@@ -20,8 +20,8 @@
 // fp32 gradients into fp64 bins, so fp32 accumulation is not good enough to reproduce its
 // tree structure.  We therefore split a 36-bit fixed-point value into two 18-bit fields and
 // accumulate each with a native 32-bit atomic; 2^14 rows can be added before a field can
-// overflow, then the CTA flushes its sub-histogram into the int64 leaf histogram in L2 with
-// RED.ADD.64.  Integer sums are exact and order-independent, so the result is bit-reproducible
+// overflow, then the CTA flushes its sub-histogram into the int64 leaf histogram in L2 (v2: RED.ADD.64
+// per bin; v3: TMA bulk reductions, UBLKRED.G.S.ADD.U64).  Integer sums are exact and order-independent, so the result is bit-reproducible
 // run to run and across ranks (the NCCL reduction is an int64 sum).
 //
 // Bank mapping: the sub-histogram planes are laid out [bin][feature-of-tile], so feature f lives in
@@ -42,6 +42,9 @@ constexpr int kTileFeat = 32;                      // features per tile == lanes
 constexpr int kBins = 256;                         // uint8 bin ids
 constexpr int kLoBits = 18;                        // low fixed-point field
 constexpr int kFlushRows = 1 << (32 - kLoBits);    // rows a sub-histogram may absorb (16384)
+// Cost-model builds of k4_hist_build_ws for tools/ubench_hist.cu; every mode but 0 computes WRONG histograms.
+//   1 / 2 / 3: the scatter loop issues 0 / 1 / 2 shared atomics per cell;
+//   4: full scatter loop, the flush reads and zeroes the planes but sends nothing to the global histogram.
 #ifndef B200GBM_K4_EXPERIMENT
 #define B200GBM_K4_EXPERIMENT 0
 #endif
@@ -260,7 +263,16 @@ constexpr int kWsProducerWarps = B200GBM_WS_PRODUCERS;            // 1 lane issu
 constexpr int kWsThreads = (kWsConsumerWarps + kWsProducerWarps) * 32;
 constexpr int kWsStageRows = 512;
 constexpr int kWsStages = 3;
-constexpr int kWsSmemBytes = 4 * kPlaneWords * 4 + kWsStages * (kWsStageRows * 32 + kWsStageRows * 16) + 64;
+// Flush staging: one slab of 32 bins x 32 features as int64 (g,h) pairs laid out like the global histogram ([feature][bin][2]),
+// one 512-byte row per feature.  Lane l handles feature l and slab bin (j + l) & 31 for j = warp and warp + 16: its plane word sits in bank l
+// and the 8 lanes of a quarter-warp store their 16-byte pairs at 8 consecutive bin slots mod 8, so reads and stores are conflict-free
+// without padding and every row stays 128-byte aligned for the bulk reduction.
+constexpr int kFlushSlabBins = 32;
+constexpr int kFlushRowBytes = kFlushSlabBins * 16;
+constexpr int kFlushStageBytes = kTileFeat * kFlushRowBytes;     // 16 KB
+constexpr int kWsSmemBytes = 4 * kPlaneWords * 4 + kWsStages * (kWsStageRows * 32 + kWsStageRows * 16) + kFlushStageBytes + 64;
+static_assert(kWsSmemBytes <= 227 * 1024, "K4 shared memory exceeds the 227 KB per block of sm_90");
+static_assert(kFlushSlabBins * kTileFeat == 2 * kWsConsumerWarps * 32, "a flush slab is two (g,h) pairs per consumer thread");
 
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
@@ -294,6 +306,19 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(unsigned long long* bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
+// TMA bulk reduction: gmem[i] += smem[i] for bytes/8 u64 elements (UBLKRED.G.S.ADD.U64), tracked by the issuing thread's bulk groups.
+// The PTX ISA (cp.reduce.async.bulk, ISA 8.0) gives each element's reduction .relaxed.gpu memory-ordering semantics, i.e. every
+// element is an atomic read-modify-write at GPU scope, so the reductions of CTAs that flush the same feature tile concurrently all land.
+__device__ __forceinline__ void bulk_reduce_add_u64(unsigned long long* gmem_dst, const void* smem_src, unsigned bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;\n" ::"l"(gmem_dst), "r"(smem_u32(smem_src)),
+               "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }   // sources read
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }             // writes done
+// generic-proxy shared-memory writes before this fence are visible to the async proxy (TMA) after the following barrier
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 template <int NATOM>
 __global__ void __launch_bounds__(kWsThreads, 1)
@@ -304,7 +329,8 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
   unsigned* plane = reinterpret_cast<unsigned*>(smem_raw);
   unsigned char* stage_bins = smem_raw + 4 * kPlaneWords * 4;
   int4* stage_q = reinterpret_cast<int4*>(stage_bins + kWsStages * kWsStageRows * 32);
-  unsigned long long* full_bar = reinterpret_cast<unsigned long long*>(reinterpret_cast<unsigned char*>(stage_q) + kWsStages * kWsStageRows * 16);
+  unsigned char* flush_stage = reinterpret_cast<unsigned char*>(stage_q) + kWsStages * kWsStageRows * 16;   // [feature][kFlushRowBytes]
+  unsigned long long* full_bar = reinterpret_cast<unsigned long long*>(flush_stage + kFlushStageBytes);
   unsigned long long* empty_bar = full_bar + kWsStages;
 
   const HistWork w = *work;
@@ -393,7 +419,7 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
     // 16-byte q load (4 LSU wavefronts for a warp) is paid once per 1024 cells instead of once per 128.  At step k the lane reads
     // bin word w = ((lane>>2)+k)&7 of its row: bank = 8*(lane&3)+w, all 32 distinct.  Inside the word the byte order is rotated
     // by lane&3, so the 32 atomics of one instruction hit features 4w+kk = 32 distinct banks (plane index = bin*32 + feature).
-#if B200GBM_K4_EXPERIMENT != 0
+#if B200GBM_K4_EXPERIMENT >= 1 && B200GBM_K4_EXPERIMENT <= 3
     unsigned exp_sink = 0;
 #endif
     const int sub = lane >> 2, rot = lane & 3;
@@ -424,7 +450,7 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
                 const int kk = (j + rot) & 3;
                 const unsigned b = (word >> (8 * kk)) & 0xFFu;
                 const unsigned a = b * 32u + static_cast<unsigned>(w8 * 4 + kk);
-#if B200GBM_K4_EXPERIMENT == 0
+#if B200GBM_K4_EXPERIMENT == 0 || B200GBM_K4_EXPERIMENT == 4
                 atomicAdd(&plane[a], static_cast<unsigned>(q.x));
                 atomicAdd(&plane[kPlaneWords + a], static_cast<unsigned>(q.y));
                 atomicAdd(&plane[2 * kPlaneWords + a], static_cast<unsigned>(q.z));
@@ -438,7 +464,7 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
             }
           }
         }
-#if B200GBM_K4_EXPERIMENT != 0
+#if B200GBM_K4_EXPERIMENT >= 1 && B200GBM_K4_EXPERIMENT <= 3
         if (exp_sink == 0x12345679u) plane[lane] = exp_sink;
 #endif
         __syncwarp();
@@ -453,29 +479,67 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
       }
       if (!flush) continue;
       acc_rows = 0;
-      // all consumers finished: flush the sub-histogram (consumer-only named barrier; the producers keep staging)
+      // All consumers finished: flush the sub-histogram into the int64 leaf histogram (consumer-only named barriers; the producers
+      // keep staging).  Slab by slab (32 bins x 32 features), every consumer thread reads and re-zeroes the plane words of two
+      // (bin, feature) cells, combines them into int64 (g,h) and stores the pairs into the staging buffer in the histogram's own
+      // [feature][bin][2] order; thread 0 then sends each feature's 512-byte run to L2 with one TMA bulk reduction.  Scattered
+      // 64-bit REDs (one cache line per lane, all through the LSU) cost 19-40 % of the kernel's time on H100 (DESIGN.md §3); the bulk
+      // reductions run in the TMA unit beside the next slab's plane reads and the next item's atomics.
       asm volatile("bar.sync 1, %0;\n" ::"n"(kWsConsumerWarps * 32) : "memory");
-      for (int e = tid; e < kPlaneWords; e += kWsConsumerWarps * 32) {
-        unsigned ghi = plane[e], glo = plane[kPlaneWords + e];
-        unsigned hhi = plane[2 * kPlaneWords + e];
-        unsigned hlo = (NATOM == 4) ? plane[3 * kPlaneWords + e] : 0u;
-        if (ghi | glo | hhi | hlo) {
-          const int f = tile * 32 + (e & 31);
-          const int b = e >> 5;
-          long long g = (static_cast<long long>(static_cast<int>(ghi)) << kLoBits) + static_cast<long long>(glo);
-          long long h = (NATOM == 4) ? (static_cast<long long>(static_cast<int>(hhi)) << kLoBits) + static_cast<long long>(hlo)
-                                     : static_cast<long long>(hhi);
-          const size_t o = (static_cast<size_t>(f) * kBins + b) * 2;
-          if (g) atomicAdd(&hist[o], static_cast<unsigned long long>(g));
-          if (h) atomicAdd(&hist[o + 1], static_cast<unsigned long long>(h));
+      unsigned long long* htile = hist + static_cast<size_t>(tile) * kTileFeat * kBins * 2;
+      int sbin[2];                                                  // slab bin of this thread's two cells; its feature is `lane`
+#pragma unroll
+      for (int i = 0; i < 2; ++i) sbin[i] = (warp + i * kWsConsumerWarps + lane) & (kFlushSlabBins - 1);
+      for (int b0 = 0; b0 < kBins; b0 += kFlushSlabBins) {
+        long long g[2], h[2];
+        bool nz = false;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int e = (b0 + sbin[i]) * kTileFeat + lane;          // plane index = bin*32 + feature
+          const unsigned ghi = plane[e], glo = plane[kPlaneWords + e], hhi = plane[2 * kPlaneWords + e];
+          const unsigned hlo = (NATOM == 4) ? plane[3 * kPlaneWords + e] : 0u;
           plane[e] = 0u;
           plane[kPlaneWords + e] = 0u;
           plane[2 * kPlaneWords + e] = 0u;
           if (NATOM == 4) plane[3 * kPlaneWords + e] = 0u;
+          nz |= (ghi | glo | hhi | hlo) != 0u;
+          g[i] = (static_cast<long long>(static_cast<int>(ghi)) << kLoBits) + static_cast<long long>(glo);
+          h[i] = (NATOM == 4) ? (static_cast<long long>(static_cast<int>(hhi)) << kLoBits) + static_cast<long long>(hlo)
+                              : static_cast<long long>(hhi);   // plain row count
         }
+        // the previous slab's reductions must have read the staging buffer before it is overwritten
+        if (tid == 0) bulk_wait_read_all();
+        asm volatile("bar.sync 1, %0;\n" ::"n"(kWsConsumerWarps * 32) : "memory");
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          *reinterpret_cast<longlong2*>(flush_stage + lane * kFlushRowBytes + sbin[i] * 16) = make_longlong2(g[i], h[i]);
+        fence_proxy_async_smem();
+        // barrier + OR of "this slab has a non-zero cell": an all-zero slab (small leaves) sends nothing
+        int any;
+        asm volatile(
+            "{\n"
+            ".reg .pred p, q;\n"
+            "setp.ne.u32 p, %1, 0;\n"
+            "bar.red.or.pred q, 1, %2, p;\n"
+            "selp.s32 %0, 1, 0, q;\n"
+            "}\n"
+            : "=r"(any)
+            : "r"(static_cast<unsigned>(nz)), "n"(kWsConsumerWarps * 32)
+            : "memory");
+#if B200GBM_K4_EXPERIMENT != 4
+        if (tid == 0 && any) {
+          for (int f = 0; f < kTileFeat; ++f)
+            bulk_reduce_add_u64(htile + (static_cast<size_t>(f) * kBins + b0) * 2, flush_stage + f * kFlushRowBytes, kFlushSlabBins * 16);
+          bulk_commit();
+        }
+#else
+        (void)any; (void)htile;
+#endif
       }
-      asm volatile("bar.sync 1, %0;\n" ::"n"(kWsConsumerWarps * 32) : "memory");
+      // the planes are zero again (every plane write precedes the last barrier above); the staging buffer is guarded by the wait
     }
+    // the bulk reductions read shared memory and write the histogram that the next kernel scans: complete them before exiting
+    if (tid == 0) bulk_wait_all();
   }
 }
 
