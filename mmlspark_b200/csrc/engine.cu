@@ -570,7 +570,7 @@ void Dataset::GetBinsOfRows(const int32_t* rows, int nrows, uint16_t* out) const
 
 void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const {
   EnsureDevice();
-  B200_CUDA(cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes));
+  B200_CUDA(set_k4_smem_limit());
   const int n = num_data;
   DevBuf<float> g, h; g.Alloc(n); h.Alloc(n);
   g.Upload(grad, n, stream); h.Upload(hess, n, stream);
@@ -590,8 +590,8 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   B200_CUDA(cudaMemcpyAsync(&ctrl.p->hist_work, &w, sizeof(w), cudaMemcpyHostToDevice, stream));
   DevBuf<int4> qo; qo.Alloc(std::max(cnt, 1));
   k_gather_q<<<sms * 4, 256, 0, stream>>>(&ctrl.p->hist_work, didx.p, didx.p, q.p, qo.p);
-  k4_hist_build_ws<4><<<sms, kWsThreads, kWsSmemBytes, stream>>>(bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
-                                                                 reinterpret_cast<unsigned long long*>(H.p));
+  launch_k4(/*const_hessian=*/false, bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
+            reinterpret_cast<unsigned long long*>(H.p), sms, stream);
   k_hist_to_double<<<sms * 4, 256, 0, stream>>>(H.p, D.p, elems, ctrl.p);
   B200_CUDA(cudaGetLastError());
   std::vector<double> hd(elems);
@@ -1010,8 +1010,7 @@ void Booster::InitTraining() {
   // A hint for the sparse leaf passes; streamed passes read whole sectors anyway.
   cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   cudaGetLastError();
-  B200_CUDA(cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes));
-  B200_CUDA(cudaFuncSetAttribute(k4_hist_build_ws<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes));
+  B200_CUDA(set_k4_smem_limit());
   B200_CUDA(cudaFuncSetAttribute(k_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
 
   sp_.l1 = cfg.lambda_l1; sp_.l2 = cfg.lambda_l2; sp_.max_delta_step = cfg.max_delta_step;
@@ -1685,12 +1684,8 @@ void Booster::TrainOneTree(int k, HostTree* out) {
     mark();
     // the scratch histogram H is zero here: zeroed at set-up and by every partition kernel after the scan consumed it
     nvtxRangePushA("b200gbm:K4 histogram");
-    if (const_hessian_)
-      k4_hist_build_ws<3><<<num_sms_, kWsThreads, kWsSmemBytes, s>>>(d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-                                                                     reinterpret_cast<unsigned long long*>(H_.p));
-    else
-      k4_hist_build_ws<4><<<num_sms_, kWsThreads, kWsSmemBytes, s>>>(d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-                                                                     reinterpret_cast<unsigned long long*>(H_.p));
+    launch_k4(const_hessian_, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
+              reinterpret_cast<unsigned long long*>(H_.p), num_sms_, s);
     if (d.nw > 0) {      // the features with more than 256 bins: own sub-histogram layout (k4_hist_wide)
       int max_nb = 0;
       for (const WideMeta& wm : d.wide_host) max_nb = std::max(max_nb, wm.num_bin);

@@ -20,18 +20,16 @@
 // fp32 gradients into fp64 bins, so fp32 accumulation is not good enough to reproduce its
 // tree structure.  We therefore split a 36-bit fixed-point value into two 18-bit fields and
 // accumulate each with a native 32-bit atomic; 2^14 rows can be added before a field can
-// overflow, then the CTA flushes its sub-histogram into the int64 leaf histogram in L2 (v2: RED.ADD.64
-// per bin; v3: TMA bulk reductions, UBLKRED.G.S.ADD.U64).  Integer sums are exact and order-independent, so the result is bit-reproducible
+// overflow, then the CTA flushes its sub-histogram into the int64 leaf histogram in L2 with TMA bulk
+// reductions (UBLKRED.G.S.ADD.U64).  Integer sums are exact and order-independent, so the result is bit-reproducible
 // run to run and across ranks (the NCCL reduction is an int64 sum).
 //
 // Bank mapping: the sub-histogram planes are laid out [bin][feature-of-tile], so feature f lives in
-// bank f.  Every ATOMS instruction of a warp addresses 32 DIFFERENT features, so it is conflict-free by
-// construction regardless of the bin distribution (ncu: 1.0 wavefront per ATOMS).
-//   k4_hist_build    (v2): warp step = 4 rows x 32 features, lane = (row selector, bin word), bytes rotated by the row selector.
-//   k4_hist_build_ws (v3, the engine's kernel): warp step = 32 rows x 4 features, lane = row for 8 steps; the lane's (g,h)
-//     quadruple stays in registers (one 16-byte LDS per 32 cells instead of one per 4), bin word and byte rotated by the lane id.
-// The LSU data pipe is the binding unit (ncu: ~94 % busy): an ATOMS wavefront costs ~0.93 cycles, so the v3 loop spends
-// 16 x 0.93 (atomics) + 1 (bin word) + 0.5 (q) cycles per 128 cells.
+// bank f.  A consumer warp step is 32 rows x 4 features: lane = row for 8 steps, its (g,h) quadruple stays in registers
+// (one 16-byte LDS per 32 cells), and the bin word and byte are rotated by the lane id, so every ATOMS instruction of a warp
+// addresses 32 DIFFERENT features: conflict-free by construction regardless of the bin distribution (ncu: 1.0 wavefront per ATOMS).
+// The LSU data pipe is the binding unit (ncu: ~94 % busy): an ATOMS wavefront costs ~0.93 cycles, so the loop spends
+// 16 x 0.93 (atomics) + 1 (bin word) + 0.5 (q) cycles per 128 cells.  DESIGN.md §3 has the measurements and the rejected variants.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -48,23 +46,7 @@ constexpr int kFlushRows = 1 << (32 - kLoBits);    // rows a sub-histogram may a
 #ifndef B200GBM_K4_EXPERIMENT
 #define B200GBM_K4_EXPERIMENT 0
 #endif
-#ifndef B200GBM_STAGE_ROWS
-#define B200GBM_STAGE_ROWS 512
-#endif
-#ifndef B200GBM_STAGES
-#define B200GBM_STAGES 3
-#endif
-#ifndef B200GBM_HIST_THREADS
-#define B200GBM_HIST_THREADS 512
-#endif
-constexpr int kStageRows = B200GBM_STAGE_ROWS;     // rows per staged sub-chunk
-constexpr int kStages = B200GBM_STAGES;            // cp.async ring depth
-constexpr int kHistThreads = B200GBM_HIST_THREADS;
-constexpr int kStageSlots = (kStageRows * 2 + kHistThreads - 1) / kHistThreads;   // half-rows a thread stages per stage
-constexpr int kHistWarps = kHistThreads / 32;
 constexpr int kPlaneWords = kBins * kTileFeat;     // 8192 words per plane
-constexpr int kHistSmemBytes =
-    4 * kPlaneWords * 4 + kStages * (kStageRows * 32 + kStageRows * 16);
 
 // Device-resident work descriptor: the controller kernels write it, so the host never has to
 // know leaf sizes (no host sync inside a tree).
@@ -94,172 +76,23 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool va
   int sz = valid ? 16 : 0;   // src-size 0 => zero fill, nothing is read
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(sz));
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
-// NATOM selects how many planes are accumulated: 4 = (g_hi,g_lo,h_hi,h_lo) general case,
-// 3 = constant-hessian objectives (g_hi,g_lo,count) [UPSTREAM is_constant_hessian path].
-template <int NATOM>
-__global__ void __launch_bounds__(kHistThreads, 1)
-k4_hist_build(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles,
-              const int4* __restrict__ qgh, const int* __restrict__ idx0, const int* __restrict__ idx1,
-              const HistWork* __restrict__ work, unsigned long long* __restrict__ hist) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  unsigned* plane = reinterpret_cast<unsigned*>(smem_raw);              // [4][kPlaneWords]
-  unsigned char* stage_bins = smem_raw + 4 * kPlaneWords * 4;           // [kStages][256][32]
-  int4* stage_q = reinterpret_cast<int4*>(stage_bins + kStages * kStageRows * 32);  // [kStages][256]
-
-  const HistWork w = *work;
-  const int n = w.count;
-  if (n <= 0) return;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int* __restrict__ idx = w.buf ? idx1 : idx0;
-
-  // rows per work item: large enough to amortise the flush, small enough to fill the grid
-  long long cells_rows = static_cast<long long>(n) * num_tiles;
-  int rpi = static_cast<int>((cells_rows + gridDim.x - 1) / gridDim.x);
-  rpi = max(rpi, 2048);
-  rpi = min(rpi, kFlushRows);
-  rpi = (rpi + kStageRows - 1) / kStageRows * kStageRows;
-  const int chunks = (n + rpi - 1) / rpi;
-  const int items = chunks * num_tiles;
-
-  for (int e = tid; e < 4 * kPlaneWords; e += kHistThreads) plane[e] = 0u;
-  __syncthreads();
-
-  for (int item = blockIdx.x; item < items; item += gridDim.x) {
-    const int tile = item % num_tiles;
-    const int chunk = item / num_tiles;
-    const int row0 = chunk * rpi;                       // position inside the leaf
-    const int nrows = min(rpi, n - row0);
-    const int nst = (nrows + kStageRows - 1) / kStageRows;
-    const uint8_t* tbins = bins + static_cast<size_t>(tile) * rows_stride * 32;
-
-    // a "slot" = half a row of bins (16 B); the thread that stages half 0 also stages the row's qgh word
-    auto row_of = [&](int st, int slot) -> int {
-      int hrow = slot * kHistThreads + tid;
-      if (hrow >= kStageRows * 2) return -1;
-      int p = row0 + st * kStageRows + (hrow >> 1);
-      if (p >= row0 + nrows) return -1;
-      return w.use_idx ? idx[w.begin + p] : (w.begin + p);
-    };
-    auto issue = [&](int st, int slot, int r) {
-      int hrow = slot * kHistThreads + tid;
-      if (hrow >= kStageRows * 2) return;
-      int srow = hrow >> 1, shalf = hrow & 1;
-      int buf = st % kStages;
-      bool ok = r >= 0;
-      size_t rr = ok ? static_cast<size_t>(r) : 0;
-      cp_async16(stage_bins + (buf * kStageRows + srow) * 32 + shalf * 16,
-                 tbins + rr * 32 + shalf * 16, ok);
-      if (shalf == 0) cp_async16(stage_q + buf * kStageRows + srow, qgh + rr, ok);
-    };
-
-    int rnext[kStageSlots];
-#pragma unroll
-    for (int sl = 0; sl < kStageSlots; ++sl) rnext[sl] = row_of(0, sl);
-#pragma unroll
-    for (int s = 0; s < kStages - 1; ++s) {
-      if (s < nst) {
-#pragma unroll
-        for (int sl = 0; sl < kStageSlots; ++sl) {
-          int r = rnext[sl];
-          rnext[sl] = (s + 1 < nst) ? row_of(s + 1, sl) : -1;
-          issue(s, sl, r);
-        }
-      }
-      cp_async_commit();
-    }
-    for (int s = 0; s < nst; ++s) {
-      cp_async_wait<kStages - 2>();
-      __syncthreads();
-      int sn = s + kStages - 1;
-      if (sn < nst) {
-#pragma unroll
-        for (int sl = 0; sl < kStageSlots; ++sl) {
-          int r = rnext[sl];
-          rnext[sl] = (sn + 1 < nst) ? row_of(sn + 1, sl) : -1;
-          issue(sn, sl, r);
-        }
-      }
-      cp_async_commit();
-
-      const int buf = s % kStages;
-      const unsigned* sw = reinterpret_cast<const unsigned*>(stage_bins + buf * kStageRows * 32);   // 8 words per row
-      const int4* sq = stage_q + buf * kStageRows;
-      // One warp step = 4 rows x 32 features.  Lane = (rsel = lane>>3, word = lane&7) reads the 4 bins of features
-      // 4*word..4*word+3 of row r0+rsel with ONE LDS.32 (the warp reads 128 contiguous bytes) and that row's 4
-      // fixed-point words with one LDS.128.  In sub-step k it handles feature 4*word + ((k+rsel)&3): for fixed k the map
-      // (rsel, word) -> feature is a bijection onto 0..31, and plane[.][bin*32+feature] puts feature f in bank f, so all
-      // 32 lanes hit distinct banks for ANY bin values: 16 conflict-free ATOMS per 128 cells, loads amortised 4x.
-      const int rsel = lane >> 3, wsel = lane & 7;
-#pragma unroll 2
-      for (int k4 = 0; k4 < kStageRows / (4 * kHistWarps); ++k4) {
-        const int r = (warp + k4 * kHistWarps) * 4 + rsel;
-        const unsigned word = sw[r * 8 + wsel];
-        const int4 q = sq[r];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int kk = (k + rsel) & 3;
-          const unsigned b = (word >> (8 * kk)) & 0xFFu;
-          const unsigned a = b * 32u + static_cast<unsigned>(wsel * 4 + kk);
-          atomicAdd(&plane[a], static_cast<unsigned>(q.x));
-          atomicAdd(&plane[kPlaneWords + a], static_cast<unsigned>(q.y));
-          atomicAdd(&plane[2 * kPlaneWords + a], static_cast<unsigned>(q.z));
-          if (NATOM == 4) atomicAdd(&plane[3 * kPlaneWords + a], static_cast<unsigned>(q.w));
-        }
-      }
-    }
-    cp_async_wait<0>();
-    __syncthreads();
-    // flush the sub-histogram into the leaf histogram (int64, L2-resident) and re-zero it
-    for (int e = tid; e < kPlaneWords; e += kHistThreads) {
-      unsigned ghi = plane[e], glo = plane[kPlaneWords + e];
-      unsigned hhi = plane[2 * kPlaneWords + e];
-      unsigned hlo = (NATOM == 4) ? plane[3 * kPlaneWords + e] : 0u;
-      if (ghi | glo | hhi | hlo) {
-        int f = tile * 32 + (e & 31);
-        int b = e >> 5;
-        long long g = (static_cast<long long>(static_cast<int>(ghi)) << kLoBits) +
-                      static_cast<long long>(glo);
-        long long h;
-        if (NATOM == 4)
-          h = (static_cast<long long>(static_cast<int>(hhi)) << kLoBits) +
-              static_cast<long long>(hlo);
-        else
-          h = static_cast<long long>(hhi);   // plain row count
-        size_t o = (static_cast<size_t>(f) * kBins + b) * 2;
-        if (g) atomicAdd(&hist[o], static_cast<unsigned long long>(g));
-        if (h) atomicAdd(&hist[o + 1], static_cast<unsigned long long>(h));
-        plane[e] = 0u;
-        plane[kPlaneWords + e] = 0u;
-        plane[2 * kPlaneWords + e] = 0u;
-        if (NATOM == 4) plane[3 * kPlaneWords + e] = 0u;
-      }
-    }
-    __syncthreads();
-  }
-}
-
-
 // ===================================================================================================
-// K4 v3 — warp-specialised variant: one PRODUCER warp stages rows into a ring of shared-memory stages,
+// k4_hist_build_ws is warp-specialised: two PRODUCER warps stage rows into a ring of shared-memory stages,
 // 16 CONSUMER warps do nothing but the conflict-free scatter.  Stages are handed over with mbarriers
-// (full / empty), so there is no block-wide barrier per stage and the producer runs ahead across work
-// items (it prefetches the next item while the consumers flush the current sub-histogram).
+// (full / empty), so there is no block-wide barrier per stage and the producers run ahead across work
+// items (they prefetch the next item while the consumers flush the current sub-histogram).
 //   * contiguous row ranges (root pass, use_idx == 0): TMA bulk copies — one elected lane issues
 //     cp.async.bulk (UBLKCP) for the stage's bins (rows*32 B) and qgh (rows*16 B), completion is signalled
 //     by the mbarrier's transaction count;
-//   * index-list leaves: the 32 producer lanes issue 16-byte cp.async gathers (LDGSTS) and arrive on the
+//   * index-list leaves: all producer lanes issue 16-byte cp.async gathers (LDGSTS) and arrive on the
 //     mbarrier with cp.async.mbarrier.arrive.noinc when their copies have landed.
 constexpr int kWsConsumerWarps = 16;
-#ifndef B200GBM_WS_PRODUCERS
-#define B200GBM_WS_PRODUCERS 2
-#endif
-constexpr int kWsProducerWarps = B200GBM_WS_PRODUCERS;            // 1 lane issues the TMA bulk copies; all lanes share the gathers
+constexpr int kWsProducerWarps = 2;                               // 1 lane issues the TMA bulk copies; all lanes share the gathers
 constexpr int kWsThreads = (kWsConsumerWarps + kWsProducerWarps) * 32;
 constexpr int kWsStageRows = 512;
 constexpr int kWsStages = 3;
@@ -320,6 +153,8 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 // generic-proxy shared-memory writes before this fence are visible to the async proxy (TMA) after the following barrier
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
+// NATOM selects how many planes are accumulated: 4 = (g_hi,g_lo,h_hi,h_lo) general case,
+// 3 = constant-hessian objectives (g_hi,g_lo,count) [UPSTREAM is_constant_hessian path].
 template <int NATOM>
 __global__ void __launch_bounds__(kWsThreads, 1)
 k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
@@ -543,5 +378,21 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
   }
 }
 
+// K4's shared memory exceeds the 48 KB default: raise the limit of both instantiations on the current device.  Call it once per
+// device at set-up; it is host work that does not belong in the per-split launches.
+inline cudaError_t set_k4_smem_limit() {
+  const cudaError_t e = cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(k4_hist_build_ws<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
+}
+
+// One persistent K4 launch: `grid` is one CTA per SM; constant-hessian objectives accumulate 3 planes (g_hi, g_lo, count).
+inline void launch_k4(bool const_hessian, const uint8_t* bins, size_t rows_stride, int num_tiles, const int4* qgh, const int4* qord,
+                      const int* idx0, const int* idx1, const HistWork* work, unsigned long long* hist, int grid, cudaStream_t stream) {
+  if (const_hessian)
+    k4_hist_build_ws<3><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist);
+  else
+    k4_hist_build_ws<4><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist);
+}
 
 }  // namespace b200gbm

@@ -1,16 +1,19 @@
 // Microbenchmarks that decide the K4 histogram design (build() compiles it to build/ubench_hist).
 //  Part A: shared-memory scatter-add throughput per SM for the candidate accumulator schemes
 //          (native ATOMS.ADD.32 owner-bank / random-bank, CAS float, non-atomic owner RMW ...).
-//  Part B: the production k4_hist_build kernel on synthetic tile-major bins, checked against a
-//          host computation, timed with CUDA events, reported as cells/s and algorithmic GB/s.
-// Output: one JSON document on stdout.
+//  Part B: the engine's K4 kernel (k4_hist_build_ws<4> and <3>, launched through launch_k4) on synthetic
+//          tile-major bins: checked exactly against an int64 host computation, then timed with CUDA events
+//          and reported as cells/s and algorithmic GB/s.
+// Usage: ubench_hist [ROWS] [SKIP_PART_A]   (ROWS defaults to 10M; SKIP_PART_A = 1 skips Part A)
+// Output: one JSON document on stdout.  Exit status 1 if the exact check finds a mismatch, except in the
+// B200GBM_K4_EXPERIMENT cost-model builds, whose histograms are wrong by design.
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
 #include <cmath>
 #include "../mmlspark_b200/csrc/hist_kernel.cuh"
-#include "k4_direct_load_experiment.cuh"
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { fprintf(stderr, "CUDA %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); exit(1);} } while (0)
 
@@ -34,7 +37,7 @@ ubench(int iters, unsigned long long* cyc_out, unsigned* sink) {
   for (int e = tid; e < 256; e += blockDim.x) sq[e] = make_int4(e - 100, e * 7 + 1, 3, e + 5);
   __syncthreads();
   long long t0 = clock64();
-  if (MODE == 9 || MODE == 10) {   // 4 rows x 32 features per warp step (the production mapping); 10 = 3 planes
+  if (MODE == 9 || MODE == 10) {   // 4 rows x 32 features per warp step, lane = (row selector, bin word), bytes rotated by the row selector; 10 = 3 planes
     const unsigned* sw = reinterpret_cast<const unsigned*>(sb);
     const int rsel = lane >> 3, wsel = lane & 7;
     for (int it = 0; it < iters; ++it) {
@@ -145,7 +148,7 @@ int main(int argc, char** argv) {
   printf(" \"smem_scatter_cells_per_cycle_per_sm\": {\n");
   const int it = 400;
   for (int threads : {512, 1024}) {
-    if (argc > 3 && atoi(argv[3]) == 1) { printf("  \"t%d\": {}%s\n", threads, threads == 512 ? "," : ""); continue; }
+    if (argc > 2 && atoi(argv[2]) == 1) { printf("  \"t%d\": {}%s\n", threads, threads == 512 ? "," : ""); continue; }
     printf("  \"t%d\": {", threads);
     printf("\"u32x4_rows4x32_rotated\": %.3f, ", run_mode<9>(threads, it, nsm));
     printf("\"u32x3_rows4x32_rotated\": %.3f, ", run_mode<10>(threads, it, nsm));
@@ -175,61 +178,55 @@ int main(int argc, char** argv) {
   CK(cudaMalloc(&d_q, N * sizeof(int4)));
   CK(cudaMalloc(&d_qord, N * sizeof(int4)));
   CK(cudaMalloc(&d_idx, N * sizeof(int)));
-  CK(cudaMalloc(&d_hist, slot_elems * 8 * 2));
-  CK(cudaMalloc(&d_work, sizeof(HistWork) * 4));
+  CK(cudaMalloc(&d_hist, slot_elems * 8));
+  CK(cudaMalloc(&d_work, sizeof(HistWork) * 2));
   gen_bins<<<nsm * 8, 256>>>(d_bins, rows_stride, num_tiles, N, 12345u);
   gen_q<<<nsm * 8, 256>>>(d_q, N, 777u);
   CK(cudaDeviceSynchronize());
-  CK(cudaFuncSetAttribute(k4_hist_build<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHistSmemBytes));
-  CK(cudaFuncSetAttribute(k4_hist_build<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHistSmemBytes));
-  CK(cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes));
-  CK(cudaFuncSetAttribute(k4_hist_build_ws<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes));
-  const int variant = argc > 2 ? atoi(argv[2]) : 0;      // 0 = v2, 1 = v3/v4 warp-specialised (production in round 1), 2 = v5 direct-load
-  const bool use_ws = variant == 1;
-  const bool use_dl = variant == 2;
-  CK(cudaFuncSetAttribute(k4_hist_build_dl<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDlSmemBytes));
-  CK(cudaFuncSetAttribute(k4_hist_build_dl<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDlSmemBytes));
+  CK(set_k4_smem_limit());
 
-  // correctness on the first 1M rows (contiguous) and on a strided index list
+  // exact int64 check of both instantiations on the first 1M rows: a contiguous pass and a strided index-list pass (every 3rd
+  // row), each with CTAs sharing feature tiles.  NATOM = 3 sums the count field q.z as h, as the kernel does.
+  size_t k4_bad = 0;
   {
-    int n_chk = (int)std::min<size_t>(N, 1000000);
+    const int n_chk = (int)std::min<size_t>(N, 1000000);
     HistWork hw[2] = {{0, n_chk, 0, 0}, {0, n_chk / 3, 1, 0}};
     CK(cudaMemcpy(d_work, hw, sizeof(hw), cudaMemcpyHostToDevice));
     gen_idx<<<nsm, 256>>>(d_idx, n_chk / 3, 3);
-    CK(cudaMemset(d_hist, 0, slot_elems * 8 * 2));
-    if (use_dl) {
-      k4_hist_build_dl<4><<<nsm, kDlThreads, kDlSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-      k_gather_q<<<nsm * 8, 256>>>(d_work + 1, d_idx, d_idx, d_q, d_qord);
-      k4_hist_build_dl<4><<<nsm, kDlThreads, kDlSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work + 1, d_hist + slot_elems);
-    } else if (use_ws) {
-      k4_hist_build_ws<4><<<nsm, kWsThreads, kWsSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-      k_gather_q<<<nsm * 8, 256>>>(d_work + 1, d_idx, d_idx, d_q, d_qord);
-      k4_hist_build_ws<4><<<nsm, kWsThreads, kWsSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work + 1, d_hist + slot_elems);
-    } else {
-    k4_hist_build<4><<<nsm, kHistThreads, kHistSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_idx, d_idx, d_work, d_hist);
-    k4_hist_build<4><<<nsm, kHistThreads, kHistSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_idx, d_idx, d_work + 1, d_hist + slot_elems);
-    }
+    k_gather_q<<<nsm * 8, 256>>>(d_work + 1, d_idx, d_idx, d_q, d_qord);
     CK(cudaDeviceSynchronize());
-    std::vector<long long> got(slot_elems * 2), want(slot_elems * 2, 0);
-    CK(cudaMemcpy(got.data(), d_hist, slot_elems * 16, cudaMemcpyDeviceToHost));
     std::vector<uint8_t> hb((size_t)num_tiles * rows_stride * 32);
     CK(cudaMemcpy(hb.data(), d_bins, hb.size(), cudaMemcpyDeviceToHost));
     std::vector<int4> hq(n_chk);
     CK(cudaMemcpy(hq.data(), d_q, (size_t)n_chk * 16, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < n_chk; ++i) {
-      long long g = ((long long)hq[i].x << kLoBits) + hq[i].y, h = ((long long)hq[i].z << kLoBits) + hq[i].w;
-      bool in2 = (i % 3 == 0) && (i / 3 < n_chk / 3);
-      for (int t = 0; t < num_tiles; ++t) {
-        const uint8_t* row = &hb[((size_t)t * rows_stride + i) * 32];
-        for (int l = 0; l < 32; ++l) {
-          size_t o = ((size_t)(t * 32 + l) * 256 + row[l]) * 2;
-          want[o] += g; want[o + 1] += h;
-          if (in2) { want[slot_elems + o] += g; want[slot_elems + o + 1] += h; }
+    std::vector<long long> got(slot_elems), want(slot_elems);
+    printf(" \"k4_check\": {\"rows\": %d, \"mismatches\": {", n_chk);
+    for (int natom : {4, 3}) {
+      for (int pass = 0; pass < 2; ++pass) {
+        CK(cudaMemset(d_hist, 0, slot_elems * 8));
+        launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work + pass, d_hist, nsm, 0);
+        CK(cudaGetLastError());
+        CK(cudaDeviceSynchronize());
+        CK(cudaMemcpy(got.data(), d_hist, slot_elems * 8, cudaMemcpyDeviceToHost));
+        std::fill(want.begin(), want.end(), 0LL);
+        const int step = pass ? 3 : 1;
+        for (int i = 0; i < hw[pass].count * step; i += step) {
+          const long long g = ((long long)hq[i].x << kLoBits) + hq[i].y;
+          const long long h = natom == 4 ? ((long long)hq[i].z << kLoBits) + hq[i].w : (long long)hq[i].z;
+          for (int t = 0; t < num_tiles; ++t) {
+            const uint8_t* row = &hb[((size_t)t * rows_stride + i) * 32];
+            for (int l = 0; l < 32; ++l) {
+              size_t o = ((size_t)(t * 32 + l) * 256 + row[l]) * 2;
+              want[o] += g; want[o + 1] += h;
+            }
+          }
         }
+        size_t bad = 0; for (size_t i = 0; i < want.size(); ++i) bad += (got[i] != want[i]);
+        printf("%s\"natom%d_%s\": %zu", natom == 4 && pass == 0 ? "" : ", ", natom, pass ? "gathered" : "contiguous", bad);
+        k4_bad += bad;
       }
     }
-    size_t bad = 0; for (size_t i = 0; i < want.size(); ++i) bad += (got[i] != want[i]);
-    printf(" \"k4_check\": {\"rows\": %d, \"mismatches\": %zu},\n", n_chk, bad);
+    printf("}},\n");
   }
 
   // timing: full pass (contiguous) and gathered pass (every 2nd row), NATOM 4 and 3
@@ -241,15 +238,8 @@ int main(int argc, char** argv) {
     for (int r = 0; r < reps + 2; ++r) {
       CK(cudaMemsetAsync(d_hist, 0, slot_elems * 8));
       CK(cudaEventRecord(e0));
-      if ((use_ws || use_dl) && use_idx) k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);     // part of a leaf pass: timed
-      if (use_dl) {
-        if (natom == 4) k4_hist_build_dl<4><<<nsm, kDlThreads, kDlSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-        else k4_hist_build_dl<3><<<nsm, kDlThreads, kDlSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-      } else if (use_ws) {
-        if (natom == 4) k4_hist_build_ws<4><<<nsm, kWsThreads, kWsSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-        else k4_hist_build_ws<3><<<nsm, kWsThreads, kWsSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist);
-      } else if (natom == 4) k4_hist_build<4><<<nsm, kHistThreads, kHistSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_idx, d_idx, d_work, d_hist);
-      else k4_hist_build<3><<<nsm, kHistThreads, kHistSmemBytes>>>(d_bins, rows_stride, num_tiles, d_q, d_idx, d_idx, d_work, d_hist);
+      if (use_idx) k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);     // part of a leaf pass: timed
+      launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, nsm, 0);
       CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
       float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
       if (r >= 2) { best = std::min(best, ms); tot += ms; }
@@ -265,11 +255,10 @@ int main(int argc, char** argv) {
     if (cfgs[c].use_idx) { gen_idx<<<nsm, 256>>>(d_idx, n, (int)(1.0 / cfgs[c].frac)); CK(cudaDeviceSynchronize()); }
     float ms = time_it(cfgs[c].natom, n, cfgs[c].use_idx, 5);
     double cells = (double)n * F;
-    double bytes = (double)n * F + (double)n * 16 * num_tiles / num_tiles /*qgh once per tile below*/;
-    bytes = (double)n * (F + 16.0 * num_tiles + (cfgs[c].use_idx ? 4.0 * num_tiles : 0.0)) + (double)F * 256 * 16;
+    double bytes = (double)n * (F + 16.0 * num_tiles + (cfgs[c].use_idx ? 4.0 * num_tiles : 0.0)) + (double)F * 256 * 16;
     printf("  {\"natom\": %d, \"rows\": %d, \"gather\": %d, \"ms\": %.4f, \"gcells_per_s\": %.2f, \"algo_GBps\": %.1f}%s\n",
            cfgs[c].natom, n, cfgs[c].use_idx, ms, cells / ms * 1e-6, bytes / ms * 1e-6, c + 1 < sizeof(cfgs) / sizeof(cfgs[0]) ? "," : "");
   }
   printf(" ]\n}\n");
-  return 0;
+  return (B200GBM_K4_EXPERIMENT == 0 && k4_bad != 0) ? 1 : 0;
 }
