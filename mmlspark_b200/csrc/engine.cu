@@ -32,6 +32,33 @@ struct NvtxRange {
   ~NvtxRange() { nvtxRangePop(); }
 };
 
+// Device time of the work enqueued on `stream` between construction and Ms() (CUDA events).  The events are destroyed on every
+// way out of the scope, a throw included.
+class StreamTimer {
+ public:
+  explicit StreamTimer(cudaStream_t stream) : stream_(stream) {
+    B200_CUDA(cudaEventCreate(&start_.e)); B200_CUDA(cudaEventCreate(&stop_.e));
+    B200_CUDA(cudaEventRecord(start_.e, stream_));
+  }
+  StreamTimer(const StreamTimer&) = delete;
+  StreamTimer& operator=(const StreamTimer&) = delete;
+  float Ms() {
+    B200_CUDA(cudaEventRecord(stop_.e, stream_));
+    B200_CUDA(cudaEventSynchronize(stop_.e));
+    float ms = 0;
+    B200_CUDA(cudaEventElapsedTime(&ms, start_.e, stop_.e));
+    return ms;
+  }
+
+ private:
+  struct Event {      // a member, so that an event made before a throw in the constructor is destroyed too
+    cudaEvent_t e = nullptr;
+    ~Event() { if (e) cudaEventDestroy(e); }
+  };
+  cudaStream_t stream_;
+  Event start_, stop_;
+};
+
 // =============================================================================== device / network
 static thread_local int t_device = -1;
 static thread_local Network t_net;
@@ -240,66 +267,45 @@ static FeatureBins UnpackMapper(const double* r) {
   return fb;
 }
 
-void Dataset::FindBins(const void* data, bool on_device, int data_type, int is_row_major) {
+// device, stream, sizes and parameters of a new dataset (the caller has run EnsureDevice)
+std::unique_ptr<Dataset> Dataset::NewShell(int nrow, int ncol, const char* params) {
+  std::unique_ptr<Dataset> d(new Dataset());
+  d->device = CurrentDevice();
+  B200_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
+  d->num_data = nrow; d->num_total_features = ncol;
+  d->cfg.Parse(params);
+  return d;
+}
+
+// the rows whose values define the bins
+std::vector<int> Dataset::SampleRows() const {
+  LcgRandom rnd(cfg.data_random_seed);
+  return rnd.Sample(num_data, std::min(num_data, cfg.bin_construct_sample_cnt));
+}
+
+// Mappers and feature names of a new dataset.  With a reference they are the reference's and the bin parameters are not checked.
+// Otherwise the bin parameters are checked, then sample(&nz, f0, f1) fills nz[f] with the sampled values of feature f that are
+// NaN or have |v| > 1e-35 (at least for this rank's features f0 <= f < f1) and returns the number of sampled rows.
+template <typename Sample>
+void Dataset::SetMappers(const Dataset* reference, Sample sample) {
   const int n = num_data, F = num_total_features;
+  if (reference) {
+    if (reference->num_total_features != F) Fatal("Validation data has a different number of features than the reference dataset");
+    mappers = reference->mappers;
+    feature_names = reference->feature_names;
+    return;
+  }
   if (cfg.max_bin >= kWideMaxBins) Fatal("max_bin >= " + std::to_string(kWideMaxBins) + " is not supported");
   if (cfg.max_bin < 2) Fatal("max_bin should be >= 2");
   if (cfg.zero_as_missing) Fatal("zero_as_missing=true is not supported by this build");
-  LcgRandom rnd(cfg.data_random_seed);
-  int sample_cnt = n < cfg.bin_construct_sample_cnt ? n : cfg.bin_construct_sample_cnt;
-  std::vector<int> rows = rnd.Sample(n, sample_cnt);
-  sample_cnt = static_cast<int>(rows.size());
-  std::vector<double> S(static_cast<size_t>(sample_cnt) * F);
-  if (on_device) {
-    DevBuf<int> d_rows; d_rows.Alloc(sample_cnt);
-    DevBuf<double> d_S; d_S.Alloc(S.size());
-    d_rows.Upload(rows.data(), sample_cnt, stream);
-    int grid = static_cast<int>(std::min<size_t>((S.size() + 255) / 256, static_cast<size_t>(DeviceSMs()) * 32));
-    if (data_type == 0) k_gather_rows<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
-    else k_gather_rows<double><<<grid, 256, 0, stream>>>(static_cast<const double*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
-    B200_CUDA(cudaGetLastError());
-    d_S.Download(S.data(), S.size(), stream);
-    B200_CUDA(cudaStreamSynchronize(stream));
-  } else {
-#pragma omp parallel for schedule(static)
-    for (int s = 0; s < sample_cnt; ++s) {
-      const long long r = rows[s];
-      for (int f = 0; f < F; ++f) {
-        double v;
-        if (data_type == 0) v = is_row_major ? static_cast<const float*>(data)[r * F + f] : static_cast<const float*>(data)[static_cast<long long>(f) * n + r];
-        else v = is_row_major ? static_cast<const double*>(data)[r * F + f] : static_cast<const double*>(data)[static_cast<long long>(f) * n + r];
-        S[static_cast<size_t>(s) * F + f] = v;
-      }
-    }
-  }
-  std::vector<std::vector<double>> nz(F);
-  {
-    const int world = Net().active ? Net().world : 1, rank = Net().active ? Net().rank : 0;
-    int step = std::max(1, (F + world - 1) / world);
-    const int f0 = world == 1 ? 0 : std::min(F, rank * step), f1 = world == 1 ? F : std::min(F, f0 + step);
-#pragma omp parallel for schedule(dynamic)
-    for (int f = f0; f < f1; ++f) {
-      nz[f].reserve(sample_cnt);
-      for (int s = 0; s < sample_cnt; ++s) {
-        double v = S[static_cast<size_t>(s) * F + f];
-        if (std::fabs(v) > kZeroThr || std::isnan(v)) nz[f].push_back(v);
-      }
-    }
-  }
-  FindBinsFromColumns(&nz, sample_cnt);
-}
-
-// nz[f] = sampled values of feature f with |v| > 1e-35 or NaN (only this rank's slice needs filling)
-void Dataset::FindBinsFromColumns(std::vector<std::vector<double>>* nzp, int sample_cnt) {
-  NvtxRange nvtx("b200gbm:find bins (host) + C5 mapper all-gather");
-  std::vector<std::vector<double>>& nz = *nzp;
-  const int n = num_data, F = num_total_features;
-  const int filter_cnt = static_cast<int>(static_cast<double>(cfg.min_data_in_leaf) * sample_cnt / n);
   // feature ownership for distributed bin finding (SURVEY.md fact 9, A.2): contiguous slices of ceil(F/R)
   const int world = Net().active ? Net().world : 1, rank = Net().active ? Net().rank : 0;
-  int step = (F + world - 1) / world;
-  if (step < 1) step = 1;
+  const int step = std::max(1, (F + world - 1) / world);
   const int f0 = world == 1 ? 0 : std::min(F, rank * step), f1 = world == 1 ? F : std::min(F, f0 + step);
+  std::vector<std::vector<double>> nz(F);
+  const int sample_cnt = sample(&nz, f0, f1);
+  NvtxRange nvtx("b200gbm:find bins (host) + C5 mapper all-gather");
+  const int filter_cnt = static_cast<int>(static_cast<double>(cfg.min_data_in_leaf) * sample_cnt / n);
   mappers.assign(F, FeatureBins());
 #pragma omp parallel for schedule(dynamic)
   for (int f = f0; f < f1; ++f) {
@@ -330,6 +336,8 @@ void Dataset::FindBinsFromColumns(std::vector<std::vector<double>>* nzp, int sam
       mappers[f] = UnpackMapper(&recv[(static_cast<size_t>(owner) * step + off) * kMapperRecord]);
     }
   }
+  feature_names.resize(F);
+  for (int f = 0; f < F; ++f) feature_names[f] = "Column_" + std::to_string(f);
 }
 
 void Dataset::UploadMeta() {
@@ -399,10 +407,12 @@ void Dataset::UploadMeta() {
   B200_CUDA(cudaStreamSynchronize(stream));
 }
 
-// bins (tiles + wide columns) of a freshly created dataset
-static void AllocBins(Dataset* d) {
-  d->bins.Alloc(static_cast<size_t>(d->num_tiles) * d->rows_stride * 32);
-  if (d->nw > 0) d->bins16.Alloc(static_cast<size_t>(d->nw) * d->rows_stride);
+// last step of every create once the mappers are set: their device tables, and the bins (tiles + wide columns) of num_data rows
+void Dataset::AllocBins() {
+  UploadMeta();
+  rows_stride = static_cast<size_t>(num_data);
+  bins.Alloc(static_cast<size_t>(num_tiles) * rows_stride * 32);
+  if (nw > 0) bins16.Alloc(static_cast<size_t>(nw) * rows_stride);
 }
 
 template <typename T>
@@ -483,20 +493,12 @@ Dataset* Dataset::CreateFromSampledColumn(double** sample_data, int** sample_ind
   (void)sample_indices;
   EnsureDevice();
   if (num_total_row <= 0 || ncol <= 0) Fatal("Dataset should have at least one row and one column");
-  std::unique_ptr<Dataset> d(new Dataset());
-  d->device = CurrentDevice();
-  B200_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-  d->num_data = num_total_row; d->num_total_features = ncol;
-  d->cfg.Parse(params);
-  if (d->cfg.max_bin >= kWideMaxBins) Fatal("max_bin >= " + std::to_string(kWideMaxBins) + " is not supported");
-  std::vector<std::vector<double>> nz(ncol);
-  for (int f = 0; f < ncol; ++f) nz[f].assign(sample_data[f], sample_data[f] + num_per_col[f]);
-  d->FindBinsFromColumns(&nz, num_sample_row);
-  d->feature_names.resize(ncol);
-  for (int f = 0; f < ncol; ++f) d->feature_names[f] = "Column_" + std::to_string(f);
-  d->UploadMeta();
-  d->rows_stride = static_cast<size_t>(num_total_row);
-  AllocBins(d.get());
+  std::unique_ptr<Dataset> d = NewShell(num_total_row, ncol, params);
+  d->SetMappers(nullptr, [&](std::vector<std::vector<double>>* nz, int, int) {      // the caller sampled the rows and dropped the zeros
+    for (int f = 0; f < ncol; ++f) (*nz)[f].assign(sample_data[f], sample_data[f] + num_per_col[f]);
+    return num_sample_row;
+  });
+  d->AllocBins();
   return d.release();
 }
 
@@ -504,38 +506,29 @@ void Dataset::PushRows(const void* data, int data_type, int nrow, int ncol, int 
   EnsureDevice();
   if (ncol != num_total_features) Fatal("PushRows: wrong number of columns");
   if (data_type != 0 && data_type != 1) Fatal("PushRows: unknown data type");
-  cudaEvent_t e0, e1;
-  B200_CUDA(cudaEventCreate(&e0)); B200_CUDA(cudaEventCreate(&e1));
-  B200_CUDA(cudaEventRecord(e0, stream));
+  StreamTimer timer(stream);
   BinBlock(data, IsDevicePointer(data), data_type, 1, nrow, start_row);
-  B200_CUDA(cudaEventRecord(e1, stream));
-  B200_CUDA(cudaEventSynchronize(e1));
-  float ms = 0;
-  B200_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  ingest_ms += ms;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  ingest_ms += timer.Ms();
 }
 
-void Dataset::GetBinsRowMajor(uint8_t* out) const {
-  if (nw > 0) Fatal("this dataset has features with more than 256 bins: use B200GBM_DatasetGetBins16");
+// the uint8 tile features' bins into out[num_data][num_total_features]; every other column is zero
+template <typename T>
+void Dataset::UnpackTiles(T* out) const {
   std::vector<uint8_t> h(bins.n);
   B200_CUDA(cudaMemcpy(h.data(), bins.p, bins.n, cudaMemcpyDeviceToHost));
-  std::memset(out, 0, static_cast<size_t>(num_data) * num_total_features);
+  std::memset(out, 0, static_cast<size_t>(num_data) * num_total_features * sizeof(T));
   for (int u = 0; u < nfn; ++u) {
     const int f = used[u];
     const uint8_t* src = h.data() + (static_cast<size_t>(u >> 5) * rows_stride) * 32 + (u & 31);
     for (int i = 0; i < num_data; ++i) out[static_cast<size_t>(i) * num_total_features + f] = src[static_cast<size_t>(i) * 32];
   }
 }
+void Dataset::GetBinsRowMajor(uint8_t* out) const {
+  if (nw > 0) Fatal("this dataset has features with more than 256 bins: use B200GBM_DatasetGetBins16");
+  UnpackTiles(out);
+}
 void Dataset::GetBinsRowMajor16(uint16_t* out) const {
-  std::vector<uint8_t> h(bins.n);
-  B200_CUDA(cudaMemcpy(h.data(), bins.p, bins.n, cudaMemcpyDeviceToHost));
-  std::memset(out, 0, static_cast<size_t>(num_data) * num_total_features * sizeof(uint16_t));
-  for (int u = 0; u < nfn; ++u) {
-    const int f = used[u];
-    const uint8_t* src = h.data() + (static_cast<size_t>(u >> 5) * rows_stride) * 32 + (u & 31);
-    for (int i = 0; i < num_data; ++i) out[static_cast<size_t>(i) * num_total_features + f] = src[static_cast<size_t>(i) * 32];
-  }
+  UnpackTiles(out);
   if (nw > 0) {
     std::vector<uint16_t> hw(bins16.n);
     B200_CUDA(cudaMemcpy(hw.data(), bins16.p, bins16.n * sizeof(uint16_t), cudaMemcpyDeviceToHost));
@@ -606,34 +599,49 @@ Dataset* Dataset::CreateFromMat(const void* data, int data_type, int nrow, int n
   EnsureDevice();
   if (data_type != 0 && data_type != 1) Fatal("Unknown data type in CreateFromMat (expect C_API_DTYPE_FLOAT32 or FLOAT64)");
   if (nrow <= 0 || ncol <= 0) Fatal("Dataset should have at least one row and one column");
-  std::unique_ptr<Dataset> d(new Dataset());
-  d->device = CurrentDevice();
-  B200_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-  d->num_data = nrow; d->num_total_features = ncol;
-  d->cfg.Parse(params);
-  cudaEvent_t e0, e1;
-  B200_CUDA(cudaEventCreate(&e0)); B200_CUDA(cudaEventCreate(&e1));
-  B200_CUDA(cudaEventRecord(e0, d->stream));
+  std::unique_ptr<Dataset> d = NewShell(nrow, ncol, params);
+  StreamTimer timer(d->stream);
   const bool on_device = IsDevicePointer(data);
-  if (reference) {
-    if (reference->num_total_features != ncol) Fatal("Validation data has a different number of features than the reference dataset");
-    d->mappers = reference->mappers;
-    d->feature_names = reference->feature_names;
-  } else {
-    d->FindBins(data, on_device, data_type, is_row_major);
-    d->feature_names.resize(ncol);
-    for (int f = 0; f < ncol; ++f) d->feature_names[f] = "Column_" + std::to_string(f);
-  }
-  d->UploadMeta();
-  d->rows_stride = static_cast<size_t>(nrow);
-  AllocBins(d.get());
+  d->SetMappers(reference, [&](std::vector<std::vector<double>>* nz, int f0, int f1) {      // the sampled rows, gathered where the data is
+    const int n = nrow, F = ncol;
+    const std::vector<int> rows = d->SampleRows();
+    const int sample_cnt = static_cast<int>(rows.size());
+    std::vector<double> S(static_cast<size_t>(sample_cnt) * F);
+    if (on_device) {
+      DevBuf<int> d_rows; d_rows.Alloc(sample_cnt);
+      DevBuf<double> d_S; d_S.Alloc(S.size());
+      d_rows.Upload(rows.data(), sample_cnt, d->stream);
+      int grid = static_cast<int>(std::min<size_t>((S.size() + 255) / 256, static_cast<size_t>(DeviceSMs()) * 32));
+      if (data_type == 0) k_gather_rows<float><<<grid, 256, 0, d->stream>>>(static_cast<const float*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
+      else k_gather_rows<double><<<grid, 256, 0, d->stream>>>(static_cast<const double*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
+      B200_CUDA(cudaGetLastError());
+      d_S.Download(S.data(), S.size(), d->stream);
+      B200_CUDA(cudaStreamSynchronize(d->stream));
+    } else {
+#pragma omp parallel for schedule(static)
+      for (int s = 0; s < sample_cnt; ++s) {
+        const long long r = rows[s];
+        for (int f = 0; f < F; ++f) {
+          double v;
+          if (data_type == 0) v = is_row_major ? static_cast<const float*>(data)[r * F + f] : static_cast<const float*>(data)[static_cast<long long>(f) * n + r];
+          else v = is_row_major ? static_cast<const double*>(data)[r * F + f] : static_cast<const double*>(data)[static_cast<long long>(f) * n + r];
+          S[static_cast<size_t>(s) * F + f] = v;
+        }
+      }
+    }
+#pragma omp parallel for schedule(dynamic)
+    for (int f = f0; f < f1; ++f) {
+      (*nz)[f].reserve(sample_cnt);
+      for (int s = 0; s < sample_cnt; ++s) {
+        double v = S[static_cast<size_t>(s) * F + f];
+        if (std::fabs(v) > kZeroThr || std::isnan(v)) (*nz)[f].push_back(v);
+      }
+    }
+    return sample_cnt;
+  });
+  d->AllocBins();
   d->BinBlock(data, on_device, data_type, is_row_major, nrow, 0);
-  B200_CUDA(cudaEventRecord(e1, d->stream));
-  B200_CUDA(cudaEventSynchronize(e1));
-  float ms = 0;
-  B200_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  d->ingest_ms = ms;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  d->ingest_ms = timer.Ms();
   return d.release();
 }
 
@@ -722,40 +730,19 @@ Dataset* Dataset::CreateFromCSR(const void* indptr, int indptr_type, const int32
     if (bad & 1) Fatal("CreateFromCSR: indptr is not non-decreasing");
     if (bad & 2) Fatal("CreateFromCSR: a column index is negative or >= num_col");
   }
-  std::unique_ptr<Dataset> d(new Dataset());
-  d->device = CurrentDevice();
-  B200_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-  d->num_data = static_cast<int>(nrow); d->num_total_features = static_cast<int>(num_col);
-  d->cfg.Parse(params);
-  cudaEvent_t e0, e1;
-  B200_CUDA(cudaEventCreate(&e0)); B200_CUDA(cudaEventCreate(&e1));
-  B200_CUDA(cudaEventRecord(e0, d->stream));
+  std::unique_ptr<Dataset> d = NewShell(static_cast<int>(nrow), static_cast<int>(num_col), params);
+  StreamTimer timer(d->stream);
   const int F = d->num_total_features;
-  if (reference) {
-    if (reference->num_total_features != F) Fatal("Validation data has a different number of features than the reference dataset");
-    d->mappers = reference->mappers;
-    d->feature_names = reference->feature_names;
-  } else {
-    if (d->cfg.max_bin >= kWideMaxBins) Fatal("max_bin >= " + std::to_string(kWideMaxBins) + " is not supported");
-    if (d->cfg.max_bin < 2) Fatal("max_bin should be >= 2");
-    if (d->cfg.zero_as_missing) Fatal("zero_as_missing=true is not supported by this build");
-    LcgRandom rnd(d->cfg.data_random_seed);
-    int sample_cnt = d->num_data < d->cfg.bin_construct_sample_cnt ? d->num_data : d->cfg.bin_construct_sample_cnt;
-    std::vector<int> rows = rnd.Sample(d->num_data, sample_cnt);
-    sample_cnt = static_cast<int>(rows.size());
-    std::vector<std::vector<double>> nz(F);
+  d->SetMappers(reference, [&](std::vector<std::vector<double>>* nz, int, int) {
+    const std::vector<int> rows = d->SampleRows();
     for (int r : rows)
       for (int64_t k = ip(r); k < ip(r + 1); ++k) {
         const double v = val(k);
-        if (std::fabs(v) > kZeroThr || std::isnan(v)) nz[indices[k]].push_back(v);
+        if (std::fabs(v) > kZeroThr || std::isnan(v)) (*nz)[indices[k]].push_back(v);
       }
-    d->FindBinsFromColumns(&nz, sample_cnt);
-    d->feature_names.resize(F);
-    for (int f = 0; f < F; ++f) d->feature_names[f] = "Column_" + std::to_string(f);
-  }
-  d->UploadMeta();
-  d->rows_stride = static_cast<size_t>(nrow);
-  AllocBins(d.get());
+    return static_cast<int>(rows.size());
+  });
+  d->AllocBins();
   const int sms = DeviceSMs();
   k_fill_default_bins<<<sms * 8, 256, 0, d->stream>>>(d->meta.p, d->nfn, d->bins.p, d->rows_stride, nrow, d->num_tiles);
   if (d->nw > 0) k_fill_default_wide<<<sms * 8, 256, 0, d->stream>>>(d->wide_meta.p, d->nw, d->bins16.p, d->rows_stride, nrow);
@@ -782,28 +769,25 @@ Dataset* Dataset::CreateFromCSR(const void* indptr, int indptr_type, const int32
       if (ne > 0) {
         const int grid = static_cast<int>(std::min<int64_t>((nr + 7) / 8, sms * 8));
         uint8_t* base = d->bins.p + static_cast<size_t>(r0) * 32;       // row offset inside every tile
-#define B200_CSR_LAUNCH(TI, TV)                                                                                                              \
-        k_bin_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),               \
-                                                      reinterpret_cast<const TV*>(d_v.p), nr, d_inner.p, d->meta.p, d->ub.p, d->catbin.p, base,  \
-                                                      d->rows_stride, e0k, d->nfn, d->wide_meta.p, d->wide_cats.p, d->wide_catbin.p, d->wide_ub.p,  \
-                                                      d->bins16.p ? d->bins16.p + r0 : nullptr)
-        if (indptr_type == 2 && data_type == 0) B200_CSR_LAUNCH(int32_t, float);
-        else if (indptr_type == 2) B200_CSR_LAUNCH(int32_t, double);
-        else if (data_type == 0) B200_CSR_LAUNCH(int64_t, float);
-        else B200_CSR_LAUNCH(int64_t, double);
-#undef B200_CSR_LAUNCH
+        auto launch = [&](auto index_type, auto value_type) {
+          using TI = decltype(index_type);
+          using TV = decltype(value_type);
+          k_bin_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),
+                                                        reinterpret_cast<const TV*>(d_v.p), nr, d_inner.p, d->meta.p, d->ub.p, d->catbin.p, base,
+                                                        d->rows_stride, e0k, d->nfn, d->wide_meta.p, d->wide_cats.p, d->wide_catbin.p, d->wide_ub.p,
+                                                        d->bins16.p ? d->bins16.p + r0 : nullptr);
+        };
+        if (indptr_type == 2 && data_type == 0) launch(int32_t{}, float{});
+        else if (indptr_type == 2) launch(int32_t{}, double{});
+        else if (data_type == 0) launch(int64_t{}, float{});
+        else launch(int64_t{}, double{});
         B200_CUDA(cudaGetLastError());
       }
       B200_CUDA(cudaStreamSynchronize(d->stream));      // the staging buffers are reused by the next block
       r0 = r1;
     }
   }
-  B200_CUDA(cudaEventRecord(e1, d->stream));
-  B200_CUDA(cudaEventSynchronize(e1));
-  float ms = 0;
-  B200_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  d->ingest_ms = ms;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  d->ingest_ms = timer.Ms();
   return d.release();
 }
 
@@ -2231,9 +2215,7 @@ int64_t Booster::PredictBatch(const void* data, int data_type, int64_t nrow, int
   DevBuf<unsigned char> xin;
   if (!on_device) xin.Alloc(static_cast<size_t>(chunk) * ncol * esz);
   DevBuf<double> dout; dout.Alloc(static_cast<size_t>(std::min(chunk, nrow)) * per_row);
-  cudaEvent_t e0, e1;
-  B200_CUDA(cudaEventCreate(&e0)); B200_CUDA(cudaEventCreate(&e1));
-  B200_CUDA(cudaEventRecord(e0, stream_));
+  StreamTimer timer(stream_);
   for (int64_t r0 = 0; r0 < nrow; r0 += chunk) {
     const int64_t rows = std::min(chunk, nrow - r0);
     const void* x = static_cast<const unsigned char*>(data) + static_cast<size_t>(r0) * ncol * esz;
@@ -2254,12 +2236,7 @@ int64_t Booster::PredictBatch(const void* data, int data_type, int64_t nrow, int
     B200_CUDA(cudaMemcpyAsync(out + r0 * per_row, dout.p, static_cast<size_t>(rows) * per_row * sizeof(double), cudaMemcpyDeviceToHost, stream_));
     B200_CUDA(cudaStreamSynchronize(stream_));
   }
-  B200_CUDA(cudaEventRecord(e1, stream_));
-  B200_CUDA(cudaEventSynchronize(e1));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  last_predict_ms = ms;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  last_predict_ms = timer.Ms();
   const bool avg = model.average_output && t1 > t0 && predict_type < 2;       // rf: raw score = mean over the iterations
   if (avg && predict_type == 1)
     for (int64_t i = 0; i < nrow * Kc; ++i) out[i] /= ((t1 - t0) / Kc);

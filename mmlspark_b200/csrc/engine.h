@@ -121,11 +121,15 @@ class Dataset {
   DevBuf<int> d_qb;
   std::vector<std::string> feature_names;
   cudaStream_t stream = nullptr;
-  double ingest_ms = 0.0;                    // H2D + binning time of the last create (CUDA events)
+  double ingest_ms = 0.0;                    // H2D + binning time of a matrix / CSR create, or the sum over PushRows calls (CUDA events)
 
  private:
-  void FindBins(const void* data, bool on_device, int data_type, int is_row_major);
-  void FindBinsFromColumns(std::vector<std::vector<double>>* nz, int sample_cnt);
+  // every create runs NewShell, SetMappers and AllocBins, in that order
+  static std::unique_ptr<Dataset> NewShell(int nrow, int ncol, const char* params);
+  template <typename Sample> void SetMappers(const Dataset* reference, Sample sample);
+  std::vector<int> SampleRows() const;
+  void AllocBins();
+  template <typename T> void UnpackTiles(T* out) const;
   void BinBlock(const void* data, bool on_device, int data_type, int is_row_major, long long nrow, long long start_row);
   // persistent H2D staging of the host ingestion path (two device chunks, a copy stream, events); released once every row is in
   DevBuf<unsigned char> ingest_buf_[2];
