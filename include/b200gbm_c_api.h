@@ -185,6 +185,9 @@ int B200GBM_DatasetGetIngestMs(DatasetHandle handle, double* out_ms);
  * fp64 [num_feature][256][2]; grad/hess/idx are host arrays; idx == NULL means rows 0..cnt-1 */
 int B200GBM_DatasetHistogram(DatasetHandle handle, const float* grad, const float* hess, const int32_t* idx,
                              int32_t cnt, double* out);
+/* kernel-level entry: the objective's gradients and hessians (K1/K2) at the booster's current training scores, class-major [K][n]
+ * host arrays; classes the objective does not train read back as 0.  Training state and the model are not changed. */
+int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess);
 /* timing of the engine stream, CUDA events: out = {hist_ms, total_ms, hist_rows, hist_launches, launches, iterations} */
 int B200GBM_BoosterSetProfile(BoosterHandle handle, int profile_hist);
 int B200GBM_BoosterGetTiming(BoosterHandle handle, double* out6, int reset);

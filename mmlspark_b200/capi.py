@@ -438,6 +438,15 @@ class Booster:
         check(load().B200GBM_BoosterGetScores(self.handle, C.c_int(data_idx), _ptr(out)))
         return out
 
+    def get_gradients(self):
+        """(grad, hess) of the objective at the current training scores, float32 class-major [K * n] (B200GBM_BoosterGetGradients)."""
+        n = C.c_int64(0)
+        check(load().LGBM_BoosterGetNumPredict(self.handle, C.c_int(0), C.byref(n)))
+        g = np.zeros(n.value, dtype=np.float32)
+        h = np.zeros(n.value, dtype=np.float32)
+        check(load().B200GBM_BoosterGetGradients(self.handle, _ptr(g), _ptr(h)))
+        return g, h
+
     def free(self):
         if self.handle:
             check(load().LGBM_BoosterFree(self.handle))

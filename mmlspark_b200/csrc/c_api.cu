@@ -571,6 +571,11 @@ int B200GBM_DatasetHistogram(DatasetHandle handle, const float* grad, const floa
   DS(handle)->Histogram(grad, hess, idx, cnt, out);
   API_END();
 }
+int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess) {
+  API_BEGIN();
+  BS(handle)->GetGradients(grad, hess);
+  API_END();
+}
 int B200GBM_BoosterSetProfile(BoosterHandle handle, int profile_hist) {
   API_BEGIN();
   BS(handle)->profile_hist = profile_hist != 0;

@@ -1894,6 +1894,18 @@ void Booster::GetRawScores(int data_idx, double* out) {
   B200_CUDA(cudaStreamSynchronize(stream_));
 }
 
+void Booster::GetGradients(float* grad, float* hess) {
+  if (!train) Fatal("this booster was loaded from a model string: it holds no training data to take gradients on");
+  EnsureDevice();
+  const size_t m = static_cast<size_t>(K) * train->num_data;
+  DevBuf<float> g, h;      // zero-filled: classes the objective does not train (NeedTrain) read back as 0
+  g.Alloc(m); h.Alloc(m); g.Zero(stream_); h.Zero(stream_);
+  obj_->LaunchGradients(score_.p, g.p, h.p, num_sms_);
+  B200_CUDA(cudaGetLastError());
+  g.Download(grad, m, stream_); h.Download(hess, m, stream_);
+  B200_CUDA(cudaStreamSynchronize(stream_));
+}
+
 void Booster::UploadForest() {
   if (forest_ && forest_->trees == model.trees.size()) return;
   forest_.reset(new ForestBufs());

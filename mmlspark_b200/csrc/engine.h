@@ -165,6 +165,9 @@ class Booster {
   void GetPredict(int data_idx, int64_t* out_len, double* out);
   int64_t NumPredict(int data_idx) const;
   void GetRawScores(int data_idx, double* out);
+  // the objective's gradients at the current training scores, class-major [K][n], computed into scratch buffers: the training state
+  // (grad_ / hess_, which rf keeps from construction and GOSS rescales in place) is not touched
+  void GetGradients(float* grad, float* hess);
   // batched GPU prediction over a row-major matrix (host or device pointer); predict_type 0 normal, 1 raw, 2 leaf index.
   // Returns the number of doubles written to `out` (host).  last_predict_ms = kernel time (CUDA events), incl. H2D for host input.
   int64_t PredictBatch(const void* data, int data_type, int64_t nrow, int ncol, int predict_type, int start_iteration, int num_iteration, double* out);

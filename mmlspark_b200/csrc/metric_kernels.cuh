@@ -120,8 +120,13 @@ __device__ __forceinline__ unsigned long long d_sortable(double v) {
   unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(v));
   return (b >> 63) ? ~b : (b | 0x8000000000000000ULL);
 }
+// -0.0 is keyed as +0.0: the two compare equal, so they are one tie group, as in [UPSTREAM AUCMetric] `cur_score != threshold` and in
+// scikit-learn's roc_auc_score (an init_score can hold -0.0)
 __global__ void k_auc_keys(const double* __restrict__ score, int n, unsigned long long* __restrict__ keys, int* __restrict__ rows) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) { keys[i] = d_sortable(score[i]); rows[i] = i; }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const double s = score[i];
+    keys[i] = d_sortable(s == 0.0 ? 0.0 : s); rows[i] = i;
+  }
 }
 // sorted position i (descending score): weights of the row split by class, and the head marker of its tie group
 __global__ void k_auc_weights(const unsigned long long* __restrict__ keys, const int* __restrict__ rows, const float* __restrict__ label,

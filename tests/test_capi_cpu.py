@@ -156,6 +156,16 @@ def test_feature_importance_dump_and_merge(capi):
     np.testing.assert_allclose(a.predict_for_mat_single(x, capi.PREDICT_RAW_SCORE), 2 * b.predict_for_mat_single(x, capi.PREDICT_RAW_SCORE), rtol=1e-12)
 
 
+def test_gradients_of_a_loaded_model_fail_loudly(capi):
+    """B200GBM_BoosterGetGradients needs training data: a booster loaded from a model string has none."""
+    b = capi.Booster(model_str=GOLDEN["models"]["regression"]["model"])
+    g, h = np.zeros(1, np.float32), np.zeros(1, np.float32)
+    with pytest.raises(capi.LightGBMError, match="model string"):
+        capi.check(capi.load().B200GBM_BoosterGetGradients(b.handle, capi._ptr(g), capi._ptr(h)))
+    with pytest.raises(capi.LightGBMError, match="model string"):
+        b.get_gradients()
+
+
 def test_save_model_small_buffer_protocol(capi):
     """saveToString passes a 10 000-byte buffer and retries with out_len (LightGBMBooster.scala:269-274)."""
     g = GOLDEN["models"]["binary"]["model"]

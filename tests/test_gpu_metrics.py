@@ -148,6 +148,145 @@ def test_ranking_metrics_ndcg_and_map(built):
         np.testing.assert_allclose(got[4:], mp, rtol=1e-6)          # [UPSTREAM] accumulates num_hit / (j + 1.0f) in float
 
 
+# ------------------------------------------------------------------------------------------------ metrics at chosen scores
+# get_eval before the first iteration evaluates the init scores exactly, so the scores can sit where each metric clips.
+N_EDGE = 300_001        # the metric kernels' blocks take contiguous row ranges; this n spans many of them and ends on a ragged tail
+EDGE_SCORES = np.array([0.0, -0.0, 1e-8, -1e-8, 0.5, -0.5, 5.0, -5.0, 23.0, -23.0, 23.1, -23.1, 30.0, -30.0, 37.0, -37.0, 40.0, -40.0])
+
+
+def _edge_scores(rng, n, spread=3.0):
+    s = spread * rng.standard_normal(n)
+    pick = rng.random(n) < 0.5
+    s[pick] = EDGE_SCORES[rng.integers(0, len(EDGE_SCORES), int(pick.sum()))]
+    return s
+
+
+def _eval_at_init(params, y, s, w=None):
+    from mmlspark_b200 import capi
+    X = np.random.default_rng(9).standard_normal((len(y), 2))
+    ds = capi.Dataset.from_mat(X, DS_PARAMS).set_field("label", y).set_field("init_score", s)
+    if w is not None:
+        ds.set_field("weight", w)
+    b = capi.Booster(ds, BASE + params)
+    try:
+        return dict(zip(b.eval_names(), b.get_eval(0)))
+    finally:
+        b.free()
+        ds.free()
+
+
+def _safe_log(x):
+    return np.where(x > 0, np.log(np.where(x > 0, x, 1.0)), -np.inf)
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+def test_regression_metrics_at_clipping_scores(built, weighted):
+    """poisson and tweedie clip exp(score) at 1e-10 (score <= -23.03); the exp-link metrics are evaluated with their objectives."""
+    rng = np.random.default_rng(10 + weighted)
+    n = N_EDGE
+    y = (0.1 + rng.gamma(2.0, 1.5, n)).astype(np.float32)          # > 0: gamma's log(label)
+    s = _edge_scores(rng, n)
+    w = (0.5 + rng.random(n)).astype(np.float32) if weighted else None
+    y64 = y.astype(np.float64)
+    with np.errstate(all="ignore"):
+        d = s - y64
+        got = _eval_at_init("objective=regression alpha=0.7 fair_c=1.3 metric=l2,rmse,l1,huber,fair,quantile,mape", y, s, w)
+        want = {
+            "l2": _wavg(d * d, w), "rmse": np.sqrt(_wavg(d * d, w)), "l1": _wavg(np.abs(d), w),
+            "huber": _wavg(np.where(np.abs(d) <= 0.7, 0.5 * d * d, 0.7 * (np.abs(d) - 0.35)), w),
+            "fair": _wavg(1.3 * np.abs(d) - 1.69 * np.log(1 + np.abs(d) / 1.3), w),
+            "quantile": _wavg(np.where(y64 - s < 0, (0.7 - 1) * (y64 - s), 0.7 * (y64 - s)), w),
+            "mape": _wavg(np.abs(y64 - s) / np.maximum(1.0, np.abs(y64)), w),
+        }
+        sc = np.maximum(np.exp(s), 1e-10)
+        got.update(_eval_at_init("objective=poisson metric=poisson", y, s, w))
+        want["poisson"] = _wavg(sc - y64 * np.log(sc), w)
+        got.update(_eval_at_init("objective=tweedie tweedie_variance_power=1.4 metric=tweedie", y, s, w))
+        want["tweedie"] = _wavg(-y64 * np.exp((1 - 1.4) * np.log(sc)) / (1 - 1.4) + np.exp((2 - 1.4) * np.log(sc)) / (2 - 1.4), w)
+        got.update(_eval_at_init("objective=gamma metric=gamma,gamma_deviance", y, s, w))
+        e = np.exp(s)
+        theta = -1.0 / e
+        want["gamma"] = _wavg(-((y64 * theta + _safe_log(-theta)) + (_safe_log(y64) - _safe_log(y64))), w)
+        tmp = y64 / (e + 1e-9)
+        want["gamma_deviance"] = _wavg(tmp - _safe_log(tmp) - 1, w)
+    assert (s <= -23.1).any() and sorted(got) == sorted(want)
+    for k, v in want.items():
+        np.testing.assert_allclose(got[k], v, rtol=1e-11, err_msg=k)
+
+
+@pytest.mark.parametrize("sigmoid", [1.0, 2.0])
+def test_binary_and_xentropy_metrics_at_saturating_scores(built, sigmoid):
+    """|sigmoid * score| >= 37 rounds p to 1 in fp64: logloss takes its epsilon branch, cross_entropy its 1e-12 branch."""
+    rng = np.random.default_rng(20 + int(sigmoid))
+    n = N_EDGE
+    s = _edge_scores(rng, n, spread=20.0)
+    y = (rng.random(n) < 0.3).astype(np.float32)
+    w = (0.5 + rng.random(n)).astype(np.float32)
+    w[rng.random(n) < 0.05] = 0.0
+    got = _eval_at_init("objective=binary sigmoid=%g metric=binary_logloss,binary_error" % sigmoid, y, s, w)
+    p = 1.0 / (1.0 + np.exp(-sigmoid * s))
+    pl = np.where(y > 0, p, 1.0 - p)
+    assert (pl == 0).any()
+    np.testing.assert_allclose(got["binary_logloss"], _wavg(np.where(pl > 1e-15, -np.log(np.maximum(pl, 1e-300)), -np.log(1e-15)), w), rtol=1e-12)
+    np.testing.assert_allclose(got["binary_error"], _wavg(((p <= 0.5) == (y > 0)).astype(np.float64), w), rtol=1e-12)
+    yx = np.where(rng.random(n) < 0.5, y, rng.random(n)).astype(np.float32)      # probabilities: 0, 1 and fractions
+    got = _eval_at_init("objective=cross_entropy metric=cross_entropy", yx, s, w)
+    y64 = yx.astype(np.float64)
+    with np.errstate(all="ignore"):
+        p = 1.0 / (1.0 + np.exp(-s))
+        a = y64 * np.where(p > 1e-12, np.log(np.maximum(p, 1e-300)), np.log(1e-12))
+        b = (1.0 - y64) * np.where(1.0 - p > 1e-12, np.log(np.maximum(1.0 - p, 1e-300)), np.log(1e-12))
+    np.testing.assert_allclose(got["cross_entropy"], _wavg(-(a + b), w), rtol=1e-12)
+
+
+@pytest.mark.parametrize("objective", ["multiclass", "multiclassova"])
+def test_multiclass_metrics_at_extreme_scores(built, objective):
+    rng = np.random.default_rng(30)
+    n, K = N_EDGE, 5
+    y = rng.integers(0, K, n).astype(np.float32)
+    s = np.concatenate([_edge_scores(rng, n, spread=10.0) for _ in range(K)])
+    got = _eval_at_init("objective=%s num_class=%d metric=multi_logloss,multi_error" % (objective, K), y, s)
+    sk = s.reshape(K, n).T
+    if objective == "multiclass":
+        e = np.exp(sk - sk.max(axis=1, keepdims=True))
+        p = e / e.sum(axis=1, keepdims=True)
+    else:
+        p = 1.0 / (1.0 + np.exp(-sk))
+    pl = p[np.arange(n), y.astype(int)]
+    assert (pl <= 1e-15).any()
+    np.testing.assert_allclose(got["multi_logloss"], np.mean(np.where(pl > 1e-15, -np.log(np.maximum(pl, 1e-300)), -np.log(1e-15))), rtol=1e-12)
+    np.testing.assert_allclose(got["multi_error"], np.mean((p >= pl[:, None]).sum(axis=1) > 1), rtol=1e-12)
+
+
+def test_auc_treats_signed_zeros_as_one_tie(built):
+    """-0.0 == +0.0, so they form one tie group, as in LightGBM's `cur_score != threshold` and in sklearn; a user init_score can hold -0.0."""
+    from sklearn.metrics import roc_auc_score
+    n = N_EDGE
+    y = (np.arange(n) % 3 == 0).astype(np.float32)
+    s = np.where(y > 0, 0.0, -0.0)             # positives at +0.0, negatives at -0.0: one tie, AUC 1/2
+    assert _eval_at_init("objective=binary metric=auc", y, s)["auc"] == 0.5
+    rng = np.random.default_rng(40)
+    y = (rng.random(n) < 0.4).astype(np.float32)
+    s = np.array([0.0, -0.0, 1e-8, -1e-8, 0.5, -0.5])[rng.integers(0, 6, n)]
+    w = (0.5 + rng.random(n)).astype(np.float32)
+    got = _eval_at_init("objective=binary metric=auc", y, s, w)["auc"]
+    np.testing.assert_allclose(got, roc_auc_score(y, s, sample_weight=w), rtol=1e-10)
+
+
+def test_auc_weighted_ties_and_single_class(built):
+    from sklearn.metrics import roc_auc_score
+    rng = np.random.default_rng(41)
+    n = N_EDGE
+    s = np.round(_edge_scores(rng, n), 0)       # few distinct values: large weighted tie groups
+    y = (rng.random(n) < 1.0 / (1.0 + np.exp(-np.clip(s, -30, 30)))).astype(np.float32)
+    w = (10.0 ** rng.uniform(-3, 3, n)).astype(np.float32)
+    w[rng.random(n) < 0.05] = 0.0
+    got = _eval_at_init("objective=binary metric=auc", y, s, w)["auc"]
+    np.testing.assert_allclose(got, roc_auc_score(y, s, sample_weight=w), rtol=1e-10)
+    for label in (0.0, 1.0):                    # one class only: LightGBM reports 1
+        assert _eval_at_init("objective=binary metric=auc", np.full(n, label, np.float32), s, w)["auc"] == 1.0
+
+
 def test_unknown_metric_fails_at_booster_create(built):
     from mmlspark_b200 import capi
     rng = np.random.default_rng(5)
