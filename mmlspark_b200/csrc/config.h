@@ -56,6 +56,7 @@ struct Config {
   double scale_pos_weight = 1.0, sigmoid = 1.0;
   bool boost_from_average = true;
   double alpha = 0.9, tweedie_variance_power = 1.5, fair_c = 1.0, poisson_max_delta_step = 0.7;
+  int objective_seed = 5;                   // rank_xendcg's random states
   int lambdarank_truncation_level = 30;
   bool lambdarank_norm = true;
   std::vector<double> label_gain;
@@ -106,6 +107,7 @@ struct Config {
     if (o == "xentropy") return "cross_entropy";
     if (o == "xentlambda") return "cross_entropy_lambda";
     if (o == "rank" ) return "lambdarank";
+    if (o == "xendcg" || o == "xe_ndcg" || o == "xe_ndcg_mart" || o == "xendcg_mart") return "rank_xendcg";
     if (o == "l1" || o == "mean_absolute_error" || o == "mae") return "regression_l1";
     if (o == "mean_absolute_percentage_error") return "mape";
     return o;
@@ -118,9 +120,12 @@ struct Config {
     if (m == "multi_logloss" || m == "multiclass" || m == "softmax" || m == "multiclassova" || m == "multiclass_ova" ||
         m == "ova" || m == "ovr")
       return "multi_logloss";
-    if (m == "ndcg" || m == "lambdarank" || m == "rank_xendcg" || m == "xendcg") return "ndcg";
+    if (m == "ndcg" || m == "lambdarank" || m == "rank_xendcg" || m == "xendcg" || m == "xe_ndcg" || m == "xe_ndcg_mart" || m == "xendcg_mart")
+      return "ndcg";
     if (m == "map" || m == "mean_average_precision") return "map";
     if (m == "xentropy" || m == "cross_entropy") return "cross_entropy";
+    if (m == "xentlambda" || m == "cross_entropy_lambda") return "cross_entropy_lambda";
+    if (m == "kldiv" || m == "kullback_leibler") return "kullback_leibler";
     if (m == "mean_absolute_percentage_error") return "mape";
     return m;
   }
@@ -177,7 +182,8 @@ struct Config {
     S("max_bin_by_feature", &max_bin_by_feature);
     I("num_class", &num_class); B("is_unbalance", &is_unbalance); D("scale_pos_weight", &scale_pos_weight);
     D("sigmoid", &sigmoid); B("boost_from_average", &boost_from_average); D("alpha", &alpha);
-    D("tweedie_variance_power", &tweedie_variance_power); D("fair_c", &fair_c); D("poisson_max_delta_step", &poisson_max_delta_step); I("lambdarank_truncation_level", &lambdarank_truncation_level);
+    D("tweedie_variance_power", &tweedie_variance_power); D("fair_c", &fair_c); D("poisson_max_delta_step", &poisson_max_delta_step); I("objective_seed", &objective_seed);
+    I("lambdarank_truncation_level", &lambdarank_truncation_level);
     B("lambdarank_norm", &lambdarank_norm); I("num_machines", &num_machines);
     {
       auto it = raw.find("label_gain");
@@ -241,7 +247,7 @@ struct Config {
     s << "[is_enable_sparse: 1]\n[enable_bundle: 1]\n[use_missing: " << use_missing << "]\n[zero_as_missing: " << zero_as_missing << "]\n";
     s << "[feature_pre_filter: " << feature_pre_filter << "]\n[pre_partition: " << pre_partition << "]\n[two_round: 0]\n[header: 0]\n";
     s << "[label_column: ]\n[weight_column: ]\n[group_column: ]\n[ignore_column: ]\n[categorical_feature: " << join_i(categorical_feature) << "]\n";
-    s << "[forcedbins_filename: ]\n[objective_seed: 5]\n[num_class: " << num_class << "]\n[is_unbalance: " << is_unbalance << "]\n";
+    s << "[forcedbins_filename: ]\n[objective_seed: " << objective_seed << "]\n[num_class: " << num_class << "]\n[is_unbalance: " << is_unbalance << "]\n";
     s << "[scale_pos_weight: " << Num(scale_pos_weight) << "]\n[sigmoid: " << Num(sigmoid) << "]\n[boost_from_average: " << boost_from_average << "]\n";
     s << "[reg_sqrt: 0]\n[alpha: " << Num(alpha) << "]\n[fair_c: " << Num(fair_c) << "]\n[poisson_max_delta_step: " << Num(poisson_max_delta_step) << "]\n";
     s << "[tweedie_variance_power: " << Num(tweedie_variance_power) << "]\n[lambdarank_truncation_level: " << lambdarank_truncation_level << "]\n";

@@ -1278,7 +1278,7 @@ double Booster::BoostFromAverage(int k) {
 
 void Booster::ComputeGradientsAt(const double* score_p) {
   NvtxRange nvtx("b200gbm:K1/K2 gradients");
-  obj_->LaunchGradients(score_p, grad_.p, hess_.p, num_sms_);
+  obj_->LaunchGradients(score_p, grad_.p, hess_.p, num_sms_, true);
   B200_CUDA(cudaGetLastError());
   timing.launches += 1;
 }
@@ -1630,10 +1630,20 @@ bool Booster::UpdateOneIterCustom(const float* grad, const float* hess) { return
 void Booster::ResetParameter(const char* params) {
   Config nc;
   nc.Parse(params);
+  const Config before = cfg;
   for (auto& kv : nc.raw) cfg.raw[kv.first] = kv.second;
   int keep_machines = cfg.num_machines;
   cfg.Refresh();
   cfg.num_machines = keep_machines;
+  if (train) {      // metrics named by the reset meet the checks of LGBM_BoosterCreate / AddValidData; a rejected reset changes nothing
+    try {
+      ValidateMetrics();
+      for (auto* v : valids_) CheckMetricData(*v->ds);
+    } catch (...) {
+      cfg = before;
+      throw;
+    }
+  }
   shrinkage_ = is_rf_ ? 1.0 : cfg.learning_rate;
   if (is_dart_) { drop_rand_ = LcgRandom(cfg.drop_seed); sum_weight_ = 0.0; }      // [LightGBM dart.hpp DART::ResetConfig]
   sp_.l1 = cfg.lambda_l1; sp_.l2 = cfg.lambda_l2; sp_.max_delta_step = cfg.max_delta_step; sp_.min_gain_to_split = cfg.min_gain_to_split;
@@ -1644,6 +1654,7 @@ void Booster::AddValidData(const Dataset* valid) {
   EnsureDevice();
   if (!train) Fatal("cannot add validation data to a prediction-only booster");
   if (valid->nf != train->nf) Fatal("validation data must be created with reference=train");
+  CheckMetricData(*valid);
   ValidSet* v = new ValidSet();
   v->ds = valid;
   v->score.Alloc(static_cast<size_t>(K) * valid->num_data);
@@ -1764,7 +1775,7 @@ static int MetricKindOf(const std::string& m) {
       {"l2", kMetL2}, {"rmse", kMetL2}, {"l1", kMetL1}, {"huber", kMetHuber}, {"fair", kMetFair}, {"poisson", kMetPoisson}, {"gamma", kMetGamma},
       {"gamma_deviance", kMetGammaDeviance}, {"tweedie", kMetTweedie}, {"quantile", kMetQuantile}, {"mape", kMetMape},
       {"binary_logloss", kMetBinLogloss}, {"binary_error", kMetBinError}, {"multi_logloss", kMetMultiLogloss}, {"multi_error", kMetMultiError},
-      {"cross_entropy", kMetXent}};
+      {"cross_entropy", kMetXent}, {"cross_entropy_lambda", kMetXentLambda}, {"kullback_leibler", kMetKLDiv}};
   auto it = kinds.find(m);
   return it == kinds.end() ? -1 : it->second;
 }
@@ -1772,6 +1783,21 @@ void Booster::ValidateMetrics() const {
   for (auto& m : cfg.metric)
     if (MetricKindOf(m) < 0 && m != "auc" && m != "ndcg" && m != "map") Fatal("Unknown metric type name: " + m);
   if (cfg.eval_at.size() > static_cast<size_t>(kMaxEvalAt)) Fatal("eval_at: at most " + std::to_string(kMaxEvalAt) + " positions are supported");
+  CheckMetricData(*train);
+}
+// [UPSTREAM CrossEntropyLambdaMetric / KullbackLeiblerDivergence ::Init] checks of the labels and weights a metric is evaluated on
+void Booster::CheckMetricData(const Dataset& ds) const {
+  for (auto& m : cfg.metric) {
+    const int kind = MetricKindOf(m);
+    if (kind != kMetXentLambda && kind != kMetKLDiv) continue;
+    if (obj_->NumTreePerIteration() > 1) Fatal("metric " + m + " needs a single-output objective");
+    for (float y : ds.label) if (!(y >= 0.0f && y <= 1.0f)) Fatal("[" + m + "]: does not tolerate label " + std::to_string(y) + " outside [0, 1]");
+    if (kind == kMetKLDiv && !ds.weight.empty()) {
+      double sw = 0;
+      for (float w : ds.weight) { if (w < 0) Fatal("[" + m + "]: at least one weight is negative"); sw += w; }
+      if (!(sw > 0)) Fatal("[" + m + "]: sum of weights is zero");
+    }
+  }
 }
 
 std::vector<double> Booster::GetEval(int data_idx) {
@@ -1804,7 +1830,9 @@ std::vector<double> Booster::GetEval(int data_idx) {
   for (auto& m : cfg.metric) {
     const int kind = MetricKindOf(m);
     if (kind >= 0) {
-      MetricParams mp{kind, K, obj_->kind() == ObjectiveKind::kMulticlassOva ? 1 : 0, 0, cfg.alpha, cfg.fair_c, cfg.tweedie_variance_power, cfg.sigmoid};
+      HostModel::OutputTransform t;
+      HostModel::ObjectiveTransform(obj_->ToString(), &t);
+      MetricParams mp{kind, K, obj_->kind() == ObjectiveKind::kMulticlassOva ? 1 : 0, t.kind, cfg.alpha, cfg.fair_c, cfg.tweedie_variance_power, cfg.sigmoid, t.sigmoid};
       if ((kind == kMetMultiLogloss || kind == kMetMultiError) && K < 2) Fatal("metric " + m + " needs a multiclass objective");
       k_metric_pointwise<<<grid, kMetricBlock, 0, s>>>(sc.p, d_y, d_w, n, mp, met_partial_.p);
       k_metric_finish<<<1, 32, 0, s>>>(met_partial_.p, grid, 2, met_out_.p);
@@ -1900,7 +1928,7 @@ void Booster::GetGradients(float* grad, float* hess) {
   const size_t m = static_cast<size_t>(K) * train->num_data;
   DevBuf<float> g, h;      // zero-filled: classes the objective does not train (NeedTrain) read back as 0
   g.Alloc(m); h.Alloc(m); g.Zero(stream_); h.Zero(stream_);
-  obj_->LaunchGradients(score_.p, g.p, h.p, num_sms_);
+  obj_->LaunchGradients(score_.p, g.p, h.p, num_sms_, false);      // training state (rank_xendcg's random states) unchanged
   B200_CUDA(cudaGetLastError());
   g.Download(grad, m, stream_); h.Download(hess, m, stream_);
   B200_CUDA(cudaStreamSynchronize(stream_));

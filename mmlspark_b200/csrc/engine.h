@@ -162,6 +162,7 @@ class Booster {
   std::vector<std::string> EvalNames() const;
   std::vector<double> GetEval(int data_idx);
   void ValidateMetrics() const;
+  void CheckMetricData(const Dataset& ds) const;
   void GetPredict(int data_idx, int64_t* out_len, double* out);
   int64_t NumPredict(int data_idx) const;
   void GetRawScores(int data_idx, double* out);

@@ -407,6 +407,109 @@ k_grad_lambdarank(const double* __restrict__ score, const float* __restrict__ la
   }
 }
 
+// [UPSTREAM RankXENDCG::GetGradientsForOneQuery] — one block per query, like k_grad_lambdarank.  Every query owns an LCG
+// (x <- 214013 x + 2531011, float = ((x >> 16) & 0x7fff) / 32768) seeded objective_seed + q; document i takes its (i+1)-th output, which
+// the jump table gives directly (x_{i+1} = jump_mul[i] * x0 + jump_add[i], as k_bag_draw).  rho (softmax of the scores) and the params
+// of the three Taylor terms live in `scratch` [2][n] fp64 at the query's rows.  The four sums (softmax denominator, sum of params,
+// sum_l1, sum_l2) are taken by one thread in document order, the reference's order, so the kernel differs from it only where the
+// device exp differs from the host's.  Products that are added are rounded separately (__dmul_rn): the reference does not fuse them.
+// advance != 0 (a training iteration) moves every query's state on by cnt draws; GetGradients reads without advancing.
+__device__ __forceinline__ float d_lcg_float(unsigned x) { return static_cast<float>((x >> 16) & 0x7FFFu) / 32768.0f; }
+constexpr int kXeThreads = 128;
+__global__ void __launch_bounds__(kXeThreads)
+k_grad_xendcg(const double* __restrict__ score, const float* __restrict__ label, const float* __restrict__ weight, const int* __restrict__ qb,
+              int nq, unsigned* __restrict__ lcg_state, const unsigned* __restrict__ jump_mul, const unsigned* __restrict__ jump_add, int advance,
+              double* __restrict__ scratch, size_t n, float* __restrict__ g, float* __restrict__ h) {
+  __shared__ double s_sum;
+  double* rho = scratch;
+  double* params = scratch + n;
+  for (int q = blockIdx.x; q < nq; q += gridDim.x) {
+    const int start = qb[q], cnt = qb[q + 1] - start;
+    if (cnt <= 1) {              // no draws
+      if (cnt == 1 && threadIdx.x == 0) { g[start] = 0.0f; h[start] = 0.0f; }
+      continue;
+    }
+    const unsigned x0 = lcg_state[q];
+    double* r = rho + start;
+    double* pa = params + start;
+    // softmax: max (order-free), exp, denominator in document order
+    double wmax = -INFINITY;
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) wmax = fmax(wmax, score[start + i]);
+    for (int o = 16; o; o >>= 1) wmax = fmax(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+    __shared__ double s_max[kXeThreads / 32];
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = wmax;
+    __syncthreads();
+    wmax = s_max[0];
+    for (int w = 1; w < kXeThreads / 32; ++w) wmax = fmax(wmax, s_max[w]);
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
+      r[i] = exp(score[start + i] - wmax);
+      const unsigned x = jump_mul[i] * x0 + jump_add[i];
+      pa[i] = ldexp(1.0, static_cast<int>(label[start + i])) - static_cast<double>(d_lcg_float(x));
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { double s = 0.0; for (int i = 0; i < cnt; ++i) s += r[i]; s_sum = s; }
+    __syncthreads();
+    const double wsum = s_sum;
+    __syncthreads();
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) r[i] /= wsum;
+    if (threadIdx.x == 0) { double s = 0.0; for (int i = 0; i < cnt; ++i) s += pa[i]; s_sum = s; }
+    __syncthreads();
+    const double inv = 1.0 / fmax(kEps, s_sum);
+    __syncthreads();
+    // first-order term
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
+      const double t = __dadd_rn(-__dmul_rn(pa[i], inv), r[i]);
+      g[start + i] = static_cast<float>(t);
+      pa[i] = t / (1.0 - r[i]);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { double s = 0.0; for (int i = 0; i < cnt; ++i) s += pa[i]; s_sum = s; }
+    __syncthreads();
+    const double sum_l1 = s_sum;
+    __syncthreads();
+    // second-order term
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
+      const double t = r[i] * (sum_l1 - pa[i]);
+      g[start + i] = __fadd_rn(g[start + i], static_cast<float>(t));
+      pa[i] = t / (1.0 - r[i]);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { double s = 0.0; for (int i = 0; i < cnt; ++i) s += pa[i]; s_sum = s; }
+    __syncthreads();
+    const double sum_l2 = s_sum;
+    // third-order term, hessian, row weight (score_t * label_t)
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
+      float lam = __fadd_rn(g[start + i], static_cast<float>(r[i] * (sum_l2 - pa[i])));
+      float hes = static_cast<float>(r[i] * (1.0 - r[i]));
+      if (weight) { lam = __fmul_rn(lam, weight[start + i]); hes = __fmul_rn(hes, weight[start + i]); }
+      g[start + i] = lam; h[start + i] = hes;
+    }
+    if (advance && threadIdx.x == 0) lcg_state[q] = jump_mul[cnt - 1] * x0 + jump_add[cnt - 1];
+    __syncthreads();
+  }
+}
+
+// [UPSTREAM CrossEntropyLambda::GetGradients]: labels are probabilities; with weights, the weight enters the link 1 - exp(-w log1p(e^s))
+__global__ void k_grad_xentlambda(const double* __restrict__ score, const float* __restrict__ label, const float* __restrict__ weight,
+                                  float* __restrict__ g, float* __restrict__ h, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const double y = label[i];
+    if (!weight) {
+      const double z = 1.0 / (1.0 + exp(-score[i]));
+      g[i] = static_cast<float>(z - y); h[i] = static_cast<float>(z * (1.0 - z));
+      continue;
+    }
+    const double w = weight[i], epf = exp(score[i]), hhat = log1p(epf), z = 1.0 - exp(-w * hhat), enf = 1.0 / epf;
+    g[i] = static_cast<float>((1.0 - y / z) * w / (1.0 + enf));
+    const double c = 1.0 / (1.0 - z);
+    double d = 1.0 + epf;
+    const double a = w * epf / (d * d);
+    d = c - 1.0;
+    const double b = (c / (d * d)) * (__dadd_rn(1.0, __dmul_rn(w, epf)) - c);
+    h[i] = static_cast<float>(a * __dadd_rn(1.0, __dmul_rn(y, b)));
+  }
+}
+
 // ---------------------------------------------------------------- quantisation + root sums (K3)
 __global__ void k_absmax(const float* __restrict__ g, const float* __restrict__ h, int n, TreeCtrl* ctrl) {
   float mg = 0.f, mh = 0.f;
@@ -2097,7 +2200,6 @@ __global__ void k_scale_add(double* __restrict__ score, int n, double pre_mul, d
 // x_{j+1} = mulA[j] * x0 + addC[j], so plain bagging is embarrassingly parallel and still bit-identical to the sequential draw.
 constexpr int kBagBlock = 1024;
 struct LcgJump { unsigned mul[kBagBlock]; unsigned add[kBagBlock]; };
-__device__ __forceinline__ float d_lcg_float(unsigned x) { return static_cast<float>((x >> 16) & 0x7FFFu) / 32768.0f; }
 
 __global__ void __launch_bounds__(256)
 k_bag_draw(unsigned* __restrict__ lcg_state, const LcgJump* __restrict__ jump, int n, double fraction, uint8_t* __restrict__ in_bag,

@@ -16,15 +16,41 @@ namespace b200gbm {
 
 enum MetricKind {
   kMetL2 = 0, kMetL1, kMetHuber, kMetFair, kMetPoisson, kMetGamma, kMetTweedie, kMetQuantile, kMetMape, kMetBinLogloss, kMetBinError,
-  kMetMultiLogloss, kMetMultiError, kMetXent, kMetGammaDeviance
+  kMetMultiLogloss, kMetMultiError, kMetXent, kMetGammaDeviance, kMetXentLambda, kMetKLDiv
 };
 struct MetricParams {
-  int kind, K, ova, pad;
+  int kind, K, ova;
+  int transform;               // the objective's single-output transform (HostModel::ObjectiveTransform kind) and its sigmoid,
   double alpha, fair_c, rho, sigmoid;
+  double transform_sigmoid;    // for cross_entropy_lambda and kullback_leibler
 };
 
-// loss of one row; r[] = raw scores of the row's K classes
-__device__ __forceinline__ double d_point_loss(const MetricParams& mp, const double* __restrict__ score, size_t n, size_t i, double lab) {
+// [UPSTREAM xentropy_metric.hpp XentLoss / YentLoss]: log arguments clipped at 1e-12; YentLoss is minus the label's entropy, so that
+// kullback_leibler = mean XentLoss + mean YentLoss is 0 where p equals the label
+__device__ __forceinline__ double d_xent_loss(double lab, double p) {
+  const double a = lab * (p > 1e-12 ? log(p) : log(1e-12)), b = (1.0 - lab) * (1.0 - p > 1e-12 ? log(1.0 - p) : log(1e-12));
+  return -(a + b);
+}
+__device__ __forceinline__ double d_yent_loss(double p) {
+  double hp = 0.0;
+  if (p > 1e-12) hp += p * log(p);
+  const double q = 1.0 - p;
+  if (q > 1e-12) hp += q * log(q);
+  return hp;
+}
+// single-output transforms of HostModel::Convert
+__device__ __forceinline__ double d_output_transform(int kind, double sigmoid, double x) {
+  switch (kind) {
+    case 1: return 1.0 / (1.0 + exp(-sigmoid * x));
+    case 3: return exp(x);
+    case 5: return log1p(exp(x));
+    case 6: return (x >= 0 ? 1.0 : -1.0) * x * x;
+    default: return x;
+  }
+}
+
+// loss of one row; score = class-major raw scores, w = the row's weight (only cross_entropy_lambda reads it)
+__device__ __forceinline__ double d_point_loss(const MetricParams& mp, const double* __restrict__ score, size_t n, size_t i, double lab, double w) {
   const double eps = 1e-15;
   double s0 = score[i];
   switch (mp.kind) {
@@ -52,11 +78,9 @@ __device__ __forceinline__ double d_point_loss(const MetricParams& mp, const dou
       const double pl = lab > 0 ? p : 1.0 - p;
       return pl > eps ? -log(pl) : -log(eps);
     }
-    case kMetXent: {
-      const double p = 1.0 / (1.0 + exp(-s0));
-      const double a = lab * (p > 1e-12 ? log(p) : log(1e-12)), b = (1.0 - lab) * (1.0 - p > 1e-12 ? log(1.0 - p) : log(1e-12));
-      return -(a + b);
-    }
+    case kMetXent: return d_xent_loss(lab, 1.0 / (1.0 + exp(-s0)));
+    case kMetXentLambda: return d_xent_loss(lab, 1.0 - exp(-w * d_output_transform(mp.transform, mp.transform_sigmoid, s0)));
+    case kMetKLDiv: return d_yent_loss(lab) + d_xent_loss(lab, d_output_transform(mp.transform, mp.transform_sigmoid, s0));
     case kMetMultiLogloss: case kMetMultiError: {
       // probabilities by the objective's ConvertOutput: softmax, or a sigmoid per class for multiclassova
       const int K = mp.K, l = static_cast<int>(lab);
@@ -100,8 +124,9 @@ k_metric_pointwise(const double* __restrict__ score, const float* __restrict__ l
   const long long r0 = per * blockIdx.x, r1 = min(r0 + per, static_cast<long long>(n));
   for (long long i = r0 + threadIdx.x; i < r1; i += kMetricBlock) {
     const double w = weight ? static_cast<double>(weight[i]) : 1.0;
-    loss += d_point_loss(mp, score, static_cast<size_t>(n), static_cast<size_t>(i), static_cast<double>(label[i])) * w;
-    sw += w;
+    const double rw = mp.kind == kMetXentLambda ? 1.0 : w;      // [UPSTREAM] cross_entropy_lambda: w is inside the loss, the mean is over rows
+    loss += d_point_loss(mp, score, static_cast<size_t>(n), static_cast<size_t>(i), static_cast<double>(label[i]), w) * rw;
+    sw += rw;
   }
   d_block_sum2(loss, sw, sm);
   if (threadIdx.x == 0) { partial[2 * blockIdx.x] = loss; partial[2 * blockIdx.x + 1] = sw; }

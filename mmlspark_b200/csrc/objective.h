@@ -9,7 +9,7 @@
 namespace b200gbm {
 
 enum class ObjectiveKind { kRegression, kHuber, kFair, kPoisson, kGamma, kTweedie, kRegressionL1, kQuantile, kMape, kBinary, kMulticlass,
-                           kMulticlassOva, kCrossEntropy, kLambdarank };
+                           kMulticlassOva, kCrossEntropy, kCrossEntropyLambda, kLambdarank, kRankXendcg };
 
 // Each objective the engine trains: its canonical name (Config has resolved the aliases) and the `kind` argument it passes to
 // k_grad_regvar (huber 1 .. tweedie 5) or k_grad_percentile (regression_l1 1, quantile 2, mape 3); 0 for the other kernels
@@ -19,7 +19,8 @@ constexpr ObjectiveName kObjectiveNames[] = {
     {"poisson", ObjectiveKind::kPoisson, 3}, {"gamma", ObjectiveKind::kGamma, 4}, {"tweedie", ObjectiveKind::kTweedie, 5},
     {"regression_l1", ObjectiveKind::kRegressionL1, 1}, {"quantile", ObjectiveKind::kQuantile, 2}, {"mape", ObjectiveKind::kMape, 3},
     {"binary", ObjectiveKind::kBinary, 0}, {"multiclass", ObjectiveKind::kMulticlass, 0}, {"multiclassova", ObjectiveKind::kMulticlassOva, 0},
-    {"cross_entropy", ObjectiveKind::kCrossEntropy, 0}, {"lambdarank", ObjectiveKind::kLambdarank, 0}};
+    {"cross_entropy", ObjectiveKind::kCrossEntropy, 0}, {"cross_entropy_lambda", ObjectiveKind::kCrossEntropyLambda, 0},
+    {"lambdarank", ObjectiveKind::kLambdarank, 0}, {"rank_xendcg", ObjectiveKind::kRankXendcg, 0}};
 inline ObjectiveKind ParseObjectiveKind(const std::string& name) {
   for (const ObjectiveName& o : kObjectiveNames) if (name == o.name) return o.kind;
   Fatal("Unknown/unsupported objective type name: " + name);
@@ -81,13 +82,13 @@ class Objective {
   using Kind = ObjectiveKind;
 
  public:
-  // Checks the name, quantile's alpha, the class count of multiclass / multiclassova and lambdarank's query information.  `cfg` is
+  // Checks the name, quantile's alpha, the class count of multiclass / multiclassova and the query information of the ranking objectives.  `cfg` is
   // read again by every later call, so that a parameter reset reaches the gradients as it reaches the rest of the booster.
   Objective(const Config& cfg, const Dataset& train) : cfg_(cfg), train_(train), kind_(ParseObjectiveKind(cfg.objective)) {
     const bool multi = kind_ == Kind::kMulticlass || kind_ == Kind::kMulticlassOva;
     if (kind_ == Kind::kQuantile && !(cfg.alpha > 0.0 && cfg.alpha < 1.0)) Fatal("Check failed: alpha_ > 0 && alpha_ < 1");
     if (multi && cfg.num_class < 2) Fatal("Number of classes should be specified and greater than 1 for multiclass training");
-    if (kind_ == Kind::kLambdarank && train.query_boundaries.empty()) Fatal("Ranking tasks require query information");
+    if ((kind_ == Kind::kLambdarank || kind_ == Kind::kRankXendcg) && train.query_boundaries.empty()) Fatal("Ranking tasks require query information");
     K_ = multi ? cfg.num_class : 1;
     if (kind_ == Kind::kQuantile) renew_alpha_ = static_cast<double>(static_cast<float>(cfg.alpha));     // quantile keeps alpha as score_t
   }
@@ -143,6 +144,26 @@ class Objective {
         double sw = 0; for (int i = 0; i < n; ++i) { if (w[i] < 0) Fatal("[cross_entropy]: at least one weight is negative"); sw += w[i]; }
         if (!(sw > 0)) Fatal("[cross_entropy]: sum of weights is zero");
       }
+    } else if (kind_ == Kind::kCrossEntropyLambda) {      // [UPSTREAM CrossEntropyLambda::Init]
+      for (int i = 0; i < n; ++i) if (!(y[i] >= 0.0f && y[i] <= 1.0f)) Fatal("[cross_entropy_lambda]: does not tolerate label " + std::to_string(y[i]) + " outside [0, 1]");
+      for (int i = 0; i < static_cast<int>(w.size()); ++i) if (!(w[i] > 0.0f)) Fatal("[cross_entropy_lambda]: at least one weight is non-positive");
+    } else if (kind_ == Kind::kRankXendcg) {
+      // one LCG per (rank-local) query, seeded objective_seed + q [UPSTREAM RankXENDCG::Init], and the jump table of its first max_q draws
+      const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
+      std::vector<unsigned> st(nq);
+      int max_q = 1;
+      for (int q = 0; q < nq; ++q) {
+        st[q] = static_cast<unsigned>(cfg_.objective_seed + q);
+        max_q = std::max(max_q, train_.query_boundaries[q + 1] - train_.query_boundaries[q]);
+      }
+      std::vector<unsigned> jump(2 * static_cast<size_t>(max_q));      // [mul][max_q], [add][max_q]: x_{j+1} = mul[j] x_0 + add[j]
+      unsigned a = 1, c = 0;
+      for (int j = 0; j < max_q; ++j) { a = a * 214013u; c = c * 214013u + 2531011u; jump[j] = a; jump[max_q + j] = c; }
+      xe_max_q_ = max_q;
+      xe_state_.Alloc(nq); xe_state_.Upload(st.data(), nq, s);
+      xe_jump_.Alloc(jump.size()); xe_jump_.Upload(jump.data(), jump.size(), s);
+      xe_scratch_.Alloc(2 * static_cast<size_t>(n));
+      B200_CUDA(cudaStreamSynchronize(s));
     } else if (kind_ == Kind::kLambdarank) {
       const std::vector<double> lg = LabelGain(cfg_);
       const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
@@ -185,7 +206,7 @@ class Objective {
   // init score of class k, the same on every rank
   double BoostFromScore(int k) {
     if (kind_ == Kind::kMulticlass) return std::log(std::max(kEps, class_init_probs_[k]));
-    if (kind_ == Kind::kLambdarank) return 0.0;
+    if (kind_ == Kind::kLambdarank || kind_ == Kind::kRankXendcg) return 0.0;
     const int n = train_.num_data; double v;
     const float* y = train_.label.data(); const std::vector<float>& w = train_.weight;
     if (kind_ == Kind::kMape) v = LabelWeightedPercentile(y, label_weight_host_.data(), n, 0.5);
@@ -201,6 +222,10 @@ class Objective {
         const double pavg = std::max(std::min(s[0] / s[1], 1.0 - kEps), kEps);
         return std::log(pavg / (1.0 - pavg)) / (kind_ == Kind::kCrossEntropy ? 1.0 : cfg_.sigmoid);
       }
+      if (kind_ == Kind::kCrossEntropyLambda) {      // [UPSTREAM CrossEntropyLambda::BoostFromScore], global sums as cross_entropy
+        AllReduceHost(s, 2, ncclSum, stream_);
+        return std::log(std::expm1(s[0] / s[1]));
+      }
       v = s[0] / s[1];
       if (kind_ == Kind::kPoisson || kind_ == Kind::kGamma || kind_ == Kind::kTweedie) v = v > 0 ? std::log(v) : -std::numeric_limits<double>::infinity();
     }
@@ -208,7 +233,8 @@ class Objective {
     return v;
   }
 
-  void LaunchGradients(const double* score, float* g, float* h, int num_sms) const {
+  // advance: a training iteration, which moves rank_xendcg's random states on; false reads the gradients without changing them
+  void LaunchGradients(const double* score, float* g, float* h, int num_sms, bool advance) const {
     const int n = train_.num_data, grid = num_sms * 8;
     const float *y = train_.d_label.p, *w = train_.weight.empty() ? nullptr : train_.d_weight.p;
     switch (kind_) {
@@ -221,6 +247,13 @@ class Objective {
       case Kind::kMulticlass: k_grad_softmax<<<grid, 256, 0, stream_>>>(score, y, w, g, h, n, K_, static_cast<double>(K_) / (K_ - 1.0)); break;
       case Kind::kMulticlassOva: k_grad_ova<<<grid, 256, 0, stream_>>>(score, y, w, g, h, n, K_, cfg_.sigmoid, ova_w_.p, ova_need_.p); break;
       case Kind::kCrossEntropy: k_grad_xent<<<grid, 256, 0, stream_>>>(score, y, w, g, h, n); break;
+      case Kind::kCrossEntropyLambda: k_grad_xentlambda<<<grid, 256, 0, stream_>>>(score, y, w, g, h, n); break;
+      case Kind::kRankXendcg: {
+        const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
+        k_grad_xendcg<<<std::max(1, std::min(nq, num_sms * 16)), kXeThreads, 0, stream_>>>(score, y, w, train_.d_qb.p, nq, xe_state_.p, xe_jump_.p,
+                                                                                         xe_jump_.p + xe_max_q_, advance ? 1 : 0, xe_scratch_.p, n, g, h);
+        break;
+      }
       case Kind::kLambdarank: {
         const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
         const size_t smem = std::max<size_t>(LambdarankSmem(lr_max_q_, cfg_.lambdarank_truncation_level), 1024);
@@ -259,6 +292,7 @@ class Objective {
   DevBuf<double> lr_inv_max_dcg_, lr_label_gain_, lr_discount_;      // lambdarank
   DevBuf<float> lr_sig_table_;
   double lr_min_in_ = -50, lr_max_in_ = 50, lr_idx_factor_ = 0; int lr_max_q_ = 0;
+  DevBuf<unsigned> xe_state_, xe_jump_; DevBuf<double> xe_scratch_; int xe_max_q_ = 1;      // rank_xendcg: LCG per query, jump table, [2][n] rho / params
 };
 
 }  // namespace b200gbm
