@@ -36,6 +36,8 @@ struct Config {
   int feature_fraction_seed = 2;
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
+  double cat_l2 = 10.0, cat_smooth = 10.0;
+  int max_cat_threshold = 32, max_cat_to_onehot = 4, min_data_per_group = 100;
   double drop_rate = 0.1, skip_drop = 0.5;
   int max_drop = 50, drop_seed = 4;
   bool xgboost_dart_mode = false, uniform_drop = false;
@@ -173,7 +175,9 @@ struct Config {
     I("bagging_freq", &bagging_freq); I("bagging_seed", &bagging_seed); D("feature_fraction", &feature_fraction);
     I("feature_fraction_seed", &feature_fraction_seed); I("early_stopping_round", &early_stopping_round);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
-    D("min_gain_to_split", &min_gain_to_split); D("drop_rate", &drop_rate); I("max_drop", &max_drop); I("drop_seed", &drop_seed);
+    D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
+    I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
+    D("drop_rate", &drop_rate); I("max_drop", &max_drop); I("drop_seed", &drop_seed);
     D("skip_drop", &skip_drop); B("xgboost_dart_mode", &xgboost_dart_mode); B("uniform_drop", &uniform_drop);
     D("top_rate", &top_rate); D("other_rate", &other_rate); I("top_k", &top_k); I("verbosity", &verbosity);
     I("max_bin", &max_bin); I("min_data_in_bin", &min_data_in_bin); I("bin_construct_sample_cnt", &bin_construct_sample_cnt);
@@ -237,7 +241,8 @@ struct Config {
     s << "[linear_lambda: 0]\n[min_gain_to_split: " << Num(min_gain_to_split) << "]\n[drop_rate: " << Num(drop_rate) << "]\n";
     s << "[max_drop: " << max_drop << "]\n[skip_drop: " << Num(skip_drop) << "]\n[xgboost_dart_mode: " << xgboost_dart_mode << "]\n";
     s << "[uniform_drop: " << uniform_drop << "]\n[drop_seed: " << drop_seed << "]\n[top_rate: " << Num(top_rate) << "]\n[other_rate: " << Num(other_rate) << "]\n";
-    s << "[min_data_per_group: 100]\n[max_cat_threshold: 32]\n[cat_l2: 10]\n[cat_smooth: 10]\n[max_cat_to_onehot: 4]\n";
+    s << "[min_data_per_group: " << min_data_per_group << "]\n[max_cat_threshold: " << max_cat_threshold << "]\n[cat_l2: " << Num(cat_l2) << "]\n";
+    s << "[cat_smooth: " << Num(cat_smooth) << "]\n[max_cat_to_onehot: " << max_cat_to_onehot << "]\n";
     s << "[top_k: " << top_k << "]\n[monotone_constraints: ]\n[monotone_constraints_method: basic]\n[monotone_penalty: 0]\n";
     s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
     s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: 0]\n[interaction_constraints: ]\n";

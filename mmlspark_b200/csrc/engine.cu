@@ -944,11 +944,10 @@ void Booster::InitTraining() {
   sp_.min_gain_to_split = cfg.min_gain_to_split; sp_.min_sum_hessian = cfg.min_sum_hessian_in_leaf;
   sp_.min_data_in_leaf = cfg.min_data_in_leaf; sp_.max_depth = cfg.max_depth; sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
   sp_.nf = train->nf; sp_.nf_pad = train->nf_pad; sp_.num_tiles = train->num_tiles; sp_.nfn = train->nfn;
-  {   // categorical split search parameters: native defaults unless given (SURVEY.md B.2)
-    auto gd = [&](const char* k, double d) { auto it = cfg.raw.find(k); return (it != cfg.raw.end() && !it->second.empty()) ? std::atof(it->second.c_str()) : d; };
-    sp_.cat_l2 = gd("cat_l2", 10.0); sp_.cat_smooth = gd("cat_smooth", 10.0);
-    sp_.max_cat_threshold = static_cast<int>(gd("max_cat_threshold", 32)); sp_.max_cat_to_onehot = static_cast<int>(gd("max_cat_to_onehot", 4));
-    sp_.min_data_per_group = static_cast<int>(gd("min_data_per_group", 100)); sp_.pad3 = 0;
+  {   // categorical split search parameters (Config keeps the native defaults unless given, SURVEY.md B.2)
+    sp_.cat_l2 = cfg.cat_l2; sp_.cat_smooth = cfg.cat_smooth;
+    sp_.max_cat_threshold = cfg.max_cat_threshold; sp_.max_cat_to_onehot = cfg.max_cat_to_onehot;
+    sp_.min_data_per_group = cfg.min_data_per_group; sp_.pad3 = 0;
     if (train->nw > 0) {
       if (sp_.max_cat_threshold > kCatListMax) Fatal("max_cat_threshold > " + std::to_string(kCatListMax) + " is not supported together with categorical features of more than 256 bins");
       if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");

@@ -714,6 +714,10 @@ __device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const l
   for (int j = 0; j < 8; ++j) cnt[j] = static_cast<int>(static_cast<double>(qh[j]) * inv_h * cnt_factor + 0.5);
 
   // ---- reverse pass: bins num_bin-1-na .. 1, candidate threshold = b-1
+  // Both passes end where the sequential scan breaks: at the first candidate, in scan order, whose far side fails min_data_in_leaf or
+  // min_sum_hessian_in_leaf.  A lane stops its own loop there; the ballot then drops every lane that comes later in scan order, so
+  // their candidates neither win nor mark the feature splittable.  With hessians >= 0 nothing after a break could pass these tests
+  // anyway (counts and hessian sums are monotone); with negative hessians (custom objectives) they could.
   double best_gain = kNegInf, best_lg = 0, best_lh = 0;
   int best_thr = -1, best_lc = 0, best_dl = 1;
   bool any_valid = false;
@@ -723,6 +727,7 @@ __device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const l
 #pragma unroll 1
     for (int j = 0; j < 8; ++j) { const int b = lane * 8 + j; if (b >= 1 && b <= hi) { lg += qg[j]; lh += qh[j]; lc += cnt[j]; } }
     long long rg = warp_suffix_excl(lg, lane), rh = warp_suffix_excl(lh, lane), rc = warp_suffix_excl(lc, lane);
+    bool stop = false;
 #pragma unroll 1
     for (int j = 7; j >= 0; --j) {
       const int b = lane * 8 + j;
@@ -733,15 +738,16 @@ __device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const l
       const int right_count = static_cast<int>(rc);
       if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) continue;
       const int left_count = num_data - right_count;
-      if (left_count < p.min_data_in_leaf) continue;
       const double slh = sum_h - srh;
-      if (slh < p.min_sum_hessian) continue;
+      if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
       const double slg = sum_g - srg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       any_valid = true;
       if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_thr = b - 1; best_lc = left_count; }
     }
+    const unsigned brk = __ballot_sync(0xffffffffu, stop);      // the reverse scan runs from lane 31 down: the highest breaking lane ends it
+    if (brk && lane < 31 - __clz(brk)) { best_gain = kNegInf; best_thr = -1; any_valid = false; }
     // warp argmax: higher gain, ties -> higher threshold (first seen in the right-to-left scan)
     for (int o = 16; o; o >>= 1) {
       double og = __shfl_xor_sync(0xffffffffu, best_gain, o);
@@ -771,6 +777,7 @@ __device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const l
       base_c = num_data - static_cast<int>(ac);
     }
     double f_gain = kNegInf, f_lg = 0, f_lh = 0; int f_thr = 1 << 30, f_lc = 0;
+    bool stop = false, f_valid = false;
 #pragma unroll 1
     for (int j = 0; j < 8; ++j) {
       const int b = lane * 8 + j;
@@ -781,15 +788,17 @@ __device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const l
       const int left_count = base_c + static_cast<int>(pc);
       if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
       const int right_count = num_data - left_count;
-      if (right_count < p.min_data_in_leaf) continue;
       const double srh = sum_h - slh;
-      if (srh < p.min_sum_hessian) continue;
+      if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { stop = true; break; }
       const double srg = sum_g - slg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
-      any_valid = true;
+      f_valid = true;
       if (gain > f_gain) { f_gain = gain; f_lg = slg; f_lh = slh; f_thr = b; f_lc = left_count; }
     }
+    const unsigned brk = __ballot_sync(0xffffffffu, stop);      // the forward scan runs from lane 0 up: the lowest breaking lane ends it
+    if (brk && lane > __ffs(brk) - 1) { f_gain = kNegInf; f_thr = 1 << 30; f_valid = false; }
+    any_valid |= f_valid;
     for (int o = 16; o; o >>= 1) {
       double og = __shfl_xor_sync(0xffffffffu, f_gain, o);
       int ot = __shfl_xor_sync(0xffffffffu, f_thr, o);
@@ -1692,7 +1701,7 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
                                                   const SplitParams& p, uint8_t* flag, SplitCand* outp) {
   __shared__ long long s_sc[24];
   __shared__ double s_bg[8], s_blg[8], s_blh[8];
-  __shared__ int s_bt[8], s_blc[8], s_any;
+  __shared__ int s_bt[8], s_blc[8], s_any, s_stop[2];
   __shared__ long long s_tot[3];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
@@ -1703,9 +1712,11 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
   const int na = two_way ? 1 : 0;
   const int S = (m.num_bin + 255) / 256;
   const int b0 = threadIdx.x * S, b1 = min(b0 + S, m.num_bin);
-  if (threadIdx.x == 0) s_any = 0;
+  if (threadIdx.x == 0) { s_any = 0; s_stop[0] = -1; s_stop[1] = blockDim.x; }     // read after the barriers of d_block_excl3
   bool any_valid = false;
-  // ---- reverse pass: bins hi .. 1, candidate threshold = b - 1
+  // ---- reverse pass: bins hi .. 1, candidate threshold = b - 1.  Both passes end at the sequential scan's first break, as in
+  // d_scan_feature: a thread stops its own bins there, and the threads after the first breaking one in scan order drop their candidates.
+  bool stop = false;
   double best_gain = kNegInf, best_lg = 0, best_lh = 0;
   int best_thr = -1, best_lc = 0, best_dl = 1;
   {
@@ -1724,15 +1735,17 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       const int right_count = static_cast<int>(rc);
       if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) continue;
       const int left_count = num_data - right_count;
-      if (left_count < p.min_data_in_leaf) continue;
       const double slh = sum_h - srh;
-      if (slh < p.min_sum_hessian) continue;
+      if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
       const double slg = sum_g - srg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       any_valid = true;
       if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_thr = b - 1; best_lc = left_count; }
     }
+    if (stop) atomicMax(&s_stop[0], static_cast<int>(threadIdx.x));     // the reverse scan runs from the last thread down
+    __syncthreads();
+    if (static_cast<int>(threadIdx.x) < s_stop[0]) { best_gain = kNegInf; best_thr = -1; any_valid = false; }
     for (int o = 16; o; o >>= 1) {
       const double og = __shfl_xor_sync(0xffffffffu, best_gain, o);
       const int ot = __shfl_xor_sync(0xffffffffu, best_thr, o);
@@ -1774,6 +1787,7 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       base_c = num_data - static_cast<int>(ac);
     }
     double f_gain = kNegInf, f_lg = 0, f_lh = 0; int f_thr = 1 << 30, f_lc = 0;
+    bool f_stop = false, f_valid = false;
     for (int b = b0; b < b1; ++b) {
       if (b > hi) continue;
       if (b >= m.offset) { const long long qh = hist[b * 2 + 1]; pg += hist[b * 2]; ph += qh; pc += static_cast<int>(static_cast<double>(qh) * inv_h * cnt_factor + 0.5); }
@@ -1782,15 +1796,18 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       const int left_count = base_c + static_cast<int>(pc);
       if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
       const int right_count = num_data - left_count;
-      if (right_count < p.min_data_in_leaf) continue;
       const double srh = sum_h - slh;
-      if (srh < p.min_sum_hessian) continue;
+      if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { f_stop = true; break; }
       const double srg = sum_g - slg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
-      any_valid = true;
+      f_valid = true;
       if (gain > f_gain) { f_gain = gain; f_lg = slg; f_lh = slh; f_thr = b; f_lc = left_count; }
     }
+    if (f_stop) atomicMin(&s_stop[1], static_cast<int>(threadIdx.x));    // the forward scan runs from thread 0 up
+    __syncthreads();
+    if (static_cast<int>(threadIdx.x) > s_stop[1]) { f_gain = kNegInf; f_thr = 1 << 30; f_valid = false; }
+    any_valid |= f_valid;
     for (int o = 16; o; o >>= 1) {
       const double og = __shfl_xor_sync(0xffffffffu, f_gain, o);
       const int ot = __shfl_xor_sync(0xffffffffu, f_thr, o);
