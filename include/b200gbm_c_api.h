@@ -176,6 +176,9 @@ int B200GBM_DatasetGetBinToCat(DatasetHandle handle, int feature, int* out, int*
 /* bins of the selected rows only, gathered on the device: out [nrows][num_feature] uint16 (trivial features 0).  Lets a test or
  * bench.py check rows of a dataset far too large to download (the 100M x 512 benchmark matrix) against host-side binning. */
 int B200GBM_DatasetGetBinsRows(DatasetHandle handle, const int32_t* rows, int32_t nrows, uint16_t* out);
+/* storage layout of the uint8 bins: out_num_columns = storage columns (feature bundles + plain features + wide features), out_column_of
+ * [num_feature] = the column of each feature, -1 if unused.  Features of one exclusive feature bundle share a column. */
+int B200GBM_DatasetGetBundles(DatasetHandle handle, int* out_num_columns, int* out_column_of);
 /* {min, max} of the sampled values of a feature (the feature_infos entry of the model text) */
 int B200GBM_DatasetGetFeatureRange(DatasetHandle handle, int feature, double* out2);
 int B200GBM_DatasetGetFeatureInfo(DatasetHandle handle, int feature, int* out5);   /* num_bin, missing, default_bin, most_freq_bin, trivial */

@@ -249,6 +249,12 @@ class Dataset:
         check(load().B200GBM_DatasetGetBinsRows(self.handle, _ptr(rows), C.c_int32(len(rows)), _ptr(out)))
         return out
 
+    def bundles(self):
+        """(number of storage columns, storage column of every feature or -1 if unused); bundled features share a column"""
+        out = np.zeros(max(self.num_feature(), 1), dtype=np.int32); k = C.c_int(0)
+        check(load().B200GBM_DatasetGetBundles(self.handle, C.byref(k), _ptr(out)))
+        return k.value, out[:self.num_feature()].copy()
+
     def feature_range(self, f):
         out = np.zeros(2, dtype=np.float64)
         check(load().B200GBM_DatasetGetFeatureRange(self.handle, C.c_int(f), _ptr(out)))

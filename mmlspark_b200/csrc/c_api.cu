@@ -541,6 +541,11 @@ int B200GBM_DatasetGetBinsRows(DatasetHandle handle, const int32_t* rows, int32_
   DS(handle)->GetBinsOfRows(rows, nrows, out);
   API_END();
 }
+int B200GBM_DatasetGetBundles(DatasetHandle handle, int* out_num_columns, int* out_column_of) {
+  API_BEGIN();
+  DS(handle)->GetBundles(out_num_columns, out_column_of);
+  API_END();
+}
 int B200GBM_DatasetGetFeatureRange(DatasetHandle handle, int feature, double* out2) {
   API_BEGIN();
   const FeatureBins& fb = DS(handle)->mappers.at(feature);

@@ -50,6 +50,7 @@ struct Config {
   int bin_construct_sample_cnt = 200000;
   int data_random_seed = 1;
   bool use_missing = true, zero_as_missing = false, feature_pre_filter = true, pre_partition = false;
+  bool enable_bundle = true;                // exclusive feature bundling of sparse features (bundle.h)
   std::vector<int> categorical_feature;
   std::string max_bin_by_feature;
   // --- objective
@@ -92,7 +93,7 @@ struct Config {
         {"reg_lambda", "lambda_l2"}, {"lambda", "lambda_l2"}, {"min_split_gain", "min_gain_to_split"},
         {"rate_drop", "drop_rate"}, {"topk", "top_k"}, {"verbose", "verbosity"},
         {"subsample_for_bin", "bin_construct_sample_cnt"}, {"data_seed", "data_random_seed"},
-        {"is_pre_partition", "pre_partition"}, {"cat_feature", "categorical_feature"},
+        {"is_pre_partition", "pre_partition"}, {"is_enable_bundle", "enable_bundle"}, {"bundle", "enable_bundle"}, {"cat_feature", "categorical_feature"},
         {"categorical_column", "categorical_feature"}, {"cat_column", "categorical_feature"},
         {"num_classes", "num_class"}, {"unbalance", "is_unbalance"}, {"unbalanced_sets", "is_unbalance"},
         {"max_position", "lambdarank_truncation_level"}, {"metrics", "metric"}, {"metric_types", "metric"},
@@ -182,7 +183,7 @@ struct Config {
     D("top_rate", &top_rate); D("other_rate", &other_rate); I("top_k", &top_k); I("verbosity", &verbosity);
     I("max_bin", &max_bin); I("min_data_in_bin", &min_data_in_bin); I("bin_construct_sample_cnt", &bin_construct_sample_cnt);
     I("data_random_seed", &data_random_seed); B("use_missing", &use_missing); B("zero_as_missing", &zero_as_missing);
-    B("feature_pre_filter", &feature_pre_filter); B("pre_partition", &pre_partition);
+    B("feature_pre_filter", &feature_pre_filter); B("pre_partition", &pre_partition); B("enable_bundle", &enable_bundle);
     S("max_bin_by_feature", &max_bin_by_feature);
     I("num_class", &num_class); B("is_unbalance", &is_unbalance); D("scale_pos_weight", &scale_pos_weight);
     D("sigmoid", &sigmoid); B("boost_from_average", &boost_from_average); D("alpha", &alpha);
@@ -249,7 +250,7 @@ struct Config {
     s << "[verbosity: " << verbosity << "]\n[saved_feature_importance_type: 0]\n[linear_tree: 0]\n[max_bin: " << max_bin << "]\n";
     s << "[max_bin_by_feature: " << max_bin_by_feature << "]\n[min_data_in_bin: " << min_data_in_bin << "]\n";
     s << "[bin_construct_sample_cnt: " << bin_construct_sample_cnt << "]\n[data_random_seed: " << data_random_seed << "]\n";
-    s << "[is_enable_sparse: 1]\n[enable_bundle: 1]\n[use_missing: " << use_missing << "]\n[zero_as_missing: " << zero_as_missing << "]\n";
+    s << "[is_enable_sparse: 1]\n[enable_bundle: " << enable_bundle << "]\n[use_missing: " << use_missing << "]\n[zero_as_missing: " << zero_as_missing << "]\n";
     s << "[feature_pre_filter: " << feature_pre_filter << "]\n[pre_partition: " << pre_partition << "]\n[two_round: 0]\n[header: 0]\n";
     s << "[label_column: ]\n[weight_column: ]\n[group_column: ]\n[ignore_column: ]\n[categorical_feature: " << join_i(categorical_feature) << "]\n";
     s << "[forcedbins_filename: ]\n[objective_seed: " << objective_seed << "]\n[num_class: " << num_class << "]\n[is_unbalance: " << is_unbalance << "]\n";

@@ -284,10 +284,12 @@ std::vector<int> Dataset::SampleRows() const {
 }
 
 // Mappers and feature names of a new dataset.  With a reference they are the reference's and the bin parameters are not checked.
-// Otherwise the bin parameters are checked, then sample(&nz, f0, f1) fills nz[f] with the sampled values of feature f that are
-// NaN or have |v| > 1e-35 (at least for this rank's features f0 <= f < f1) and returns the number of sampled rows.
+// Otherwise the bin parameters are checked, then sample(&nz, &nz_rows, f0, f1) fills nz[f] with the sampled values of feature f that are
+// NaN or have |v| > 1e-35 (at least for this rank's features f0 <= f < f1) and returns the number of sampled rows.  When nz_rows is not
+// null (bundling), it fills every feature, and nz_rows[f] with the sample position (0 .. count-1) of each value of nz[f].
+// Bundles are grouped on rank 0's sample and broadcast, so every rank starts from the same candidate bundles.
 template <typename Sample>
-void Dataset::SetMappers(const Dataset* reference, Sample sample) {
+void Dataset::SetMappers(const Dataset* reference, bool may_bundle, Sample sample) {
   const int n = num_data, F = num_total_features;
   if (reference) {
     if (reference->num_total_features != F) Fatal("Validation data has a different number of features than the reference dataset");
@@ -302,16 +304,21 @@ void Dataset::SetMappers(const Dataset* reference, Sample sample) {
   const int world = Net().active ? Net().world : 1, rank = Net().active ? Net().rank : 0;
   const int step = std::max(1, (F + world - 1) / world);
   const int f0 = world == 1 ? 0 : std::min(F, rank * step), f1 = world == 1 ? F : std::min(F, f0 + step);
+  const bool bundle = may_bundle && cfg.enable_bundle;
   std::vector<std::vector<double>> nz(F);
-  const int sample_cnt = sample(&nz, f0, f1);
+  std::vector<std::vector<int>> nz_rows(bundle ? F : 0);
+  const int sample_cnt = sample(&nz, bundle ? &nz_rows : nullptr, f0, f1);
   NvtxRange nvtx("b200gbm:find bins (host) + C5 mapper all-gather");
   const int filter_cnt = static_cast<int>(static_cast<double>(cfg.min_data_in_leaf) * sample_cnt / n);
   mappers.assign(F, FeatureBins());
 #pragma omp parallel for schedule(dynamic)
   for (int f = f0; f < f1; ++f) {
+    std::vector<double> vals;      // the bin finders reorder their input; bundling needs nz[f] in step with nz_rows[f]
+    std::vector<double>* v = &nz[f];
+    if (bundle) { vals = nz[f]; v = &vals; }
     const bool is_cat = std::find(cfg.categorical_feature.begin(), cfg.categorical_feature.end(), f) != cfg.categorical_feature.end();
-    if (is_cat) mappers[f] = FindCategoricalBins(&nz[f], sample_cnt, cfg.max_bin, cfg.min_data_in_bin, filter_cnt, cfg.feature_pre_filter);
-    else mappers[f] = FindFeatureBins(&nz[f], sample_cnt, cfg.max_bin, cfg.min_data_in_bin, filter_cnt, cfg.feature_pre_filter, cfg.use_missing,
+    if (is_cat) mappers[f] = FindCategoricalBins(v, sample_cnt, cfg.max_bin, cfg.min_data_in_bin, filter_cnt, cfg.feature_pre_filter);
+    else mappers[f] = FindFeatureBins(v, sample_cnt, cfg.max_bin, cfg.min_data_in_bin, filter_cnt, cfg.feature_pre_filter, cfg.use_missing,
                                       cfg.zero_as_missing);
   }
   for (int f = f0; f < f1; ++f)
@@ -338,6 +345,79 @@ void Dataset::SetMappers(const Dataset* reference, Sample sample) {
   }
   feature_names.resize(F);
   for (int f = 0; f < F; ++f) feature_names[f] = "Column_" + std::to_string(f);
+  bundles.clear();
+  if (!bundle) return;
+  if (rank == 0) {
+    std::vector<std::vector<int>> off_mfb(F);
+#pragma omp parallel for schedule(dynamic)
+    for (int f = 0; f < F; ++f) {
+      const FeatureBins& fb = mappers[f];
+      if (!BundleCandidate(fb)) continue;
+      for (size_t i = 0; i < nz[f].size(); ++i)
+        if (fb.ValueToBin(nz[f][i]) != fb.most_freq_bin) off_mfb[f].push_back(nz_rows[f][i]);
+    }
+    bundles = FindBundles(mappers, off_mfb, sample_cnt);
+  }
+  if (world > 1) {      // broadcast rank 0's grouping: bundle index + 1 of every feature, summed over ranks that send zeros
+    std::vector<double> of(F, 0.0);
+    for (size_t k = 0; k < bundles.size(); ++k) for (int f : bundles[k]) of[f] = static_cast<double>(k + 1);
+    AllReduceHost(of.data(), F, ncclSum, stream);
+    int nb = 0;
+    for (int f = 0; f < F; ++f) nb = std::max(nb, static_cast<int>(of[f]));
+    bundles.assign(nb, {});
+    for (int f = 0; f < F; ++f) if (of[f] > 0) bundles[static_cast<int>(of[f]) - 1].push_back(f);
+  }
+}
+
+// The device table of the bundle members (BundleMember, kernels.cuh).  inner / base / the bundle columns are valid after UploadMeta.
+void Dataset::UploadBundleMembers() {
+  std::vector<BundleMember> mem;
+  std::vector<int> start(1, 0), bcol;
+  for (const std::vector<int>& b : bundles) {
+    int base = 0;
+    for (int f : b) {
+      const FeatureBins& fb = mappers[f];
+      const int db = static_cast<int>(fb.default_bin);
+      BundleMember m{};
+      m.zlo = db == 0 ? -std::numeric_limits<double>::infinity() : fb.upper[db - 1];
+      m.zhi = fb.upper[db];
+      m.real_index = f;
+      m.inner = inner_of.empty() ? -1 : inner_of[f];
+      m.base = base;
+      m.bundle = static_cast<int>(start.size()) - 1;
+      m.nan_moves = fb.missing_type == MISSING_NAN ? 1 : 0;
+      mem.push_back(m);
+      base += fb.num_bin - 1;
+    }
+    start.push_back(static_cast<int>(mem.size()));
+    bcol.push_back(inner_of.empty() ? -1 : meta_host[inner_of[b[0]]].hist_off >> 8);
+  }
+  d_members.Alloc(std::max<size_t>(mem.size(), 1)); d_bundle_start.Alloc(start.size()); d_bundle_col.Alloc(std::max<size_t>(bcol.size(), 1));
+  if (!mem.empty()) { d_members.Upload(mem.data(), mem.size(), stream); d_bundle_col.Upload(bcol.data(), bcol.size(), stream); }
+  d_bundle_start.Upload(start.data(), start.size(), stream);
+  B200_CUDA(cudaStreamSynchronize(stream));
+}
+
+// Every row of the input is checked before any bin is written; with data-parallel training the counts of all ranks are combined, so
+// every rank keeps the same bundles (and the histogram all-reduce one buffer shape).
+template <typename Count>
+void Dataset::DissolveConflictingBundles(Count count) {
+  const bool parallel = Net().active && Net().world > 1;
+  if (bundles.empty()) return;
+  NvtxRange nvtx("b200gbm:bundle row check");
+  UploadBundleMembers();
+  const int nb = static_cast<int>(bundles.size());
+  DevBuf<unsigned long long> conflicts; conflicts.Alloc(nb); conflicts.Zero(stream);
+  count(conflicts.p);
+  B200_CUDA(cudaGetLastError());
+  std::vector<unsigned long long> h(nb);
+  conflicts.Download(h.data(), nb, stream);
+  B200_CUDA(cudaStreamSynchronize(stream));
+  std::vector<double> c(h.begin(), h.end());
+  if (parallel) AllReduceHost(c.data(), nb, ncclMax, stream);
+  std::vector<std::vector<int>> kept;
+  for (int k = 0; k < nb; ++k) if (c[k] == 0.0) kept.push_back(std::move(bundles[k]));
+  bundles = std::move(kept);
 }
 
 void Dataset::UploadMeta() {
@@ -356,11 +436,28 @@ void Dataset::UploadMeta() {
   nw = nf - nfn;
   sample_order.clear();
   for (int f = 0; f < num_total_features; ++f) if (inner_of[f] >= 0) sample_order.push_back(inner_of[f]);
-  num_tiles = std::max(1, (nfn + 31) / 32);
-  nf_pad = num_tiles * 32 + nw;
+  // storage columns in inner-feature order: a plain feature's column, or its bundle's column where the bundle's first feature comes
+  std::vector<int> bundle_of(num_total_features, -1), col_of(nfn, 0), base_of(nfn, -1), bundle_col(bundles.size(), -1);
+  for (size_t k = 0; k < bundles.size(); ++k) {
+    int base = 0;
+    for (int f : bundles[k]) { bundle_of[f] = static_cast<int>(k); base_of[inner_of[f]] = base; base += mappers[f].num_bin - 1; }
+  }
+  num_columns = 0;
+  for (int u = 0; u < nfn; ++u) {
+    const int k = bundle_of[used[u]];
+    if (k < 0) col_of[u] = num_columns++;
+    else { if (bundle_col[k] < 0) bundle_col[k] = num_columns++; col_of[u] = bundle_col[k]; }
+  }
+  num_tiles = std::max(1, (num_columns + 31) / 32);
+  col_feat.assign(static_cast<size_t>(num_tiles) * 32, -1);
+  for (int u = 0; u < nfn; ++u) if (base_of[u] < 0) col_feat[col_of[u]] = u;
+  const int nft = std::max(1, (nfn + 31) / 32) * 32;      // inner slots of the tile features
+  nf_pad = nft + nw;
   meta_host.assign(nf_pad, FeatMeta{1, 0, 0, 0, 0, 0, 0, 0});
-  std::vector<double> ubh(static_cast<size_t>(num_tiles) * 32 * 256, 0.0);
-  std::vector<uint8_t> cbh(static_cast<size_t>(num_tiles) * 32 * 256, 0);
+  bundle_base.assign(nf_pad, -1);
+  for (int u = 0; u < nfn; ++u) bundle_base[u] = base_of[u];
+  std::vector<double> ubh(static_cast<size_t>(nft) * 256, 0.0);
+  std::vector<uint8_t> cbh(static_cast<size_t>(nft) * 256, 0);
   has_categorical = false;
   hist_pairs = static_cast<size_t>(num_tiles) * 32 * 256;
   wide_host.clear();
@@ -369,7 +466,7 @@ void Dataset::UploadMeta() {
   std::vector<double> wub;
   for (int u = 0; u < nf; ++u) {
     const FeatureBins& fb = mappers[used[u]];
-    int hist_off = u * 256;
+    int hist_off = u < nfn ? col_of[u] * 256 : 0;
     if (u >= nfn) {
       hist_off = static_cast<int>(hist_pairs);
       WideMeta wm{fb.num_bin, hist_off, static_cast<int>(fb.categorical ? wcats.size() : wub.size()), static_cast<int>(fb.sorted_cats.size()),
@@ -395,6 +492,9 @@ void Dataset::UploadMeta() {
   }
   meta.Alloc(nf_pad); ub.Alloc(ubh.size()); catbin.Alloc(cbh.size());
   meta.Upload(meta_host.data(), nf_pad, stream);
+  d_col_feat.Alloc(col_feat.size()); d_col_feat.Upload(col_feat.data(), col_feat.size(), stream);
+  d_bundle_base.Alloc(nf_pad); d_bundle_base.Upload(bundle_base.data(), nf_pad, stream);
+  if (!bundles.empty()) UploadBundleMembers();
   ub.Upload(ubh.data(), ubh.size(), stream);
   catbin.Upload(cbh.data(), cbh.size(), stream);
   if (nw > 0) {
@@ -422,7 +522,10 @@ static void LaunchBin(const T* X, long long nrow, int ncol, int row_major, long 
   const int sms = DeviceSMs();
   dim3 grid(static_cast<unsigned>(std::min<long long>((nrow + 7) / 8, sms * 8)), d.num_tiles);
   if (grid.x == 0) grid.x = 1;
-  k_bin_rows<T><<<grid, 256, 65536, s>>>(X, nrow, ncol, row_major, ld, d.meta.p, d.ub.p, d.catbin.p, d.nfn, d.bins.p, static_cast<long long>(d.rows_stride), row_offset);
+  k_bin_rows<T><<<grid, 256, 65536, s>>>(X, nrow, ncol, row_major, ld, d.meta.p, d.ub.p, d.catbin.p, d.d_col_feat.p, d.bins.p, static_cast<long long>(d.rows_stride), row_offset);
+  if (!d.bundles.empty())      // after k_bin_rows (same stream): it left the bundle columns at slot 0
+    k_bin_bundles<T><<<sms * 8, 256, 0, s>>>(X, nrow, row_major, ld, d.d_members.p, d.d_bundle_start.p, d.d_bundle_col.p, static_cast<int>(d.bundles.size()),
+                                             d.meta.p, d.ub.p, d.bins.p, static_cast<long long>(d.rows_stride), row_offset);
   if (d.nw > 0)
     k_bin_wide<T><<<sms * 8, 256, 0, s>>>(X, nrow, row_major, ld, d.wide_meta.p, d.nw, d.wide_cats.p, d.wide_catbin.p, d.wide_ub.p, d.bins16.p, d.rows_stride, row_offset);
   B200_CUDA(cudaGetLastError());
@@ -431,12 +534,22 @@ static void LaunchBin(const T* X, long long nrow, int ncol, int row_major, long 
 void Dataset::BinBlock(const void* data, bool on_device, int data_type, int is_row_major, long long n, long long start_row) {
   NvtxRange nvtx("b200gbm:K0 bin rows (H2D + value->bin)");
   const int F = num_total_features;
-  const size_t esz = data_type == 0 ? 4 : 8;
   if (start_row < 0 || start_row + n > num_data) Fatal("row block out of range");
+  ForEachDeviceBlock(data, on_device, data_type, is_row_major, n, [&](const void* x, long long rows, long long ld, long long r0) {
+    if (data_type == 0) LaunchBin<float>(static_cast<const float*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
+    else LaunchBin<double>(static_cast<const double*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
+  });
+  if (on_device) return;
+  ingest_rows_done_ += n;
+  if (ingest_rows_done_ >= num_data) ReleaseIngestStaging();
+}
+
+template <typename Fn>
+void Dataset::ForEachDeviceBlock(const void* data, bool on_device, int data_type, int is_row_major, long long n, Fn fn) {
+  const int F = num_total_features;
+  const size_t esz = data_type == 0 ? 4 : 8;
   if (on_device) {
-    const long long ld = is_row_major ? F : n;
-    if (data_type == 0) LaunchBin<float>(static_cast<const float*>(data), n, F, is_row_major, ld, *this, start_row, stream);
-    else LaunchBin<double>(static_cast<const double*>(data), n, F, is_row_major, ld, *this, start_row, stream);
+    fn(data, n, is_row_major ? F : n, 0LL);
     B200_CUDA(cudaStreamSynchronize(stream));
     return;
   }
@@ -469,14 +582,10 @@ void Dataset::BinBlock(const void* data, bool on_device, int data_type, int is_r
     }
     B200_CUDA(cudaEventRecord(ingest_copied_[b], copy_stream));
     B200_CUDA(cudaStreamWaitEvent(stream, ingest_copied_[b], 0));
-    const long long ld = is_row_major ? F : rows;
-    if (data_type == 0) LaunchBin<float>(reinterpret_cast<const float*>(ingest_buf_[b].p), rows, F, is_row_major, ld, *this, start_row + r0, stream);
-    else LaunchBin<double>(reinterpret_cast<const double*>(ingest_buf_[b].p), rows, F, is_row_major, ld, *this, start_row + r0, stream);
+    fn(static_cast<const void*>(ingest_buf_[b].p), rows, is_row_major ? F : rows, r0);
     B200_CUDA(cudaEventRecord(ingest_binned_[b], stream));
   }
   B200_CUDA(cudaStreamSynchronize(stream));          // all copies are consumed: the caller may reuse its buffer
-  ingest_rows_done_ += n;
-  if (ingest_rows_done_ >= num_data) ReleaseIngestStaging();
 }
 
 void Dataset::ReleaseIngestStaging() {
@@ -494,7 +603,7 @@ Dataset* Dataset::CreateFromSampledColumn(double** sample_data, int** sample_ind
   EnsureDevice();
   if (num_total_row <= 0 || ncol <= 0) Fatal("Dataset should have at least one row and one column");
   std::unique_ptr<Dataset> d = NewShell(num_total_row, ncol, params);
-  d->SetMappers(nullptr, [&](std::vector<std::vector<double>>* nz, int, int) {      // the caller sampled the rows and dropped the zeros
+  d->SetMappers(nullptr, false, [&](std::vector<std::vector<double>>* nz, std::vector<std::vector<int>>*, int, int) {      // the caller sampled the rows and dropped the zeros
     for (int f = 0; f < ncol; ++f) (*nz)[f].assign(sample_data[f], sample_data[f] + num_per_col[f]);
     return num_sample_row;
   });
@@ -519,8 +628,11 @@ void Dataset::UnpackTiles(T* out) const {
   std::memset(out, 0, static_cast<size_t>(num_data) * num_total_features * sizeof(T));
   for (int u = 0; u < nfn; ++u) {
     const int f = used[u];
-    const uint8_t* src = h.data() + (static_cast<size_t>(u >> 5) * rows_stride) * 32 + (u & 31);
-    for (int i = 0; i < num_data; ++i) out[static_cast<size_t>(i) * num_total_features + f] = src[static_cast<size_t>(i) * 32];
+    const FeatMeta& m = meta_host[u];
+    const int c = m.hist_off >> 8;
+    const uint8_t* src = h.data() + (static_cast<size_t>(c >> 5) * rows_stride) * 32 + (c & 31);
+    for (int i = 0; i < num_data; ++i)
+      out[static_cast<size_t>(i) * num_total_features + f] = static_cast<T>(d_unbundle(src[static_cast<size_t>(i) * 32], bundle_base[u], m.default_bin, m.num_bin));
   }
 }
 void Dataset::GetBinsRowMajor(uint8_t* out) const {
@@ -573,7 +685,8 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   if (idx) didx.Upload(idx, cnt, stream);
   const size_t elems = static_cast<size_t>(num_tiles) * 32 * 512;      // tile features only (wide features are covered by the model-level tests)
   DevBuf<long long> H; H.Alloc(elems); H.Zero(stream);
-  DevBuf<double> D; D.Alloc(elems);
+  const size_t felems = static_cast<size_t>(std::max(nfn, 1)) * 512;     // per feature
+  DevBuf<double> D; D.Alloc(felems);
   int sms = 0;
   B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   k_absmax<<<sms * 4, 256, 0, stream>>>(g.p, h.p, n, ctrl.p);
@@ -585,10 +698,30 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   k_gather_q<<<sms * 4, 256, 0, stream>>>(&ctrl.p->hist_work, didx.p, didx.p, q.p, qo.p);
   launch_k4(/*const_hessian=*/false, bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
             reinterpret_cast<unsigned long long*>(H.p), sms, stream);
-  k_hist_to_double<<<sms * 4, 256, 0, stream>>>(H.p, D.p, elems, ctrl.p);
+  // per-feature histograms out of the column histograms, exact int64 as in k_scan: a bundle member's most frequent bin is the column total
+  // minus the member's other bins
+  std::vector<long long> hc(elems), hf(felems, 0);
+  H.Download(hc.data(), elems, stream);
+  B200_CUDA(cudaStreamSynchronize(stream));
+  for (int u = 0; u < nfn; ++u) {
+    const FeatMeta& m = meta_host[u];
+    const long long* c = hc.data() + static_cast<size_t>(m.hist_off) * 2;
+    long long* o = hf.data() + static_cast<size_t>(u) * 512;
+    if (bundle_base[u] < 0) { std::copy(c, c + 512, o); continue; }
+    long long tot[2] = {0, 0};
+    for (int s = 0; s < 256; ++s) { tot[0] += c[s * 2]; tot[1] += c[s * 2 + 1]; }
+    for (int b = 0; b < m.num_bin; ++b) {
+      if (b == m.default_bin) continue;
+      const unsigned s = d_bundle_slot(static_cast<unsigned>(b), bundle_base[u], m.default_bin);
+      for (int j = 0; j < 2; ++j) { o[b * 2 + j] = c[s * 2 + j]; tot[j] -= c[s * 2 + j]; }
+    }
+    o[m.default_bin * 2] = tot[0]; o[m.default_bin * 2 + 1] = tot[1];
+  }
+  DevBuf<long long> HF; HF.Alloc(felems); HF.Upload(hf.data(), felems, stream);
+  k_hist_to_double<<<sms * 4, 256, 0, stream>>>(HF.p, D.p, felems, ctrl.p);
   B200_CUDA(cudaGetLastError());
-  std::vector<double> hd(elems);
-  D.Download(hd.data(), elems, stream);
+  std::vector<double> hd(felems);
+  D.Download(hd.data(), felems, stream);
   B200_CUDA(cudaStreamSynchronize(stream));
   std::memset(out, 0, sizeof(double) * static_cast<size_t>(num_total_features) * 512);
   for (int u = 0; u < nfn; ++u) std::memcpy(out + static_cast<size_t>(used[u]) * 512, hd.data() + static_cast<size_t>(u) * 512, sizeof(double) * 512);
@@ -602,7 +735,7 @@ Dataset* Dataset::CreateFromMat(const void* data, int data_type, int nrow, int n
   std::unique_ptr<Dataset> d = NewShell(nrow, ncol, params);
   StreamTimer timer(d->stream);
   const bool on_device = IsDevicePointer(data);
-  d->SetMappers(reference, [&](std::vector<std::vector<double>>* nz, int f0, int f1) {      // the sampled rows, gathered where the data is
+  d->SetMappers(reference, true, [&](std::vector<std::vector<double>>* nz, std::vector<std::vector<int>>* nz_rows, int f0, int f1) {      // the sampled rows, gathered where the data is
     const int n = nrow, F = ncol;
     const std::vector<int> rows = d->SampleRows();
     const int sample_cnt = static_cast<int>(rows.size());
@@ -629,15 +762,25 @@ Dataset* Dataset::CreateFromMat(const void* data, int data_type, int nrow, int n
         }
       }
     }
+    if (nz_rows) { f0 = 0; f1 = F; }
 #pragma omp parallel for schedule(dynamic)
     for (int f = f0; f < f1; ++f) {
-      (*nz)[f].reserve(sample_cnt);
       for (int s = 0; s < sample_cnt; ++s) {
         double v = S[static_cast<size_t>(s) * F + f];
-        if (std::fabs(v) > kZeroThr || std::isnan(v)) (*nz)[f].push_back(v);
+        if (std::fabs(v) > kZeroThr || std::isnan(v)) {
+          (*nz)[f].push_back(v);
+          if (nz_rows) (*nz_rows)[f].push_back(s);
+        }
       }
     }
     return sample_cnt;
+  });
+  d->DissolveConflictingBundles([&](unsigned long long* conflicts) {
+    const int nb = static_cast<int>(d->bundles.size()), grid = DeviceSMs() * 8;
+    d->ForEachDeviceBlock(data, on_device, data_type, is_row_major, nrow, [&](const void* x, long long rows, long long ld, long long) {
+      if (data_type == 0) k_bundle_conflicts<float><<<grid, 256, 0, d->stream>>>(static_cast<const float*>(x), rows, is_row_major, ld, d->d_members.p, d->d_bundle_start.p, nb, conflicts);
+      else k_bundle_conflicts<double><<<grid, 256, 0, d->stream>>>(static_cast<const double*>(x), rows, is_row_major, ld, d->d_members.p, d->d_bundle_start.p, nb, conflicts);
+    });
   });
   d->AllocBins();
   d->BinBlock(data, on_device, data_type, is_row_major, nrow, 0);
@@ -654,22 +797,25 @@ __global__ void k_fill_default_wide(const WideMeta* __restrict__ wm, int nw, uin
     bins16[static_cast<size_t>(w) * rows_stride + (e - static_cast<long long>(w) * nrow)] = static_cast<uint16_t>(wm[w].default_bin);
   }
 }
-__global__ void k_fill_default_bins(const FeatMeta* __restrict__ meta, int nf, uint8_t* __restrict__ bins, size_t rows_stride, long long nrow, int num_tiles) {
+// every column's default: a plain feature's default bin, slot 0 of a bundle column (all members at their default bin), 0 for padding
+__global__ void k_fill_default_bins(const FeatMeta* __restrict__ meta, const int* __restrict__ col_feat, uint8_t* __restrict__ bins, size_t rows_stride,
+                                    long long nrow, int num_tiles) {
   const long long total = nrow * num_tiles * 32;
   for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total; e += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int lane = static_cast<int>(e & 31);
     const long long rt = e >> 5;
     const int tile = static_cast<int>(rt / nrow);
     const long long r = rt - static_cast<long long>(tile) * nrow;
-    const int u = tile * 32 + lane;
-    bins[(static_cast<size_t>(tile) * rows_stride + r) * 32 + lane] = u < nf ? static_cast<uint8_t>(meta[u].default_bin) : 0;
+    const int u = col_feat[tile * 32 + lane];
+    bins[(static_cast<size_t>(tile) * rows_stride + r) * 32 + lane] = u >= 0 ? static_cast<uint8_t>(meta[u].default_bin) : 0;
   }
 }
 template <typename TI, typename TV>
 __global__ void k_bin_csr(const TI* __restrict__ indptr, const int* __restrict__ indices, const TV* __restrict__ vals, long long nrow, const int* __restrict__ inner_of,
                           const FeatMeta* __restrict__ meta, const double* __restrict__ ub, const uint8_t* __restrict__ catbin, uint8_t* __restrict__ bins,
                           size_t rows_stride, long long elem_base, int nfn, const WideMeta* __restrict__ wm, const int* __restrict__ wcats,
-                          const unsigned short* __restrict__ wcatbin, const double* __restrict__ wub, uint16_t* __restrict__ bins16) {
+                          const unsigned short* __restrict__ wcatbin, const double* __restrict__ wub, uint16_t* __restrict__ bins16,
+                          const int* __restrict__ bundle_base) {
   const int lane = threadIdx.x & 31;
   const long long warp = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5, nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
   for (long long r = warp; r < nrow; r += nwarps) {
@@ -702,7 +848,12 @@ __global__ void k_bin_csr(const TI* __restrict__ indptr, const int* __restrict__
           bin = lo;
         }
       }
-      bins[(static_cast<size_t>(u >> 5) * rows_stride + r) * 32 + (u & 31)] = static_cast<uint8_t>(bin);
+      const int base = bundle_base[u], c = m.hist_off >> 8;
+      if (base >= 0) {      // a bundle member: its default bin is the column's slot 0, already filled
+        if (bin == static_cast<unsigned>(m.default_bin)) continue;
+        bin = d_bundle_slot(bin, base, m.default_bin);
+      }
+      bins[(static_cast<size_t>(c >> 5) * rows_stride + r) * 32 + (c & 31)] = static_cast<uint8_t>(bin);
     }
   }
 }
@@ -733,59 +884,82 @@ Dataset* Dataset::CreateFromCSR(const void* indptr, int indptr_type, const int32
   std::unique_ptr<Dataset> d = NewShell(static_cast<int>(nrow), static_cast<int>(num_col), params);
   StreamTimer timer(d->stream);
   const int F = d->num_total_features;
-  d->SetMappers(reference, [&](std::vector<std::vector<double>>* nz, int, int) {
+  d->SetMappers(reference, true, [&](std::vector<std::vector<double>>* nz, std::vector<std::vector<int>>* nz_rows, int, int) {
     const std::vector<int> rows = d->SampleRows();
-    for (int r : rows)
-      for (int64_t k = ip(r); k < ip(r + 1); ++k) {
+    for (int s = 0; s < static_cast<int>(rows.size()); ++s)
+      for (int64_t k = ip(rows[s]); k < ip(rows[s] + 1); ++k) {
         const double v = val(k);
-        if (std::fabs(v) > kZeroThr || std::isnan(v)) (*nz)[indices[k]].push_back(v);
+        if (std::fabs(v) > kZeroThr || std::isnan(v)) {
+          (*nz)[indices[k]].push_back(v);
+          if (nz_rows) (*nz_rows)[indices[k]].push_back(s);
+        }
       }
     return static_cast<int>(rows.size());
   });
-  d->AllocBins();
   const int sms = DeviceSMs();
-  k_fill_default_bins<<<sms * 8, 256, 0, d->stream>>>(d->meta.p, d->nfn, d->bins.p, d->rows_stride, nrow, d->num_tiles);
-  if (d->nw > 0) k_fill_default_wide<<<sms * 8, 256, 0, d->stream>>>(d->wide_meta.p, d->nw, d->bins16.p, d->rows_stride, nrow);
-  B200_CUDA(cudaGetLastError());
-  if (d->nf > 0) {
-    DevBuf<int> d_inner; d_inner.Alloc(F); d_inner.Upload(d->inner_of.data(), F, d->stream);
-    // row blocks of bounded element count: the stored elements are staged through one device buffer per block
-    const size_t isz = indptr_type == 2 ? 4 : 8, vsz = data_type == 0 ? 4 : 8;
+  // row blocks of bounded element count: the stored elements are staged through one device buffer per block; fn(indptr, indices,
+  // values, rows, first row, first element) runs on each.  The block staged last stays on the device: when the whole CSR is one block
+  // (up to 64M stored values), the bundle row check and the binning share a single upload.
+  const size_t isz = indptr_type == 2 ? 4 : 8, vsz = data_type == 0 ? 4 : 8;
+  DevBuf<unsigned char> d_ip, d_ix, d_v;
+  int64_t staged_r0 = -1, staged_r1 = -1;
+  auto for_each_block = [&](auto fn) {
     const int64_t kBlockElems = 64LL << 20;
-    DevBuf<unsigned char> d_ip, d_ix, d_v;
     int64_t r0 = 0;
     while (r0 < nrow) {
       int64_t r1 = r0 + 1;
       while (r1 < nrow && ip(r1 + 1) - ip(r0) <= kBlockElems) ++r1;
       const int64_t e0k = ip(r0), ne = ip(r1) - e0k, nr = r1 - r0;
-      if (d_ip.n < static_cast<size_t>(nr + 1) * isz) d_ip.Alloc(static_cast<size_t>(nr + 1) * isz);
-      if (ne > 0) {
-        if (d_ix.n < static_cast<size_t>(ne) * 4) d_ix.Alloc(static_cast<size_t>(ne) * 4);
-        if (d_v.n < static_cast<size_t>(ne) * vsz) d_v.Alloc(static_cast<size_t>(ne) * vsz);
-        B200_CUDA(cudaMemcpyAsync(d_ix.p, indices + e0k, static_cast<size_t>(ne) * 4, cudaMemcpyHostToDevice, d->stream));
-        B200_CUDA(cudaMemcpyAsync(d_v.p, static_cast<const unsigned char*>(data) + static_cast<size_t>(e0k) * vsz, static_cast<size_t>(ne) * vsz, cudaMemcpyHostToDevice, d->stream));
+      if (r0 != staged_r0 || r1 != staged_r1) {
+        if (d_ip.n < static_cast<size_t>(nr + 1) * isz) d_ip.Alloc(static_cast<size_t>(nr + 1) * isz);
+        if (ne > 0) {
+          if (d_ix.n < static_cast<size_t>(ne) * 4) d_ix.Alloc(static_cast<size_t>(ne) * 4);
+          if (d_v.n < static_cast<size_t>(ne) * vsz) d_v.Alloc(static_cast<size_t>(ne) * vsz);
+          B200_CUDA(cudaMemcpyAsync(d_ix.p, indices + e0k, static_cast<size_t>(ne) * 4, cudaMemcpyHostToDevice, d->stream));
+          B200_CUDA(cudaMemcpyAsync(d_v.p, static_cast<const unsigned char*>(data) + static_cast<size_t>(e0k) * vsz, static_cast<size_t>(ne) * vsz, cudaMemcpyHostToDevice, d->stream));
+        }
+        B200_CUDA(cudaMemcpyAsync(d_ip.p, static_cast<const unsigned char*>(indptr) + static_cast<size_t>(r0) * isz, static_cast<size_t>(nr + 1) * isz, cudaMemcpyHostToDevice, d->stream));
+        staged_r0 = r0; staged_r1 = r1;
       }
-      B200_CUDA(cudaMemcpyAsync(d_ip.p, static_cast<const unsigned char*>(indptr) + static_cast<size_t>(r0) * isz, static_cast<size_t>(nr + 1) * isz, cudaMemcpyHostToDevice, d->stream));
       if (ne > 0) {
-        const int grid = static_cast<int>(std::min<int64_t>((nr + 7) / 8, sms * 8));
-        uint8_t* base = d->bins.p + static_cast<size_t>(r0) * 32;       // row offset inside every tile
-        auto launch = [&](auto index_type, auto value_type) {
-          using TI = decltype(index_type);
-          using TV = decltype(value_type);
-          k_bin_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),
-                                                        reinterpret_cast<const TV*>(d_v.p), nr, d_inner.p, d->meta.p, d->ub.p, d->catbin.p, base,
-                                                        d->rows_stride, e0k, d->nfn, d->wide_meta.p, d->wide_cats.p, d->wide_catbin.p, d->wide_ub.p,
-                                                        d->bins16.p ? d->bins16.p + r0 : nullptr);
-        };
-        if (indptr_type == 2 && data_type == 0) launch(int32_t{}, float{});
-        else if (indptr_type == 2) launch(int32_t{}, double{});
-        else if (data_type == 0) launch(int64_t{}, float{});
-        else launch(int64_t{}, double{});
+        if (indptr_type == 2 && data_type == 0) fn(int32_t{}, float{}, nr, r0, e0k);
+        else if (indptr_type == 2) fn(int32_t{}, double{}, nr, r0, e0k);
+        else if (data_type == 0) fn(int64_t{}, float{}, nr, r0, e0k);
+        else fn(int64_t{}, double{}, nr, r0, e0k);
         B200_CUDA(cudaGetLastError());
       }
       B200_CUDA(cudaStreamSynchronize(d->stream));      // the staging buffers are reused by the next block
       r0 = r1;
     }
+  };
+  d->DissolveConflictingBundles([&](unsigned long long* conflicts) {
+    std::vector<int> member_of(F, -1);
+    for (size_t k = 0, i = 0; k < d->bundles.size(); ++k) for (int f : d->bundles[k]) member_of[f] = static_cast<int>(i++);
+    DevBuf<int> d_member_of; d_member_of.Alloc(F); d_member_of.Upload(member_of.data(), F, d->stream);
+    for_each_block([&](auto index_type, auto value_type, int64_t nr, int64_t, int64_t e0k) {
+      using TI = decltype(index_type);
+      using TV = decltype(value_type);
+      const int grid = static_cast<int>(std::min<int64_t>((nr + 7) / 8, sms * 8));
+      k_bundle_conflicts_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),
+                                                                 reinterpret_cast<const TV*>(d_v.p), nr, e0k, d_member_of.p, d->d_members.p, conflicts);
+    });
+  });
+  d->AllocBins();
+  k_fill_default_bins<<<sms * 8, 256, 0, d->stream>>>(d->meta.p, d->d_col_feat.p, d->bins.p, d->rows_stride, nrow, d->num_tiles);
+  if (d->nw > 0) k_fill_default_wide<<<sms * 8, 256, 0, d->stream>>>(d->wide_meta.p, d->nw, d->bins16.p, d->rows_stride, nrow);
+  B200_CUDA(cudaGetLastError());
+  if (d->nf > 0) {
+    DevBuf<int> d_inner; d_inner.Alloc(F); d_inner.Upload(d->inner_of.data(), F, d->stream);
+    for_each_block([&](auto index_type, auto value_type, int64_t nr, int64_t r0, int64_t e0k) {
+      using TI = decltype(index_type);
+      using TV = decltype(value_type);
+      const int grid = static_cast<int>(std::min<int64_t>((nr + 7) / 8, sms * 8));
+      uint8_t* base = d->bins.p + static_cast<size_t>(r0) * 32;       // row offset inside every tile
+      k_bin_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),
+                                                    reinterpret_cast<const TV*>(d_v.p), nr, d_inner.p, d->meta.p, d->ub.p, d->catbin.p, base,
+                                                    d->rows_stride, e0k, d->nfn, d->wide_meta.p, d->wide_cats.p, d->wide_catbin.p, d->wide_ub.p,
+                                                    d->bins16.p ? d->bins16.p + r0 : nullptr, d->d_bundle_base.p);
+    });
   }
   d->ingest_ms = timer.Ms();
   return d.release();
@@ -837,6 +1011,14 @@ void Dataset::GetField(const char* name, int* out_len, const void** out_ptr, int
   else if (s == "init_score") { *out_len = static_cast<int>(init_score.size()); *out_ptr = init_score.empty() ? nullptr : init_score.data(); *out_type = 1; }
   else if (s == "group" || s == "query") { *out_len = static_cast<int>(query_boundaries.size()); *out_ptr = query_boundaries.empty() ? nullptr : query_boundaries.data(); *out_type = 2; }
   else Fatal("Unknown field name: " + s);
+}
+
+void Dataset::GetBundles(int* out_num_columns, int* out_column_of) const {
+  *out_num_columns = num_columns + nw;
+  for (int f = 0; f < num_total_features; ++f) {
+    const int u = inner_of[f];
+    out_column_of[f] = u < 0 ? -1 : (u < nfn ? meta_host[u].hist_off >> 8 : num_columns + (u - nfn));
+  }
 }
 
 void Dataset::SetFeatureNames(const char** names, int n) {
@@ -1194,7 +1376,8 @@ void Booster::SetupPeerReduce() {
   // Default = NCCL all-reduce of the 2 MB histogram; the peer-memory modes (two cross-GPU flag barriers per split) are opt-in.
   // Their speed relative to NCCL has not been measured on H100.
   int mode = env ? std::atoi(env) : 0;      // 0 NCCL, 1 fused reduce-scatter + scan of the owned slice, 2 two-shot P2P all-reduce + replicated scan
-  if (mode == 1 && train->has_categorical) mode = 0;      // the fused scan handles numerical tile features only (same decision on every rank)
+  // the fused scan handles unbundled numerical tile features only (same decision on every rank)
+  if (mode == 1 && (train->has_categorical || !train->bundles.empty())) mode = 0;
   mine.ok = (R <= kMaxPeers && (mode == 1 || mode == 2)) ? 1 : 0;
   void* bufs[3] = {H_.p, mailbox_.p, peer_flags_.p};
   for (int i = 0; i < 3; ++i) {
@@ -1373,8 +1556,9 @@ void Booster::LaunchPartition(int grid, int last) {
   const uint8_t* cols = bins_cols_.p;
   size_t cols_stride = cols_stride_;
   int* super_tot = part_chunks_.p + (train->num_data / kPartChunk + 2);
+  const int* bundle_base = d.BundleBase();
   void* args[] = {&ctrl, &leaves, &tree, &flags, &meta, &sp, &last, &bins, &rows_stride, &i0, &i1, &bits, &chunks, &qgh, &qord, &H, &h_elems, &bins16, &tickets_per_block,
-                  &cols, &cols_stride, &super_tot};
+                  &cols, &cols_stride, &super_tot, &bundle_base};
   B200_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(k_partition), dim3(grid), dim3(256), args, 0, stream_));
 }
 
@@ -1466,8 +1650,8 @@ void Booster::TrainOneTree(int k, HostTree* out) {
         k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
         timing.launches += 1;
       }
-      // scan + (last block) pick; the dynamic scratch is only touched by categorical features
-      k_scan<<<sgrid, 256, d.has_categorical ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
+      // scan + (last block) pick; the dynamic scratch is only touched by categorical features and bundle members
+      k_scan<<<sgrid, 256, (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase());
     }
     nvtxRangePop();
     mark();

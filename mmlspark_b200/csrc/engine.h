@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "bin_mapper.h"
+#include "bundle.h"
 #include "config.h"
 #include "kernels.cuh"
 #include "model.h"
@@ -85,11 +86,12 @@ class Dataset {
   void GetBinsRowMajor(uint8_t* out) const;                 // fails when a feature has more than 256 bins
   void GetBinsRowMajor16(uint16_t* out) const;
   void GetBinsOfRows(const int32_t* rows, int nrows, uint16_t* out) const;      // [nrows][num_total_features], gathered on the device
-  // K4 on this dataset's bins for the given rows (kernel-level parity entry), fp64 [F][256][2]
+  // K4 on this dataset's bins for the given rows (kernel-level parity entry), fp64 [F][256][2] per feature (bundle columns expanded)
   void Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const;
   void SetField(const char* name, const void* data, int n, int type);
   void GetField(const char* name, int* out_len, const void** out_ptr, int* out_type) const;
   void SetFeatureNames(const char** names, int n);
+  void GetBundles(int* out_num_columns, int* out_column_of) const;      // storage column of every feature (-1: unused)
 
   int device = 0;
   int num_data = 0, num_total_features = 0;
@@ -100,6 +102,15 @@ class Dataset {
   std::vector<FeatMeta> meta_host;
   int nf = 0, nf_pad = 0, num_tiles = 0;
   int nfn = 0, nw = 0;                       // inner features [0, nfn) live in uint8 tiles, [nfn, nf) are wide (> 256 bins, uint16 columns)
+  // storage columns of the uint8 tiles: one per plain tile feature and one per feature bundle (bundle.h); without a bundle column = feature
+  int num_columns = 0;
+  std::vector<std::vector<int>> bundles;     // real indices of the members of each bundle (two or more each)
+  std::vector<int> col_feat;                 // [num_tiles * 32] the plain inner feature of a column, -1 for a bundle column or padding
+  DevBuf<int> d_col_feat;
+  std::vector<int> bundle_base;              // [nf_pad] per inner feature: -1 alone in its column, else its base in a bundle column (d_unbundle)
+  DevBuf<int> d_bundle_base;
+  DevBuf<BundleMember> d_members;            // members of all bundles, bundle by bundle
+  DevBuf<int> d_bundle_start, d_bundle_col;  // [bundles + 1] first member of each bundle, [bundles] its storage column
   size_t hist_pairs = 0;                     // (g,h) pairs of one histogram slot: num_tiles*32*256 for the tiles + the wide features' bins
   std::vector<int> sample_order;             // used features in real-index order -> inner index (ColSampler draws in that order)
   size_t rows_stride = 0;
@@ -110,7 +121,8 @@ class Dataset {
   DevBuf<int> wide_cats;                     // sorted category values of all wide features (slices per WideMeta)
   DevBuf<unsigned short> wide_catbin;        // ... and their bins
   DevBuf<double> wide_ub;                    // bin upper bounds of the wide numerical features (max_bin > 255)
-  BinView View() const { return BinView{bins.p, rows_stride, bins16.p, nfn}; }
+  const int* BundleBase() const { return bundles.empty() ? nullptr : d_bundle_base.p; }      // null: no feature bundle, no decode
+  BinView View() const { return BinView{bins.p, rows_stride, bins16.p, nfn, meta.p, BundleBase()}; }
   DevBuf<FeatMeta> meta;
   DevBuf<double> ub;                         // [nf][256] bin upper bounds (categorical: sorted category values)
   DevBuf<uint8_t> catbin;                    // [nf][256] categorical: bin of the i-th sorted category
@@ -127,11 +139,17 @@ class Dataset {
  private:
   // every create runs NewShell, SetMappers and AllocBins, in that order
   static std::unique_ptr<Dataset> NewShell(int nrow, int ncol, const char* params);
-  template <typename Sample> void SetMappers(const Dataset* reference, Sample sample);
+  // may_bundle: the create path can check every row before binning (matrix and CSR input)
+  template <typename Sample> void SetMappers(const Dataset* reference, bool may_bundle, Sample sample);
+  // drops every bundle with a row in which two members are away from their most frequent bin; count(conflicts) runs the row check
+  template <typename Count> void DissolveConflictingBundles(Count count);
+  void UploadBundleMembers();
   std::vector<int> SampleRows() const;
   void AllocBins();
   template <typename T> void UnpackTiles(T* out) const;
   void BinBlock(const void* data, bool on_device, int data_type, int is_row_major, long long nrow, long long start_row);
+  // fn(device rows, rows, leading dimension, first row) for each block of rows of a matrix, staged through device memory if on the host
+  template <typename Fn> void ForEachDeviceBlock(const void* data, bool on_device, int data_type, int is_row_major, long long nrow, Fn fn);
   // persistent H2D staging of the host ingestion path (two device chunks, a copy stream, events); released once every row is in
   DevBuf<unsigned char> ingest_buf_[2];
   cudaStream_t ingest_copy_stream_ = nullptr;

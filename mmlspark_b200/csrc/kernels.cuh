@@ -19,8 +19,23 @@ struct FeatMeta {          // per inner (used) feature
   int real_index;
   int is_categorical;      // bins are category ranks; splits are bin bitsets
   int num_sorted_cats;     // categorical: entries of the sorted category table (ub row = categories, catbin row = their bins)
-  int hist_off;            // first (g,h) pair of the feature in a histogram slot: u * 256 for a tile feature, beyond the tiles for a wide one
+  int hist_off;            // first (g,h) pair of the feature's storage column in a histogram slot: col * 256 for a tile feature (col = u
+                           // without feature bundles), beyond the tiles for a wide one
 };
+
+// Exclusive feature bundles (bundle.h): a bundle column holds several features of which at most one is away from its most frequent bin
+// (mfb = default_bin for a member) in any row.  Slot 0 = every member at its mfb; member bin b != mfb is stored at
+// base + 1 + (b < mfb ? b : b - 1).  Decoding a stored slot back to the member's bin:
+__host__ __device__ __forceinline__ unsigned d_unbundle(unsigned slot, int base, int mfb, int num_bin) {
+  if (base < 0) return slot;
+  const int v = static_cast<int>(slot) - base - 1;
+  if (v < 0 || v >= num_bin - 1) return static_cast<unsigned>(mfb);
+  return static_cast<unsigned>(v < mfb ? v : v + 1);
+}
+// slot of member bin `bin` (the caller has checked bin != mfb)
+__host__ __device__ __forceinline__ unsigned d_bundle_slot(unsigned bin, int base, int mfb) {
+  return static_cast<unsigned>(base + 1) + (bin < static_cast<unsigned>(mfb) ? bin : bin - 1);
+}
 
 // "Wide" features: more than 256 bins.  LightGBM does not cap a categorical feature at max_bin — it keeps categories until 99 % of the
 // sampled mass is covered (BinMapper::FindBin) — so a 10^3..10^5-cardinality column (BASELINE.json configs[4]) needs thousands of bins.
@@ -37,8 +52,12 @@ struct WideMeta {
 };
 struct BinView {                         // where a row's bin of inner feature u is stored
   const uint8_t* bins; size_t rows_stride; const uint16_t* bins16; int nfn;
+  const FeatMeta* meta; const int* bundle_base;      // bundle_base null: no feature bundle, column = feature, no decode
   __device__ __forceinline__ unsigned at(int u, size_t row) const {
-    return u < nfn ? bins[(static_cast<size_t>(u >> 5) * rows_stride + row) * 32 + (u & 31)] : bins16[static_cast<size_t>(u - nfn) * rows_stride + row];
+    if (u >= nfn) return bins16[static_cast<size_t>(u - nfn) * rows_stride + row];
+    if (!bundle_base) return bins[(static_cast<size_t>(u >> 5) * rows_stride + row) * 32 + (u & 31)];
+    const int c = meta[u].hist_off >> 8;
+    return d_unbundle(bins[(static_cast<size_t>(c >> 5) * rows_stride + row) * 32 + (c & 31)], bundle_base[u], meta[u].default_bin, meta[u].num_bin);
   }
 };
 
@@ -75,6 +94,9 @@ struct LeafState {
   int global_count, identity, hist_slot, parent_node;
   double sum_g, sum_h;
   LeafBest best;
+  // exact fixed-point (g,h) totals, kept only for datasets with feature bundles: qtot = this leaf's (written by k_scan), qpar = its
+  // parent's (written by the round controller); a bundle member's most frequent bin is the leaf total minus its other bins
+  long long qtot[2], qpar[2];
 };
 
 struct TreeCtrl {
@@ -132,29 +154,44 @@ __device__ __noinline__ double d_leaf_gain(double g, double h, const SplitParams
 }
 
 // ---------------------------------------------------------------- binning (dataset creation)
-// One warp per row-of-a-tile: lane = feature of the tile.  Upper bounds of the tile's 32 features sit
-// in shared memory ([32][256] doubles = 64 KB).  ValueToBin: lower-bound search `value <= ub[m]`.
+// numerical value -> bin (ValueToBin): lower-bound search `value <= ub[m * stride]`
+__device__ __forceinline__ unsigned d_num_bin(double v, const FeatMeta& m, const double* ub, int stride) {
+  if (isnan(v)) {
+    if (m.missing_type == 2) return static_cast<unsigned>(m.num_bin - 1);
+    v = 0.0;
+  }
+  int lo = 0, hi = m.num_bin - 1 - (m.missing_type == 2 ? 1 : 0);
+  while (lo < hi) {
+    int mid = (hi + lo - 1) / 2;
+    if (v <= ub[mid * stride]) hi = mid; else lo = mid + 1;
+  }
+  return static_cast<unsigned>(lo);
+}
+
+// One warp per row-of-a-tile: lane = storage column of the tile.  Upper bounds of the tile's (at most 32) plain features sit
+// in shared memory ([32][256] doubles = 64 KB).  col_feat[column] = the plain feature of the column, or -1: a bundle column (left at
+// slot 0 here, k_bin_bundles writes its non-default rows) or padding.
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_bin_rows(const T* __restrict__ X, long long nrow, int ncol, int row_major, long long ld, const FeatMeta* __restrict__ meta,
-           const double* __restrict__ ub, const uint8_t* __restrict__ catbin, int nf, uint8_t* __restrict__ bins, long long rows_stride,
-           long long row_offset) {
+           const double* __restrict__ ub, const uint8_t* __restrict__ catbin, const int* __restrict__ col_feat, uint8_t* __restrict__ bins,
+           long long rows_stride, long long row_offset) {
   extern __shared__ double s_ub[];   // [256 bins][32 lanes]: lane l always hits bank pair 2l -> no conflicts beyond the 64-bit 2-phase
   const int tile = blockIdx.y;
   for (int e = threadIdx.x; e < 32 * 256; e += blockDim.x) {
-    int f = tile * 32 + (e >> 8);
-    s_ub[(e & 255) * 32 + (e >> 8)] = f < nf ? ub[static_cast<size_t>(f) * 256 + (e & 255)] : 0.0;
+    const int f = col_feat[tile * 32 + (e >> 8)];
+    s_ub[(e & 255) * 32 + (e >> 8)] = f >= 0 ? ub[static_cast<size_t>(f) * 256 + (e & 255)] : 0.0;
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int u = tile * 32 + lane;
+  const int u = col_feat[tile * 32 + lane];
   FeatMeta m;
   m.num_bin = 1; m.missing_type = 0; m.real_index = 0; m.is_categorical = 0; m.num_sorted_cats = 0;
-  if (u < nf) m = meta[u];
+  if (u >= 0) m = meta[u];
   const double* myub = s_ub + lane;
   for (long long r = blockIdx.x * 8LL + warp; r < nrow; r += gridDim.x * 8LL) {
     unsigned bin = 0;
-    if (u < nf) {
+    if (u >= 0) {
       double v = row_major ? static_cast<double>(X[r * ld + m.real_index]) : static_cast<double>(X[static_cast<long long>(m.real_index) * ld + r]);
       if (m.is_categorical) {     // category -> bin: binary search in the sorted category table; NaN / negative / unseen -> bin 0
         if (!isnan(v)) {
@@ -166,20 +203,102 @@ k_bin_rows(const T* __restrict__ X, long long nrow, int ncol, int row_major, lon
           }
         }
       } else {
-        if (isnan(v)) {
-          if (m.missing_type == 2) bin = m.num_bin - 1; else v = 0.0;
-        }
-        if (!isnan(v)) {
-          int lo = 0, hi = m.num_bin - 1 - (m.missing_type == 2 ? 1 : 0);
-          while (lo < hi) {
-            int mid = (hi + lo - 1) / 2;
-            if (v <= myub[mid * 32]) hi = mid; else lo = mid + 1;
-          }
-          bin = lo;
-        }
+        bin = d_num_bin(v, m, myub, 32);
       }
     }
     bins[(static_cast<size_t>(tile) * rows_stride + row_offset + r) * 32 + lane] = static_cast<uint8_t>(bin);
+  }
+}
+
+// ---------------------------------------------------------------- exclusive feature bundles (bundle.h): row check and binning
+// One member of a bundle; the members of bundle k are [start[k], start[k+1]).  A value is away from the member's most frequent bin
+// iff it is NaN and NaN has its own bin, or it lies outside (zlo, zhi] — exactly the values whose bin differs from the mfb.  zlo = -inf
+// when the mfb is bin 0, whose range has no lower end (-inf itself lands there).
+struct BundleMember {
+  double zlo, zhi;
+  int real_index, inner, base, bundle;     // inner / base: set once the layout is final (the row check needs neither)
+  int nan_moves, pad;
+};
+__device__ __forceinline__ bool d_off_mfb(double v, const BundleMember& m) {
+  return isnan(v) ? m.nan_moves != 0 : !((v > m.zlo || isinf(m.zlo)) && v <= m.zhi);
+}
+// per bundle: the rows (of this block of rows) in which two or more members are away from their mfb; one thread per (bundle, row)
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_bundle_conflicts(const T* __restrict__ X, long long nrow, int row_major, long long ld, const BundleMember* __restrict__ mem,
+                   const int* __restrict__ start, int nb, unsigned long long* __restrict__ conflicts) {
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < nrow * nb; e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int b = static_cast<int>(e / nrow);
+    const long long r = e - static_cast<long long>(b) * nrow;
+    int off = 0;
+    for (int k = start[b]; k < start[b + 1]; ++k) {
+      const int f = mem[k].real_index;
+      const double v = row_major ? static_cast<double>(X[r * ld + f]) : static_cast<double>(X[static_cast<long long>(f) * ld + r]);
+      if (d_off_mfb(v, mem[k]) && ++off == 2) { atomicAdd(conflicts + b, 1ull); break; }
+    }
+  }
+}
+// CSR: one warp per row.  The bundles that already had a member away from its mfb in this row are listed in shared memory; a second
+// one is a conflict.  A row that touches more than kSeenPerWarp bundles counts its further bundles as conflicts (dissolving is always safe).
+// conflicts[k] > 0 iff some row has two members of bundle k away from their mfb.
+constexpr int kSeenPerWarp = 256;
+template <typename TI, typename TV>
+__global__ void __launch_bounds__(256)
+k_bundle_conflicts_csr(const TI* __restrict__ indptr, const int* __restrict__ indices, const TV* __restrict__ vals, long long nrow, long long elem_base,
+                       const int* __restrict__ member_of, const BundleMember* __restrict__ mem, unsigned long long* __restrict__ conflicts) {
+  __shared__ int s_seen[8][kSeenPerWarp];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  int* seen_list = s_seen[wib];
+  const long long warp = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5, nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  for (long long r = warp; r < nrow; r += nwarps) {
+    const long long a = static_cast<long long>(indptr[r]) - elem_base, e = static_cast<long long>(indptr[r + 1]) - elem_base;
+    int nseen = 0;
+    for (long long k0 = a; k0 < e; k0 += 32) {
+      const long long k = k0 + lane;
+      int bundle = -1;
+      if (k < e) {
+        const int mi = member_of[indices[k]];
+        if (mi >= 0 && d_off_mfb(static_cast<double>(vals[k]), mem[mi])) bundle = mem[mi].bundle;
+      }
+      const unsigned peers = __match_any_sync(0xffffffffu, bundle);
+      const bool leader = bundle >= 0 && __ffs(peers) - 1 == lane;
+      bool seen = false;
+      if (bundle >= 0) for (int i = 0; i < nseen; ++i) seen |= seen_list[i] == bundle;
+      if (leader && (seen || __popc(peers) > 1)) atomicAdd(conflicts + bundle, 1ull);
+      const bool add = leader && !seen;
+      const unsigned adds = __ballot_sync(0xffffffffu, add);
+      __syncwarp();
+      if (add) {
+        const int pos = nseen + __popc(adds & ((1u << lane) - 1u));
+        if (pos < kSeenPerWarp) seen_list[pos] = bundle;
+        else atomicAdd(conflicts + bundle, 1ull);
+      }
+      nseen = min(kSeenPerWarp, nseen + __popc(adds));
+      __syncwarp();
+    }
+  }
+}
+// the non-default rows of the bundle columns (k_bin_rows left them at slot 0); one thread per (bundle, row).  The row check guarantees
+// at most one member per row is away from its mfb.
+template <typename T>
+__global__ void __launch_bounds__(256)
+k_bin_bundles(const T* __restrict__ X, long long nrow, int row_major, long long ld, const BundleMember* __restrict__ mem, const int* __restrict__ start,
+              const int* __restrict__ bundle_col, int nb, const FeatMeta* __restrict__ meta, const double* __restrict__ ub, uint8_t* __restrict__ bins,
+              long long rows_stride, long long row_offset) {
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < nrow * nb; e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int b = static_cast<int>(e / nrow);
+    const long long r = e - static_cast<long long>(b) * nrow;
+    for (int k = start[b]; k < start[b + 1]; ++k) {
+      const BundleMember bm = mem[k];
+      const double v = row_major ? static_cast<double>(X[r * ld + bm.real_index]) : static_cast<double>(X[static_cast<long long>(bm.real_index) * ld + r]);
+      if (!d_off_mfb(v, bm)) continue;
+      const FeatMeta m = meta[bm.inner];
+      const unsigned bin = d_num_bin(v, m, ub + static_cast<size_t>(bm.inner) * 256, 1);
+      if (bin == static_cast<unsigned>(m.default_bin)) continue;      // never written as a slot (d_bundle_slot needs bin != mfb)
+      const int c = bundle_col[b];
+      bins[(static_cast<size_t>(c >> 5) * rows_stride + row_offset + r) * 32 + (c & 31)] = static_cast<uint8_t>(d_bundle_slot(bin, bm.base, m.default_bin));
+      break;
+    }
   }
 }
 
@@ -598,6 +717,7 @@ d_round_ctl(TreeCtrl* ctrl, LeafState* leaves, const TreeDev& tree, uint8_t* fla
       const int leaf = ctrl->split_leaf, nl = ctrl->new_leaf;
       LeafState& L = leaves[leaf];
       LeafState& R = leaves[nl];
+      L.qpar[0] = R.qpar[0] = L.qtot[0]; L.qpar[1] = R.qpar[1] = L.qtot[1];
       LeafBest b = L.best;
       // written by another block of the same kernel when this runs as the tail of k_partition: read through L2
       const int true_left = __ldcg(&ctrl->part_left_total), true_right = ctrl->part_count - true_left;
@@ -1359,7 +1479,8 @@ __global__ void __launch_bounds__(256, 3)
 k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, const FeatMeta* __restrict__ meta, SplitParams p, int last,
             const uint8_t* __restrict__ bins, size_t rows_stride, int* __restrict__ idx0, int* __restrict__ idx1, unsigned* __restrict__ bits,
             int* __restrict__ chunk_left, const int4* __restrict__ qgh, int4* __restrict__ qord, long long* __restrict__ H, size_t h_elems,
-            const uint16_t* __restrict__ bins16, int tickets_per_block, const uint8_t* __restrict__ cols, size_t cols_stride, int* __restrict__ super_tot) {
+            const uint16_t* __restrict__ bins16, int tickets_per_block, const uint8_t* __restrict__ cols, size_t cols_stride, int* __restrict__ super_tot,
+            const int* __restrict__ bundle_base) {
   __shared__ int s_pref[kPartLocalScan + 1];
   __shared__ unsigned short s_list[kCatListMax];
   __shared__ int s_wl[64];
@@ -1382,9 +1503,11 @@ k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
     const int begin = ctrl->part_begin, identity = ctrl->part_identity;
     const int f = ctrl->split_feature;
     const int wide = ctrl->split_wide;
-    const uint8_t* col = bins + (static_cast<size_t>((wide >= 0 ? 0 : f) >> 5) * rows_stride) * 32 + ((wide >= 0 ? 0 : f) & 31);
+    const int sc = wide >= 0 ? 0 : meta[f].hist_off >> 8;         // storage column of the split feature
+    const int bbase = (wide >= 0 || !bundle_base) ? -1 : bundle_base[f], bmfb = meta[f].default_bin, bnb = meta[f].num_bin;
+    const uint8_t* col = bins + (static_cast<size_t>(sc >> 5) * rows_stride) * 32 + (sc & 31);
     const uint16_t* wcol = wide >= 0 ? bins16 + static_cast<size_t>(wide) * rows_stride : nullptr;
-    const uint8_t* ccol = (cols != nullptr && wide < 0) ? cols + static_cast<size_t>(f) * cols_stride : nullptr;      // column-major copy, if kept
+    const uint8_t* ccol = (cols != nullptr && wide < 0) ? cols + static_cast<size_t>(sc) * cols_stride : nullptr;      // column-major copy, if kept
     const bool wide_cat = wide >= 0 && ctrl->split_is_cat;
     const int list_len = wide_cat ? ctrl->split_cat_list_len : 0;
     if (threadIdx.x < list_len) s_list[threadIdx.x] = ctrl->split_cat_list[threadIdx.x];
@@ -1422,7 +1545,7 @@ k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
       for (int k = 0; k < 8; ++k) {
         bool left = false;
         if (rr[k] >= 0) {
-          const unsigned bin = bb[k];
+          const unsigned bin = d_unbundle(bb[k], bbase, bmfb, bnb);
           if (wide_cat) { for (int kk = 0; kk < list_len; ++kk) left |= (bin == s_list[kk]); }
           else left = d_goes_left(bin, ctrl);
         }
@@ -2094,6 +2217,39 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   __threadfence();
 }
 
+// A bundle member's histogram out of its bundle column, by the member's k_scan block (thread t = column slot t).  The member's slots of
+// the column become its bins != mfb; this block alone updates them in the pool (smaller leaf: H, larger: parent - H).  Every column of a leaf
+// sums to the leaf total, so the smaller leaf's total is this column of H summed, and the larger's is its parent's total minus that; the
+// member's mfb is the total minus its other bins.  All exact int64, so `out` equals the unbundled feature's histogram bit for bit.
+__device__ __noinline__ void d_unbundle_hist(const long long* __restrict__ src, long long* __restrict__ dst, int num_bin, int mfb, int base, int which,
+                                             LeafState* L, longlong2* out) {
+  __shared__ long long s_red[4][8];
+  const int b = threadIdx.x, lane = b & 31, warp = b >> 5;
+  const longlong2 hv = reinterpret_cast<const longlong2*>(src)[b];
+  const bool own = b > base && b < base + num_bin;
+  longlong2 sv = hv;
+  if (own) {
+    if (which) { const longlong2 pr = reinterpret_cast<const longlong2*>(dst)[b]; sv.x = pr.x - hv.x; sv.y = pr.y - hv.y; }
+    reinterpret_cast<longlong2*>(dst)[b] = sv;
+    const int v = b - base - 1;
+    out[v < mfb ? v : v + 1] = sv;
+  }
+  long long r[4] = {hv.x, hv.y, own ? sv.x : 0, own ? sv.y : 0};
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    for (int o = 16; o; o >>= 1) r[i] += __shfl_xor_sync(0xffffffffu, r[i], o);
+  if (lane == 0) for (int i = 0; i < 4; ++i) s_red[i][warp] = r[i];
+  __syncthreads();
+  if (b == 0) {
+    long long t[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 4; ++i) for (int w = 0; w < 8; ++w) t[i] += s_red[i][w];
+    const long long tg = which ? L->qpar[0] - t[0] : t[0], th = which ? L->qpar[1] - t[1] : t[1];
+    L->qtot[0] = tg; L->qtot[1] = th;      // every member block of this leaf writes the same value
+    out[mfb] = make_longlong2(tg - t[2], th - t[3]);
+  }
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------- K5/K6 for the tile features: one BLOCK per (smaller|larger, feature)
 // Thread t = bin t.  The block reduces the feature into the leaf's pool slot (larger child: parent - smaller, exact int64), then runs the
 // same block-wide two-pass scan as the wide numerical features (d_scan_wide_numeric with one bin per thread: exclusive block scans of
@@ -2104,7 +2260,10 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base) {
+  // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
+  // or a bundle member's histogram (d_unbundle_hist)
+  extern __shared__ double scan_ws[];
   const int which = blockIdx.y;
   const int leaf = which ? ctrl->larger : ctrl->smaller;
   const int u = blockIdx.x;
@@ -2117,20 +2276,22 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     if (*flag) {
       const LeafState& L = leaves[leaf];
       const FeatMeta fm = meta[u];
-      long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(u) * 512;
-      const long long* src = H + static_cast<size_t>(u) * 512;
-      {
+      long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(fm.hist_off) * 2;
+      const long long* src = H + static_cast<size_t>(fm.hist_off) * 2;
+      if (!bundle_base || bundle_base[u] < 0) {
         const int b = threadIdx.x;
         longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
         if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
         *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
+        __syncthreads();      // the scan reads bins other threads of this block reduced
+      } else {
+        d_unbundle_hist(src, dst, fm.num_bin, fm.default_bin, bundle_base[u], which, leaves + leaf, reinterpret_cast<longlong2*>(scan_ws));
+        dst = reinterpret_cast<long long*>(scan_ws);
       }
-      __syncthreads();      // the scan reads bins other threads of this block reduced
       if (!fm.is_categorical) {
         const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
         d_scan_wide_numeric(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out);
       } else if (threadIdx.x < 32) {
-        extern __shared__ double scan_ws[];      // (3*256 doubles + 2*256 bytes) of scratch for the categorical search
         long long qg[8], qh[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
