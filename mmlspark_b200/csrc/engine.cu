@@ -535,6 +535,10 @@ void Dataset::BinBlock(const void* data, bool on_device, int data_type, int is_r
   NvtxRange nvtx("b200gbm:K0 bin rows (H2D + value->bin)");
   const int F = num_total_features;
   if (start_row < 0 || start_row + n > num_data) Fatal("row block out of range");
+  {
+    std::lock_guard<std::mutex> lock(block_bound_mu_);
+    block_bound_.Free();      // a bound of earlier bins would let K4 overflow a cell
+  }
   ForEachDeviceBlock(data, on_device, data_type, is_row_major, n, [&](const void* x, long long rows, long long ld, long long r0) {
     if (data_type == 0) LaunchBin<float>(static_cast<const float*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
     else LaunchBin<double>(static_cast<const double*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
@@ -673,16 +677,37 @@ void Dataset::GetBinsOfRows(const int32_t* rows, int nrows, uint16_t* out) const
   B200_CUDA(cudaStreamSynchronize(stream));
 }
 
+RowBlockBound Dataset::BlockBound() const {
+  std::lock_guard<std::mutex> lock(block_bound_mu_);
+  if (!block_bound_.p) {
+    block_bound_.Alloc(static_cast<size_t>(num_tiles) * (bound_blocks(num_data) + 1));
+    launch_block_bound(bins.p, rows_stride, num_data, num_tiles, num_columns, block_bound_.p, stream);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaStreamSynchronize(stream));      // the boosters launch K4 on their own streams
+  }
+  return RowBlockBound{block_bound_.p, bound_blocks(num_data)};
+}
+
 void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const {
   EnsureDevice();
   B200_CUDA(set_k4_smem_limit());
   const int n = num_data;
+  // K4 bounds an index-list item by the row blocks between its first and last row, so it needs a strictly ascending list; the
+  // histogram does not depend on the order.  A list that repeats a row is bounded by row counts instead.
+  std::vector<int32_t> rows;
+  RowBlockBound bound = BlockBound();
+  if (idx) {
+    rows.assign(idx, idx + cnt);
+    std::sort(rows.begin(), rows.end());
+    if (cnt > 0 && (rows.front() < 0 || rows.back() >= n)) Fatal("Histogram: row index out of range");
+    if (std::adjacent_find(rows.begin(), rows.end()) != rows.end()) bound.prefix = nullptr;
+  }
   DevBuf<float> g, h; g.Alloc(n); h.Alloc(n);
   g.Upload(grad, n, stream); h.Upload(hess, n, stream);
   DevBuf<int4> q; q.Alloc(n);
   DevBuf<TreeCtrl> ctrl; ctrl.Alloc(1); ctrl.Zero(stream);
   DevBuf<int> didx; didx.Alloc(std::max(cnt, 1));
-  if (idx) didx.Upload(idx, cnt, stream);
+  if (idx) didx.Upload(rows.data(), cnt, stream);
   const size_t elems = static_cast<size_t>(num_tiles) * 32 * 512;      // tile features only (wide features are covered by the model-level tests)
   DevBuf<long long> H; H.Alloc(elems); H.Zero(stream);
   const size_t felems = static_cast<size_t>(std::max(nfn, 1)) * 512;     // per feature
@@ -697,7 +722,7 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   DevBuf<int4> qo; qo.Alloc(std::max(cnt, 1));
   k_gather_q<<<sms * 4, 256, 0, stream>>>(&ctrl.p->hist_work, didx.p, didx.p, q.p, qo.p);
   launch_k4(/*const_hessian=*/false, bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
-            reinterpret_cast<unsigned long long*>(H.p), sms, stream);
+            reinterpret_cast<unsigned long long*>(H.p), bound, sms, stream);
   // per-feature histograms out of the column histograms, exact int64 as in k_scan: a bundle member's most frequent bin is the column total
   // minus the member's other bins
   std::vector<long long> hc(elems), hf(felems, 0);
@@ -1590,6 +1615,7 @@ void Booster::TrainOneTree(int k, HostTree* out) {
   timing.launches += 4;
   const int pgrid = std::max(1, std::min(n / kPartChunk + 1, part_max_blocks_));
   const dim3 sgrid(std::max(1, d.nfn), 2);      // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates
+  const RowBlockBound bound = d.BlockBound();
   std::vector<cudaEvent_t> evs;
   // B200GBM_SPLIT_TIMING=1 (debug): an event after every operation of a split; per-operation averages go to stderr when the booster is freed
   static const bool split_timing = getenv("B200GBM_SPLIT_TIMING") != nullptr;
@@ -1607,7 +1633,7 @@ void Booster::TrainOneTree(int k, HostTree* out) {
     // the scratch histogram H is zero here: zeroed at set-up and by every partition kernel after the scan consumed it
     nvtxRangePushA("b200gbm:K4 histogram");
     launch_k4(const_hessian_, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-              reinterpret_cast<unsigned long long*>(H_.p), num_sms_, s);
+              reinterpret_cast<unsigned long long*>(H_.p), bound, num_sms_, s);
     if (d.nw > 0) {      // the features with more than 256 bins: own sub-histogram layout (k4_hist_wide)
       int max_nb = 0;
       for (const WideMeta& wm : d.wide_host) max_nb = std::max(max_nb, wm.num_bin);

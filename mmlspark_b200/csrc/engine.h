@@ -10,6 +10,7 @@
 #include <memory>
 #include <stdexcept>
 #include <map>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -92,6 +93,9 @@ class Dataset {
   void GetField(const char* name, int* out_len, const void** out_ptr, int* out_type) const;
   void SetFeatureNames(const char** names, int n);
   void GetBundles(int* out_num_columns, int* out_column_of) const;      // storage column of every feature (-1: unused)
+  // K4's per-block bin-count bound of the uint8 tiles (hist_kernel.cuh): computed from the bins on first use, reused by every
+  // booster on this dataset and by Histogram, dropped when rows are binned again.  Safe to call from several host threads.
+  RowBlockBound BlockBound() const;
 
   int device = 0;
   int num_data = 0, num_total_features = 0;
@@ -157,6 +161,8 @@ class Dataset {
   long long ingest_rows_done_ = 0;
   void ReleaseIngestStaging();
   void UploadMeta();
+  mutable DevBuf<int> block_bound_;          // [num_tiles][bound_blocks(num_data) + 1], empty until BlockBound()
+  mutable std::mutex block_bound_mu_;        // boosters on other host threads may ask for the bound at the same time
 };
 
 // ---- booster -----------------------------------------------------------------------------------

@@ -19,10 +19,15 @@
 // ATOMS.CAST.SPIN compare-and-swap loop (checked with cuobjdump).  The reference accumulates
 // fp32 gradients into fp64 bins, so fp32 accumulation is not good enough to reproduce its
 // tree structure.  We therefore split a 36-bit fixed-point value into two 18-bit fields and
-// accumulate each with a native 32-bit atomic; 2^14 rows can be added before a field can
+// accumulate each with a native 32-bit atomic; one (column, bin) cell can take 2^14 additions before a field can
 // overflow, then the CTA flushes its sub-histogram into the int64 leaf histogram in L2 with TMA bulk
 // reductions (UBLKRED.G.S.ADD.U64).  Integer sums are exact and order-independent, so the result is bit-reproducible
 // run to run and across ranks (the NCCL reduction is an int64 sum).
+//
+// When to flush: a per-block bin-count bound of the dataset (k_block_maxcnt: for every tile and block of 4096 rows, the largest
+// row count of any cell) bounds the additions a run of work items can put into one cell.  A CTA flushes when that bound would pass
+// 2^14, when the tile changes, and after its last item.  Uniform 255-bin columns put ~16 rows per cell into a block, so a root-pass
+// CTA flushes every few dozen 2^14-row items instead of after every one; a column with one dominant bin falls back to the latter.
 //
 // Bank mapping: the sub-histogram planes are laid out [bin][feature-of-tile], so feature f lives in
 // bank f.  A consumer warp step is 32 rows x 4 features: lane = row for 8 steps, its (g,h) quadruple stays in registers
@@ -33,6 +38,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include <cub/block/block_scan.cuh>
 
 namespace b200gbm {
 
@@ -68,6 +74,80 @@ k_gather_q(const HistWork* __restrict__ work, const int* __restrict__ idx0, cons
     const int p = w.begin + i;
     qord[p] = qgh[idx[p]];
   }
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Per-block bin-count bound of K4's flush rule.  The rows are cut into blocks of kBoundBlockRows; maxcnt(tile, block) is the largest
+// number of the block's rows that fall into one (storage column, bin) cell of the tile.  It is kept as an exclusive prefix over the
+// blocks of each tile, prefix[tile * (blocks + 1) + b] = sum of maxcnt over blocks < b, so any subset of the rows of blocks [b0, b1]
+// adds at most prefix[b1 + 1] - prefix[b0] to one cell of the tile.  A tile's total is at most num_data <= 2^31 - 1: int does not
+// overflow.  It depends on the bins only, so a dataset computes it once (Dataset::BlockBound).
+constexpr int kBoundBlockRows = 4096;
+struct RowBlockBound {
+  const int* prefix;   // [num_tiles][blocks + 1]; nullptr: no bound, an item is bounded by its row count
+  int blocks;
+};
+inline int bound_blocks(int num_data) { return (num_data + kBoundBlockRows - 1) / kBoundBlockRows; }
+
+// grid (blocks, num_tiles): maxcnt of one (tile, block) into prefix[tile][block] (k_block_bound_prefix turns it into the prefix)
+__global__ void __launch_bounds__(256)
+k_block_maxcnt(const uint8_t* __restrict__ bins, size_t rows_stride, int num_data, int num_columns, int* __restrict__ prefix) {
+  __shared__ unsigned cnt[kBins * kTileFeat];   // [bin][column of the tile]
+  __shared__ unsigned wmax[8];
+  const int tile = blockIdx.y, tid = threadIdx.x;
+  for (int e = tid; e < kBins * kTileFeat; e += blockDim.x) cnt[e] = 0u;
+  __syncthreads();
+  const int r0 = blockIdx.x * kBoundBlockRows, rows = min(kBoundBlockRows, num_data - r0);
+  const unsigned* wp = reinterpret_cast<const unsigned*>(bins + (static_cast<size_t>(tile) * rows_stride + r0) * kTileFeat);
+  for (int e = tid; e < rows * 8; e += blockDim.x) {      // one 4-byte word = 4 columns of one row
+    const unsigned word = wp[e];
+    const int c0 = (e & 7) * 4, rot = (e >> 3) & 3;       // byte order rotated by the row: a warp's atomics hit 32 banks
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int kk = (k + rot) & 3;
+      atomicAdd(&cnt[((word >> (8 * kk)) & 0xFFu) * kTileFeat + c0 + kk], 1u);
+    }
+  }
+  __syncthreads();
+  // Storage columns that no feature maps to (padding of the last tile) are left out: their bytes may put every row into one bin,
+  // which would bound nothing.  No reader looks at their cells, and a 32-bit field that wraps there is defined behaviour.
+  const int ncol = min(kTileFeat, num_columns - tile * kTileFeat);
+  unsigned m = 0u;
+  for (int e = tid; e < kBins * kTileFeat; e += blockDim.x)
+    if ((e & (kTileFeat - 1)) < ncol) m = max(m, cnt[e]);
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((tid & 31) == 0) wmax[tid >> 5] = m;
+  __syncthreads();
+  if (tid == 0) {
+    for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) m = max(m, wmax[i]);
+    prefix[static_cast<size_t>(tile) * (gridDim.x + 1) + blockIdx.x] = static_cast<int>(m);
+  }
+}
+
+// grid num_tiles: prefix[tile][0 .. blocks) holds maxcnt on entry; on exit prefix[tile][b] = sum of maxcnt over blocks < b, b = 0 .. blocks
+__global__ void __launch_bounds__(1024) k_block_bound_prefix(int blocks, int* __restrict__ prefix) {
+  using Scan = cub::BlockScan<int, 1024>;
+  __shared__ typename Scan::TempStorage tmp;
+  int* p = prefix + static_cast<size_t>(blockIdx.x) * (blocks + 1);
+  int carry = 0;
+  for (int b0 = 0; b0 < blocks; b0 += 1024) {
+    const int b = b0 + threadIdx.x;
+    const int v = b < blocks ? p[b] : 0;
+    int ex, total;
+    Scan(tmp).ExclusiveSum(v, ex, total);
+    if (b < blocks) p[b] = carry + ex;
+    carry += total;
+    __syncthreads();      // tmp is reused by the next chunk
+  }
+  if (threadIdx.x == 0) p[blocks] = carry;
+}
+
+// prefix: [num_tiles][bound_blocks(num_data) + 1] ints
+inline void launch_block_bound(const uint8_t* bins, size_t rows_stride, int num_data, int num_tiles, int num_columns, int* prefix,
+                               cudaStream_t stream) {
+  const int blocks = bound_blocks(num_data);
+  if (blocks > 0) k_block_maxcnt<<<dim3(blocks, num_tiles), 256, 0, stream>>>(bins, rows_stride, num_data, num_columns, prefix);
+  k_block_bound_prefix<<<num_tiles, 1024, 0, stream>>>(blocks, prefix);
 }
 
 
@@ -159,7 +239,7 @@ template <int NATOM>
 __global__ void __launch_bounds__(kWsThreads, 1)
 k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
                  const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1,
-                 const HistWork* __restrict__ work, unsigned long long* __restrict__ hist) {
+                 const HistWork* __restrict__ work, unsigned long long* __restrict__ hist, RowBlockBound bound) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned* plane = reinterpret_cast<unsigned*>(smem_raw);
   unsigned char* stage_bins = smem_raw + 4 * kPlaneWords * 4;
@@ -176,7 +256,7 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
 
   // Work items are (tile, row chunk) pairs in TILE-MAJOR order; every CTA takes one contiguous range of them, so
   // consecutive items of a CTA mostly belong to the same feature tile and the sub-histogram is flushed only when the
-  // tile changes or the 2^14-row field headroom is used up (small and medium leaves: one flush per CTA).
+  // tile changes or the bound of the items absorbed since the last flush could pass the 2^14 additions per cell (below).
   long long cells_rows = static_cast<long long>(n) * num_tiles;
   int rpi = static_cast<int>((cells_rows + 4LL * gridDim.x - 1) / (4LL * gridDim.x));
   rpi = (rpi + kWsStageRows - 1) / kWsStageRows * kWsStageRows;
@@ -258,12 +338,40 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
     unsigned exp_sink = 0;
 #endif
     const int sub = lane >> 2, rot = lane & 3;
-    int acc_rows = 0;                                             // rows absorbed by the sub-histogram since the last flush
+    // Most additions one cell of the item's tile can take from the item: its row count, or the block bound of the rows between its
+    // first and last row.  Index-list items take those two rows from the list: every leaf's row list is strictly ascending (the
+    // identity root, k_bag_compact's in-bag list and the stable k_partition scatter all keep the row order), so all rows of the
+    // item lie in between.  Every consumer thread reads the same values and so reaches the same flush decision.
+    // The loads run two items ahead, so no consumer waits on them: the first and last row of item k + 2 and the bound of item
+    // k + 1 are loaded when item k starts, and that bound is first used when item k ends.
+    auto item_rows = [&](int it, int& first, int& last) {
+      const int t = it / chunks, r0 = (it - t * chunks) * rpi;
+      first = w.begin + r0;
+      last = first + min(rpi, n - r0) - 1;
+      if (w.use_idx && bound.prefix) { first = idx[first]; last = idx[last]; }
+    };
+    auto item_bound = [&](int it, int first, int last) -> int {
+      const int t = it / chunks, nr = min(rpi, n - (it - t * chunks) * rpi);
+      if (!bound.prefix) return nr;
+      const int* p = bound.prefix + static_cast<size_t>(t) * (bound.blocks + 1);
+      return min(nr, p[last / kBoundBlockRows + 1] - p[first / kBoundBlockRows]);
+    };
+    int first, last;                                              // first and last row of the item whose bound is loaded next
+    item_rows(i0, first, last);
+    int next_bound = item_bound(i0, first, last);
+    if (i0 + 1 < i1) item_rows(i0 + 1, first, last);
+    int acc_bound = 0;                                            // bound of the items absorbed since the last flush, <= kFlushRows
     for (int item = i0; item < i1; ++item) {
       const int tile = item / chunks, chunk = item - tile * chunks;
       const int row0 = chunk * rpi;
       const int nrows = min(rpi, n - row0);
       const int nst = (nrows + kWsStageRows - 1) / kWsStageRows;
+      acc_bound += next_bound;
+      next_bound = 0;
+      if (item + 1 < i1) {
+        next_bound = item_bound(item + 1, first, last);
+        if (item + 2 < i1) item_rows(item + 2, first, last);
+      }
       for (int s = 0; s < nst; ++s, ++gs) {
         const int slot = gs % kWsStages;
         mbar_wait(&full_bar[slot], (gs / kWsStages) & 1u);
@@ -305,15 +413,10 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[slot]);
       }
-      acc_rows += nrows;
-      bool flush = (item + 1 == i1);
-      if (!flush) {
-        const int ntile = (item + 1) / chunks, nchunk = (item + 1) - ntile * chunks;
-        const int nnext = min(rpi, n - nchunk * rpi);
-        flush = (ntile != tile) || (acc_rows + nnext > kFlushRows);
-      }
+      // rpi <= kFlushRows, so a single item never breaks the 2^14 bound
+      const bool flush = (item + 1 == i1) || ((item + 1) / chunks != tile) || (acc_bound + next_bound > kFlushRows);
       if (!flush) continue;
-      acc_rows = 0;
+      acc_bound = 0;
       // All consumers finished: flush the sub-histogram into the int64 leaf histogram (consumer-only named barriers; the producers
       // keep staging).  Slab by slab (32 bins x 32 features), every consumer thread reads and re-zeroes the plane words of two
       // (bin, feature) cells, combines them into int64 (g,h) and stores the pairs into the staging buffer in the histogram's own
@@ -387,12 +490,14 @@ inline cudaError_t set_k4_smem_limit() {
 }
 
 // One persistent K4 launch: `grid` is one CTA per SM; constant-hessian objectives accumulate 3 planes (g_hi, g_lo, count).
+// `bound` is the bins' per-block bound (launch_block_bound); index lists given with it must be strictly ascending.
 inline void launch_k4(bool const_hessian, const uint8_t* bins, size_t rows_stride, int num_tiles, const int4* qgh, const int4* qord,
-                      const int* idx0, const int* idx1, const HistWork* work, unsigned long long* hist, int grid, cudaStream_t stream) {
+                      const int* idx0, const int* idx1, const HistWork* work, unsigned long long* hist, RowBlockBound bound, int grid,
+                      cudaStream_t stream) {
   if (const_hessian)
-    k4_hist_build_ws<3><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist);
+    k4_hist_build_ws<3><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound);
   else
-    k4_hist_build_ws<4><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist);
+    k4_hist_build_ws<4><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound);
 }
 
 }  // namespace b200gbm

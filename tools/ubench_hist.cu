@@ -1,9 +1,9 @@
 // Microbenchmarks that decide the K4 histogram design (build() compiles it to build/ubench_hist).
 //  Part A: shared-memory scatter-add throughput per SM for the candidate accumulator schemes
 //          (native ATOMS.ADD.32 owner-bank / random-bank, CAS float, non-atomic owner RMW ...).
-//  Part B: the engine's K4 kernel (k4_hist_build_ws<4> and <3>, launched through launch_k4) on synthetic
-//          tile-major bins: checked exactly against an int64 host computation, then timed with CUDA events
-//          and reported as cells/s and algorithmic GB/s.
+//  Part B: the engine's K4 kernel (k4_hist_build_ws<4> and <3>, launched through launch_k4 with the per-block bin-count
+//          bound of launch_block_bound) on synthetic tile-major bins, uniform and skewed: checked exactly against an int64
+//          host computation, then timed with CUDA events and reported as cells/s and algorithmic GB/s.
 // Usage: ubench_hist [ROWS] [SKIP_PART_A]   (ROWS defaults to 10M; SKIP_PART_A = 1 skips Part A)
 // Output: one JSON document on stdout.  Exit status 1 if the exact check finds a mismatch, except in the
 // B200GBM_K4_EXPERIMENT cost-model builds, whose histograms are wrong by design.
@@ -125,17 +125,26 @@ __global__ void gen_bins(uint8_t* bins, size_t rows_stride, int num_tiles, size_
     reinterpret_cast<unsigned*>(bins)[i] = w;
   }
 }
+// (g,h) words with signed ~36-bit g and unsigned ~35-bit h whose 18-bit low fields lie in [2^18 - 2^12, 2^18): one cell's low
+// field fits 2^14 additions and wraps its 32-bit accumulator within ~16.6K, so a window that misses a needed flush gives a mismatch
 __global__ void gen_q(int4* q, size_t n, unsigned seed) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   for (; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    long long g = (long long)(int)hash32((unsigned)i ^ seed) * 11LL;                 // signed ~36 bit
-    long long h = (long long)(hash32((unsigned)i * 3u + seed) >> 1) * 9LL;           // unsigned ~35 bit
-    q[i] = make_int4((int)(g >> kLoBits), (int)(g & ((1 << kLoBits) - 1)), (int)(h >> kLoBits), (int)(h & ((1 << kLoBits) - 1)));
+    const int g_hi = (int)hash32((unsigned)i ^ seed) >> 14, h_hi = (int)(hash32((unsigned)i * 3u + seed) >> 15);
+    const int g_lo = (1 << kLoBits) - 1 - (int)(hash32((unsigned)i * 5u + seed) & 4095u);
+    const int h_lo = (1 << kLoBits) - 1 - (int)(hash32((unsigned)i * 7u + seed) & 4095u);
+    q[i] = make_int4(g_hi, g_lo, h_hi, h_lo);
   }
 }
 __global__ void gen_idx(int* idx, int n, int stride) {   // every `stride`-th row, ascending
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   for (; i < n; i += gridDim.x * blockDim.x) idx[i] = i * stride;
+}
+// skew: column `col` of `tile` takes bin 7 in every row of [r0, r1) except every 64th, so one cell collects far more than 2^14
+// rows of a CTA's range and the flush bound has to force flushes
+__global__ void skew_bins(uint8_t* bins, size_t rows_stride, int tile, int col, int r0, int r1) {
+  for (int r = r0 + blockIdx.x * blockDim.x + threadIdx.x; r < r1; r += gridDim.x * blockDim.x)
+    if (r % 64 != 0) bins[((size_t)tile * rows_stride + r) * 32 + col] = 7;
 }
 
 int main(int argc, char** argv) {
@@ -180,57 +189,84 @@ int main(int argc, char** argv) {
   CK(cudaMalloc(&d_idx, N * sizeof(int)));
   CK(cudaMalloc(&d_hist, slot_elems * 8));
   CK(cudaMalloc(&d_work, sizeof(HistWork) * 2));
-  gen_bins<<<nsm * 8, 256>>>(d_bins, rows_stride, num_tiles, N, 12345u);
+  // the per-block bin-count bound of the flush rule, computed by the engine's kernels whenever the bins change
+  int* d_bound; CK(cudaMalloc(&d_bound, sizeof(int) * num_tiles * (bound_blocks((int)N) + 1)));
+  const RowBlockBound kb{d_bound, bound_blocks((int)N)};
+  auto set_bins = [&](int skew_r0, int skew_r1) {      // uniform bins, optionally skewed in rows [skew_r0, skew_r1), and their bound
+    gen_bins<<<nsm * 8, 256>>>(d_bins, rows_stride, num_tiles, N, 12345u);
+    if (skew_r1 > skew_r0) skew_bins<<<nsm * 8, 256>>>(d_bins, rows_stride, 1, 5, skew_r0, skew_r1);
+    launch_block_bound(d_bins, rows_stride, (int)N, num_tiles, F, d_bound, 0);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+  };
   gen_q<<<nsm * 8, 256>>>(d_q, N, 777u);
-  CK(cudaDeviceSynchronize());
+  set_bins(0, 0);
   CK(set_k4_smem_limit());
 
-  // exact int64 check of both instantiations on the first 1M rows: a contiguous pass and a strided index-list pass (every 3rd
-  // row), each with CTAs sharing feature tiles.  NATOM = 3 sums the count field q.z as h, as the kernel does.
+  // exact int64 check of both instantiations on the first 1M rows, every pass with CTAs sharing feature tiles: a contiguous pass
+  // and an ascending index-list pass, on three bin states.  "uniform": the generated bins, every 3rd row gathered.  "skew": column 5
+  // of tile 1 has nearly every row in one bin, so the bound must force flushes; every 2nd row gathered.  "skew_second_half": the
+  // same skew in the second half of the rows only, so a window that starts uniform must flush in time; every 37th row gathered (a
+  // leaf of low density).  NATOM = 3 sums the count field q.z as h, as the kernel does.
   size_t k4_bad = 0;
   {
     const int n_chk = (int)std::min<size_t>(N, 1000000);
-    HistWork hw[2] = {{0, n_chk, 0, 0}, {0, n_chk / 3, 1, 0}};
-    CK(cudaMemcpy(d_work, hw, sizeof(hw), cudaMemcpyHostToDevice));
-    gen_idx<<<nsm, 256>>>(d_idx, n_chk / 3, 3);
-    k_gather_q<<<nsm * 8, 256>>>(d_work + 1, d_idx, d_idx, d_q, d_qord);
-    CK(cudaDeviceSynchronize());
-    std::vector<uint8_t> hb((size_t)num_tiles * rows_stride * 32);
-    CK(cudaMemcpy(hb.data(), d_bins, hb.size(), cudaMemcpyDeviceToHost));
+    std::vector<uint8_t> hb((size_t)num_tiles * n_chk * 32);      // [tile][row][32] of the checked rows
     std::vector<int4> hq(n_chk);
     CK(cudaMemcpy(hq.data(), d_q, (size_t)n_chk * 16, cudaMemcpyDeviceToHost));
-    std::vector<long long> got(slot_elems), want(slot_elems);
+    std::vector<long long> got(slot_elems), want4(slot_elems), want3(slot_elems);
     printf(" \"k4_check\": {\"rows\": %d, \"mismatches\": {", n_chk);
-    for (int natom : {4, 3}) {
+    struct State { const char* name; int skew_r0, skew_r1, stride; };
+    const State states[] = {{"uniform", 0, 0, 3}, {"skew", 0, n_chk, 2}, {"skew_second_half", n_chk / 2, n_chk, 37}};
+    bool first = true;
+    for (const State& st : states) {
+      set_bins(st.skew_r0, st.skew_r1);
+      for (int t = 0; t < num_tiles; ++t)
+        CK(cudaMemcpy(&hb[(size_t)t * n_chk * 32], d_bins + (size_t)t * rows_stride * 32, (size_t)n_chk * 32, cudaMemcpyDeviceToHost));
       for (int pass = 0; pass < 2; ++pass) {
-        CK(cudaMemset(d_hist, 0, slot_elems * 8));
-        launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work + pass, d_hist, nsm, 0);
-        CK(cudaGetLastError());
-        CK(cudaDeviceSynchronize());
-        CK(cudaMemcpy(got.data(), d_hist, slot_elems * 8, cudaMemcpyDeviceToHost));
-        std::fill(want.begin(), want.end(), 0LL);
-        const int step = pass ? 3 : 1;
-        for (int i = 0; i < hw[pass].count * step; i += step) {
+        const int step = pass ? st.stride : 1;
+        const HistWork hw = {0, n_chk / step, pass, 0};
+        CK(cudaMemcpy(d_work, &hw, sizeof(hw), cudaMemcpyHostToDevice));
+        if (pass) {
+          gen_idx<<<nsm, 256>>>(d_idx, hw.count, step);
+          k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);
+        }
+        std::fill(want4.begin(), want4.end(), 0LL);
+        std::fill(want3.begin(), want3.end(), 0LL);
+        for (int i = 0; i < hw.count * step; i += step) {
           const long long g = ((long long)hq[i].x << kLoBits) + hq[i].y;
-          const long long h = natom == 4 ? ((long long)hq[i].z << kLoBits) + hq[i].w : (long long)hq[i].z;
+          const long long h4 = ((long long)hq[i].z << kLoBits) + hq[i].w, h3 = hq[i].z;
           for (int t = 0; t < num_tiles; ++t) {
-            const uint8_t* row = &hb[((size_t)t * rows_stride + i) * 32];
+            const uint8_t* row = &hb[((size_t)t * n_chk + i) * 32];
             for (int l = 0; l < 32; ++l) {
               size_t o = ((size_t)(t * 32 + l) * 256 + row[l]) * 2;
-              want[o] += g; want[o + 1] += h;
+              want4[o] += g; want4[o + 1] += h4;
+              want3[o] += g; want3[o + 1] += h3;
             }
           }
         }
-        size_t bad = 0; for (size_t i = 0; i < want.size(); ++i) bad += (got[i] != want[i]);
-        printf("%s\"natom%d_%s\": %zu", natom == 4 && pass == 0 ? "" : ", ", natom, pass ? "gathered" : "contiguous", bad);
-        k4_bad += bad;
+        for (int natom : {4, 3}) {
+          CK(cudaMemset(d_hist, 0, slot_elems * 8));
+          launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, kb, nsm, 0);
+          CK(cudaGetLastError());
+          CK(cudaDeviceSynchronize());
+          CK(cudaMemcpy(got.data(), d_hist, slot_elems * 8, cudaMemcpyDeviceToHost));
+          const std::vector<long long>& want = natom == 4 ? want4 : want3;
+          size_t bad = 0; for (size_t i = 0; i < want.size(); ++i) bad += (got[i] != want[i]);
+          printf("%s\"%s_natom%d_%s\": %zu", first ? "" : ", ", st.name, natom, pass ? "gathered" : "contiguous", bad);
+          first = false;
+          k4_bad += bad;
+        }
       }
     }
     printf("}},\n");
+    set_bins(0, 0);
   }
 
-  // timing: full pass (contiguous) and gathered pass (every 2nd row), NATOM 4 and 3
-  auto time_it = [&](int natom, int n, int use_idx, int reps) -> float {
+  // timing: full pass (contiguous) and gathered passes, NATOM 4 and 3.  The two skew = 1 rows run on bins whose column 5 of tile 1
+  // has nearly every row in one bin, where the block bound lets that tile flush only every ~2^14 rows: once with the block bound
+  // and once (bound = 0) with the row-count bound, i.e. a flush every 2^14 rows, what the kernel does for an index list that repeats rows.
+  auto time_it = [&](int natom, int n, int use_idx, RowBlockBound rb, int reps) -> float {
     HistWork hw = {0, n, use_idx, 0};
     CK(cudaMemcpy(d_work, &hw, sizeof(hw), cudaMemcpyHostToDevice));
     cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
@@ -239,7 +275,7 @@ int main(int argc, char** argv) {
       CK(cudaMemsetAsync(d_hist, 0, slot_elems * 8));
       CK(cudaEventRecord(e0));
       if (use_idx) k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);     // part of a leaf pass: timed
-      launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, nsm, 0);
+      launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, rb, nsm, 0);
       CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
       float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
       if (r >= 2) { best = std::min(best, ms); tot += ms; }
@@ -247,17 +283,28 @@ int main(int argc, char** argv) {
     (void)best;
     return tot / reps;
   };
+  {  // one-time cost of the flush bound (a dataset computes it on first use): every bin byte read once, one shared atomic per byte
+    cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    CK(cudaEventRecord(e0));
+    launch_block_bound(d_bins, rows_stride, (int)N, num_tiles, F, d_bound, 0);
+    CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
+    float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+    printf(" \"block_bound\": {\"ms\": %.3f, \"bin_bytes\": %zu},\n", ms, (size_t)num_tiles * N * 32);
+  }
   printf(" \"k4_timing\": [\n");
-  struct Cfg { int natom; double frac; int use_idx; };
-  Cfg cfgs[] = {{4, 1.0, 0}, {3, 1.0, 0}, {4, 0.5, 1}, {4, 0.1, 1}, {4, 0.01, 1}, {4, 0.001, 1}};
+  struct Cfg { int natom; double frac; int use_idx; int skew; int bound; };
+  Cfg cfgs[] = {{4, 1.0, 0, 0, 1}, {3, 1.0, 0, 0, 1}, {4, 0.5, 1, 0, 1}, {4, 0.1, 1, 0, 1}, {4, 0.01, 1, 0, 1}, {4, 0.001, 1, 0, 1},
+                {4, 1.0, 0, 1, 1}, {4, 1.0, 0, 1, 0}};
   for (size_t c = 0; c < sizeof(cfgs) / sizeof(cfgs[0]); ++c) {
     int n = (int)(N * cfgs[c].frac);
     if (cfgs[c].use_idx) { gen_idx<<<nsm, 256>>>(d_idx, n, (int)(1.0 / cfgs[c].frac)); CK(cudaDeviceSynchronize()); }
-    float ms = time_it(cfgs[c].natom, n, cfgs[c].use_idx, 5);
+    if (cfgs[c].skew && !cfgs[c - 1].skew) set_bins(0, (int)N);
+    float ms = time_it(cfgs[c].natom, n, cfgs[c].use_idx, cfgs[c].bound ? kb : RowBlockBound{nullptr, 0}, 5);
     double cells = (double)n * F;
     double bytes = (double)n * (F + 16.0 * num_tiles + (cfgs[c].use_idx ? 4.0 * num_tiles : 0.0)) + (double)F * 256 * 16;
-    printf("  {\"natom\": %d, \"rows\": %d, \"gather\": %d, \"ms\": %.4f, \"gcells_per_s\": %.2f, \"algo_GBps\": %.1f}%s\n",
-           cfgs[c].natom, n, cfgs[c].use_idx, ms, cells / ms * 1e-6, bytes / ms * 1e-6, c + 1 < sizeof(cfgs) / sizeof(cfgs[0]) ? "," : "");
+    printf("  {\"natom\": %d, \"rows\": %d, \"gather\": %d, \"skew\": %d, \"bound\": %d, \"ms\": %.4f, \"gcells_per_s\": %.2f, \"algo_GBps\": %.1f}%s\n",
+           cfgs[c].natom, n, cfgs[c].use_idx, cfgs[c].skew, cfgs[c].bound, ms, cells / ms * 1e-6, bytes / ms * 1e-6,
+           c + 1 < sizeof(cfgs) / sizeof(cfgs[0]) ? "," : "");
   }
   printf(" ]\n}\n");
   return (B200GBM_K4_EXPERIMENT == 0 && k4_bad != 0) ? 1 : 0;
