@@ -204,9 +204,12 @@ int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, i
 /* out = {num_machines, rank, histogram reduce mode (0 = ncclAllReduce, 1 = reduce-scatter + scan of the owned feature slice over NVLink
  * peer memory, 2 = two-shot all-reduce kernel over peer memory + replicated scan), constant_hessian} */
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4);
-/* out = {bytes of the optional column-major copy of the training bins kept for the partition kernel (0 = not kept: it is built before the
- * first tree only if it leaves a reserve of device memory, B200GBM_COLUMN_COPY=0 disables it), free device memory in bytes} */
+/* out = {bytes of the optional column-major copy of the training bins kept for the partition kernel (0 = not kept: it is set up before the
+ * first tree only within a reserve of device memory, B200GBM_COLUMN_COPY=0 disables it; when the full copy does not fit, the bytes of
+ * the column cache's slot pool), free device memory in bytes} */
 int B200GBM_BoosterGetMemoryInfo(BoosterHandle handle, int64_t* out2);
+/* out = {slots of the column cache (0 = no cache: full copy or none), slots in use, columns built into slots so far, evictions so far} */
+int B200GBM_BoosterGetColumnCacheInfo(BoosterHandle handle, int64_t* out4);
 
 #ifdef __cplusplus
 }

@@ -437,6 +437,11 @@ class Booster:
         check(load().B200GBM_BoosterGetMemoryInfo(self.handle, _ptr(out)))
         return dict(partition_column_copy_bytes=int(out[0]), device_free_bytes=int(out[1]))
 
+    def get_column_cache_info(self):
+        out = np.zeros(4, dtype=np.int64)
+        check(load().B200GBM_BoosterGetColumnCacheInfo(self.handle, _ptr(out)))
+        return dict(slots=int(out[0]), slots_used=int(out[1]), builds=int(out[2]), evictions=int(out[3]))
+
     def get_scores(self, data_idx=0):
         n = C.c_int64(0)
         check(load().LGBM_BoosterGetNumPredict(self.handle, C.c_int(data_idx), C.byref(n)))

@@ -612,6 +612,11 @@ int B200GBM_BoosterGetMemoryInfo(BoosterHandle handle, int64_t* out2) {
   BS(handle)->GetMemoryInfo(out2);
   API_END();
 }
+int B200GBM_BoosterGetColumnCacheInfo(BoosterHandle handle, int64_t* out4) {
+  API_BEGIN();
+  BS(handle)->GetColumnCacheInfo(out4);
+  API_END();
+}
 int B200GBM_BoosterGetScores(BoosterHandle handle, int data_idx, double* out) {
   API_BEGIN();
   BS(handle)->GetRawScores(data_idx, out);

@@ -1525,29 +1525,95 @@ void Booster::RenewTreeOutput(int k, double rf_pred) {
 }
 
 // k_partition is launched cooperatively: its software grid barriers need every block resident
-// Column-major copy of the training tiles for k_partition (kernels.cuh: k_tiles_to_columns).  Built once, before the first tree, after every
-// other buffer of the booster exists, and only if it leaves a reserve of device memory (validation scores, metric and prediction scratch
-// come later); B200GBM_COLUMN_COPY=0 disables it.  Without it the partition reads one 32-byte sector per row — same results.
+// Column-major copies of the training tiles for k_partition, so that its phase 1 reads one byte per row instead of a 32-byte sector —
+// same results either way.  Set up once, before the first tree, after every other buffer of the booster exists, and only within a
+// reserve of device memory (validation scores, metric and prediction scratch come later); B200GBM_COLUMN_COPY=0 disables it.
+//   full copy     every storage column (kernels.cuh: k_tiles_to_columns), if it fits
+//   column cache  otherwise a pool of as many column slots as fit, filled between trees with the columns the trees split on
+//                 (UpdateColumnCache); B200GBM_COLUMN_CACHE_COLUMNS=k forces this mode with at most k slots
 void Booster::EnsureColumnCopy() {
   if (cols_tried_) return;
   cols_tried_ = true;
   const Dataset& d = *train;
   const char* env = std::getenv("B200GBM_COLUMN_COPY");
   if ((env && std::atoi(env) == 0) || d.nfn == 0 || d.num_data == 0) return;
+  const char* force = std::getenv("B200GBM_COLUMN_CACHE_COLUMNS");
   const size_t stride = (static_cast<size_t>(d.num_data) + 255) & ~static_cast<size_t>(255);
-  const size_t need = static_cast<size_t>(d.num_tiles) * 32 * stride;
+  const int ncols = d.num_tiles * 32;
+  const size_t need = static_cast<size_t>(ncols) * stride;
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return; }
   const size_t reserve = std::max<size_t>(static_cast<size_t>(8) << 30, total_b / 10);
-  if (free_b < need + reserve) return;
+  const bool full = !force && free_b >= need + reserve;
+  int slots = ncols;
+  if (!full) {
+    slots = static_cast<int>(std::min<size_t>(d.num_columns, free_b > reserve ? (free_b - reserve) / stride : 0));
+    if (force) slots = std::min(slots, std::max(0, std::atoi(force)));
+    if (slots == 0) return;
+  }
+  const size_t bytes = static_cast<size_t>(slots) * stride;
   uint8_t* p = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&p), need) != cudaSuccess) { cudaGetLastError(); return; }
-  bins_cols_.p = p; bins_cols_.n = need;
+  if (cudaMalloc(reinterpret_cast<void**>(&p), bytes) != cudaSuccess) { cudaGetLastError(); return; }
+  bins_cols_.p = p; bins_cols_.n = bytes;
   cols_stride_ = stride;
-  const long long work = ((static_cast<long long>(d.num_data) + 255) / 256) * d.num_tiles;
-  k_tiles_to_columns<<<static_cast<unsigned>(std::min<long long>(work, static_cast<long long>(num_sms_) * 16)), 256, 0, stream_>>>(
-      d.bins.p, d.rows_stride, d.num_tiles, d.num_data, bins_cols_.p, stride);
+  col_slot_host_.assign(ncols, -1);
+  if (full) {
+    for (int c = 0; c < ncols; ++c) col_slot_host_[c] = c;
+    const long long work = ((static_cast<long long>(d.num_data) + 255) / 256) * d.num_tiles;
+    k_tiles_to_columns<<<static_cast<unsigned>(std::min<long long>(work, static_cast<long long>(num_sms_) * 16)), 256, 0, stream_>>>(
+        d.bins.p, d.rows_stride, d.num_tiles, d.num_data, bins_cols_.p, stride);
+    B200_CUDA(cudaGetLastError());
+  } else {
+    slot_col_.assign(slots, -1);
+    col_splits_.assign(ncols, 0);
+  }
+  col_slot_.Alloc(ncols);
+  col_slot_.Upload(col_slot_host_.data(), ncols, stream_);
+}
+
+// Column cache, after each tree (its host copy is read back, the stream is idle): count the tree's splits per storage column (wide
+// features have their own uint16 columns and are not counted), then copy the most split-on columns that are not cached into free slots.
+// When the pool is full, a candidate replaces the least split-on cached column only if that one has fewer splits, so columns that are
+// split on often stay.  At most kColumnBuildsMax columns (N x 32 bytes read each) are built per tree, in one launch on the stream;
+// the next tree's partitions see the new slot table in stream order, with no host sync inside the tree.
+void Booster::UpdateColumnCache(const HostTree& t) {
+  if (slot_col_.empty()) return;
+  const Dataset& d = *train;
+  for (int i = 0; i + 1 < t.num_leaves; ++i) {
+    const int f = t.split_feature_inner[i];
+    if (f < d.nfn) ++col_splits_[d.meta_host[f].hist_off >> 8];
+  }
+  std::vector<int> cand;
+  for (int c = 0; c < static_cast<int>(col_splits_.size()); ++c)
+    if (col_splits_[c] > 0 && col_slot_host_[c] < 0) cand.push_back(c);
+  std::stable_sort(cand.begin(), cand.end(), [&](int a, int b) { return col_splits_[a] > col_splits_[b]; });
+  ColumnJobs jobs{};
+  for (int c : cand) {
+    if (jobs.n == kColumnBuildsMax) break;
+    int slot = -1, victim = -1;
+    for (int s = 0; s < static_cast<int>(slot_col_.size()) && slot < 0; ++s) {
+      const int held = slot_col_[s];
+      if (held < 0) slot = s;
+      else if (victim < 0 || col_splits_[held] < col_splits_[slot_col_[victim]]) victim = s;
+    }
+    if (slot < 0) {
+      if (col_splits_[slot_col_[victim]] >= col_splits_[c]) break;      // candidates come in descending order: none later wins either
+      slot = victim;
+      col_slot_host_[slot_col_[slot]] = -1;
+      ++cache_evictions_;
+    }
+    slot_col_[slot] = c;
+    col_slot_host_[c] = slot;
+    jobs.col[jobs.n] = c; jobs.slot[jobs.n] = slot; ++jobs.n;
+  }
+  if (jobs.n == 0) return;
+  const long long words = (static_cast<long long>(d.num_data) + 3) / 4;
+  const unsigned gx = static_cast<unsigned>(std::max<long long>(1, std::min<long long>((words + 255) / 256, static_cast<long long>(num_sms_) * 8)));
+  k_tiles_to_column_slots<<<dim3(gx, jobs.n), 256, 0, stream_>>>(d.bins.p, d.rows_stride, d.num_data, jobs, bins_cols_.p, cols_stride_);
   B200_CUDA(cudaGetLastError());
+  col_slot_.Upload(col_slot_host_.data(), col_slot_host_.size(), stream_);
+  cache_builds_ += jobs.n;
+  timing.launches += 1;
 }
 
 void Booster::GetMemoryInfo(int64_t* out2) {
@@ -1556,6 +1622,13 @@ void Booster::GetMemoryInfo(int64_t* out2) {
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
   out2[0] = static_cast<int64_t>(bins_cols_.n);
   out2[1] = static_cast<int64_t>(free_b);
+}
+
+void Booster::GetColumnCacheInfo(int64_t* out4) const {
+  out4[0] = static_cast<int64_t>(slot_col_.size());
+  out4[1] = static_cast<int64_t>(std::count_if(slot_col_.begin(), slot_col_.end(), [](int c) { return c >= 0; }));
+  out4[2] = cache_builds_;
+  out4[3] = cache_evictions_;
 }
 
 void Booster::LaunchPartition(int grid, int last) {
@@ -1580,10 +1653,11 @@ void Booster::LaunchPartition(int grid, int last) {
   int tickets_per_block = tickets;
   const uint8_t* cols = bins_cols_.p;
   size_t cols_stride = cols_stride_;
+  const int* col_slot = col_slot_.p;
   int* super_tot = part_chunks_.p + (train->num_data / kPartChunk + 2);
   const int* bundle_base = d.BundleBase();
   void* args[] = {&ctrl, &leaves, &tree, &flags, &meta, &sp, &last, &bins, &rows_stride, &i0, &i1, &bits, &chunks, &qgh, &qord, &H, &h_elems, &bins16, &tickets_per_block,
-                  &cols, &cols_stride, &super_tot, &bundle_base};
+                  &cols, &cols_stride, &col_slot, &super_tot, &bundle_base};
   B200_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(k_partition), dim3(grid), dim3(256), args, 0, stream_));
 }
 
@@ -1764,6 +1838,7 @@ void Booster::TrainOneTree(int k, HostTree* out) {
   } else {
     out->leaf_value[0] = 0.0;
   }
+  UpdateColumnCache(*out);
 }
 
 bool Booster::TrainTrees(const float* custom_g, const float* custom_h) {

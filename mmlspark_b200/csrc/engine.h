@@ -282,12 +282,21 @@ class Booster {
   unsigned char* tree_host_ = nullptr;   // pinned mirror of tree_blob_
   TreeCtrl* ctrl_host_ = nullptr;        // pinned
   LeafState* leaves_host_ = nullptr;     // pinned
-  DevBuf<uint8_t> bins_cols_;      // optional [feature][row] copy of the uint8 tiles for the partition kernel
+  // optional [column][row] copies of the uint8 tiles' storage columns for the partition kernel: all of them (full copy), or a pool of
+  // slots that UpdateColumnCache fills with the columns the trees split on (column cache)
+  DevBuf<uint8_t> bins_cols_;
   size_t cols_stride_ = 0;
   bool cols_tried_ = false;
+  DevBuf<int> col_slot_;                   // [num_tiles * 32] slot of each storage column in bins_cols_, -1: not copied
+  std::vector<int> col_slot_host_;
+  std::vector<int> slot_col_;              // column cache: storage column held by each slot, -1: free (empty for the full copy)
+  std::vector<long long> col_splits_;      // column cache: splits on each storage column so far
+  long long cache_builds_ = 0, cache_evictions_ = 0;
   void EnsureColumnCopy();
+  void UpdateColumnCache(const HostTree& t);
  public:
   void GetMemoryInfo(int64_t* out2);
+  void GetColumnCacheInfo(int64_t* out4) const;
  private:
   DevBuf<unsigned> part_bits_;
   DevBuf<int> part_chunks_;

@@ -1444,6 +1444,29 @@ k_tiles_to_columns(const uint8_t* __restrict__ bins, size_t rows_stride, int num
   }
 }
 
+// When the whole copy does not fit, the booster keeps a pool of column slots instead and fills them, between trees, with the storage
+// columns the trees split on (Booster::UpdateColumnCache).  This kernel copies up to kColumnBuildsMax storage columns into given slots:
+// blockIdx.y is the job, each thread packs 4 consecutive rows into one 32-bit store.  The 4 bytes lie in 4 sectors of one 128-byte
+// line, so every sector of the column's tile is read from DRAM once per job (32 bytes per row).
+constexpr int kColumnBuildsMax = 8;
+struct ColumnJobs { int n; int col[kColumnBuildsMax]; int slot[kColumnBuildsMax]; };
+__global__ void __launch_bounds__(256)
+k_tiles_to_column_slots(const uint8_t* __restrict__ bins, size_t rows_stride, long long nrow, ColumnJobs jobs, uint8_t* __restrict__ cols,
+                        size_t cols_stride) {
+  const int c = jobs.col[blockIdx.y];
+  const uint8_t* src = bins + static_cast<size_t>(c >> 5) * rows_stride * 32 + (c & 31);
+  unsigned* dst = reinterpret_cast<unsigned*>(cols + static_cast<size_t>(jobs.slot[blockIdx.y]) * cols_stride);     // cols_stride: multiple of 256
+  const long long words = (nrow + 3) / 4;
+  for (long long w = blockIdx.x * 256LL + threadIdx.x; w < words; w += static_cast<long long>(gridDim.x) * 256) {
+    const long long r0 = w * 4;
+    unsigned v = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (r0 + j < nrow) v |= static_cast<unsigned>(src[static_cast<size_t>(r0 + j) * 32]) << (8 * j);
+    dst[w] = v;
+  }
+}
+
 // ---------------------------------------------------------------- K7 row partition (stable), one cooperative kernel per split
 // Replaces [UPSTREAM] DataPartition::Split.  Round 1 ran three kernels (decision bits + per-chunk left counts, single-block scan of the
 // chunk counts, scatter) plus a memset of the scratch histogram and the next round's controller: five launches on the per-split
@@ -1479,8 +1502,8 @@ __global__ void __launch_bounds__(256, 3)
 k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, const FeatMeta* __restrict__ meta, SplitParams p, int last,
             const uint8_t* __restrict__ bins, size_t rows_stride, int* __restrict__ idx0, int* __restrict__ idx1, unsigned* __restrict__ bits,
             int* __restrict__ chunk_left, const int4* __restrict__ qgh, int4* __restrict__ qord, long long* __restrict__ H, size_t h_elems,
-            const uint16_t* __restrict__ bins16, int tickets_per_block, const uint8_t* __restrict__ cols, size_t cols_stride, int* __restrict__ super_tot,
-            const int* __restrict__ bundle_base) {
+            const uint16_t* __restrict__ bins16, int tickets_per_block, const uint8_t* __restrict__ cols, size_t cols_stride,
+            const int* __restrict__ col_slot, int* __restrict__ super_tot, const int* __restrict__ bundle_base) {
   __shared__ int s_pref[kPartLocalScan + 1];
   __shared__ unsigned short s_list[kCatListMax];
   __shared__ int s_wl[64];
@@ -1507,7 +1530,9 @@ k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
     const int bbase = (wide >= 0 || !bundle_base) ? -1 : bundle_base[f], bmfb = meta[f].default_bin, bnb = meta[f].num_bin;
     const uint8_t* col = bins + (static_cast<size_t>(sc >> 5) * rows_stride) * 32 + (sc & 31);
     const uint16_t* wcol = wide >= 0 ? bins16 + static_cast<size_t>(wide) * rows_stride : nullptr;
-    const uint8_t* ccol = (cols != nullptr && wide < 0) ? cols + static_cast<size_t>(sc) * cols_stride : nullptr;      // column-major copy, if kept
+    // column-major copy of the split's storage column, if the booster keeps one: col_slot maps a storage column to its slot (-1: none)
+    const int cslot = (col_slot != nullptr && wide < 0) ? col_slot[sc] : -1;
+    const uint8_t* ccol = cslot >= 0 ? cols + static_cast<size_t>(cslot) * cols_stride : nullptr;
     const bool wide_cat = wide >= 0 && ctrl->split_is_cat;
     const int list_len = wide_cat ? ctrl->split_cat_list_len : 0;
     if (threadIdx.x < list_len) s_list[threadIdx.x] = ctrl->split_cat_list[threadIdx.x];
