@@ -201,6 +201,15 @@ int B200GBM_BoosterGetScores(BoosterHandle handle, int data_idx, double* out);  
  * NULL) = CUDA-event time.  Replaces the per-row UDF calls of LightGBMBooster.scala:390-423,528-545 for whole partitions. */
 int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol, int predict_type,
                                        int start_iteration, int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms);
+/* batched GPU prediction of a host CSR matrix (indptr INT32 or INT64, data FLOAT64), arguments of LGBM_BoosterPredictForCSRSingle plus
+ * elapsed_ms.  Every output equals B200GBM_BoosterPredictForMatDevice on the densified rows bit for bit (a missing entry is 0, of
+ * repeated indices the last wins, indices outside the model's features are ignored), and so LGBM_BoosterPredictForCSRSingle on the row:
+ * bit for bit, contributions to 1e-12.  Contributions keep the dense layout [nrow][num_class][num_feature+1].  Only the features the
+ * trees split on are built on the device, so a row costs O(its nonzeros + the split features) however wide num_col is.  Unlike the
+ * single-row entry, a bad indptr (decreasing, negative, or past nelem) is an error. */
+int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
+                                       int data_type, int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration,
+                                       int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms);
 /* out = {num_machines, rank, histogram reduce mode (0 = ncclAllReduce, 1 = reduce-scatter + scan of the owned feature slice over NVLink
  * peer memory, 2 = two-shot all-reduce kernel over peer memory + replicated scan), constant_hessian} */
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4);

@@ -419,6 +419,30 @@ class Booster:
         res = out[:n.value].reshape(nrow, -1)
         return (res, ms.value) if return_ms else res
 
+    def predict_csr_device(self, indptr, indices=None, data=None, num_col=None, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1,
+                           return_ms=False):
+        """Batched GPU prediction of CSR rows (B200GBM_BoosterPredictForCSRDevice): host indptr (int32/int64), indices, float64 data,
+        or a scipy.sparse matrix as the first argument.  Same values as predict_for_csr_single row by row."""
+        if not isinstance(indptr, np.ndarray) and hasattr(indptr, "tocsr"):      # scipy.sparse
+            m = indptr.tocsr()
+            indptr, indices, data, num_col = m.indptr, m.indices, m.data, m.shape[1]
+        indptr = np.ascontiguousarray(indptr)
+        if indptr.dtype not in (np.int32, np.int64):
+            indptr = indptr.astype(np.int64)
+        indices = np.ascontiguousarray(indices, dtype=np.int32)
+        data = np.ascontiguousarray(data, dtype=np.float64)
+        nrow = len(indptr) - 1
+        n = C.c_int64(0)
+        check(load().LGBM_BoosterCalcNumPredict(self.handle, C.c_int(max(nrow, 0)), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n)))
+        out = np.zeros(max(n.value, 1), dtype=np.float64)
+        ms = C.c_double(0)
+        check(load().B200GBM_BoosterPredictForCSRDevice(self.handle, _ptr(indptr), C.c_int(DTYPE_INT32 if indptr.dtype == np.int32 else DTYPE_INT64),
+                                                        _ptr(indices), _ptr(data), C.c_int(DTYPE_FLOAT64), C.c_int64(len(indptr)), C.c_int64(len(data)),
+                                                        C.c_int64(num_col), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration),
+                                                        C.byref(n), _ptr(out), C.byref(ms)))
+        res = out[:n.value].reshape(nrow, n.value // max(nrow, 1))
+        return (res, ms.value) if return_ms else res
+
     def set_profile(self, on=True):
         check(load().B200GBM_BoosterSetProfile(self.handle, C.c_int(1 if on else 0)))
 

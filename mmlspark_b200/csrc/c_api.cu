@@ -602,6 +602,16 @@ int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, i
   if (elapsed_ms) *elapsed_ms = b->last_predict_ms;
   API_END();
 }
+int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
+                                       int data_type, int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration,
+                                       int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms) {
+  API_BEGIN();
+  (void)num_col;      // like LGBM_BoosterPredictForCSRSingle: columns past the model's features are never read
+  Booster* b = BS(handle);
+  *out_len = b->PredictBatchCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, predict_type, start_iteration, num_iteration, out_result);
+  if (elapsed_ms) *elapsed_ms = b->last_predict_ms;
+  API_END();
+}
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4) {
   API_BEGIN();
   BS(handle)->GetInfo(out4);

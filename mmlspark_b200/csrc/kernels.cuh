@@ -2716,6 +2716,47 @@ k_predict_contrib(ForestDev f, const T* __restrict__ X, long long nrow, int ncol
   }
 }
 
+// ---------------------------------------------------------------- batched prediction of CSR rows
+// The predict kernels above read a CSR row through a dense [rows][U] row of "slots": one per distinct split feature of the trees
+// walked, with the forest's split_feature remapped to slots.  One warp per row zero-fills its slots, then stores the row's entries
+// 32 at a time in CSR order.  Values match LGBM_BoosterPredictForCSRSingle's densified row: a missing entry is 0, stored zeros and
+// NaN are kept, an index outside [0, num_feature) or of a feature no tree splits on is dropped, and of repeated indices the last
+// wins: within a stride the highest lane of each slot stores, and __syncwarp orders the strides.
+__global__ void __launch_bounds__(256)
+k_csr_to_slots(const long long* __restrict__ indptr, const int* __restrict__ indices, const double* __restrict__ data, long long nrow,
+               const int* __restrict__ slot_of_feature, int num_feature, int U, double* __restrict__ X) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  for (long long r = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5; r < nrow; r += warps) {
+    double* row = X + r * U;
+    for (int s = lane; s < U; s += 32) row[s] = 0.0;
+    __syncwarp();
+    const long long b = indptr[r + 1];
+    for (long long k0 = indptr[r]; k0 < b; k0 += 32) {
+      const long long k = k0 + lane;
+      int slot = -1;
+      double v = 0.0;
+      if (k < b) {
+        const int j = indices[k];
+        if (j >= 0 && j < num_feature) { slot = slot_of_feature[j]; v = data[k]; }
+      }
+      const unsigned same = __match_any_sync(0xffffffffu, slot);
+      if (slot >= 0 && lane == 31 - __clz(same)) row[slot] = v;
+      __syncwarp();
+    }
+  }
+}
+// contributions per slot [rows][K][U+1] (expected value last) -> LightGBM's dense layout [rows][K][F1] in a zero-filled `out`
+__global__ void k_contrib_slots_to_features(const double* __restrict__ in, long long rows_k, int U, const int* __restrict__ feature_of_slot,
+                                            int F1, double* __restrict__ out) {
+  const long long total = rows_k * (U + 1);
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total; e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long rk = e / (U + 1);
+    const int s = static_cast<int>(e - rk * (U + 1));
+    out[rk * F1 + (s == U ? F1 - 1 : feature_of_slot[s])] = in[e];
+  }
+}
+
 __global__ void k_hist_to_double(const long long* __restrict__ H, double* __restrict__ out, size_t elems, const TreeCtrl* ctrl) {
   const double ig = ctrl->inv_g, ih = ctrl->inv_h;
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < elems; i += static_cast<size_t>(gridDim.x) * blockDim.x)

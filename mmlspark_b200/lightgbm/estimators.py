@@ -2,7 +2,7 @@
 lightgbm/src/main/scala/com/microsoft/ml/spark/lightgbm/{LightGBMBase,LightGBMClassifier,LightGBMRegressor,
 LightGBMRanker,LightGBMModelMethods}.scala and booster/LightGBMBooster.scala, driving the b200gbm engine through the
 C ABI.  There is no JVM/Spark in this environment, so a "DataFrame" is a `Frame` (dict of numpy columns, the
-features column being a 2-D array) or a pandas DataFrame; a Spark partition is a contiguous row block and a Spark
+features column being a 2-D array or a scipy.sparse matrix) or a pandas DataFrame; a Spark partition is a contiguous row block and a Spark
 task is a rank-thread bound to one GPU (SURVEY.md fact 8: in local mode all tasks are threads of one JVM)."""
 import logging
 import os
@@ -17,15 +17,59 @@ from .params import COMMON_DEFAULTS, Params, TrainParams, dataset_params
 log = logging.getLogger("mmlspark_b200.lightgbm")
 
 
+def _is_sparse(x):
+    """A scipy.sparse matrix or array (told apart without importing scipy)."""
+    return not isinstance(x, np.ndarray) and hasattr(x, "tocsr") and hasattr(x, "nnz")
+
+
+def _canonical_csr(x):
+    """CSR with sorted, distinct indices per row: scipy's meaning of repeated entries (their sum) in every path that reads them."""
+    m = x.tocsr()
+    if not m.has_canonical_format:
+        m = m.copy()
+        m.sum_duplicates()
+    return m
+
+
+def _to_sparse(X):
+    """Dense rows to CSR the way Spark's DenseVector.toSparse does: every value != 0 is kept, NaN included."""
+    import scipy.sparse as sp
+    X = np.asarray(X, dtype=np.float64)
+    keep = X != 0
+    indptr = np.concatenate([[0], np.cumsum(keep.sum(axis=1))]).astype(np.int64)
+    return sp.csr_matrix((X[keep], np.nonzero(keep)[1].astype(np.int32), indptr), shape=X.shape)
+
+
+def resolve_matrix_type(matrix_type, features):
+    """The features column as the fit will read it, sparse or dense (SharedState.scala:28-36; DatasetAggregator.scala:142-150).
+    auto: as given (in a column of one kind the reference's vote over the first 10 rows always picks that kind); sparse: dense rows go
+    through toSparse; dense: sparse rows are densified."""
+    if matrix_type not in ("auto", "sparse", "dense"):
+        raise ValueError("Invalid parameter matrix type specified: %s" % matrix_type)
+    if _is_sparse(features):
+        m = _canonical_csr(features)
+        return m.toarray() if matrix_type == "dense" else m
+    return _to_sparse(features) if matrix_type == "sparse" else features
+
+
+def _row_features(x):
+    return x if _is_sparse(x) else np.asarray(x, dtype=np.float64)
+
+
+def _batch_features(col):
+    return _canonical_csr(col) if _is_sparse(col) else np.ascontiguousarray(col, dtype=np.float64)
+
+
 class Frame(dict):
-    """Minimal columnar frame: column name -> numpy array (the features column is [n_rows, n_features])."""
+    """Minimal columnar frame: column name -> numpy array.  The features column is [n_rows, n_features], a 2-D array of dense rows
+    or a scipy.sparse matrix of sparse rows."""
 
     @classmethod
     def of(cls, data):
         if isinstance(data, Frame):
             return data
         if isinstance(data, dict):
-            return cls({k: np.asarray(v) for k, v in data.items()})
+            return cls({k: v if _is_sparse(v) else np.asarray(v) for k, v in data.items()})
         try:
             import pandas as pd
             if isinstance(data, pd.DataFrame):
@@ -42,10 +86,14 @@ class Frame(dict):
         raise TypeError("expected Frame, dict or pandas.DataFrame")
 
     def num_rows(self):
-        return len(next(iter(self.values()))) if self else 0
+        if not self:
+            return 0
+        v = next(iter(self.values()))
+        return v.shape[0] if _is_sparse(v) else len(v)
 
     def rows(self, sl):
-        return Frame({k: v[sl] for k, v in self.items()})
+        """Rows by slice, boolean mask or index array."""
+        return Frame({k: v.tocsr()[sl] if _is_sparse(v) else v[sl] for k, v in self.items()})
 
     def with_column(self, name, values):
         out = Frame(self)
@@ -94,21 +142,38 @@ class LightGBMBooster:
             return np.array([-p, p]) if raw else np.array([1 - p, p])
         return np.asarray(pred[:self.numClasses], dtype=np.float64)
 
+    def _predict_row(self, features, kind):
+        """One row: dense through LGBM_BoosterPredictForMatSingle, a one-row scipy.sparse matrix through
+        LGBM_BoosterPredictForCSRSingle (the SparseVector branch, :510-526)."""
+        if _is_sparse(features):
+            m = _canonical_csr(features)
+            if m.shape[0] != 1:
+                raise ValueError("expected one sparse row, got %d" % m.shape[0])
+            return self._handle().predict_for_csr_single(m.indices, m.data, m.shape[1], kind, self.startIteration, self.numIterations)
+        return self._handle().predict_for_mat_single(features, kind, self.startIteration, self.numIterations)
+
+    def predict_batch(self, X, kind):
+        """Many rows on the GPU: a 2-D array through predict_device, a scipy.sparse matrix through predict_csr_device."""
+        h = self._handle()
+        if _is_sparse(X):
+            return h.predict_csr_device(X, predict_type=kind, start_iteration=self.startIteration, num_iteration=self.numIterations)
+        return h.predict_device(X, kind, self.startIteration, self.numIterations)
+
     def score(self, features, raw, classification):             # :390-398
         kind = capi.PREDICT_RAW_SCORE if raw else capi.PREDICT_NORMAL
-        out = self._handle().predict_for_mat_single(features, kind, self.startIteration, self.numIterations)
+        out = self._predict_row(features, kind)
         return self._pred_to_array(classification, out, raw)
 
     def predictLeaf(self, features):                            # :400-410
-        return self._handle().predict_for_mat_single(features, capi.PREDICT_LEAF_INDEX, self.startIteration, self.numIterations)
+        return self._predict_row(features, capi.PREDICT_LEAF_INDEX)
 
     def featuresShap(self, features):                           # :412-423
-        return self._handle().predict_for_mat_single(features, capi.PREDICT_CONTRIB, self.startIteration, self.numIterations)
+        return self._predict_row(features, capi.PREDICT_CONTRIB)
 
     def score_batch(self, X, raw, classification):
         """transform(): one batched GPU prediction instead of the reference's per-row UDF (SURVEY §8f-2); same values as score()."""
         kind = capi.PREDICT_RAW_SCORE if raw else capi.PREDICT_NORMAL
-        out = self._handle().predict_device(X, kind, self.startIteration, self.numIterations)
+        out = self.predict_batch(X, kind)
         if classification and self.numClasses == 1:
             p = out[:, 0]
             return np.stack([-p, p], axis=1) if raw else np.stack([1 - p, p], axis=1)
@@ -142,7 +207,7 @@ class _ModelBase(Params):
     def saveNativeModel(self, filename, overwrite=True): self.booster.saveNativeModel(filename, overwrite)
     def getNativeModel(self): return self.booster.modelStr
     def getFeatureImportances(self, importance_type="split"): return self.booster.getFeatureImportances(importance_type)
-    def getFeatureShaps(self, vector): return self.booster.featuresShap(np.asarray(vector, dtype=np.float64)).tolist()
+    def getFeatureShaps(self, vector): return self.booster.featuresShap(_row_features(vector)).tolist()
     def getDenseFeatureShaps(self, features): return self.getFeatureShaps(features)          # LightGBMModelMethods.scala:33-36
 
     def getSparseFeatureShaps(self, size, indices, values):                                  # LightGBMModelMethods.scala:38-46
@@ -161,12 +226,10 @@ class _ModelBase(Params):
 
     def _extra_columns(self, out, X):
         if self.get("leafPredictionCol"):
-            out = out.with_column(self.get("leafPredictionCol"), self.booster._handle().predict_device(
-                X, capi.PREDICT_LEAF_INDEX, self.booster.startIteration, self.booster.numIterations))
+            out = out.with_column(self.get("leafPredictionCol"), self.booster.predict_batch(X, capi.PREDICT_LEAF_INDEX))
         if self.get("featuresShapCol"):
             # batched TreeSHAP on the GPU (k_predict_contrib); same values as the per-row featuresShap() the reference's UDF calls
-            out = out.with_column(self.get("featuresShapCol"), self.booster._handle().predict_device(
-                X, capi.PREDICT_CONTRIB, self.booster.startIteration, self.booster.numIterations))
+            out = out.with_column(self.get("featuresShapCol"), self.booster.predict_batch(X, capi.PREDICT_CONTRIB))
         return out
 
     @classmethod
@@ -189,7 +252,7 @@ class LightGBMClassificationModel(_ModelBase):
     def transform(self, data):
         df = Frame.of(data)
         self._update_booster_params()
-        X = np.ascontiguousarray(df[self.get("featuresCol")], dtype=np.float64)
+        X = _batch_features(df[self.get("featuresCol")])
         out = df
         raw = prob = None
         if self.get("rawPredictionCol"):
@@ -219,13 +282,13 @@ class LightGBMRegressionModel(_ModelBase):
     def transform(self, data):
         df = Frame.of(data)
         self._update_booster_params()
-        X = np.ascontiguousarray(df[self.get("featuresCol")], dtype=np.float64)
+        X = _batch_features(df[self.get("featuresCol")])
         out = df.with_column(self.get("predictionCol"), self.booster.score_batch(X, False, False)[:, 0])
         return self._extra_columns(out, X)
 
     def predict(self, features):
         self._update_booster_params()
-        return float(self.booster.score(np.asarray(features, dtype=np.float64), False, False)[0])
+        return float(self.booster.score(_row_features(features), False, False)[0])
 
 
 class LightGBMRankerModel(LightGBMRegressionModel):
@@ -293,6 +356,8 @@ class LightGBMBase(Params):
 
     def _inner_train(self, df, batch_index):     # innerTrain (:440-489)
         num_tasks = self.get("numTasks") if self.get("numTasks") > 0 else self._num_devices()
+        fcol = self.get("featuresCol")
+        df = df.with_column(fcol, resolve_matrix_type(self.get("matrixType"), df[fcol]))      # once per fit, train and validation alike
         vcol = self.get("validationIndicatorCol")
         valid = None
         if vcol and vcol in df:
@@ -334,7 +399,10 @@ class LightGBMBase(Params):
 
     def _make_dataset(self, part, params_str, reference=None):
         X = part[self.get("featuresCol")]
-        ds = capi.Dataset.from_mat(np.ascontiguousarray(X, dtype=np.float64), params_str, reference=reference)
+        if _is_sparse(X):      # CSR from resolve_matrix_type
+            ds = capi.Dataset.from_csr(X.indptr, X.indices, X.data, X.shape[1], params_str, reference=reference)
+        else:
+            ds = capi.Dataset.from_mat(np.ascontiguousarray(X, dtype=np.float64), params_str, reference=reference)
         ds.set_field("label", np.asarray(part[self.get("labelCol")], dtype=np.float32))       # narrowed to f32 (DatasetAggregator.scala:89-92)
         if self.get("weightCol"):
             ds.set_field("weight", np.asarray(part[self.get("weightCol")], dtype=np.float32))
