@@ -42,8 +42,12 @@ const char* LGBM_GetLastError(void);
 /* ---- network (replaces LightGBM's TCP collectives with NCCL over NVLink) ------------------ */
 /* LGB/TrainUtils.scala:279-295: LGBM_NetworkInit(nodes, localListenPort, 120, numNodes).
  * `machines` = "ip:port,ip:port,..."; the rank is the position of the entry whose port equals
- * local_listen_port.  Rank 0 hands its ncclUniqueId to every other rank over one TCP connection
- * to that rank's listen port; afterwards all traffic is NCCL. */
+ * local_listen_port.  Rank 0 connects to every other rank's listen port, collects each rank's process
+ * token and device UUID, and sends back the layout it chose: every rank on its own device -> NCCL (with
+ * rank 0's ncclUniqueId), every rank a thread of this process on one device -> the in-process
+ * same-device collective (at most 16 ranks).  Any other layout returns -1 on every rank with a message
+ * naming the ranks that share a device.  listen_time_out also bounds every same-device collective, and a
+ * rank that calls LGBM_NetworkFree early makes the others' collectives fail ("left the network"). */
 int LGBM_NetworkInit(const char* machines, int local_listen_port, int listen_time_out, int num_machines);
 /* LGB/LightGBMBase.scala:379 */
 int LGBM_NetworkFree(void);

@@ -17,8 +17,11 @@
 #include <sys/types.h>
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
+#include <condition_variable>
 #include <functional>
+#include <random>
 #include <mutex>
 #include <omp.h>
 #include <cstring>
@@ -124,9 +127,183 @@ static void RecvAll(int fd, void* buf, size_t n) {
   while (n) { ssize_t k = ::recv(fd, p, n, 0); if (k <= 0) Fatal("network bootstrap: recv failed"); p += k; n -= k; }
 }
 
-// Replaces LGBM_NetworkInit's TCP mesh (reference call site TrainUtils.scala:279-295): the machine list
-// is only used to agree on ranks and to hand rank 0's ncclUniqueId to the others over one TCP
-// connection each; all training traffic then goes over NCCL (NVLink / NVSwitch).
+// ---- same-device communicator
+// Rank-threads of one process that share one CUDA device (numTasks above the GPU count, the reference's local mode) cannot use NCCL, which
+// refuses two ranks on one device.  They meet in one SameDeviceComm: a collective posts each rank's device pointer into its slot, and the
+// last rank to arrive enqueues the whole collective on the device's shared stream (AcquireStream), then releases the others.  Every rank
+// enqueued its earlier work on that stream before arriving, and its later work after being released, so stream order is the only
+// synchronisation the device needs; no kernel ever waits on another rank.
+struct SameDeviceComm {
+  int world = 0;
+  cudaStream_t stream = nullptr;
+  std::chrono::seconds timeout{120};      // NetworkInit's listen_time_out bounds every wait
+  std::mutex mu;
+  std::condition_variable cv;
+  unsigned long long generation = 0;      // completed collectives
+  int arrived = 0;
+  int left = -1;                          // the first rank that left the network (LGBM_NetworkFree, a timeout or a failed collective)
+  void* buf[kMaxPeers] = {};
+  const void* src[kMaxPeers] = {};
+  size_t bytes[kMaxPeers] = {};
+};
+
+static std::string LeftMessage(int r) {
+  return "rank " + std::to_string(r) + " left the network: the same-device collective cannot complete";
+}
+
+// The rendezvous of one collective.  The last rank to arrive checks that every rank passed the same size, runs enqueue() under the lock and
+// advances the generation; the others wait for that, for a rank leaving, or for the timeout.  A failure marks this rank as left, so that
+// no rank waits for it.
+template <typename Enqueue>
+static void Rendezvous(SameDeviceComm& c, int me, void* buf, const void* src, size_t bytes, Enqueue enqueue) {
+  std::unique_lock<std::mutex> lk(c.mu);
+  if (c.left >= 0) Fatal(LeftMessage(c.left));
+  c.buf[me] = buf; c.src[me] = src; c.bytes[me] = bytes;
+  const unsigned long long gen = c.generation;
+  if (++c.arrived == c.world) {
+    std::string err;
+    for (int r = 0; r < c.world; ++r)
+      if (c.bytes[r] != bytes) err = "same-device collective: rank " + std::to_string(r) + " passed " + std::to_string(c.bytes[r]) + " bytes, rank " + std::to_string(me) + " " + std::to_string(bytes);
+    if (err.empty()) {
+      try { enqueue(); } catch (const std::exception& e) { err = e.what(); }
+    }
+    if (!err.empty()) { c.left = me; c.cv.notify_all(); Fatal(err); }
+    c.arrived = 0;
+    ++c.generation;
+    c.cv.notify_all();
+    return;
+  }
+  const bool woke = c.cv.wait_for(lk, c.timeout, [&] { return c.generation != gen || c.left >= 0; });
+  if (c.generation != gen) return;      // completed, even if a rank left afterwards
+  if (!woke) {
+    c.left = me; c.cv.notify_all();
+    Fatal("rank " + std::to_string(me) + ": a same-device collective timed out after " + std::to_string(c.timeout.count()) + " s waiting for the other ranks");
+  }
+  Fatal(LeftMessage(c.left));
+}
+
+static void LaunchAllReduceSameDevice(void* const* bufs, int R, size_t count, ncclDataType_t type, ncclRedOp_t op, cudaStream_t s) {
+  SameDevicePtrs t{};
+  int vec = 1;
+  for (int r = 0; r < R; ++r) { t.p[r] = bufs[r]; vec &= (reinterpret_cast<uintptr_t>(bufs[r]) & 15) == 0 ? 1 : 0; }
+  int sms = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, CurrentDevice()));
+  const size_t esz = type == ncclUint32 ? 4 : 8;
+  const size_t work = std::max<size_t>(1, count / (16 / esz) + 16 / esz);      // vectors plus the scalar tail
+  const unsigned grid = static_cast<unsigned>(std::min<size_t>((work + 255) / 256, static_cast<size_t>(sms) * 16));
+  const long long n = static_cast<long long>(count);
+  if (type == ncclDouble && op == ncclSum) k_allreduce_same_device<double, RedSum<double>><<<grid, 256, 0, s>>>(t, R, n, vec);
+  else if (type == ncclDouble && op == ncclMax) k_allreduce_same_device<double, RedMax<double>><<<grid, 256, 0, s>>>(t, R, n, vec);
+  else if (type == ncclDouble && op == ncclMin) k_allreduce_same_device<double, RedMin<double>><<<grid, 256, 0, s>>>(t, R, n, vec);
+  else if (type == ncclInt64 && op == ncclSum) k_allreduce_same_device<long long, RedSum<long long>><<<grid, 256, 0, s>>>(t, R, n, vec);
+  else if (type == ncclUint32 && op == ncclMax) k_allreduce_same_device<unsigned, RedMax<unsigned>><<<grid, 256, 0, s>>>(t, R, n, vec);
+  else Fatal("same-device all-reduce: unsupported type / operation");
+  B200_CUDA(cudaGetLastError());
+}
+
+void Network::AllReduce(void* buf, size_t count, ncclDataType_t type, ncclRedOp_t op, cudaStream_t s) const {
+  if (!active) Fatal("collective called without an initialised network (LGBM_NetworkInit)");
+  if (!same_device) { B200_NCCL(ncclAllReduce(buf, buf, count, type, op, comm, s)); return; }
+  SameDeviceComm& c = *same_device;
+  if (s != c.stream) Fatal("same-device collective on a stream other than the device's shared stream");
+  const size_t esz = type == ncclUint32 ? 4 : 8;
+  Rendezvous(c, rank, buf, nullptr, count * esz, [&] { LaunchAllReduceSameDevice(c.buf, c.world, count, type, op, s); });
+}
+
+void Network::AllGather(const void* send, void* recv, size_t bytes, cudaStream_t s) const {
+  if (!active) Fatal("collective called without an initialised network (LGBM_NetworkInit)");
+  if (!same_device) { B200_NCCL(ncclAllGather(send, recv, bytes, ncclChar, comm, s)); return; }
+  SameDeviceComm& c = *same_device;
+  if (s != c.stream) Fatal("same-device collective on a stream other than the device's shared stream");
+  Rendezvous(c, rank, recv, send, bytes, [&] {      // every send into rank 0's recv, then rank 0's recv into the others'
+    char* r0 = static_cast<char*>(c.buf[0]);
+    for (int r = 0; r < c.world; ++r) B200_CUDA(cudaMemcpyAsync(r0 + r * bytes, c.src[r], bytes, cudaMemcpyDeviceToDevice, s));
+    for (int r = 1; r < c.world; ++r) B200_CUDA(cudaMemcpyAsync(c.buf[r], r0, bytes * c.world, cudaMemcpyDeviceToDevice, s));
+  });
+}
+
+// one non-blocking stream per device for every rank-thread of a same-device network; never destroyed
+static std::mutex g_shared_streams_mu;
+static std::map<int, cudaStream_t> g_shared_streams;
+static cudaStream_t SharedStream(int device) {
+  std::lock_guard<std::mutex> lk(g_shared_streams_mu);
+  cudaStream_t& s = g_shared_streams[device];
+  if (!s) B200_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  return s;
+}
+cudaStream_t AcquireStream() {
+  if (t_net.active && t_net.same_device) return t_net.same_device->stream;
+  cudaStream_t s = nullptr;
+  B200_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  return s;
+}
+void ReleaseStream(cudaStream_t s) {
+  if (!s) return;
+  {
+    std::lock_guard<std::mutex> lk(g_shared_streams_mu);
+    for (auto& kv : g_shared_streams) if (kv.second == s) return;
+  }
+  cudaStreamDestroy(s);
+}
+
+// same-device communicators between NetworkInit's rank 0 creating one and every other rank attaching to it
+static std::mutex g_comm_registry_mu;
+static std::map<std::pair<unsigned long long, unsigned long long>, std::shared_ptr<SameDeviceComm>> g_comm_registry;      // (token, sequence)
+
+// A random token of this process, made once when the library loads: it tells rank 0 which ranks are threads of one process (a pid alone
+// does not, pids repeat across containers).
+static const unsigned long long g_process_token = [] {
+  std::random_device rd;
+  return (static_cast<unsigned long long>(rd()) << 32) ^ rd() ^ static_cast<unsigned long long>(std::chrono::steady_clock::now().time_since_epoch().count());
+}();
+static std::atomic<unsigned long long> g_comm_sequence{0};
+
+// what every rank reports to rank 0, and rank 0's decision
+struct RankHello { unsigned long long token; unsigned char uuid[16]; };
+enum : int { kLayoutNccl = 0, kLayoutSameDevice = 1, kLayoutRejected = 2 };
+struct LayoutDecision { int layout; unsigned long long sequence; ncclUniqueId id; char message[1024]; };
+
+static std::string UuidString(const unsigned char* u) {
+  char b[48];
+  std::snprintf(b, sizeof(b), "GPU-%02x%02x%02x%02x-%02x%02x-%02x%02x-%02x%02x-%02x%02x%02x%02x%02x%02x", u[0], u[1], u[2], u[3], u[4], u[5], u[6], u[7], u[8],
+                u[9], u[10], u[11], u[12], u[13], u[14], u[15]);
+  return b;
+}
+
+// Rank 0's choice from every rank's process token and device UUID: NCCL when all devices differ, the same-device communicator when all
+// ranks are threads of one process on one device, a message naming the ranks that share a device otherwise.
+static LayoutDecision DecideLayout(const std::vector<RankHello>& h) {
+  LayoutDecision d{};
+  const int R = static_cast<int>(h.size());
+  std::map<std::string, std::vector<int>> by_device;
+  bool one_process = true;
+  for (int r = 0; r < R; ++r) { by_device[UuidString(h[r].uuid)].push_back(r); one_process &= h[r].token == h[0].token; }
+  if (static_cast<int>(by_device.size()) == R) { d.layout = kLayoutNccl; return d; }
+  if (by_device.size() == 1 && one_process && R <= kMaxPeers) { d.layout = kLayoutSameDevice; return d; }
+  std::string m = "LGBM_NetworkInit: unsupported layout:";
+  for (auto& kv : by_device) {
+    if (kv.second.size() < 2) continue;
+    m += " ranks";
+    for (size_t i = 0; i < kv.second.size(); ++i) m += (i ? "," : " ") + std::to_string(kv.second[i]);
+    m += " share CUDA device " + kv.first + ";";
+  }
+  if (by_device.size() == 1 && one_process) m += " more than " + std::to_string(kMaxPeers) + " ranks on one device;";
+  m += " supported layouts are one device per rank (NCCL) or every rank a thread of one process on one device (same-device collective)";
+  d.layout = kLayoutRejected;
+  std::snprintf(d.message, sizeof(d.message), "%s", m.c_str());
+  return d;
+}
+
+static void SetSocketTimeout(int fd, int sec) {
+  timeval tv{std::max(sec, 1), 0};
+  setsockopt(fd, SOL_SOCKET, SO_RCVTIMEO, &tv, sizeof(tv));
+  setsockopt(fd, SOL_SOCKET, SO_SNDTIMEO, &tv, sizeof(tv));
+}
+
+// Replaces LGBM_NetworkInit's TCP mesh (reference call site TrainUtils.scala:279-295): the machine list is only used to agree on ranks.
+// Rank 0 connects to every other rank, collects each rank's process token and device UUID, decides the layout (DecideLayout) and sends
+// the decision — with its ncclUniqueId when NCCL was chosen — back over the same connections.  NCCL training traffic then goes over
+// NVLink / NVSwitch; a same-device network never leaves the process.  A rejected layout fails on every rank with the same message.
 void NetworkInit(const char* machines, int local_listen_port, int listen_time_out_sec, int num_machines) {
   NetworkFree();
   if (num_machines <= 1) return;
@@ -155,9 +332,19 @@ void NetworkInit(const char* machines, int local_listen_port, int listen_time_ou
   }
   EnsureDevice();
   const auto deadline = std::chrono::steady_clock::now() + std::chrono::seconds(std::max(listen_time_out_sec, 1));
-  ncclUniqueId id;
+  RankHello mine{};
+  mine.token = g_process_token;
+  {
+    cudaDeviceProp prop;
+    B200_CUDA(cudaGetDeviceProperties(&prop, t_device));
+    std::memcpy(mine.uuid, prop.uuid.bytes, 16);
+  }
+  LayoutDecision dec{};
+  std::shared_ptr<SameDeviceComm> sd;
   if (rank == 0) {
-    B200_NCCL(ncclGetUniqueId(&id));
+    struct Conns { std::vector<int> fd; ~Conns() { for (int f : fd) ::close(f); } } conns;
+    std::vector<RankHello> hello(num_machines);
+    hello[0] = mine;
     for (int r = 1; r < num_machines; ++r) {
       int fd = -1;
       while (true) {
@@ -174,10 +361,29 @@ void NetworkInit(const char* machines, int local_listen_port, int listen_time_ou
         if (std::chrono::steady_clock::now() > deadline) Fatal("network bootstrap: cannot reach " + nodes[r].first + ":" + std::to_string(nodes[r].second));
         std::this_thread::sleep_for(std::chrono::milliseconds(20));
       }
-      SendAll(fd, &id, sizeof(id));
+      conns.fd.push_back(fd);
+      SetSocketTimeout(fd, listen_time_out_sec);
+      RecvAll(fd, &hello[r], sizeof(RankHello));
+    }
+    dec = DecideLayout(hello);
+    if (dec.layout == kLayoutNccl) B200_NCCL(ncclGetUniqueId(&dec.id));
+    if (dec.layout == kLayoutSameDevice) {      // created before any rank hears the decision, so every rank finds it
+      sd = std::make_shared<SameDeviceComm>();
+      sd->world = num_machines;
+      sd->stream = SharedStream(t_device);
+      sd->timeout = std::chrono::seconds(std::max(listen_time_out_sec, 1));
+      dec.sequence = ++g_comm_sequence;
+      std::lock_guard<std::mutex> lk(g_comm_registry_mu);
+      g_comm_registry[{g_process_token, dec.sequence}] = sd;
+    }
+    struct Unregister {      // once every rank attached, or when the bootstrap fails; the ranks hold the communicator
+      unsigned long long seq;
+      ~Unregister() { if (seq) { std::lock_guard<std::mutex> lk(g_comm_registry_mu); g_comm_registry.erase({g_process_token, seq}); } }
+    } unregister{dec.sequence};
+    for (int fd : conns.fd) {      // the ack comes after the rank attached to a same-device communicator
+      SendAll(fd, &dec, sizeof(dec));
       char ack = 0;
       RecvAll(fd, &ack, 1);
-      ::close(fd);
     }
   } else {
     int ls = ::socket(AF_INET, SOCK_STREAM, 0);
@@ -193,19 +399,40 @@ void NetworkInit(const char* machines, int local_listen_port, int listen_time_ou
     timeval tv{std::max(listen_time_out_sec, 1), 0};
     if (::select(ls + 1, &fds, nullptr, nullptr, &tv) <= 0) { ::close(ls); Fatal("network bootstrap: timed out waiting for rank 0"); }
     int fd = ::accept(ls, nullptr, nullptr);
-    if (fd < 0) { ::close(ls); Fatal("network bootstrap: accept failed"); }
-    RecvAll(fd, &id, sizeof(id));
+    ::close(ls);
+    if (fd < 0) Fatal("network bootstrap: accept failed");
+    struct Conn { int fd; ~Conn() { ::close(fd); } } conn{fd};
+    SetSocketTimeout(fd, listen_time_out_sec);
+    SendAll(fd, &mine, sizeof(mine));
+    RecvAll(fd, &dec, sizeof(dec));
+    if (dec.layout == kLayoutSameDevice) {
+      std::lock_guard<std::mutex> lk(g_comm_registry_mu);
+      auto it = g_comm_registry.find({g_process_token, dec.sequence});
+      if (it == g_comm_registry.end()) Fatal("network bootstrap: rank 0's same-device communicator is not in this process");
+      sd = it->second;
+    }
     char ack = 1;
     SendAll(fd, &ack, 1);
-    ::close(fd);
-    ::close(ls);
+  }
+  if (dec.layout == kLayoutRejected) Fatal(std::string(dec.message, strnlen(dec.message, sizeof(dec.message))));
+  if (sd) {
+    t_net.active = true; t_net.rank = rank; t_net.world = num_machines; t_net.same_device = sd;
+    return;
   }
   ncclComm_t comm;
-  B200_NCCL(ncclCommInitRank(&comm, num_machines, id, rank));
+  B200_NCCL(ncclCommInitRank(&comm, num_machines, dec.id, rank));
   t_net.active = true; t_net.rank = rank; t_net.world = num_machines; t_net.comm = comm;
 }
+// Leaving a same-device network marks the rank as left: ranks waiting in a collective, or entering one later, fail instead of waiting for
+// it.  Ranks that already completed every collective are not affected.
 void NetworkFree() {
   if (t_net.active && t_net.comm) { ncclCommDestroy(t_net.comm); }
+  if (t_net.same_device) {
+    SameDeviceComm& c = *t_net.same_device;
+    std::lock_guard<std::mutex> lk(c.mu);
+    if (c.left < 0) c.left = t_net.rank;
+    c.cv.notify_all();
+  }
   t_net = Network();
 }
 
@@ -213,7 +440,7 @@ void AllReduceHost(double* v, int n, ncclRedOp_t op, cudaStream_t s) {
   if (!Net().active) return;
   DevBuf<double> d; d.Alloc(n);
   d.Upload(v, n, s);
-  B200_NCCL(ncclAllReduce(d.p, d.p, n, ncclDouble, op, Net().comm, s));
+  Net().AllReduce(d.p, n, ncclDouble, op, s);
   d.Download(v, n, s);
   B200_CUDA(cudaStreamSynchronize(s));
 }
@@ -221,7 +448,7 @@ void AllReduceHost(double* v, int n, ncclRedOp_t op, cudaStream_t s) {
 // =============================================================================== dataset
 Dataset::~Dataset() {
   ReleaseIngestStaging();
-  if (stream) cudaStreamDestroy(stream);
+  ReleaseStream(stream);
 }
 
 template <typename T>
@@ -271,7 +498,7 @@ static FeatureBins UnpackMapper(const double* r) {
 std::unique_ptr<Dataset> Dataset::NewShell(int nrow, int ncol, const char* params) {
   std::unique_ptr<Dataset> d(new Dataset());
   d->device = CurrentDevice();
-  B200_CUDA(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
+  d->stream = AcquireStream();
   d->num_data = nrow; d->num_total_features = ncol;
   d->cfg.Parse(params);
   return d;
@@ -335,7 +562,7 @@ void Dataset::SetMappers(const Dataset* reference, bool may_bundle, Sample sampl
     for (int f = f0; f < f1; ++f) PackMapper(mappers[f], &send[static_cast<size_t>(f - f0) * kMapperRecord], slots);
     DevBuf<double> ds, dr; ds.Alloc(send.size()); dr.Alloc(recv.size());
     ds.Upload(send.data(), send.size(), stream);
-    B200_NCCL(ncclAllGather(ds.p, dr.p, send.size(), ncclDouble, Net().comm, stream));
+    Net().AllGather(ds.p, dr.p, send.size() * sizeof(double), stream);
     dr.Download(recv.data(), recv.size(), stream);
     B200_CUDA(cudaStreamSynchronize(stream));
     for (int f = 0; f < F; ++f) {
@@ -1092,14 +1319,14 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   if (train->label.empty()) Fatal("label should not be empty for training");
   K = obj_->NumTreePerIteration();
   parallel_ = Net().active && Net().world > 1;
+  same_device_ = parallel_ && Net().same_device != nullptr;
   cfg.num_machines = parallel_ ? Net().world : 1;
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
-      cudaStream_t ts;
-      B200_CUDA(cudaStreamCreateWithFlags(&ts, cudaStreamNonBlocking));
-      AllReduceHost(&npos, 1, ncclSum, ts);
-      B200_CUDA(cudaStreamDestroy(ts));
+      cudaStream_t ts = AcquireStream();
+      try { AllReduceHost(&npos, 1, ncclSum, ts); } catch (...) { ReleaseStream(ts); throw; }
+      ReleaseStream(ts);
     }
     if (!(npos > 0)) { balanced_bagging_ = false; bagging_ = cfg.bagging_freq > 0 && cfg.bagging_fraction < 1.0; }
   }
@@ -1129,7 +1356,7 @@ Booster::~Booster() {
   if (leaves_host_) cudaFreeHost(leaves_host_);
   if (ev_a_) cudaEventDestroy(ev_a_);
   if (ev_b_) cudaEventDestroy(ev_b_);
-  if (stream_) cudaStreamDestroy(stream_);
+  ReleaseStream(stream_);
 }
 
 void Booster::InitTraining() {
@@ -1138,7 +1365,7 @@ void Booster::InitTraining() {
   cudaDeviceProp prop;
   B200_CUDA(cudaGetDeviceProperties(&prop, device_));
   num_sms_ = prop.multiProcessorCount;
-  B200_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+  stream_ = AcquireStream();
   B200_CUDA(cudaEventCreate(&ev_a_)); B200_CUDA(cudaEventCreate(&ev_b_));
   // leaf passes gather single 32-byte sectors: ask L2 not to fetch the neighbouring sector from DRAM on a miss (default 64 B).
   // A hint for the sparse leaf passes; streamed passes read whole sectors anyway.
@@ -1390,6 +1617,9 @@ struct PeerInfo {
   cudaIpcMemHandle_t ipc[3];
 };
 void Booster::SetupPeerReduce() {
+  // Ranks on one device take the same-device all-reduce whatever B200GBM_FUSED_REDUCE asks: the peer-memory modes spin on flags that
+  // other ranks' kernels raise, and those kernels run after this rank's on the shared stream.
+  if (same_device_) return;
   const char* env = std::getenv("B200GBM_FUSED_REDUCE");
   const int R = Net().world, me = Net().rank;
   mailbox_.Alloc(static_cast<size_t>(kMaxPeers) * 2); mailbox_.Zero(stream_);
@@ -1413,7 +1643,7 @@ void Booster::SetupPeerReduce() {
   {
     DevBuf<unsigned char> ds, dr; ds.Alloc(sizeof(PeerInfo)); dr.Alloc(sizeof(PeerInfo) * R);
     B200_CUDA(cudaMemcpyAsync(ds.p, &mine, sizeof(PeerInfo), cudaMemcpyHostToDevice, stream_));
-    B200_NCCL(ncclAllGather(ds.p, dr.p, sizeof(PeerInfo), ncclChar, Net().comm, stream_));
+    Net().AllGather(ds.p, dr.p, sizeof(PeerInfo), stream_);
     B200_CUDA(cudaMemcpyAsync(all.data(), dr.p, sizeof(PeerInfo) * R, cudaMemcpyDeviceToHost, stream_));
     B200_CUDA(cudaStreamSynchronize(stream_));
   }
@@ -1518,7 +1748,7 @@ void Booster::RenewTreeOutput(int k, double rf_pred) {
     k_renew_cdf<<<L, 1024, 0, s>>>(ctrl, rn_seg_.p, rn_pos_a_.p, rn_row_.p, wptr, rn_cdf_.p);
     k_renew_weighted<<<lgrid, 128, 0, s>>>(ctrl, rn_seg_.p, rn_pos_a_.p, rn_res_.p, rn_cdf_.p, obj_->RenewAlpha(), out, has);
   }
-  if (parallel_) B200_NCCL(ncclAllReduce(out, out, 2 * static_cast<size_t>(L), ncclDouble, ncclSum, Net().comm, s));
+  if (parallel_) Net().AllReduce(out, 2 * static_cast<size_t>(L), ncclDouble, ncclSum, s);
   k_renew_apply<<<lgrid, 128, 0, s>>>(ctrl, tree_dev_, out, has, parallel_ ? 1 : 0);
   B200_CUDA(cudaGetLastError());
   timing.launches += wptr ? 7 : 6;
@@ -1531,23 +1761,38 @@ void Booster::RenewTreeOutput(int k, double rf_pred) {
 //   full copy     every storage column (kernels.cuh: k_tiles_to_columns), if it fits
 //   column cache  otherwise a pool of as many column slots as fit, filled between trees with the columns the trees split on
 //                 (UpdateColumnCache); B200GBM_COLUMN_CACHE_COLUMNS=k forces this mode with at most k slots
+// With R ranks on one device (same-device network) all of them reach this point at their first tree, when every rank's training buffers
+// exist: they measure the free memory before any of them allocates a copy, and each takes at most 1/R of what lies above the reserve.
 void Booster::EnsureColumnCopy() {
   if (cols_tried_) return;
   cols_tried_ = true;
   const Dataset& d = *train;
   const char* env = std::getenv("B200GBM_COLUMN_COPY");
-  if ((env && std::atoi(env) == 0) || d.nfn == 0 || d.num_data == 0) return;
+  if ((env && std::atoi(env) == 0) || d.nfn == 0) return;      // the same on every rank: the ranks share the bin layout and the process
+  size_t free_b = 0, total_b = 0;
+  const bool mem_ok = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
+  if (!mem_ok) cudaGetLastError();
+  size_t share = 1;
+  if (same_device_) {
+    double arrived = 0.0;
+    AllReduceHost(&arrived, 1, ncclSum, stream_);      // every rank built its buffers
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
+    double f = mem_ok ? static_cast<double>(free_b) : 0.0;
+    AllReduceHost(&f, 1, ncclMin, stream_);            // every rank measured before any allocates
+    free_b = static_cast<size_t>(f);
+    share = static_cast<size_t>(Net().world);
+  }
+  if (!mem_ok || d.num_data == 0) return;
   const char* force = std::getenv("B200GBM_COLUMN_CACHE_COLUMNS");
   const size_t stride = (static_cast<size_t>(d.num_data) + 255) & ~static_cast<size_t>(255);
   const int ncols = d.num_tiles * 32;
   const size_t need = static_cast<size_t>(ncols) * stride;
-  size_t free_b = 0, total_b = 0;
-  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); return; }
   const size_t reserve = std::max<size_t>(static_cast<size_t>(8) << 30, total_b / 10);
-  const bool full = !force && free_b >= need + reserve;
+  const size_t spare = free_b > reserve ? (free_b - reserve) / share : 0;
+  const bool full = !force && spare >= need;
   int slots = ncols;
   if (!full) {
-    slots = static_cast<int>(std::min<size_t>(d.num_columns, free_b > reserve ? (free_b - reserve) / stride : 0));
+    slots = static_cast<int>(std::min<size_t>(d.num_columns, spare / stride));
     if (force) slots = std::min(slots, std::max(0, std::atoi(force)));
     if (slots == 0) return;
   }
@@ -1677,10 +1922,10 @@ void Booster::TrainOneTree(int k, HostTree* out) {
   nvtxRangePushA("b200gbm:K3 quantize + C1 root sums");
   B200_CUDA(cudaMemsetAsync(&ctrl->absmax_bits[0], 0, 8, s));
   k_absmax<<<egrid, 256, 0, s>>>(g, h, n, ctrl);
-  if (parallel_) B200_NCCL(ncclAllReduce(&ctrl->absmax_bits[0], &ctrl->absmax_bits[0], 2, ncclUint32, ncclMax, Net().comm, s));
+  if (parallel_) Net().AllReduce(&ctrl->absmax_bits[0], 2, ncclUint32, ncclMax, s);
   k_set_scale<<<1, 1, 0, s>>>(ctrl, const_hessian_ ? 1 : 0, 1.0);
   k_quantize<<<egrid, 256, 0, s>>>(g, h, n, qgh_.p, ctrl, const_hessian_ ? 1 : 0, use_bag_ ? in_bag_.p : nullptr, bag_count_);
-  if (parallel_) B200_NCCL(ncclAllReduce(&ctrl->root_q[0], &ctrl->root_q[0], 3, ncclInt64, ncclSum, Net().comm, s));
+  if (parallel_) Net().AllReduce(&ctrl->root_q[0], 3, ncclInt64, ncclSum, s);
   ResetFeaturesByTree();
   if (use_bag_)      // the root leaf is the ascending in-bag row list (SetBaggingData); partitions then ping-pong idx0/idx1 as usual
     B200_CUDA(cudaMemcpyAsync(idx0_.p, bag_idx_.p, static_cast<size_t>(bag_count_) * sizeof(int), cudaMemcpyDeviceToDevice, s));
@@ -1743,7 +1988,7 @@ void Booster::TrainOneTree(int k, HostTree* out) {
         k_allreduce_p2p<<<agrid, 256, 0, s>>>(ctrl, peers_, slot_elems_, epoch_, peer_flags_.p + 48);
         timing.launches += 1;
       } else if (parallel_) {
-        B200_NCCL(ncclAllReduce(H_.p, H_.p, slot_elems_, ncclInt64, ncclSum, Net().comm, s));   // C2
+        Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
       }
       mark();
       if (d.nw > 0) {
@@ -2244,7 +2489,7 @@ void Booster::UploadForest() {
     }
     for (int i = 0; i < tr.num_leaves; ++i) { lv.push_back(tr.leaf_value[i]); lcnt.push_back(tr.leaf_count[i]); }
   }
-  if (!stream_) B200_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+  if (!stream_) stream_ = AcquireStream();
   auto up_i = [&](DevBuf<int>& d, std::vector<int>& h) { d.Alloc(std::max<size_t>(h.size(), 1)); if (!h.empty()) d.Upload(h.data(), h.size(), stream_); };
   auto up_d = [&](DevBuf<double>& d, std::vector<double>& h) { d.Alloc(std::max<size_t>(h.size(), 1)); if (!h.empty()) d.Upload(h.data(), h.size(), stream_); };
   up_i(f.tree_offset, toff); up_i(f.leaf_offset, loff); up_i(f.num_leaves, nl); up_i(f.split_feature, sf); up_i(f.decision_type, dt);

@@ -38,10 +38,19 @@ namespace b200gbm {
 [[noreturn]] inline void Fatal(const std::string& m) { throw std::runtime_error(m); }
 
 // ---- per-thread device + network state -------------------------------------------------------
+struct SameDeviceComm;          // engine.cu: rank-threads of one process on one device
+// The data-parallel communicator of one rank.  NetworkInit picks the backend from the layout it observes: NCCL when every rank has its
+// own device, the same-device communicator when every rank is a thread of this process on one device.  Every collective of the engine
+// goes through AllReduce / AllGather, which make the same NCCL calls as before on the NCCL backend.
 struct Network {
   bool active = false;
   int rank = 0, world = 1;
   ncclComm_t comm = nullptr;
+  std::shared_ptr<SameDeviceComm> same_device;
+  // in place on `count` elements of buf; (type, op) in (double: sum / max / min), (int64: sum), (uint32: max)
+  void AllReduce(void* buf, size_t count, ncclDataType_t type, ncclRedOp_t op, cudaStream_t s) const;
+  // recv[r * bytes, (r + 1) * bytes) = rank r's send, on every rank
+  void AllGather(const void* send, void* recv, size_t bytes, cudaStream_t s) const;
 };
 Network& Net();                 // thread-local
 int CurrentDevice();            // thread-local CUDA ordinal (selects on first use)
@@ -51,6 +60,11 @@ int DeviceSMs();                // multiprocessor count of CurrentDevice() (grid
 void NetworkInit(const char* machines, int local_listen_port, int listen_time_out_sec, int num_machines);
 void NetworkFree();
 void AllReduceHost(double* v, int n, ncclRedOp_t op, cudaStream_t s);      // small host-value collectives, staged through device memory
+// The stream of a new dataset or booster on CurrentDevice().  With the same-device communicator it is the one process-wide stream of
+// the device, so the ranks' kernels run one after another (k_partition's cooperative grid needs the whole device) and the collectives
+// are ordered by the stream alone; that stream lives until the process ends, so objects may outlive LGBM_NetworkFree.
+cudaStream_t AcquireStream();
+void ReleaseStream(cudaStream_t s);      // destroys a stream of AcquireStream unless it is a shared one
 
 template <typename T>
 struct DevBuf {
@@ -201,7 +215,7 @@ class Booster {
   int64_t PredictBatchCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
                           int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out);
   double last_predict_ms = 0.0;
-  void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = fused_ ? 1 : (p2p_allreduce_ ? 2 : 0); out4[3] = const_hessian_ ? 1 : 0; }
+  void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = fused_ ? 1 : (p2p_allreduce_ ? 2 : (same_device_ ? 3 : 0)); out4[3] = const_hessian_ ? 1 : 0; }
   std::string SaveModelToString(int start_iteration, int num_iteration, int importance_type) const;
   std::string DumpModelJson(int start_iteration, int num_iteration) const;
 
@@ -231,6 +245,7 @@ class Booster {
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool parallel_ = false;
+  bool same_device_ = false;            // parallel_ over the same-device communicator: all ranks are threads of this process on this device
   bool const_hessian_ = false;
   bool has_init_score_ = false;
   double shrinkage_ = 0.1;

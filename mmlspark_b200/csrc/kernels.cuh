@@ -1319,6 +1319,54 @@ k_allreduce_p2p(const TreeCtrl* __restrict__ ctrl, PeerTables pt, size_t elems, 
   __syncthreads();
 }
 
+// ---------------------------------------------------------------- same-device all-reduce (rank-threads of one process on one device)
+// Every rank's buffer is on this device, so one launch, enqueued by the last rank to reach the collective (engine.cu SameDeviceComm), does
+// the whole all-reduce: element i of every buffer becomes Op over the R buffers' element i, accumulated in rank order.  The order never
+// changes, so double sums are deterministic; for R = 2 they equal NCCL's a + b bit for bit.  Each thread owns whole 16-byte vectors (the
+// per-split C2 histogram is 1-2 MB of int64), so reading and then overwriting all R copies in place needs no barrier.  The rank loops are
+// unrolled to kMaxPeers with a guard, so the pointer table stays in the parameter bank instead of a local copy.
+struct SameDevicePtrs { void* p[kMaxPeers]; };
+template <typename T> struct RedSum { __device__ __forceinline__ static T f(T a, T b) { return a + b; } };
+template <typename T> struct RedMax { __device__ __forceinline__ static T f(T a, T b) { return b > a ? b : a; } };
+template <typename T> struct RedMin { __device__ __forceinline__ static T f(T a, T b) { return b < a ? b : a; } };
+// fmax / fmin for doubles (the host values reduced this way are never NaN): the compare-and-select form spills at -O3
+template <> struct RedMax<double> { __device__ __forceinline__ static double f(double a, double b) { return fmax(a, b); } };
+template <> struct RedMin<double> { __device__ __forceinline__ static double f(double a, double b) { return fmin(a, b); } };
+template <typename T> struct alignas(16) Vec16 { T v[16 / sizeof(T)]; };
+
+// vec: every buffer is 16-byte aligned, so count / (16 / sizeof(T)) vectors go as 16-byte loads and stores and the rest as scalars
+template <typename T, typename Op>
+__global__ void __launch_bounds__(256)
+k_allreduce_same_device(SameDevicePtrs bufs, int R, long long count, int vec) {
+  constexpr int V = 16 / sizeof(T);
+  const long long nvec = vec ? count / V : 0;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long tid = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  for (long long i = tid; i < nvec; i += stride) {
+    Vec16<T> acc = reinterpret_cast<const Vec16<T>*>(bufs.p[0])[i];
+#pragma unroll
+    for (int r = 1; r < kMaxPeers; ++r) {
+      if (r < R) {
+        const Vec16<T> x = reinterpret_cast<const Vec16<T>*>(bufs.p[r])[i];
+#pragma unroll
+        for (int k = 0; k < V; ++k) acc.v[k] = Op::f(acc.v[k], x.v[k]);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < kMaxPeers; ++r)
+      if (r < R) reinterpret_cast<Vec16<T>*>(bufs.p[r])[i] = acc;
+  }
+  for (long long i = nvec * V + tid; i < count; i += stride) {
+    T acc = static_cast<const T*>(bufs.p[0])[i];
+#pragma unroll
+    for (int r = 1; r < kMaxPeers; ++r)
+      if (r < R) acc = Op::f(acc, static_cast<const T*>(bufs.p[r])[i]);
+#pragma unroll
+    for (int r = 0; r < kMaxPeers; ++r)
+      if (r < R) static_cast<T*>(bufs.p[r])[i] = acc;
+  }
+}
+
 // leaf choice by warp 0: ArgMax over leaves with SplitInfo::operator> (gain desc, real feature asc, first index), stop on gain <= 0
 
 // argmax over features per leaf (gain desc, real feature index asc), then over leaves
