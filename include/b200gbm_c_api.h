@@ -60,6 +60,18 @@ int LGBM_DatasetCreateFromMat(const void* data, int data_type, int32_t nrow, int
 int LGBM_DatasetCreateFromCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data,
                               int data_type, int64_t nindptr, int64_t nelem, int64_t num_col,
                               const char* parameters, const DatasetHandle reference, DatasetHandle* out);
+/* [UPSTREAM] LightGBM's LGBM_DatasetCreateFromMats: one dataset from nmat row parts that count as one matrix (part 0's
+ * rows, then part 1's, ...).  Each data[i] holds nrow[i] rows and may be a host or a device pointer.  Bins, bundles and
+ * mappers, and so every model trained on it, are bit-identical to LGBM_DatasetCreateFromMat on the concatenation; no host
+ * copy of the parts is made.  Rejects nmat < 1, a part without rows and null pointers. */
+int LGBM_DatasetCreateFromMats(int32_t nmat, const void** data, int data_type, int32_t* nrow, int32_t ncol, int is_row_major,
+                               const char* parameters, const DatasetHandle reference, DatasetHandle* out);
+/* The same for nparts host CSR parts (no upstream equivalent): part i is indptr[i] (nindptr[i] entries, need not start at
+ * 0), indices[i] and data[i] (nelem[i] stored values).  Equal to LGBM_DatasetCreateFromCSR on the concatenated rows; every
+ * part is checked as LGBM_DatasetCreateFromCSR checks its input. */
+int B200GBM_DatasetCreateFromCSRs(int32_t nparts, const void** indptr, int indptr_type, const int32_t** indices,
+                                  const void** data, int data_type, const int64_t* nindptr, const int64_t* nelem,
+                                  int64_t num_col, const char* parameters, const DatasetHandle reference, DatasetHandle* out);
 /* LightGBM streaming ingestion (not used by the reference revision; offered as the bulk path of
  * SURVEY.md §8f-1): create from a column-wise sample, then push row blocks (host or device). */
 int LGBM_DatasetCreateFromSampledColumn(double** sample_data, int** sample_indices, int32_t ncol,

@@ -172,6 +172,49 @@ class Dataset:
         return cls(h)
 
     @classmethod
+    def from_mats(cls, parts, params="", reference=None):
+        """One dataset from a list of 2-D row-major arrays that count as one matrix (LGBM_DatasetCreateFromMats): the same bins and
+        models as from_mat on their concatenation, without making it.  Every part is float32 or float64, C-contiguous, of one dtype
+        and one column count."""
+        parts = [np.asarray(X) for X in parts]
+        if not parts:
+            raise LightGBMError("from_mats needs at least one part")
+        for X in parts:
+            if X.ndim != 2 or X.dtype != parts[0].dtype or X.shape[1] != parts[0].shape[1] or not X.flags.c_contiguous:
+                raise LightGBMError("from_mats: every part must be a C-contiguous 2-D array of one dtype and one column count")
+        code = _np_dtype_code(parts[0])
+        ptrs = (C.c_void_p * len(parts))(*[X.ctypes.data for X in parts])
+        nrow = np.array([X.shape[0] for X in parts], dtype=np.int32)
+        h = C.c_void_p()
+        check(load().LGBM_DatasetCreateFromMats(C.c_int32(len(parts)), ptrs, C.c_int(code), _ptr(nrow), C.c_int32(parts[0].shape[1]), C.c_int(1),
+                                                params.encode(), reference.handle if reference is not None else None, C.byref(h)))
+        return cls(h)
+
+    @classmethod
+    def from_csrs(cls, parts, num_col, params="", reference=None):
+        """One dataset from a list of CSR row parts (B200GBM_DatasetCreateFromCSRs): scipy.sparse matrices or (indptr, indices, data)
+        tuples, each indptr starting anywhere.  The same bins and models as from_csr on the concatenated rows."""
+        ips, ixs, vals = [], [], []
+        for p in parts:
+            if not isinstance(p, tuple) and hasattr(p, "tocsr"):      # scipy.sparse
+                m = p.tocsr()
+                p = (m.indptr, m.indices, m.data)
+            ip, ix, v = p
+            ips.append(np.ascontiguousarray(ip, dtype=np.int64))
+            ixs.append(np.ascontiguousarray(ix, dtype=np.int32))
+            vals.append(np.ascontiguousarray(v, dtype=np.float64))
+        if not ips:
+            raise LightGBMError("from_csrs needs at least one part")
+        n = len(ips)
+        h = C.c_void_p()
+        check(load().B200GBM_DatasetCreateFromCSRs(C.c_int32(n), (C.c_void_p * n)(*[a.ctypes.data for a in ips]), C.c_int(DTYPE_INT64),
+                                                   (C.c_void_p * n)(*[a.ctypes.data for a in ixs]), (C.c_void_p * n)(*[a.ctypes.data for a in vals]),
+                                                   C.c_int(DTYPE_FLOAT64), _ptr(np.array([len(a) for a in ips], dtype=np.int64)),
+                                                   _ptr(np.array([len(a) for a in vals], dtype=np.int64)), C.c_int64(num_col), params.encode(),
+                                                   reference.handle if reference is not None else None, C.byref(h)))
+        return cls(h)
+
+    @classmethod
     def from_sampled_columns(cls, sample, num_total_row, params=""):
         """sample: [num_sample_row][ncol] float64 (dense sample of rows); zeros are dropped per column as LightGBM expects."""
         sample = np.ascontiguousarray(sample, dtype=np.float64)

@@ -53,14 +53,28 @@ int LGBM_NetworkFree(void) {
 int LGBM_DatasetCreateFromMat(const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, const char* parameters,
                               const DatasetHandle reference, DatasetHandle* out) {
   API_BEGIN();
-  *out = Dataset::CreateFromMat(data, data_type, nrow, ncol, is_row_major, parameters, static_cast<const Dataset*>(reference));
+  *out = Dataset::CreateFromMats(1, &data, data_type, &nrow, ncol, is_row_major, parameters, static_cast<const Dataset*>(reference));
+  API_END();
+}
+int LGBM_DatasetCreateFromMats(int32_t nmat, const void** data, int data_type, int32_t* nrow, int32_t ncol, int is_row_major,
+                               const char* parameters, const DatasetHandle reference, DatasetHandle* out) {
+  API_BEGIN();
+  *out = Dataset::CreateFromMats(nmat, data, data_type, nrow, ncol, is_row_major, parameters, static_cast<const Dataset*>(reference));
   API_END();
 }
 int LGBM_DatasetCreateFromCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
                               int64_t nelem, int64_t num_col, const char* parameters, const DatasetHandle reference, DatasetHandle* out) {
   API_BEGIN();
-  *out = Dataset::CreateFromCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, num_col, parameters,
-                                static_cast<const Dataset*>(reference));
+  *out = Dataset::CreateFromCSRs(1, &indptr, indptr_type, &indices, &data, data_type, &nindptr, &nelem, num_col, parameters,
+                                 static_cast<const Dataset*>(reference));
+  API_END();
+}
+int B200GBM_DatasetCreateFromCSRs(int32_t nparts, const void** indptr, int indptr_type, const int32_t** indices, const void** data, int data_type,
+                                  const int64_t* nindptr, const int64_t* nelem, int64_t num_col, const char* parameters, const DatasetHandle reference,
+                                  DatasetHandle* out) {
+  API_BEGIN();
+  *out = Dataset::CreateFromCSRs(nparts, indptr, indptr_type, indices, data, data_type, nindptr, nelem, num_col, parameters,
+                                 static_cast<const Dataset*>(reference));
   API_END();
 }
 int LGBM_DatasetCreateFromSampledColumn(double** sample_data, int** sample_indices, int32_t ncol, const int* num_per_col, int32_t num_sample_row,

@@ -758,65 +758,77 @@ static void LaunchBin(const T* X, long long nrow, int ncol, int row_major, long 
   B200_CUDA(cudaGetLastError());
 }
 
-void Dataset::BinBlock(const void* data, bool on_device, int data_type, int is_row_major, long long n, long long start_row) {
+void Dataset::BinBlock(const std::vector<MatPart>& parts, int data_type, int is_row_major, long long start_row) {
   NvtxRange nvtx("b200gbm:K0 bin rows (H2D + value->bin)");
   const int F = num_total_features;
+  long long n = 0, host_rows = 0;
+  for (const MatPart& p : parts) { n += p.nrow; if (!p.on_device) host_rows += p.nrow; }
   if (start_row < 0 || start_row + n > num_data) Fatal("row block out of range");
   {
     std::lock_guard<std::mutex> lock(block_bound_mu_);
     block_bound_.Free();      // a bound of earlier bins would let K4 overflow a cell
   }
-  ForEachDeviceBlock(data, on_device, data_type, is_row_major, n, [&](const void* x, long long rows, long long ld, long long r0) {
+  ForEachDeviceBlock(parts, data_type, is_row_major, [&](const void* x, long long rows, long long ld, long long r0) {
     if (data_type == 0) LaunchBin<float>(static_cast<const float*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
     else LaunchBin<double>(static_cast<const double*>(x), rows, F, is_row_major, ld, *this, start_row + r0, stream);
   });
-  if (on_device) return;
-  ingest_rows_done_ += n;
+  if (host_rows == 0) return;
+  ingest_rows_done_ += host_rows;
   if (ingest_rows_done_ >= num_data) ReleaseIngestStaging();
 }
 
 template <typename Fn>
-void Dataset::ForEachDeviceBlock(const void* data, bool on_device, int data_type, int is_row_major, long long n, Fn fn) {
+void Dataset::ForEachDeviceBlock(const std::vector<MatPart>& parts, int data_type, int is_row_major, Fn fn) {
   const int F = num_total_features;
   const size_t esz = data_type == 0 ? 4 : 8;
-  if (on_device) {
-    fn(data, n, is_row_major ? F : n, 0LL);
-    B200_CUDA(cudaStreamSynchronize(stream));
-    return;
-  }
-  // host source: stream row chunks through two device buffers, copy of chunk i+1 overlaps binning of chunk i.  The staging
-  // buffers, copy stream and events persist across LGBM_DatasetPushRows calls (a cudaMalloc/cudaFree pair per call costs as much
-  // as the copy itself) and are released when the last row has arrived.
+  // host parts: stream row chunks through two device buffers, copy of chunk i+1 overlaps binning of chunk i, also where chunk i is
+  // the last of one part and chunk i+1 the first of the next.  The staging buffers, copy stream and events persist across
+  // LGBM_DatasetPushRows calls (a cudaMalloc/cudaFree pair per call costs as much as the copy itself) and are released when the
+  // last row has arrived.
   const size_t kStageBytes = 256u << 20;
-  long long chunk = std::max<long long>(1, std::min<long long>(n, static_cast<long long>(kStageBytes) / (static_cast<long long>(F) * esz)));
-  const size_t need = static_cast<size_t>(chunk) * F * esz;
-  if (!ingest_copy_stream_) {
-    B200_CUDA(cudaStreamCreateWithFlags(&ingest_copy_stream_, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      B200_CUDA(cudaEventCreateWithFlags(&ingest_copied_[i], cudaEventDisableTiming));
-      B200_CUDA(cudaEventCreateWithFlags(&ingest_binned_[i], cudaEventDisableTiming));
+  long long host_max = 0;
+  for (const MatPart& p : parts) if (!p.on_device) host_max = std::max(host_max, p.nrow);
+  const long long chunk = std::max<long long>(1, std::min<long long>(host_max, static_cast<long long>(kStageBytes) / (static_cast<long long>(F) * esz)));
+  if (host_max > 0) {
+    const size_t need = static_cast<size_t>(chunk) * F * esz;
+    if (!ingest_copy_stream_) {
+      B200_CUDA(cudaStreamCreateWithFlags(&ingest_copy_stream_, cudaStreamNonBlocking));
+      for (int i = 0; i < 2; ++i) {
+        B200_CUDA(cudaEventCreateWithFlags(&ingest_copied_[i], cudaEventDisableTiming));
+        B200_CUDA(cudaEventCreateWithFlags(&ingest_binned_[i], cudaEventDisableTiming));
+      }
     }
+    for (int i = 0; i < 2; ++i) if (ingest_buf_[i].n < need) ingest_buf_[i].Alloc(std::max(need, std::min(kStageBytes, static_cast<size_t>(num_data) * F * esz)));
   }
-  for (int i = 0; i < 2; ++i) if (ingest_buf_[i].n < need) ingest_buf_[i].Alloc(std::max(need, std::min(kStageBytes, static_cast<size_t>(num_data) * F * esz)));
   cudaStream_t copy_stream = ingest_copy_stream_;
-  int it = 0;
-  for (long long r0 = 0; r0 < n; r0 += chunk, ++it) {
-    const int b = it & 1;
-    const long long rows = std::min(chunk, n - r0);
-    if (it >= 2) B200_CUDA(cudaStreamWaitEvent(copy_stream, ingest_binned_[b], 0));
-    if (is_row_major) {
-      B200_CUDA(cudaMemcpyAsync(ingest_buf_[b].p, static_cast<const unsigned char*>(data) + static_cast<size_t>(r0) * F * esz, static_cast<size_t>(rows) * F * esz,
-                                cudaMemcpyHostToDevice, copy_stream));
-    } else {   // column-major: F column segments of `rows` elements, device chunk keeps ld = rows
-      B200_CUDA(cudaMemcpy2DAsync(ingest_buf_[b].p, static_cast<size_t>(rows) * esz, static_cast<const unsigned char*>(data) + static_cast<size_t>(r0) * esz,
-                                  static_cast<size_t>(n) * esz, static_cast<size_t>(rows) * esz, F, cudaMemcpyHostToDevice, copy_stream));
+  int it = 0;                 // host chunks so far, over all parts: the buffer of chunk it is it & 1
+  long long first = 0;        // first row of the part
+  for (const MatPart& p : parts) {
+    const long long n = p.nrow;
+    if (p.on_device) {
+      fn(p.data, n, is_row_major ? F : n, first);
+      first += n;
+      continue;
     }
-    B200_CUDA(cudaEventRecord(ingest_copied_[b], copy_stream));
-    B200_CUDA(cudaStreamWaitEvent(stream, ingest_copied_[b], 0));
-    fn(static_cast<const void*>(ingest_buf_[b].p), rows, is_row_major ? F : rows, r0);
-    B200_CUDA(cudaEventRecord(ingest_binned_[b], stream));
+    for (long long r0 = 0; r0 < n; r0 += chunk, ++it) {
+      const int b = it & 1;
+      const long long rows = std::min(chunk, n - r0);
+      if (it >= 2) B200_CUDA(cudaStreamWaitEvent(copy_stream, ingest_binned_[b], 0));
+      if (is_row_major) {
+        B200_CUDA(cudaMemcpyAsync(ingest_buf_[b].p, static_cast<const unsigned char*>(p.data) + static_cast<size_t>(r0) * F * esz, static_cast<size_t>(rows) * F * esz,
+                                  cudaMemcpyHostToDevice, copy_stream));
+      } else {   // column-major: F column segments of `rows` elements, device chunk keeps ld = rows
+        B200_CUDA(cudaMemcpy2DAsync(ingest_buf_[b].p, static_cast<size_t>(rows) * esz, static_cast<const unsigned char*>(p.data) + static_cast<size_t>(r0) * esz,
+                                    static_cast<size_t>(n) * esz, static_cast<size_t>(rows) * esz, F, cudaMemcpyHostToDevice, copy_stream));
+      }
+      B200_CUDA(cudaEventRecord(ingest_copied_[b], copy_stream));
+      B200_CUDA(cudaStreamWaitEvent(stream, ingest_copied_[b], 0));
+      fn(static_cast<const void*>(ingest_buf_[b].p), rows, is_row_major ? F : rows, first + r0);
+      B200_CUDA(cudaEventRecord(ingest_binned_[b], stream));
+    }
+    first += n;
   }
-  B200_CUDA(cudaStreamSynchronize(stream));          // all copies are consumed: the caller may reuse its buffer
+  B200_CUDA(cudaStreamSynchronize(stream));          // all copies are consumed: the caller may reuse its buffers
 }
 
 void Dataset::ReleaseIngestStaging() {
@@ -847,7 +859,7 @@ void Dataset::PushRows(const void* data, int data_type, int nrow, int ncol, int 
   if (ncol != num_total_features) Fatal("PushRows: wrong number of columns");
   if (data_type != 0 && data_type != 1) Fatal("PushRows: unknown data type");
   StreamTimer timer(stream);
-  BinBlock(data, IsDevicePointer(data), data_type, 1, nrow, start_row);
+  BinBlock({MatPart{data, nrow, IsDevicePointer(data)}}, data_type, 1, start_row);
   ingest_ms += timer.Ms();
 }
 
@@ -979,39 +991,65 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   for (int u = 0; u < nfn; ++u) std::memcpy(out + static_cast<size_t>(used[u]) * 512, hd.data() + static_cast<size_t>(u) * 512, sizeof(double) * 512);
 }
 
-Dataset* Dataset::CreateFromMat(const void* data, int data_type, int nrow, int ncol, int is_row_major, const char* params,
-                                const Dataset* reference) {
+// " (part i)" in the messages of a multi-part create
+static std::string PartSuffix(int nparts, int i) { return nparts > 1 ? " (part " + std::to_string(i) + ")" : std::string(); }
+
+Dataset* Dataset::CreateFromMats(int nmat, const void* const* data, int data_type, const int32_t* nrow, int ncol, int is_row_major,
+                                 const char* params, const Dataset* reference) {
   EnsureDevice();
   if (data_type != 0 && data_type != 1) Fatal("Unknown data type in CreateFromMat (expect C_API_DTYPE_FLOAT32 or FLOAT64)");
-  if (nrow <= 0 || ncol <= 0) Fatal("Dataset should have at least one row and one column");
-  std::unique_ptr<Dataset> d = NewShell(nrow, ncol, params);
+  if (nmat < 1) Fatal("CreateFromMats: nmat must be at least 1");
+  if (!data || !nrow) Fatal("CreateFromMats: data and nrow must not be null");
+  std::vector<MatPart> parts(nmat);
+  std::vector<long long> first(nmat + 1, 0);          // first row of every part, then the total
+  for (int i = 0; i < nmat; ++i) {
+    if (nrow[i] <= 0 || ncol <= 0) Fatal("Dataset should have at least one row and one column" + PartSuffix(nmat, i));
+    if (!data[i]) Fatal("CreateFromMats: the data pointer is null" + PartSuffix(nmat, i));
+    parts[i] = MatPart{data[i], nrow[i], IsDevicePointer(data[i])};
+    first[i + 1] = first[i] + nrow[i];
+  }
+  if (first[nmat] > std::numeric_limits<int>::max()) Fatal("CreateFromMats: more than 2^31 - 1 rows in all");
+  std::unique_ptr<Dataset> d = NewShell(static_cast<int>(first[nmat]), ncol, params);
   StreamTimer timer(d->stream);
-  const bool on_device = IsDevicePointer(data);
   d->SetMappers(reference, true, [&](std::vector<std::vector<double>>* nz, std::vector<std::vector<int>>* nz_rows, int f0, int f1) {      // the sampled rows, gathered where the data is
-    const int n = nrow, F = ncol;
-    const std::vector<int> rows = d->SampleRows();
+    const int F = ncol;
+    const std::vector<int> rows = d->SampleRows();      // over the concatenated rows
     const int sample_cnt = static_cast<int>(rows.size());
     std::vector<double> S(static_cast<size_t>(sample_cnt) * F);
-    if (on_device) {
-      DevBuf<int> d_rows; d_rows.Alloc(sample_cnt);
-      DevBuf<double> d_S; d_S.Alloc(S.size());
-      d_rows.Upload(rows.data(), sample_cnt, d->stream);
-      int grid = static_cast<int>(std::min<size_t>((S.size() + 255) / 256, static_cast<size_t>(DeviceSMs()) * 32));
-      if (data_type == 0) k_gather_rows<float><<<grid, 256, 0, d->stream>>>(static_cast<const float*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
-      else k_gather_rows<double><<<grid, 256, 0, d->stream>>>(static_cast<const double*>(data), n, F, is_row_major, d_rows.p, sample_cnt, d_S.p);
+    // part and row within the part of every sampled row
+    std::vector<int> part_of(sample_cnt), local(sample_cnt);
+    for (int s = 0; s < sample_cnt; ++s) {
+      part_of[s] = static_cast<int>(std::upper_bound(first.begin() + 1, first.end(), static_cast<long long>(rows[s])) - (first.begin() + 1));
+      local[s] = static_cast<int>(rows[s] - first[part_of[s]]);
+    }
+    for (int i = 0; i < nmat; ++i) {
+      if (!parts[i].on_device) continue;
+      std::vector<int> pos, lrows;      // sample positions in this part, and their rows in it
+      for (int s = 0; s < sample_cnt; ++s) if (part_of[s] == i) { pos.push_back(s); lrows.push_back(local[s]); }
+      if (pos.empty()) continue;
+      const int cnt = static_cast<int>(pos.size());
+      std::vector<double> Sp(static_cast<size_t>(cnt) * F);
+      DevBuf<int> d_rows; d_rows.Alloc(cnt);
+      DevBuf<double> d_S; d_S.Alloc(Sp.size());
+      d_rows.Upload(lrows.data(), cnt, d->stream);
+      int grid = static_cast<int>(std::min<size_t>((Sp.size() + 255) / 256, static_cast<size_t>(DeviceSMs()) * 32));
+      if (data_type == 0) k_gather_rows<float><<<grid, 256, 0, d->stream>>>(static_cast<const float*>(parts[i].data), nrow[i], F, is_row_major, d_rows.p, cnt, d_S.p);
+      else k_gather_rows<double><<<grid, 256, 0, d->stream>>>(static_cast<const double*>(parts[i].data), nrow[i], F, is_row_major, d_rows.p, cnt, d_S.p);
       B200_CUDA(cudaGetLastError());
-      d_S.Download(S.data(), S.size(), d->stream);
+      d_S.Download(Sp.data(), Sp.size(), d->stream);
       B200_CUDA(cudaStreamSynchronize(d->stream));
-    } else {
+      for (int j = 0; j < cnt; ++j) std::memcpy(&S[static_cast<size_t>(pos[j]) * F], &Sp[static_cast<size_t>(j) * F], sizeof(double) * F);
+    }
 #pragma omp parallel for schedule(static)
-      for (int s = 0; s < sample_cnt; ++s) {
-        const long long r = rows[s];
-        for (int f = 0; f < F; ++f) {
-          double v;
-          if (data_type == 0) v = is_row_major ? static_cast<const float*>(data)[r * F + f] : static_cast<const float*>(data)[static_cast<long long>(f) * n + r];
-          else v = is_row_major ? static_cast<const double*>(data)[r * F + f] : static_cast<const double*>(data)[static_cast<long long>(f) * n + r];
-          S[static_cast<size_t>(s) * F + f] = v;
-        }
+    for (int s = 0; s < sample_cnt; ++s) {
+      const MatPart& p = parts[part_of[s]];
+      if (p.on_device) continue;
+      const long long r = local[s], n = p.nrow;
+      for (int f = 0; f < F; ++f) {
+        double v;
+        if (data_type == 0) v = is_row_major ? static_cast<const float*>(p.data)[r * F + f] : static_cast<const float*>(p.data)[static_cast<long long>(f) * n + r];
+        else v = is_row_major ? static_cast<const double*>(p.data)[r * F + f] : static_cast<const double*>(p.data)[static_cast<long long>(f) * n + r];
+        S[static_cast<size_t>(s) * F + f] = v;
       }
     }
     if (nz_rows) { f0 = 0; f1 = F; }
@@ -1029,13 +1067,14 @@ Dataset* Dataset::CreateFromMat(const void* data, int data_type, int nrow, int n
   });
   d->DissolveConflictingBundles([&](unsigned long long* conflicts) {
     const int nb = static_cast<int>(d->bundles.size()), grid = DeviceSMs() * 8;
-    d->ForEachDeviceBlock(data, on_device, data_type, is_row_major, nrow, [&](const void* x, long long rows, long long ld, long long) {
+    d->ForEachDeviceBlock(parts, data_type, is_row_major, [&](const void* x, long long rows, long long ld, long long) {
       if (data_type == 0) k_bundle_conflicts<float><<<grid, 256, 0, d->stream>>>(static_cast<const float*>(x), rows, is_row_major, ld, d->d_members.p, d->d_bundle_start.p, nb, conflicts);
       else k_bundle_conflicts<double><<<grid, 256, 0, d->stream>>>(static_cast<const double*>(x), rows, is_row_major, ld, d->d_members.p, d->d_bundle_start.p, nb, conflicts);
     });
   });
   d->AllocBins();
-  d->BinBlock(data, on_device, data_type, is_row_major, nrow, 0);
+  d->BinBlock(parts, data_type, is_row_major, 0);
+  d->ReleaseIngestStaging();      // every row is in, also when some parts were on the device
   d->ingest_ms = timer.Ms();
   return d.release();
 }
@@ -1110,78 +1149,96 @@ __global__ void k_bin_csr(const TI* __restrict__ indptr, const int* __restrict__
   }
 }
 
-Dataset* Dataset::CreateFromCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type,
-                                int64_t nindptr, int64_t nelem, int64_t num_col, const char* params, const Dataset* reference) {
+Dataset* Dataset::CreateFromCSRs(int nparts, const void* const* indptr, int indptr_type, const int32_t* const* indices, const void* const* data,
+                                 int data_type, const int64_t* nindptr, const int64_t* nelem, int64_t num_col, const char* params,
+                                 const Dataset* reference) {
   EnsureDevice();
   if (num_col <= 0) Fatal("CreateFromCSR: num_col must be given");
   if (num_col > std::numeric_limits<int>::max()) Fatal("CreateFromCSR: too many columns");
   if (indptr_type != 2 && indptr_type != 3) Fatal("CreateFromCSR: indptr must be int32 or int64");
   if (data_type != 0 && data_type != 1) Fatal("Unknown data type in CreateFromCSR (expect C_API_DTYPE_FLOAT32 or FLOAT64)");
-  const int64_t nrow = nindptr - 1;
-  if (nrow <= 0) Fatal("Dataset should have at least one row and one column");
-  if (nrow > std::numeric_limits<int>::max()) Fatal("CreateFromCSR: too many rows for one partition");
-  auto ip = [&](int64_t r) -> int64_t { return indptr_type == 2 ? static_cast<const int32_t*>(indptr)[r] : static_cast<const int64_t*>(indptr)[r]; };
-  auto val = [&](int64_t k) -> double { return data_type == 0 ? static_cast<double>(static_cast<const float*>(data)[k]) : static_cast<const double*>(data)[k]; };
-  if (ip(0) < 0 || ip(nrow) > nelem) Fatal("CreateFromCSR: indptr does not match the number of elements");
-  {
+  if (nparts < 1) Fatal("CreateFromCSRs: nparts must be at least 1");
+  if (!indptr || !indices || !data || !nindptr || !nelem) Fatal("CreateFromCSRs: the part arrays must not be null");
+  // indptr entry r of part i, stored value k of part i
+  auto ip = [&](int i, int64_t r) -> int64_t { return indptr_type == 2 ? static_cast<const int32_t*>(indptr[i])[r] : static_cast<const int64_t*>(indptr[i])[r]; };
+  auto val = [&](int i, int64_t k) -> double { return data_type == 0 ? static_cast<double>(static_cast<const float*>(data[i])[k]) : static_cast<const double*>(data[i])[k]; };
+  std::vector<int64_t> first(nparts + 1, 0);      // first row of every part, then the total
+  for (int i = 0; i < nparts; ++i) {
+    const std::string where = PartSuffix(nparts, i);
+    const int64_t nrow = nindptr[i] - 1;
+    if (nrow <= 0) Fatal("Dataset should have at least one row and one column" + where);
+    if (!indptr[i] || (nelem[i] > 0 && (!indices[i] || !data[i]))) Fatal("CreateFromCSRs: a pointer is null" + where);
+    if (ip(i, 0) < 0 || ip(i, nrow) > nelem[i]) Fatal("CreateFromCSR: indptr does not match the number of elements" + where);
+    const int32_t* ix = indices[i];
     int bad = 0;
 #pragma omp parallel for schedule(static) reduction(| : bad)
     for (int64_t r = 0; r < nrow; ++r) {
-      if (ip(r) > ip(r + 1)) bad |= 1;
-      else for (int64_t k = ip(r); k < ip(r + 1); ++k) if (indices[k] < 0 || indices[k] >= num_col) bad |= 2;
+      if (ip(i, r) > ip(i, r + 1)) bad |= 1;
+      else for (int64_t k = ip(i, r); k < ip(i, r + 1); ++k) if (ix[k] < 0 || ix[k] >= num_col) bad |= 2;
     }
-    if (bad & 1) Fatal("CreateFromCSR: indptr is not non-decreasing");
-    if (bad & 2) Fatal("CreateFromCSR: a column index is negative or >= num_col");
+    if (bad & 1) Fatal("CreateFromCSR: indptr is not non-decreasing" + where);
+    if (bad & 2) Fatal("CreateFromCSR: a column index is negative or >= num_col" + where);
+    first[i + 1] = first[i] + nrow;
   }
+  const int64_t nrow = first[nparts];
+  if (nrow > std::numeric_limits<int>::max()) Fatal("CreateFromCSR: too many rows for one partition");
   std::unique_ptr<Dataset> d = NewShell(static_cast<int>(nrow), static_cast<int>(num_col), params);
   StreamTimer timer(d->stream);
   const int F = d->num_total_features;
   d->SetMappers(reference, true, [&](std::vector<std::vector<double>>* nz, std::vector<std::vector<int>>* nz_rows, int, int) {
-    const std::vector<int> rows = d->SampleRows();
-    for (int s = 0; s < static_cast<int>(rows.size()); ++s)
-      for (int64_t k = ip(rows[s]); k < ip(rows[s] + 1); ++k) {
-        const double v = val(k);
+    const std::vector<int> rows = d->SampleRows();      // over the concatenated rows
+    for (int s = 0; s < static_cast<int>(rows.size()); ++s) {
+      const int i = static_cast<int>(std::upper_bound(first.begin() + 1, first.end(), static_cast<int64_t>(rows[s])) - (first.begin() + 1));
+      const int64_t r = rows[s] - first[i];
+      for (int64_t k = ip(i, r); k < ip(i, r + 1); ++k) {
+        const double v = val(i, k);
         if (std::fabs(v) > kZeroThr || std::isnan(v)) {
-          (*nz)[indices[k]].push_back(v);
-          if (nz_rows) (*nz_rows)[indices[k]].push_back(s);
+          (*nz)[indices[i][k]].push_back(v);
+          if (nz_rows) (*nz_rows)[indices[i][k]].push_back(s);
         }
       }
+    }
     return static_cast<int>(rows.size());
   });
   const int sms = DeviceSMs();
-  // row blocks of bounded element count: the stored elements are staged through one device buffer per block; fn(indptr, indices,
-  // values, rows, first row, first element) runs on each.  The block staged last stays on the device: when the whole CSR is one block
-  // (up to 64M stored values), the bundle row check and the binning share a single upload.
+  // row blocks of bounded element count, part by part: the stored elements are staged through one device buffer per block; fn(indptr,
+  // indices, values, rows, first row over all parts, first element in the part) runs on each.  The block staged last stays on the
+  // device: when the whole CSR is one block (up to 64M stored values), the bundle row check and the binning share a single upload.
   const size_t isz = indptr_type == 2 ? 4 : 8, vsz = data_type == 0 ? 4 : 8;
   DevBuf<unsigned char> d_ip, d_ix, d_v;
+  int staged_part = -1;
   int64_t staged_r0 = -1, staged_r1 = -1;
   auto for_each_block = [&](auto fn) {
     const int64_t kBlockElems = 64LL << 20;
-    int64_t r0 = 0;
-    while (r0 < nrow) {
-      int64_t r1 = r0 + 1;
-      while (r1 < nrow && ip(r1 + 1) - ip(r0) <= kBlockElems) ++r1;
-      const int64_t e0k = ip(r0), ne = ip(r1) - e0k, nr = r1 - r0;
-      if (r0 != staged_r0 || r1 != staged_r1) {
-        if (d_ip.n < static_cast<size_t>(nr + 1) * isz) d_ip.Alloc(static_cast<size_t>(nr + 1) * isz);
-        if (ne > 0) {
-          if (d_ix.n < static_cast<size_t>(ne) * 4) d_ix.Alloc(static_cast<size_t>(ne) * 4);
-          if (d_v.n < static_cast<size_t>(ne) * vsz) d_v.Alloc(static_cast<size_t>(ne) * vsz);
-          B200_CUDA(cudaMemcpyAsync(d_ix.p, indices + e0k, static_cast<size_t>(ne) * 4, cudaMemcpyHostToDevice, d->stream));
-          B200_CUDA(cudaMemcpyAsync(d_v.p, static_cast<const unsigned char*>(data) + static_cast<size_t>(e0k) * vsz, static_cast<size_t>(ne) * vsz, cudaMemcpyHostToDevice, d->stream));
+    for (int i = 0; i < nparts; ++i) {
+      const int64_t n = first[i + 1] - first[i];
+      int64_t r0 = 0;
+      while (r0 < n) {
+        int64_t r1 = r0 + 1;
+        while (r1 < n && ip(i, r1 + 1) - ip(i, r0) <= kBlockElems) ++r1;
+        const int64_t e0k = ip(i, r0), ne = ip(i, r1) - e0k, nr = r1 - r0;
+        if (i != staged_part || r0 != staged_r0 || r1 != staged_r1) {
+          if (d_ip.n < static_cast<size_t>(nr + 1) * isz) d_ip.Alloc(static_cast<size_t>(nr + 1) * isz);
+          if (ne > 0) {
+            if (d_ix.n < static_cast<size_t>(ne) * 4) d_ix.Alloc(static_cast<size_t>(ne) * 4);
+            if (d_v.n < static_cast<size_t>(ne) * vsz) d_v.Alloc(static_cast<size_t>(ne) * vsz);
+            B200_CUDA(cudaMemcpyAsync(d_ix.p, indices[i] + e0k, static_cast<size_t>(ne) * 4, cudaMemcpyHostToDevice, d->stream));
+            B200_CUDA(cudaMemcpyAsync(d_v.p, static_cast<const unsigned char*>(data[i]) + static_cast<size_t>(e0k) * vsz, static_cast<size_t>(ne) * vsz, cudaMemcpyHostToDevice, d->stream));
+          }
+          B200_CUDA(cudaMemcpyAsync(d_ip.p, static_cast<const unsigned char*>(indptr[i]) + static_cast<size_t>(r0) * isz, static_cast<size_t>(nr + 1) * isz, cudaMemcpyHostToDevice, d->stream));
+          staged_part = i; staged_r0 = r0; staged_r1 = r1;
         }
-        B200_CUDA(cudaMemcpyAsync(d_ip.p, static_cast<const unsigned char*>(indptr) + static_cast<size_t>(r0) * isz, static_cast<size_t>(nr + 1) * isz, cudaMemcpyHostToDevice, d->stream));
-        staged_r0 = r0; staged_r1 = r1;
+        if (ne > 0) {
+          const int64_t g0 = first[i] + r0;
+          if (indptr_type == 2 && data_type == 0) fn(int32_t{}, float{}, nr, g0, e0k);
+          else if (indptr_type == 2) fn(int32_t{}, double{}, nr, g0, e0k);
+          else if (data_type == 0) fn(int64_t{}, float{}, nr, g0, e0k);
+          else fn(int64_t{}, double{}, nr, g0, e0k);
+          B200_CUDA(cudaGetLastError());
+        }
+        B200_CUDA(cudaStreamSynchronize(d->stream));      // the staging buffers are reused by the next block
+        r0 = r1;
       }
-      if (ne > 0) {
-        if (indptr_type == 2 && data_type == 0) fn(int32_t{}, float{}, nr, r0, e0k);
-        else if (indptr_type == 2) fn(int32_t{}, double{}, nr, r0, e0k);
-        else if (data_type == 0) fn(int64_t{}, float{}, nr, r0, e0k);
-        else fn(int64_t{}, double{}, nr, r0, e0k);
-        B200_CUDA(cudaGetLastError());
-      }
-      B200_CUDA(cudaStreamSynchronize(d->stream));      // the staging buffers are reused by the next block
-      r0 = r1;
     }
   };
   d->DissolveConflictingBundles([&](unsigned long long* conflicts) {

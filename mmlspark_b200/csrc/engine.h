@@ -89,11 +89,15 @@ struct DevBuf {
 class Dataset {
  public:
   ~Dataset();
-  // data: host or device pointer (detected); data_type 0=f32 1=f64; reference != null => reuse its bins
-  static Dataset* CreateFromMat(const void* data, int data_type, int nrow, int ncol, int is_row_major, const char* params,
-                                const Dataset* reference);
-  static Dataset* CreateFromCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type,
-                                int64_t nindptr, int64_t nelem, int64_t num_col, const char* params, const Dataset* reference);
+  // One dataset from nmat row parts that count as one matrix: part 0's rows, then part 1's, ...  Bins, bundles and mappers equal those
+  // of one matrix holding the concatenation (a single matrix is nmat = 1), and no host copy of the parts is made.
+  // data[i]: host or device pointer (detected per part) of nrow[i] rows; data_type 0=f32 1=f64; reference != null => reuse its bins
+  static Dataset* CreateFromMats(int nmat, const void* const* data, int data_type, const int32_t* nrow, int ncol, int is_row_major,
+                                 const char* params, const Dataset* reference);
+  // the same for nparts host CSR parts; each part has its own indptr, which need not start at 0
+  static Dataset* CreateFromCSRs(int nparts, const void* const* indptr, int indptr_type, const int32_t* const* indices, const void* const* data,
+                                 int data_type, const int64_t* nindptr, const int64_t* nelem, int64_t num_col, const char* params,
+                                 const Dataset* reference);
   // LightGBM streaming ingestion: bins from a column-wise sample, then row blocks pushed in place
   static Dataset* CreateFromSampledColumn(double** sample_data, int** sample_indices, int ncol, const int* num_per_col,
                                           int num_sample_row, int num_total_row, const char* params);
@@ -165,9 +169,11 @@ class Dataset {
   std::vector<int> SampleRows() const;
   void AllocBins();
   template <typename T> void UnpackTiles(T* out) const;
-  void BinBlock(const void* data, bool on_device, int data_type, int is_row_major, long long nrow, long long start_row);
-  // fn(device rows, rows, leading dimension, first row) for each block of rows of a matrix, staged through device memory if on the host
-  template <typename Fn> void ForEachDeviceBlock(const void* data, bool on_device, int data_type, int is_row_major, long long nrow, Fn fn);
+  struct MatPart { const void* data; long long nrow; bool on_device; };      // rows of a matrix, one after another
+  void BinBlock(const std::vector<MatPart>& parts, int data_type, int is_row_major, long long start_row);
+  // fn(device rows, rows, leading dimension, first row counted over all parts) for each block of rows of the parts, in order; host
+  // parts are staged through device memory
+  template <typename Fn> void ForEachDeviceBlock(const std::vector<MatPart>& parts, int data_type, int is_row_major, Fn fn);
   // persistent H2D staging of the host ingestion path (two device chunks, a copy stream, events); released once every row is in
   DevBuf<unsigned char> ingest_buf_[2];
   cudaStream_t ingest_copy_stream_ = nullptr;

@@ -373,10 +373,16 @@ class LightGBMBase(Params):
         driver = tu.DriverRendezvous(num_tasks, self.get("driverListenPort"), self.get("timeout"))
         host, port = driver.start()
         results, errors = [None] * num_tasks, []
+        single = bool(self.get("useSingleDatasetMode"))
 
         def task(pid):
             try:
-                results[pid] = self._train_lightgbm(batch_index, pid, df.rows(parts[pid]), valid, train_params, host, port, num_tasks)
+                # single-dataset mode: the tasks of one device train as one rank over their partitions, in pid order.  The reference
+                # gathers those rows on the executor behind latches (SharedState); in this in-process mirror the main task reads its
+                # group's partitions from the frame directly, so no task waits for another.
+                rows = self._device_group(pid, parts, num_tasks) if single else [pid]
+                part_frames = [df.rows(parts[q]) for q in rows]
+                results[pid] = self._train_lightgbm(batch_index, pid, part_frames, valid, train_params, host, port, num_tasks)
             except Exception as e:   # noqa
                 log.exception("task %d failed", pid)
                 errors.append(e)
@@ -397,51 +403,75 @@ class LightGBMBase(Params):
     def _preprocess(self, df):
         return df
 
+    def _device_group(self, pid, parts, num_tasks):
+        """Single-dataset mode: the partitions task pid trains on.  The tasks of one device (pid % number of devices) form a group whose
+        main task is the lowest pid with a non-empty partition; it gets the group's non-empty partitions in pid order, every other task
+        none (it reports "ignore" like a disabled worker of the reference, LightGBMBase.trainLightGBM)."""
+        ndev = self._num_devices()
+        group = [q for q in range(num_tasks) if q % ndev == pid % ndev and parts[q].stop > parts[q].start]
+        return group if group and group[0] == pid else []
+
     def _make_dataset(self, part, params_str, reference=None):
-        X = part[self.get("featuresCol")]
-        if _is_sparse(X):      # CSR from resolve_matrix_type
+        """One dataset from a frame, or from a list of frames that count as one in order: a device group's partitions in single-dataset
+        mode (their feature matrices go to the library as they are, never concatenated here)."""
+        parts = part if isinstance(part, list) else [part]
+        Xs = [p[self.get("featuresCol")] for p in parts]
+        if len(Xs) > 1 and _is_sparse(Xs[0]):
+            ds = capi.Dataset.from_csrs(Xs, Xs[0].shape[1], params_str, reference=reference)
+        elif len(Xs) > 1:
+            ds = capi.Dataset.from_mats([np.ascontiguousarray(X, dtype=np.float64) for X in Xs], params_str, reference=reference)
+        elif _is_sparse(Xs[0]):      # CSR from resolve_matrix_type
+            X = Xs[0]
             ds = capi.Dataset.from_csr(X.indptr, X.indices, X.data, X.shape[1], params_str, reference=reference)
         else:
-            ds = capi.Dataset.from_mat(np.ascontiguousarray(X, dtype=np.float64), params_str, reference=reference)
-        ds.set_field("label", np.asarray(part[self.get("labelCol")], dtype=np.float32))       # narrowed to f32 (DatasetAggregator.scala:89-92)
+            ds = capi.Dataset.from_mat(np.ascontiguousarray(Xs[0], dtype=np.float64), params_str, reference=reference)
+
+        def column(name, dtype):
+            return np.concatenate([np.asarray(p[name], dtype=dtype) for p in parts])
+
+        ds.set_field("label", column(self.get("labelCol"), np.float32))       # narrowed to f32 (DatasetAggregator.scala:89-92)
         if self.get("weightCol"):
-            ds.set_field("weight", np.asarray(part[self.get("weightCol")], dtype=np.float32))
+            ds.set_field("weight", column(self.get("weightCol"), np.float32))
         if self.get("initScoreCol"):
-            init = np.asarray(part[self.get("initScoreCol")], dtype=np.float64)
+            init = column(self.get("initScoreCol"), np.float64)
             ds.set_field("init_score", init.T.reshape(-1) if init.ndim == 2 else init)    # class-major at the C ABI (Appendix D)
         gcol = self.get("groupCol") if "groupCol" in self._defaults else None
-        if gcol:
-            ds.set_field("group", np.asarray(tu.count_cardinality(part[gcol].tolist()), dtype=np.int32))
+        if gcol:      # partitions never split a query, so the parts' runs are the runs of their concatenation
+            ds.set_field("group", np.asarray([c for p in parts for c in tu.count_cardinality(p[gcol].tolist())], dtype=np.int32))
         names = list(self.get("slotNames"))
         if names:
             ds.set_feature_names(names)
         return ds
 
-    def _train_lightgbm(self, batch_index, pid, part, valid, train_params, driver_host, driver_port, num_tasks):
-        """trainLightGBM (:337-382) + translate (:292-335) for one partition / rank-thread."""
+    def _train_lightgbm(self, batch_index, pid, parts, valid, train_params, driver_host, driver_port, num_tasks):
+        """trainLightGBM (:337-382) + translate (:292-335) for one rank-thread: its partition, or in single-dataset mode its device
+        group's partitions (none for a task that is not the group's main task)."""
         capi.set_device(pid % self._num_devices())
-        empty = part.num_rows() == 0
+        parts = [p for p in parts if p.num_rows() > 0]
+        empty = not parts
         sock, local_port = tu.find_open_port(self.get("defaultListenPort"), pid)
         try:
             nodes = tu.get_network_init_nodes(driver_host, driver_port, local_port, empty)
         finally:
             sock.close()
         if empty:
-            return None                                   # "ignore" protocol for empty partitions
+            return None                                   # "ignore" protocol for empty partitions and non-main tasks
         use_net = len(nodes.split(",")) > 1
         try:
             if use_net:
                 tu.network_init(nodes, local_port)
             ds_params = dataset_params(self.get("maxBin"), self.get("binSampleCount"), self.get("numThreads"), train_params.categoricalFeatures)
-            train_ds = self._make_dataset(part, ds_params)
+            train_ds = self._make_dataset(parts if len(parts) > 1 else parts[0], ds_params)
             valid_ds = None
             try:
+                # built once per rank; in single-dataset mode the validation rows stay apart from the training rows (the reference's
+                # SharedState.merge would hand both the same shared aggregate)
                 if valid is not None and valid.num_rows() > 0:
                     valid_ds = self._make_dataset(valid, ds_params, reference=train_ds)
                 booster = tu.create_booster(train_params, train_ds, valid_ds)
                 try:
                     best = tu.train_core(batch_index, pid, train_params, booster, valid_ds is not None,
-                                         train_label=np.asarray(part[self.get("labelCol")], dtype=np.float32))
+                                         train_label=np.concatenate([np.asarray(p[self.get("labelCol")], dtype=np.float32) for p in parts]))
                     if tu.get_main_worker_port(nodes) == local_port:      # getReturnBooster (:355-363)
                         mb = LightGBMBooster(booster.save_model_to_string())
                         if best is not None:

@@ -2,8 +2,10 @@
 
 The cfg2 shape of bench.py (10M x 256 dense f32 regression, 255 bins, 31 leaves) is split into R contiguous shards, R in {1, 2, 4}, every
 rank-thread on device 0.  Ranks on one device share one stream, so their kernels run one after another: R ranks cost at least one rank over
-all rows, plus the collectives and the smaller per-rank launches.  After a warm-up the script alternates R over three rounds of 20 timed
-iterations and prints the iterations/s of every round.  A separate run under torch.profiler (R = 2) gives the device time per launch of
+all rows, plus the collectives and the smaller per-rank launches.  The "merged" arms train the same R shards as ONE rank over one dataset
+built from the R row parts (LGBM_DatasetCreateFromMats, what single-dataset mode does), and report its ingest time next to
+LGBM_DatasetCreateFromMat's on the whole matrix.  After a warm-up the script alternates the arms over three rounds of 20 timed iterations
+and prints the iterations/s of every round.  A separate run under torch.profiler (R = 2) gives the device time per launch of
 k_allreduce_same_device.  The card's name and power limit are read in the same run.
 
     python tools/shared_device_measure.py [--rows 10000000] [--features 256] [--out FILE]
@@ -77,6 +79,39 @@ def run(X, y, R, warmup, iters, port, on_timed=None):
     return max(secs)
 
 
+def run_merged(X, y, R, warmup, iters):
+    """the R shards of run() as ONE rank (single-dataset mode): one dataset from the R row parts through LGBM_DatasetCreateFromMats;
+    returns the wall time of `iters` iterations after `warmup` and the dataset's ingest time in ms"""
+    from mmlspark_b200 import capi
+    bounds = np.linspace(0, len(X), R + 1).astype(np.int64)
+    capi.set_device(0)
+    ds = capi.Dataset.from_mats([X[int(bounds[r]):int(bounds[r + 1])] for r in range(R)], DS_PARAMS).set_field("label", y)
+    ingest = ds.ingest_ms()
+    b = capi.Booster(ds, params(1))
+    try:
+        for _ in range(warmup):
+            b.update_one_iter()
+        b.get_scores()
+        t0 = time.perf_counter()
+        for _ in range(iters):
+            b.update_one_iter()
+        b.get_scores()
+        return time.perf_counter() - t0, ingest
+    finally:
+        b.free(); ds.free()
+
+
+def ingest_from_mat(X):
+    """ingest time in ms of LGBM_DatasetCreateFromMat on the whole matrix (the concatenation of the shards)"""
+    from mmlspark_b200 import capi
+    capi.set_device(0)
+    ds = capi.Dataset.from_mat(X, DS_PARAMS)
+    try:
+        return ds.ingest_ms()
+    finally:
+        ds.free()
+
+
 class _Null:
     def __enter__(self):
         return self
@@ -101,15 +136,22 @@ def main():
     rng = np.random.default_rng(2024)
     X = rng.standard_normal((a.rows, a.features), dtype=np.float32)
     y = (X[:, 0] + 0.5 * X[:, 1] * X[:, 2] + np.sin(X[:, 3]) + 0.3 * rng.standard_normal(a.rows, dtype=np.float32)).astype(np.float32)
-    rates = {1: [], 2: [], 4: []}
+    rates = {"1": [], "2": [], "4": [], "merged_2": [], "merged_4": []}
+    ingest = {"from_mat": [], "from_mats_2": [], "from_mats_4": []}
     port = 27000
     for rnd in range(a.rounds):
-        order = [1, 2, 4] if rnd % 2 == 0 else [4, 2, 1]
-        for R in order:
-            s = run(X, y, R, a.warmup, a.iters, port)
-            port += 10
-            rates[R].append(a.iters / s)
-            print("round %d R=%d: %.2f iters/s" % (rnd, R, a.iters / s), flush=True)
+        order = ["1", "2", "merged_2", "4", "merged_4"]
+        for arm in (order if rnd % 2 == 0 else order[::-1]):
+            if arm.startswith("merged_"):
+                R = int(arm[len("merged_"):])
+                s, ms = run_merged(X, y, R, a.warmup, a.iters)
+                ingest["from_mats_%d" % R].append(ms)
+            else:
+                s = run(X, y, int(arm), a.warmup, a.iters, port)
+                port += 10
+            rates[arm].append(a.iters / s)
+            print("round %d %s: %.2f iters/s" % (rnd, arm, a.iters / s), flush=True)
+        ingest["from_mat"].append(ingest_from_mat(X))
     # kernel time of the same-device all-reduce, in a run of its own
     prof_box = {}
 
@@ -123,7 +165,8 @@ def main():
     us = [e.time_range.elapsed_us() for e in ev]
     per_launch_us = float(np.mean(us)) if us else float("nan")
     out = dict(card=card, rows=a.rows, features=a.features, iters=a.iters,
-               iters_per_s={str(R): dict(median=float(np.median(v)), runs=[round(x, 3) for x in v]) for R, v in rates.items()},
+               iters_per_s={arm: dict(median=float(np.median(v)), runs=[round(x, 3) for x in v]) for arm, v in rates.items()},
+               ingest_ms={k: dict(median=float(np.median(v)), runs=[round(x, 1) for x in v]) for k, v in ingest.items()},
                allreduce_same_device=dict(launches=len(ev), mean_us=per_launch_us))
     print(json.dumps(out))
     if a.out:
