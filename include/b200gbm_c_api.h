@@ -226,8 +226,8 @@ int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, i
 int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
                                        int data_type, int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration,
                                        int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms);
-/* out = {num_machines, rank, histogram reduce mode (0 = ncclAllReduce, 1 = reduce-scatter + scan of the owned feature slice over NVLink
- * peer memory, 2 = two-shot all-reduce kernel over peer memory + replicated scan), constant_hessian} */
+/* out = {num_machines, rank, histogram reduce mode (0 = ncclAllReduce, 3 = same-device all-reduce: every rank a thread of this process
+ * on this device), constant_hessian} */
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4);
 /* out = {bytes of the optional column-major copy of the training bins kept for the partition kernel (0 = not kept: it is set up before the
  * first tree only within a reserve of device memory, B200GBM_COLUMN_COPY=0 disables it; when the full copy does not fit, the bytes of

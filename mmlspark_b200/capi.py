@@ -497,7 +497,7 @@ class Booster:
     def get_info(self):
         out = np.zeros(4, dtype=np.int32)
         check(load().B200GBM_BoosterGetInfo(self.handle, _ptr(out)))
-        return dict(num_machines=int(out[0]), rank=int(out[1]), fused_peer_reduce=int(out[2]) == 1, reduce_mode=int(out[2]), constant_hessian=bool(out[3]))
+        return dict(num_machines=int(out[0]), rank=int(out[1]), reduce_mode=int(out[2]), constant_hessian=bool(out[3]))
 
     def get_memory_info(self):
         out = np.zeros(2, dtype=np.int64)

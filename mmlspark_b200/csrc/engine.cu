@@ -1407,7 +1407,6 @@ Booster::~Booster() {
     fprintf(stderr, " (per split)\n");
   }
   for (auto* v : valids_) delete v;
-  for (void* p : ipc_opened_) cudaIpcCloseMemHandle(p);
   if (tree_host_) cudaFreeHost(tree_host_);
   if (ctrl_host_) cudaFreeHost(ctrl_host_);
   if (leaves_host_) cudaFreeHost(leaves_host_);
@@ -1511,7 +1510,6 @@ void Booster::InitTraining() {
     rn_tmp_bytes_ = std::max(t1, t2);
     rn_tmp_.Alloc(rn_tmp_bytes_ + 16);
   }
-  if (parallel_) SetupPeerReduce();
   // ColSampler: one draw at init, then one per tree ([UPSTREAM] ColSampler::SetTrainingData / ResetByTree)
   col_rand_ = LcgRandom(cfg.feature_fraction_seed);
   feature_used_host_.assign(train->nf_pad, 0);
@@ -1663,86 +1661,6 @@ void Booster::Bagging(int it) {
   B200_CUDA(cudaStreamSynchronize(s));
   timing.launches += 3;
   use_bag_ = true;
-}
-
-// Peer-memory set-up for the fused reduce+scan (k_scan_dp / k_pick_dp): every rank publishes its scratch histogram, mailbox and
-// flag block; ranks in the same process exchange raw pointers (peer access), ranks in other processes CUDA-IPC handles.
-struct PeerInfo {
-  long long pid;
-  int device, ok;
-  unsigned long long ptr[3];
-  cudaIpcMemHandle_t ipc[3];
-};
-void Booster::SetupPeerReduce() {
-  // Ranks on one device take the same-device all-reduce whatever B200GBM_FUSED_REDUCE asks: the peer-memory modes spin on flags that
-  // other ranks' kernels raise, and those kernels run after this rank's on the shared stream.
-  if (same_device_) return;
-  const char* env = std::getenv("B200GBM_FUSED_REDUCE");
-  const int R = Net().world, me = Net().rank;
-  mailbox_.Alloc(static_cast<size_t>(kMaxPeers) * 2); mailbox_.Zero(stream_);
-  peer_flags_.Alloc(64); peer_flags_.Zero(stream_);      // [0,16) "histogram ready" epochs by rank, [16,32) "second barrier" epochs, [48] block ticket
-  peer_error_.Alloc(1); peer_error_.Zero(stream_);
-  B200_CUDA(cudaStreamSynchronize(stream_));
-  PeerInfo mine{};
-  mine.pid = static_cast<long long>(getpid()); mine.device = device_;
-  // Default = NCCL all-reduce of the 2 MB histogram; the peer-memory modes (two cross-GPU flag barriers per split) are opt-in.
-  // Their speed relative to NCCL has not been measured on H100.
-  int mode = env ? std::atoi(env) : 0;      // 0 NCCL, 1 fused reduce-scatter + scan of the owned slice, 2 two-shot P2P all-reduce + replicated scan
-  // the fused scan handles unbundled numerical tile features only (same decision on every rank)
-  if (mode == 1 && (train->has_categorical || !train->bundles.empty())) mode = 0;
-  mine.ok = (R <= kMaxPeers && (mode == 1 || mode == 2)) ? 1 : 0;
-  void* bufs[3] = {H_.p, mailbox_.p, peer_flags_.p};
-  for (int i = 0; i < 3; ++i) {
-    mine.ptr[i] = reinterpret_cast<unsigned long long>(bufs[i]);
-    if (cudaIpcGetMemHandle(&mine.ipc[i], bufs[i]) != cudaSuccess) { cudaGetLastError(); mine.ok = 0; }
-  }
-  std::vector<PeerInfo> all(R);
-  {
-    DevBuf<unsigned char> ds, dr; ds.Alloc(sizeof(PeerInfo)); dr.Alloc(sizeof(PeerInfo) * R);
-    B200_CUDA(cudaMemcpyAsync(ds.p, &mine, sizeof(PeerInfo), cudaMemcpyHostToDevice, stream_));
-    Net().AllGather(ds.p, dr.p, sizeof(PeerInfo), stream_);
-    B200_CUDA(cudaMemcpyAsync(all.data(), dr.p, sizeof(PeerInfo) * R, cudaMemcpyDeviceToHost, stream_));
-    B200_CUDA(cudaStreamSynchronize(stream_));
-  }
-  int ok = 1;
-  for (int r = 0; r < R; ++r) ok &= all[r].ok;
-  PeerTables pt{};
-  if (ok) {
-    for (int r = 0; r < R && ok; ++r) {
-      void* p3[3];
-      if (r == me) { for (int i = 0; i < 3; ++i) p3[i] = bufs[i]; }
-      else if (all[r].pid == mine.pid) {          // rank-thread of the same process (the reference's local mode)
-        int can = 0;
-        cudaDeviceCanAccessPeer(&can, device_, all[r].device);
-        if (!can) { ok = 0; break; }
-        cudaError_t e = cudaDeviceEnablePeerAccess(all[r].device, 0);
-        if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); ok = 0; break; }
-        cudaGetLastError();
-        for (int i = 0; i < 3; ++i) p3[i] = reinterpret_cast<void*>(all[r].ptr[i]);
-      } else {                                    // one process per GPU (torchrun): CUDA IPC
-        for (int i = 0; i < 3; ++i) {
-          if (cudaIpcOpenMemHandle(&p3[i], all[r].ipc[i], cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); ok = 0; break; }
-          ipc_opened_.push_back(p3[i]);
-        }
-        if (!ok) break;
-      }
-      pt.H[r] = static_cast<const long long*>(p3[0]); pt.mail[r] = static_cast<SplitCand*>(p3[1]); pt.flags[r] = static_cast<unsigned*>(p3[2]);
-    }
-  }
-  // every rank must take the same path: agree on `ok`
-  double okd = ok ? 1.0 : 0.0;
-  AllReduceHost(&okd, 1, ncclMin, stream_);
-  const bool peers_ok = okd > 0.5;
-  fused_ = peers_ok && mode == 1;
-  p2p_allreduce_ = peers_ok && mode == 2;
-  if (p2p_allreduce_) { pt.rank = me; pt.world = R; pt.feat0 = 0; pt.feat1 = 0; pt.error = peer_error_.p; peers_ = pt; return; }
-  if (!fused_) return;
-  const int tiles_per_rank = (train->num_tiles + R - 1) / R;
-  pt.rank = me; pt.world = R;
-  pt.feat0 = std::min(train->nf_pad, me * tiles_per_rank * 32);
-  pt.feat1 = std::min(train->nf_pad, (me + 1) * tiles_per_rank * 32);
-  pt.error = peer_error_.p;
-  peers_ = pt;
 }
 
 void Booster::ResetFeaturesByTree() {
@@ -2031,37 +1949,21 @@ void Booster::TrainOneTree(int k, HostTree* out) {
     if (profile_hist) B200_CUDA(cudaEventRecord(evs.back(), s));
     mark();
     nvtxRangePushA(parallel_ ? "b200gbm:C2 histogram reduce + K5 scan + pick" : "b200gbm:K5 scan + pick");
-    if (fused_) {
-      // C2+K5+C3 fused over NVLink peer memory: signal "histogram ready", then the scan reduces its owned slice from all peers
-      ++epoch_;
-      const dim3 dgrid(std::max(1, (peers_.feat1 - peers_.feat0 + 7) / 8), 2);
-      k_scan_dp<<<dgrid, 256, 0, s>>>(ctrl, leaves_.p, d.meta.p, peers_, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, epoch_);
-      k_pick_dp<<<1, 256, 0, s>>>(ctrl, leaves_.p, d.meta.p, cands_.p, sp_, peers_, epoch_);
-      mark();
-    } else {
-      if (p2p_allreduce_) {       // C2 as one kernel over NVLink peer memory (k_allreduce_p2p)
-        ++epoch_;
-        const int agrid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(64, slot_elems_ / 2 / Net().world / 256 + 1)));
-        k_allreduce_p2p<<<agrid, 256, 0, s>>>(ctrl, peers_, slot_elems_, epoch_, peer_flags_.p + 48);
-        timing.launches += 1;
-      } else if (parallel_) {
-        Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
-      }
-      mark();
-      if (d.nw > 0) {
-        k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
-        timing.launches += 1;
-      }
-      // scan + (last block) pick; the dynamic scratch is only touched by categorical features and bundle members
-      k_scan<<<sgrid, 256, (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase());
+    if (parallel_) Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
+    mark();
+    if (d.nw > 0) {
+      k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
+      timing.launches += 1;
     }
+    // scan + (last block) pick; the dynamic scratch is only touched by categorical features and bundle members
+    k_scan<<<sgrid, 256, (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase());
     nvtxRangePop();
     mark();
     nvtxRangePushA("b200gbm:K7 partition + controller");
     LaunchPartition(pgrid, split == L - 2 ? 1 : 0);
     nvtxRangePop();
     mark();
-    timing.launches += fused_ ? 4 : 3; timing.hist_launches += 1;
+    timing.launches += 3; timing.hist_launches += 1;
   }
   if (obj_->RenewsLeaves()) RenewTreeOutput(k, is_rf_ ? rf_init_scores_[k] : 0.0);
   // rf keeps scores as the running average of (tree + init score) over the iterations [LightGBM rf.hpp MultiplyScore / UpdateScore]
@@ -2079,7 +1981,7 @@ void Booster::TrainOneTree(int k, HostTree* out) {
   B200_CUDA(cudaMemcpyAsync(tree_host_, tree_blob_.p, tree_blob_bytes_, cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaMemcpyAsync(ctrl_host_, ctrl, sizeof(TreeCtrl), cudaMemcpyDeviceToHost, s));
   B200_CUDA(cudaStreamSynchronize(s));
-  if (split_timing && !fused_ && !sev.empty()) {
+  if (split_timing && !sev.empty()) {
     static const char* kOps[] = {"gather_q(bagged root)", "K4", "allreduce", "scan+pick", "partition+zeroH+ctl"};
     const int per = 6;       // marks per split
     for (size_t b0 = 0; b0 + per <= sev.size(); b0 += per)
@@ -2092,11 +1994,6 @@ void Booster::TrainOneTree(int k, HostTree* out) {
     for (auto e : evs) cudaEventDestroy(e);
   }
   timing.hist_rows += ctrl_host_->trace_rows;
-  if (fused_ || p2p_allreduce_) {
-    int err = 0;
-    B200_CUDA(cudaMemcpy(&err, peer_error_.p, sizeof(int), cudaMemcpyDeviceToHost));
-    if (err) Fatal("data-parallel training: a peer rank stopped responding (peer-memory barrier timed out)");
-  }
   // ---- host copy of the tree
   const unsigned char* hb = tree_host_;
   auto at = [&](const void* devp) { return hb + (static_cast<const unsigned char*>(devp) - tree_blob_.p); };

@@ -221,7 +221,7 @@ class Booster {
   int64_t PredictBatchCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
                           int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out);
   double last_predict_ms = 0.0;
-  void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = fused_ ? 1 : (p2p_allreduce_ ? 2 : (same_device_ ? 3 : 0)); out4[3] = const_hessian_ ? 1 : 0; }
+  void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = same_device_ ? 3 : 0; out4[3] = const_hessian_ ? 1 : 0; }
   std::string SaveModelToString(int start_iteration, int num_iteration, int importance_type) const;
   std::string DumpModelJson(int start_iteration, int num_iteration) const;
 
@@ -325,16 +325,6 @@ class Booster {
  private:
   DevBuf<unsigned> part_bits_;
   DevBuf<int> part_chunks_;
-  // fused data-parallel reduce (peer memory over NVLink); falls back to NCCL when peers cannot map each other
-  bool fused_ = false;
-  bool p2p_allreduce_ = false;          // B200GBM_FUSED_REDUCE=2: the per-split histogram all-reduce is k_allreduce_p2p instead of ncclAllReduce
-  PeerTables peers_{};
-  DevBuf<SplitCand> mailbox_;
-  DevBuf<unsigned> peer_flags_;
-  DevBuf<int> peer_error_;
-  std::vector<void*> ipc_opened_;
-  unsigned epoch_ = 0;
-  void SetupPeerReduce();
   // flattened forest for PredictBatch
   // PredictBatchCSR's slots (kernels.cuh k_csr_to_slots) for the trees [t0, t1): the U distinct split features in ascending order
   struct SlotBufs { int t0 = 0, t1 = 0, U = 0; DevBuf<int> slot_of_feature, feature_of_slot, split_slot; };

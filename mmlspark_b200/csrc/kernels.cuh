@@ -803,142 +803,8 @@ k_round_ctl(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
 }
 
 // ---------------------------------------------------------------- K5/K6 split scan
-// One warp per (which in {smaller, larger}, feature).  Lane l owns bins 8l..8l+7.  All prefix sums are
-// exact int64; gains are fp64.  Replaces FeatureHistogram::FindBestThresholdSequentially (+Subtract).
-__device__ __forceinline__ long long warp_suffix_excl(long long v, int lane) {   // sum over lanes > lane
-  long long inc = v;
-  for (int o = 1; o < 32; o <<= 1) { long long t = __shfl_down_sync(0xffffffffu, inc, o); if (lane + o < 32) inc += t; }
-  return inc - v;
-}
-__device__ __forceinline__ long long warp_prefix_excl(long long v, int lane) {   // sum over lanes < lane
-  long long inc = v;
-  for (int o = 1; o < 32; o <<= 1) { long long t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-  return inc - v;
-}
-
-// the per-feature scan shared by k_scan and k_scan_dp: qg/qh = this lane's 8 bins of the (global) histogram
-// The bin loops are deliberately NOT unrolled (qg/qh/cnt are then indexed dynamically and live in L1-cached local memory): unrolled, the two
-// scan directions alone were ~5K instructions of straight-line fp64 code per warp and the kernel was bound by instruction fetch.
-__device__ __forceinline__ void d_scan_feature(const long long (&qg)[8], const long long (&qh)[8], int lane, const FeatMeta m, const LeafState& L,
-                                               double inv_g, double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* outp) {
-  SplitCand& out = *outp;
-  const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
-  const int num_data = L.global_count;
-  const double cnt_factor = num_data / sum_h;
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
-  const bool two_way = (m.num_bin > 2 && m.missing_type == 2);
-  const int na = two_way ? 1 : 0;
-
-  int cnt[8];
-#pragma unroll 1
-  for (int j = 0; j < 8; ++j) cnt[j] = static_cast<int>(static_cast<double>(qh[j]) * inv_h * cnt_factor + 0.5);
-
-  // ---- reverse pass: bins num_bin-1-na .. 1, candidate threshold = b-1
-  // Both passes end where the sequential scan breaks: at the first candidate, in scan order, whose far side fails min_data_in_leaf or
-  // min_sum_hessian_in_leaf.  A lane stops its own loop there; the ballot then drops every lane that comes later in scan order, so
-  // their candidates neither win nor mark the feature splittable.  With hessians >= 0 nothing after a break could pass these tests
-  // anyway (counts and hessian sums are monotone); with negative hessians (custom objectives) they could.
-  double best_gain = kNegInf, best_lg = 0, best_lh = 0;
-  int best_thr = -1, best_lc = 0, best_dl = 1;
-  bool any_valid = false;
-  {
-    const int hi = m.num_bin - 1 - na;
-    long long lg = 0, lh = 0, lc = 0;
-#pragma unroll 1
-    for (int j = 0; j < 8; ++j) { const int b = lane * 8 + j; if (b >= 1 && b <= hi) { lg += qg[j]; lh += qh[j]; lc += cnt[j]; } }
-    long long rg = warp_suffix_excl(lg, lane), rh = warp_suffix_excl(lh, lane), rc = warp_suffix_excl(lc, lane);
-    bool stop = false;
-#pragma unroll 1
-    for (int j = 7; j >= 0; --j) {
-      const int b = lane * 8 + j;
-      if (b < 1 || b > hi) continue;
-      rg += qg[j]; rh += qh[j]; rc += cnt[j];
-      const double srg = static_cast<double>(rg) * inv_g;
-      const double srh = kEpsD + static_cast<double>(rh) * inv_h;
-      const int right_count = static_cast<int>(rc);
-      if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) continue;
-      const int left_count = num_data - right_count;
-      const double slh = sum_h - srh;
-      if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
-      const double slg = sum_g - srg;
-      const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
-      if (gain <= min_gain_shift) continue;
-      any_valid = true;
-      if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_thr = b - 1; best_lc = left_count; }
-    }
-    const unsigned brk = __ballot_sync(0xffffffffu, stop);      // the reverse scan runs from lane 31 down: the highest breaking lane ends it
-    if (brk && lane < 31 - __clz(brk)) { best_gain = kNegInf; best_thr = -1; any_valid = false; }
-    // warp argmax: higher gain, ties -> higher threshold (first seen in the right-to-left scan)
-    for (int o = 16; o; o >>= 1) {
-      double og = __shfl_xor_sync(0xffffffffu, best_gain, o);
-      int ot = __shfl_xor_sync(0xffffffffu, best_thr, o);
-      double olg = __shfl_xor_sync(0xffffffffu, best_lg, o), olh = __shfl_xor_sync(0xffffffffu, best_lh, o);
-      int olc = __shfl_xor_sync(0xffffffffu, best_lc, o);
-      if (og > best_gain || (og == best_gain && ot > best_thr)) { best_gain = og; best_thr = ot; best_lg = olg; best_lh = olh; best_lc = olc; }
-    }
-  }
-  // ---- forward pass (NaN-as-missing features only): bins 0 .. num_bin-2, threshold = b, NaN goes right
-  if (two_way) {
-    const int hi = m.num_bin - 2;
-    long long ag = 0, ah = 0, ac = 0;     // everything stored except bin 0 (incl. the NaN bin)
-    long long lg = 0, lh = 0, lc = 0;
-#pragma unroll 1
-    for (int j = 0; j < 8; ++j) {
-      const int b = lane * 8 + j;
-      if (b >= 1 && b < m.num_bin) { ag += qg[j]; ah += qh[j]; ac += cnt[j]; }
-      if (b >= m.offset && b <= hi) { lg += qg[j]; lh += qh[j]; lc += cnt[j]; }
-    }
-    for (int o = 16; o; o >>= 1) { ag += __shfl_xor_sync(0xffffffffu, ag, o); ah += __shfl_xor_sync(0xffffffffu, ah, o); ac += __shfl_xor_sync(0xffffffffu, ac, o); }
-    long long pg = warp_prefix_excl(lg, lane), ph = warp_prefix_excl(lh, lane), pc = warp_prefix_excl(lc, lane);
-    double base_g = 0.0, base_h = kEpsD; int base_c = 0;
-    if (m.offset == 1) {   // implicit bin 0 = leaf total - everything stored  [UPSTREAM NA_AS_MISSING && offset==1]
-      base_g = sum_g - static_cast<double>(ag) * inv_g;
-      base_h = (sum_h - kEpsD) - static_cast<double>(ah) * inv_h;
-      base_c = num_data - static_cast<int>(ac);
-    }
-    double f_gain = kNegInf, f_lg = 0, f_lh = 0; int f_thr = 1 << 30, f_lc = 0;
-    bool stop = false, f_valid = false;
-#pragma unroll 1
-    for (int j = 0; j < 8; ++j) {
-      const int b = lane * 8 + j;
-      if (b > hi) continue;
-      if (b >= m.offset) { pg += qg[j]; ph += qh[j]; pc += cnt[j]; }
-      const double slg = base_g + static_cast<double>(pg) * inv_g;
-      const double slh = base_h + static_cast<double>(ph) * inv_h;
-      const int left_count = base_c + static_cast<int>(pc);
-      if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
-      const int right_count = num_data - left_count;
-      const double srh = sum_h - slh;
-      if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { stop = true; break; }
-      const double srg = sum_g - slg;
-      const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
-      if (gain <= min_gain_shift) continue;
-      f_valid = true;
-      if (gain > f_gain) { f_gain = gain; f_lg = slg; f_lh = slh; f_thr = b; f_lc = left_count; }
-    }
-    const unsigned brk = __ballot_sync(0xffffffffu, stop);      // the forward scan runs from lane 0 up: the lowest breaking lane ends it
-    if (brk && lane > __ffs(brk) - 1) { f_gain = kNegInf; f_thr = 1 << 30; f_valid = false; }
-    any_valid |= f_valid;
-    for (int o = 16; o; o >>= 1) {
-      double og = __shfl_xor_sync(0xffffffffu, f_gain, o);
-      int ot = __shfl_xor_sync(0xffffffffu, f_thr, o);
-      double olg = __shfl_xor_sync(0xffffffffu, f_lg, o), olh = __shfl_xor_sync(0xffffffffu, f_lh, o);
-      int olc = __shfl_xor_sync(0xffffffffu, f_lc, o);
-      if (og > f_gain || (og == f_gain && ot < f_thr)) { f_gain = og; f_thr = ot; f_lg = olg; f_lh = olh; f_lc = olc; }
-    }
-    if (f_gain > best_gain) { best_gain = f_gain; best_thr = f_thr; best_lg = f_lg; best_lh = f_lh; best_lc = f_lc; best_dl = 0; }
-  } else if (m.missing_type == 2) {
-    best_dl = 0;
-  }
-  any_valid = __any_sync(0xffffffffu, any_valid);
-  if (lane == 0) {
-    *flag = any_valid ? 1 : 0;
-    if (any_valid && best_gain > min_gain_shift) {
-      out.gain = best_gain - min_gain_shift; out.left_g = best_lg; out.left_h = best_lh; out.threshold = best_thr;
-      out.left_count = best_lc; out.default_left = best_dl;
-    }
-  }
-}
+// What k_scan (below) runs besides the numerical scan: the warp-level categorical search, and the pick step of its last block over the
+// candidates of every feature, the wide ones from k_scan_wide included.  All sums are exact int64; gains are fp64.
 
 // Categorical split search for one feature by one warp (FeatureHistogram::FindBestThresholdCategoricalInner [UPSTREAM]):
 // one-hot when num_bin <= max_cat_to_onehot; otherwise the bins holding >= cat_smooth rows are ranked by g/(h+cat_smooth)
@@ -1171,153 +1037,6 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
   __syncthreads();
   if (threadIdx.x < 32 && !ctrl->finished) d_choose_leaf(ctrl, leaves, meta, p, threadIdx.x);
 }
-__global__ void __launch_bounds__(256)
-k_pick(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, SplitParams p) {
-  d_pick_block(ctrl, leaves, meta, cands, p);
-}
-
-// ---------------------------------------------------------------- fused data-parallel reduce + scan (C2 + K5 + C3)
-// Replaces  K4 -> ncclAllReduce(histogram) -> K5  by LightGBM's reduce-scatter scheme executed over NVLink peer
-// memory inside the scan kernel: rank r owns a contiguous slice of feature tiles; after a flag barrier ("all local
-// histograms are complete") its scan warps read the slice from EVERY rank's scratch histogram with P2P loads, sum it
-// (exact int64), scan only the owned features, and post the rank's two best candidates into every peer's mailbox.
-constexpr int kMaxPeers = 16;
-struct PeerTables {
-  const long long* H[kMaxPeers];       // every rank's scratch histogram (own entry = local pointer)
-  SplitCand* mail[kMaxPeers];          // every rank's mailbox [world][2]
-  unsigned* flags[kMaxPeers];          // every rank's flag block: [0..15] = "hist ready" epochs, [16..31] = "candidates posted"
-  int rank, world, feat0, feat1;       // owned inner-feature range [feat0, feat1)
-  int* error;                          // set when a spin-wait times out
-};
-
-__device__ __forceinline__ void peer_wait(const volatile unsigned* f, int world, unsigned epoch, int* error) {
-  const long long t0 = clock64();
-  for (int r = 0; r < world; ++r) {
-    while (static_cast<int>(f[r] - epoch) < 0) {
-      if (clock64() - t0 > 4000000000LL) { *error = 1; return; }   // ~2 s: a peer died; fail instead of hanging the GPU
-      __nanosleep(100);
-    }
-  }
-  __threadfence_system();
-}
-// one small kernel after K4: tell every peer that this rank's scratch histogram is complete
-__global__ void k_peer_signal_hist(PeerTables pt, unsigned epoch) {
-  __threadfence_system();
-  const int r = threadIdx.x;
-  if (r < pt.world) *reinterpret_cast<volatile unsigned*>(&pt.flags[r][pt.rank]) = epoch;
-}
-
-__global__ void __launch_bounds__(256)
-k_scan_dp(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const FeatMeta* __restrict__ meta, PeerTables pt,
-          long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
-          unsigned epoch) {
-  if (!ctrl->go) return;
-  const int which = blockIdx.y;
-  const int leaf = which ? ctrl->larger : ctrl->smaller;
-  if (leaf < 0) return;
-  // "my scratch histogram is complete" (K4 finished: stream order) -> every peer; then wait for all peers
-  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x < pt.world) {
-    __threadfence_system();
-    *reinterpret_cast<volatile unsigned*>(&pt.flags[threadIdx.x][pt.rank]) = epoch;
-  }
-  if (threadIdx.x == 0) peer_wait(pt.flags[pt.rank], pt.world, epoch, pt.error);
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int u = pt.feat0 + blockIdx.x * 8 + warp;
-  if (u >= pt.feat1 || u >= p.nf) return;
-  SplitCand out;
-  out.gain = kNegInf; out.left_g = 0; out.left_h = 0; out.threshold = 0; out.left_count = 0; out.default_left = 1; out.feature = u;
-  out.l2_extra = 0; out.is_cat = 0; out.cat_list_len = 0;
-  for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
-  uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
-  if (!*flag) { if (lane == 0) cands[which * p.nf_pad + u] = out; return; }
-
-  const LeafState& L = leaves[leaf];
-  long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(u) * 512;
-  long long qg[8], qh[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { qg[j] = 0; qh[j] = 0; }
-  // reduce-scatter: sum the owned slice over all ranks.  P2P loads bypass L1 (volatile); 4 peers are in flight at a time so
-  // the ~2 us NVLink round trips overlap instead of serialising.
-  for (int r0 = 0; r0 < pt.world; r0 += 4) {
-    longlong2 v[4][8];
-#pragma unroll
-    for (int rr = 0; rr < 4; ++rr) {
-      const int r = min(r0 + rr, pt.world - 1);
-      const long long* src = pt.H[r] + static_cast<size_t>(u) * 512;
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        asm volatile("ld.volatile.global.v2.s64 {%0, %1}, [%2];\n" : "=l"(v[rr][j].x), "=l"(v[rr][j].y) : "l"(src + (lane * 8 + j) * 2));
-    }
-#pragma unroll
-    for (int rr = 0; rr < 4; ++rr) {
-      if (r0 + rr < pt.world) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { qg[j] += v[rr][j].x; qh[j] += v[rr][j].y; }
-      }
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int b = lane * 8 + j;
-    if (which) {
-      longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2);
-      qg[j] = pr.x - qg[j]; qh[j] = pr.y - qh[j];
-    }
-    longlong2 sv; sv.x = qg[j]; sv.y = qh[j];
-    *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
-  }
-  d_scan_feature(qg, qh, lane, meta[u], L, ctrl->inv_g, ctrl->inv_h, p, flag, &out);
-  if (lane == 0) cands[which * p.nf_pad + u] = out;
-}
-
-// ---------------------------------------------------------------- C2 as ONE kernel: two-shot all-reduce over NVLink peer memory
-// B200GBM_FUSED_REDUCE=2.  The histogram all-reduce of a split is 2-4 MB of int64 — far below the size where NCCL's ring / tree protocols
-// pay off; ncclAllReduce costs ~50 us of launch + protocol latency per split at 8 ranks.  Here every rank runs this kernel on its own stream:
-//   barrier A  "my scratch histogram is complete" -> flag in every peer's flag block; wait for all peers
-//   shot 1     rank r sums slice r (1/world of the histogram) over all peers' scratch histograms with 16-byte P2P loads ...
-//   shot 2     ... and stores the sums into slice r of EVERY peer's scratch histogram (nobody else touches slice r)
-//   barrier B  raised by the block that finishes last; the kernel does not return before all peers raised theirs, so the scan that follows
-//              in stream order sees the complete reduced histogram.  Exact int64 sums: identical bits on every rank.
-__global__ void __launch_bounds__(256)
-k_allreduce_p2p(const TreeCtrl* __restrict__ ctrl, PeerTables pt, size_t elems, unsigned epoch, unsigned* __restrict__ ticket) {
-  __shared__ int s_last;
-  if (!ctrl->go) return;                 // same decision on every rank (global counts); nothing was built
-  if (blockIdx.x == 0 && threadIdx.x < pt.world) {
-    __threadfence_system();
-    *reinterpret_cast<volatile unsigned*>(&pt.flags[threadIdx.x][pt.rank]) = epoch;
-  }
-  if (threadIdx.x == 0) peer_wait(pt.flags[pt.rank], pt.world, epoch, pt.error);
-  __syncthreads();
-  const size_t n2 = elems / 2;                                   // longlong2 units
-  const size_t per = (n2 + pt.world - 1) / pt.world;
-  const size_t lo = per * pt.rank, hi = min(lo + per, n2);
-  for (size_t i = lo + blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < hi; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    long long sx = 0, sy = 0;
-    for (int r0 = 0; r0 < pt.world; r0 += 4) {                   // 4 peers in flight: the NVLink round trips overlap
-      long long vx[4], vy[4];
-#pragma unroll
-      for (int rr = 0; rr < 4; ++rr) {
-        const int r = min(r0 + rr, pt.world - 1);
-        asm volatile("ld.volatile.global.v2.s64 {%0, %1}, [%2];\n" : "=l"(vx[rr]), "=l"(vy[rr]) : "l"(pt.H[r] + i * 2));
-      }
-#pragma unroll
-      for (int rr = 0; rr < 4; ++rr) if (r0 + rr < pt.world) { sx += vx[rr]; sy += vy[rr]; }
-    }
-    for (int r = 0; r < pt.world; ++r)
-      asm volatile("st.volatile.global.v2.s64 [%0], {%1, %2};\n" ::"l"(const_cast<long long*>(pt.H[r]) + i * 2), "l"(sx), "l"(sy) : "memory");
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1) ? 1 : 0;
-  __syncthreads();
-  if (!s_last) return;
-  if (threadIdx.x == 0) *ticket = 0u;
-  __threadfence_system();
-  if (threadIdx.x < pt.world) *reinterpret_cast<volatile unsigned*>(&pt.flags[threadIdx.x][16 + pt.rank]) = epoch;
-  if (threadIdx.x == 0) peer_wait(pt.flags[pt.rank] + 16, pt.world, epoch, pt.error);
-  __syncthreads();
-}
 
 // ---------------------------------------------------------------- same-device all-reduce (rank-threads of one process on one device)
 // Every rank's buffer is on this device, so one launch, enqueued by the last rank to reach the collective (engine.cu SameDeviceComm), does
@@ -1325,6 +1044,7 @@ k_allreduce_p2p(const TreeCtrl* __restrict__ ctrl, PeerTables pt, size_t elems, 
 // changes, so double sums are deterministic; for R = 2 they equal NCCL's a + b bit for bit.  Each thread owns whole 16-byte vectors (the
 // per-split C2 histogram is 1-2 MB of int64), so reading and then overwriting all R copies in place needs no barrier.  The rank loops are
 // unrolled to kMaxPeers with a guard, so the pointer table stays in the parameter bank instead of a local copy.
+constexpr int kMaxPeers = 16;      // ranks that may share one device (DecideLayout)
 struct SameDevicePtrs { void* p[kMaxPeers]; };
 template <typename T> struct RedSum { __device__ __forceinline__ static T f(T a, T b) { return a + b; } };
 template <typename T> struct RedMax { __device__ __forceinline__ static T f(T a, T b) { return b > a ? b : a; } };
@@ -1365,99 +1085,6 @@ k_allreduce_same_device(SameDevicePtrs bufs, int R, long long count, int vec) {
     for (int r = 0; r < kMaxPeers; ++r)
       if (r < R) static_cast<T*>(bufs.p[r])[i] = acc;
   }
-}
-
-// leaf choice by warp 0: ArgMax over leaves with SplitInfo::operator> (gain desc, real feature asc, first index), stop on gain <= 0
-
-// argmax over features per leaf (gain desc, real feature index asc), then over leaves
-// (SplitInfo::operator> : gain desc, feature asc; ArrayArgs::ArgMax keeps the first on full ties).
-
-
-// data-parallel pick: local argmax over the OWNED features, exchange of the per-rank winners through the peers'
-// mailboxes (C3, SyncUpGlobalBestSplit), global argmax with the same tie-breaks on every rank, then the usual leaf choice.
-__global__ void __launch_bounds__(256)
-k_pick_dp(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* __restrict__ cands, SplitParams p,
-          PeerTables pt, unsigned epoch) {
-  __shared__ double s_gain[256];
-  __shared__ int s_feat[256], s_idx[256];
-  const bool go = ctrl->go != 0;
-  if (go) {
-    for (int which = 0; which < 2; ++which) {
-      const int leaf = which ? ctrl->larger : ctrl->smaller;
-      double bg = kNegInf; int bf = 0x7fffffff, bi = -1;
-      if (leaf >= 0) {
-        for (int u = pt.feat0 + threadIdx.x; u < pt.feat1 && u < p.nf; u += blockDim.x) {
-          const SplitCand& c = cands[which * p.nf_pad + u];
-          const int rf = meta[u].real_index;
-          if (c.gain > bg || (c.gain == bg && rf < bf)) { bg = c.gain; bf = rf; bi = u; }
-        }
-      }
-      s_gain[threadIdx.x] = bg; s_feat[threadIdx.x] = bf; s_idx[threadIdx.x] = bi;
-      __syncthreads();
-      for (int s = 128; s; s >>= 1) {
-        if (threadIdx.x < s) {
-          double og = s_gain[threadIdx.x + s]; int of = s_feat[threadIdx.x + s];
-          if (og > s_gain[threadIdx.x] || (og == s_gain[threadIdx.x] && of < s_feat[threadIdx.x])) {
-            s_gain[threadIdx.x] = og; s_feat[threadIdx.x] = of; s_idx[threadIdx.x] = s_idx[threadIdx.x + s];
-          }
-        }
-        __syncthreads();
-      }
-      if (threadIdx.x < pt.world) {      // post this rank's winner into every peer's mailbox
-        SplitCand c;
-        c.gain = kNegInf; c.left_g = 0; c.left_h = 0; c.threshold = 0; c.left_count = 0; c.default_left = 1; c.feature = -1;
-        if (s_idx[0] >= 0 && s_gain[0] > kNegInf) c = cands[which * p.nf_pad + s_idx[0]];
-        SplitCand* dst = pt.mail[threadIdx.x] + pt.rank * 2 + which;
-        volatile double* dd = reinterpret_cast<volatile double*>(dst);
-        dd[0] = c.gain; dd[1] = c.left_g; dd[2] = c.left_h;
-        volatile int* di = reinterpret_cast<volatile int*>(dd + 3);
-        di[0] = c.threshold; di[1] = c.left_count; di[2] = c.default_left; di[3] = c.feature;
-      }
-      __syncthreads();
-    }
-  }
-  // barrier B: "candidates posted" (also means: every peer is done reading this rank's scratch histogram)
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x < pt.world) *reinterpret_cast<volatile unsigned*>(&pt.flags[threadIdx.x][16 + pt.rank]) = epoch;
-  if (threadIdx.x == 0) peer_wait(pt.flags[pt.rank] + 16, pt.world, epoch, pt.error);
-  __syncthreads();
-  if (threadIdx.x == 0 && go) {
-    for (int which = 0; which < 2; ++which) {
-      const int leaf = which ? ctrl->larger : ctrl->smaller;
-      if (leaf < 0) continue;
-      SplitCand best;
-      best.gain = kNegInf; best.feature = -1; best.left_g = best.left_h = 0; best.threshold = 0; best.left_count = 0; best.default_left = 1;
-      int best_rf = 0x7fffffff;
-      const SplitCand* mb = pt.mail[pt.rank];
-      for (int r = 0; r < pt.world; ++r) {
-        SplitCand c;
-        const volatile double* dd = reinterpret_cast<const volatile double*>(mb + r * 2 + which);
-        c.gain = dd[0]; c.left_g = dd[1]; c.left_h = dd[2];
-        const volatile int* di = reinterpret_cast<const volatile int*>(dd + 3);
-        c.threshold = di[0]; c.left_count = di[1]; c.default_left = di[2]; c.feature = di[3];
-        const int rf = c.feature < 0 ? 0x7fffffff : meta[c.feature].real_index;
-        if (c.gain > best.gain || (c.gain == best.gain && rf < best_rf)) { best = c; best_rf = rf; }
-      }
-      LeafState& L = leaves[leaf];
-      LeafBest b;
-      b.gain = kNegInf; b.feature = -1; b.threshold = 0; b.default_left = 1; b.left_count = 0; b.right_count = 0;
-      b.left_g = b.left_h = b.right_g = b.right_h = b.left_out = b.right_out = 0; b.is_cat = 0; b.cat_list_len = 0; b.pad = 0;
-      for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = 0u;
-      if (best.feature >= 0 && best.gain > kNegInf) {
-        const double sum_h = L.sum_h + 2 * kEpsD;
-        b.gain = best.gain; b.feature = best.feature; b.threshold = best.threshold; b.default_left = best.default_left;
-        b.left_count = best.left_count; b.right_count = L.global_count - best.left_count;
-        b.left_g = best.left_g; b.left_h = best.left_h - kEpsD;
-        b.right_g = L.sum_g - best.left_g; b.right_h = sum_h - best.left_h - kEpsD;
-        b.left_out = d_calc_output(best.left_g, best.left_h, p);
-        b.right_out = d_calc_output(L.sum_g - best.left_g, sum_h - best.left_h, p);
-      }
-      L.best = b;
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x < 32 && !ctrl->finished) d_choose_leaf(ctrl, leaves, meta, p, threadIdx.x);
 }
 
 // ---------------------------------------------------------------- column-major copy of the uint8 tiles (for the partition kernel)
@@ -1889,8 +1516,8 @@ __device__ __forceinline__ void d_block_excl3(long long& a, long long& b, long l
   __syncthreads();
 }
 
-// FeatureHistogram::FindBestThresholdSequentially for a WIDE numerical feature (max_bin > 255): the same two passes as d_scan_feature with the
-// bins spread over a 256-thread block — thread t owns the contiguous bins [t*S, (t+1)*S) — exclusive block scans of the per-thread
+// FeatureHistogram::FindBestThresholdSequentially for a numerical feature: its reverse pass and, for NaN-as-missing features, its forward
+// pass, with the bins spread over a 256-thread block — thread t owns the contiguous bins [t*S, (t+1)*S) — exclusive block scans of the per-thread
 // (g, h, count) sums, and a block argmax with the sequential scan's tie-breaks (reverse pass: the highest threshold wins, forward pass: the
 // lowest).  hist = the leaf's reduced histogram of the feature in its pool slot.  Returns through *outp (thread 0) and *flag.
 __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ hist, const WideMeta m, const LeafState& L, double inv_g, double inv_h,
@@ -1910,8 +1537,11 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
   const int b0 = threadIdx.x * S, b1 = min(b0 + S, m.num_bin);
   if (threadIdx.x == 0) { s_any = 0; s_stop[0] = -1; s_stop[1] = blockDim.x; }     // read after the barriers of d_block_excl3
   bool any_valid = false;
-  // ---- reverse pass: bins hi .. 1, candidate threshold = b - 1.  Both passes end at the sequential scan's first break, as in
-  // d_scan_feature: a thread stops its own bins there, and the threads after the first breaking one in scan order drop their candidates.
+  // ---- reverse pass: bins hi .. 1, candidate threshold = b - 1.  Both passes end where the sequential scan breaks: at the first candidate,
+  // in scan order, whose far side fails min_data_in_leaf or min_sum_hessian_in_leaf.  A thread stops its own bins there, and the threads
+  // after the first breaking one in scan order drop their candidates, so these neither win nor mark the feature splittable.  With hessians
+  // >= 0 nothing after a break could pass these tests anyway (counts and hessian sums are monotone); with negative hessians (custom
+  // objectives) they could.
   bool stop = false;
   double best_gain = kNegInf, best_lg = 0, best_lh = 0;
   int best_thr = -1, best_lc = 0, best_dl = 1;

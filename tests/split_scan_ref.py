@@ -1,5 +1,5 @@
-"""Plain NumPy/fp64 restatement of LightGBM 3.2's split search, used to pin the engine's scan kernels (K5/K6: k_scan, k_scan_wide,
-k_scan_dp) and the pick step (d_pick_block / d_choose_leaf) tree by tree.  It imports neither mmlspark_b200 nor oracle.
+"""Plain NumPy/fp64 restatement of LightGBM 3.2's split search, used to pin the engine's scan kernels (K5/K6: k_scan, k_scan_wide)
+and the pick step (d_pick_block / d_choose_leaf) tree by tree.  It imports neither mmlspark_b200 nor oracle.
 
 Restated from LightGBM 3.2 (FeatureHistogram, SerialTreeLearner):
 - FindBestThresholdNumerical: the reverse pass, the NaN-as-missing forward pass (incl. the implicit bin 0 when offset == 1) and

@@ -76,14 +76,10 @@ def run_ranks(X, y, rank_rows, params, iters, base_port, weight=None, push_chunk
     return out
 
 
-@pytest.mark.parametrize("objective,R,fused", [("regression", 2, 0), ("binary", 2, 0), ("binary", 2, 1), ("binary", 2, 2), ("regression", 2, 2),
-                                               ("binary", 4, 0), ("regression", 4, 1), ("binary", 4, 2)])
-def test_data_parallel_matches_oracle_emulation(built, objective, R, fused, monkeypatch):
-    """fused=1 selects the reduce-scatter + scan over NVLink peer memory (k_scan_dp / k_pick_dp) instead of ncclAllReduce, fused=2 the
-    two-shot all-reduce kernel over peer memory (k_allreduce_p2p) followed by the replicated scan."""
+@pytest.mark.parametrize("objective,R", [("regression", 2), ("binary", 2), ("binary", 4), ("regression", 4)])
+def test_data_parallel_matches_oracle_emulation(built, objective, R):
     if _ngpu() < R:
         pytest.skip("needs %d GPUs" % R)
-    monkeypatch.setenv("B200GBM_FUSED_REDUCE", str(fused))
     from mmlspark_b200.modeltext import parse_model, compare_models
     from oracle import oracle as O
     rng = np.random.default_rng(100 + R)
@@ -94,7 +90,7 @@ def test_data_parallel_matches_oracle_emulation(built, objective, R, fused, monk
     y = (s > 0).astype(np.float32) if objective == "binary" else s.astype(np.float32)
     rank_rows = [n // R + (7 if r == 0 else 0) - (7 if r == R - 1 else 0) for r in range(R)]     # unequal shards
     params = _params(objective, R, "is_unbalance=false" if objective == "binary" else "")
-    res = run_ranks(X, y, rank_rows, params, 15, 23000 + 40 * R + 9 * fused + (0 if objective == "binary" else 3))
+    res = run_ranks(X, y, rank_rows, params, 15, 23000 + 40 * R + (0 if objective == "binary" else 20))
     ods = O.OracleDataset(X, DS_PARAMS, rank_rows=rank_rows).set_field("label", y)
     ob = O.OracleBooster(ods, params)
     ob.train(15)
@@ -133,12 +129,11 @@ def test_rank_with_single_class_does_not_hang(built):
 
 
 @pytest.mark.parametrize("mode", ["bagging", "goss"])
-def test_data_parallel_row_sampling(built, mode, monkeypatch):
+def test_data_parallel_row_sampling(built, mode):
     """Every rank bags its own shard with its own per-block LCGs (seeded bagging_seed + local block); root counts and sums are
     all-reduced over the in-bag rows only."""
     if _ngpu() < 2:
         pytest.skip("needs 2 GPUs")
-    monkeypatch.setenv("B200GBM_FUSED_REDUCE", "0")
     from mmlspark_b200.modeltext import parse_model, compare_models
     from oracle import oracle as O
     rng = np.random.default_rng(321)
@@ -162,12 +157,11 @@ def test_data_parallel_row_sampling(built, mode, monkeypatch):
     np.testing.assert_allclose(got_scores, ob.scores(), rtol=1e-6, atol=1e-6)
 
 
-def test_data_parallel_push_rows_ingestion(built, monkeypatch):
+def test_data_parallel_push_rows_ingestion(built):
     """The path bench.py builds its shards with (LGBM_DatasetCreateFromSampledColumn + LGBM_DatasetPushRows, f32 chunks, ragged tail) on
     2 ranks: distributed bin finding from every rank's own sample, bins and trees equal to the oracle's 2-rank emulation."""
     if _ngpu() < 2:
         pytest.skip("needs 2 GPUs")
-    monkeypatch.setenv("B200GBM_FUSED_REDUCE", "0")
     from mmlspark_b200.modeltext import parse_model, compare_models
     from oracle import oracle as O
     rng = np.random.default_rng(77)

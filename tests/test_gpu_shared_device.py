@@ -42,9 +42,9 @@ def _cases(fn):
 
 
 # ------------------------------------------------------------------------------------------------ the existing scenarios on one device
-@pytest.mark.parametrize("objective,R,fused", _cases(M.test_data_parallel_matches_oracle_emulation))
-def test_multi_matches_oracle_emulation(built, one_device, objective, R, fused, monkeypatch):
-    M.test_data_parallel_matches_oracle_emulation(built, objective, R, fused, monkeypatch)
+@pytest.mark.parametrize("objective,R", _cases(M.test_data_parallel_matches_oracle_emulation))
+def test_multi_matches_oracle_emulation(built, one_device, objective, R):
+    M.test_data_parallel_matches_oracle_emulation(built, objective, R)
 
 
 def test_multi_rank_with_single_class(built, one_device):
@@ -52,12 +52,12 @@ def test_multi_rank_with_single_class(built, one_device):
 
 
 @pytest.mark.parametrize("mode", _cases(M.test_data_parallel_row_sampling))
-def test_multi_row_sampling(built, one_device, mode, monkeypatch):
-    M.test_data_parallel_row_sampling(built, mode, monkeypatch)
+def test_multi_row_sampling(built, one_device, mode):
+    M.test_data_parallel_row_sampling(built, mode)
 
 
-def test_multi_push_rows_ingestion(built, one_device, monkeypatch):
-    M.test_data_parallel_push_rows_ingestion(built, monkeypatch)
+def test_multi_push_rows_ingestion(built, one_device):
+    M.test_data_parallel_push_rows_ingestion(built)
 
 
 @pytest.mark.parametrize("fmt", _cases(B.test_two_ranks_bundled_equals_unbundled))
@@ -77,8 +77,6 @@ def test_estimator_two_tasks(built, one_device):
     E.test_two_tasks_two_gpus(built)
 
 
-@pytest.mark.xfail(reason="the driver numbers ranks in the order the tasks reach it, so the sparse and the dense fit may find the bins of "
-                          "a feature slice on different shards; this does not depend on the layout", strict=False)
 def test_sparse_estimator_two_tasks(built, one_device):
     S.test_two_tasks_sparse(built)
 
@@ -196,22 +194,17 @@ def test_three_ranks_unequal_shards(built, one_device):
     np.testing.assert_allclose(np.concatenate([res[r]["scores"] for r in range(3)]), ob.scores(), rtol=1e-6, atol=1e-6)
 
 
-def test_reduce_mode_is_same_device_under_every_fused_setting(built, monkeypatch):
-    """GetInfo reports world, rank and reduce mode 3; the peer-memory modes fall back to it, so their models equal mode 0's"""
+def test_reduce_mode_is_same_device(built):
+    """GetInfo reports world, rank and reduce mode 3, and both ranks hold the same model"""
     n = 40_000
     X_, y = _regression_data(41, n)
     rank_rows = [n // 2 + 99, n - n // 2 - 99]
     params = M._params("regression", 2)
-    models = {}
-    for fused in (0, 1, 2):
-        monkeypatch.setenv("B200GBM_FUSED_REDUCE", str(fused))
-        res, errs = _on_ranks(2, 26200 + 10 * fused, _train_shards(X_, y, rank_rows, params, 8))
-        assert not errs, errs
-        for r in range(2):
-            assert res[r]["info"]["num_machines"] == 2 and res[r]["info"]["rank"] == r and res[r]["info"]["reduce_mode"] == 3
-        assert res[1]["model"] == res[0]["model"]
-        models[fused] = res[0]["model"]
-    assert models[1] == models[0] and models[2] == models[0]
+    res, errs = _on_ranks(2, 26200, _train_shards(X_, y, rank_rows, params, 8))
+    assert not errs, errs
+    for r in range(2):
+        assert res[r]["info"]["num_machines"] == 2 and res[r]["info"]["rank"] == r and res[r]["info"]["reduce_mode"] == 3
+    assert res[1]["model"] == res[0]["model"]
 
 
 def test_column_copy_with_four_ranks_on_one_device(built, monkeypatch):

@@ -155,8 +155,12 @@ def test_two_tasks_sparse(built):
     if _ngpu() < 2:
         pytest.skip("needs 2 GPUs")
     from mmlspark_b200.lightgbm import LightGBMClassifier
-    _, X, z = _data(7, n=8000)
+    _, X, z = _data(7, n=4000)
     y = (z > np.median(z)).astype(np.float64)
+    # the two tasks get the same 4000 rows: the driver numbers ranks in the order the tasks reach it, and each rank finds the bins of
+    # a slice of the features on its own shard, so with different shards the two fits would agree only when their tasks arrive in
+    # the same order
+    X, y = np.vstack([X, X]), np.concatenate([y, y])
     md = LightGBMClassifier(numIterations=10, numTasks=2, defaultListenPort=25400).fit(_frame(X, {"label": y}))
     ms = LightGBMClassifier(numIterations=10, numTasks=2, defaultListenPort=25500).fit(_frame(sp.csr_matrix(X), {"label": y}))
     assert _model_string(ms) == _model_string(md)
