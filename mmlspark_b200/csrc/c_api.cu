@@ -597,7 +597,7 @@ int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess) 
 }
 int B200GBM_BoosterSetProfile(BoosterHandle handle, int profile_hist) {
   API_BEGIN();
-  BS(handle)->profile_hist = profile_hist != 0;
+  BS(handle)->SetProfile(profile_hist != 0);
   API_END();
 }
 int B200GBM_BoosterGetTiming(BoosterHandle handle, double* out6, int reset) {

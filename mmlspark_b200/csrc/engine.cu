@@ -1340,8 +1340,9 @@ void Dataset::SetFeatureNames(const char** names, int n) {
 }
 
 // =============================================================================== booster
-static size_t Align16(size_t x) { return (x + 15) & ~static_cast<size_t>(15); }
-constexpr int kScanSmem = (768 + 64) * 8;         // k_scan: scratch of the categorical split search (one warp per block runs it)
+}  // namespace b200gbm
+#include "tree_learner.cu"      // the booster's tree learner, in this translation unit
+namespace b200gbm {
 
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
@@ -1400,16 +1401,8 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
 }
 
 Booster::~Booster() {
-  if (split_op_trees_ > 0) {
-    double tot = 0; for (auto& kv : split_op_ms_) tot += kv.second;
-    fprintf(stderr, "[b200gbm split timing] %d trees, %.3f ms per tree in split operations:", split_op_trees_, tot / split_op_trees_);
-    for (auto& kv : split_op_ms_) fprintf(stderr, " %s=%.1fus", kv.first.c_str(), 1000.0 * kv.second / split_op_trees_ / std::max(cfg.num_leaves - 1, 1));
-    fprintf(stderr, " (per split)\n");
-  }
+  learner_.reset();
   for (auto* v : valids_) delete v;
-  if (tree_host_) cudaFreeHost(tree_host_);
-  if (ctrl_host_) cudaFreeHost(ctrl_host_);
-  if (leaves_host_) cudaFreeHost(leaves_host_);
   if (ev_a_) cudaEventDestroy(ev_a_);
   if (ev_b_) cudaEventDestroy(ev_b_);
   ReleaseStream(stream_);
@@ -1417,81 +1410,13 @@ Booster::~Booster() {
 
 void Booster::InitTraining() {
   const int n = train->num_data;
-  const int L = cfg.num_leaves;
   cudaDeviceProp prop;
   B200_CUDA(cudaGetDeviceProperties(&prop, device_));
   num_sms_ = prop.multiProcessorCount;
   stream_ = AcquireStream();
   B200_CUDA(cudaEventCreate(&ev_a_)); B200_CUDA(cudaEventCreate(&ev_b_));
-  // leaf passes gather single 32-byte sectors: ask L2 not to fetch the neighbouring sector from DRAM on a miss (default 64 B).
-  // A hint for the sparse leaf passes; streamed passes read whole sectors anyway.
-  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
-  cudaGetLastError();
-  B200_CUDA(set_k4_smem_limit());
-  B200_CUDA(cudaFuncSetAttribute(k_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
-
-  sp_.l1 = cfg.lambda_l1; sp_.l2 = cfg.lambda_l2; sp_.max_delta_step = cfg.max_delta_step;
-  sp_.min_gain_to_split = cfg.min_gain_to_split; sp_.min_sum_hessian = cfg.min_sum_hessian_in_leaf;
-  sp_.min_data_in_leaf = cfg.min_data_in_leaf; sp_.max_depth = cfg.max_depth; sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
-  sp_.nf = train->nf; sp_.nf_pad = train->nf_pad; sp_.num_tiles = train->num_tiles; sp_.nfn = train->nfn;
-  {   // categorical split search parameters (Config keeps the native defaults unless given, SURVEY.md B.2)
-    sp_.cat_l2 = cfg.cat_l2; sp_.cat_smooth = cfg.cat_smooth;
-    sp_.max_cat_threshold = cfg.max_cat_threshold; sp_.max_cat_to_onehot = cfg.max_cat_to_onehot;
-    sp_.min_data_per_group = cfg.min_data_per_group; sp_.pad3 = 0;
-    if (train->nw > 0) {
-      if (sp_.max_cat_threshold > kCatListMax) Fatal("max_cat_threshold > " + std::to_string(kCatListMax) + " is not supported together with categorical features of more than 256 bins");
-      if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");
-      B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
-      B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
-    }
-  }
-
   score_.Alloc(static_cast<size_t>(K) * n); score_.Zero(stream_);
   grad_.Alloc(static_cast<size_t>(K) * n); hess_.Alloc(static_cast<size_t>(K) * n);
-  qgh_.Alloc(n); qord_.Alloc(n); idx0_.Alloc(n); idx1_.Alloc(n);
-  slot_elems_ = train->hist_pairs * 2;
-  H_.Alloc(slot_elems_); H_.Zero(stream_); pool_.Alloc(slot_elems_ * L);
-  {
-    int per_sm = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_partition, 256, 0));
-    int coop = 0;
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device_);
-    if (!coop || per_sm < 1) Fatal("this device cannot launch the cooperative partition kernel");
-    part_max_blocks_ = per_sm * num_sms_;
-  }
-  flags_.Alloc(static_cast<size_t>(L) * train->nf_pad);
-  cands_.Alloc(2 * static_cast<size_t>(train->nf_pad));
-  leaves_.Alloc(L); ctrl_.Alloc(1); ctrl_.Zero(stream_);
-  const int chunks = n / kPartChunk + 2;
-  part_bits_.Alloc(static_cast<size_t>(chunks) * (kPartChunk / 32)); part_chunks_.Alloc(static_cast<size_t>(chunks) + chunks / kPartLocalScan + 8); part_chunks_.Zero(stream_);      // + the super-chunk totals of the two-level scan
-  // SoA tree blob
-  {
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += Align16(bytes); return o; };
-    size_t o_lc = take(4 * (L - 1)), o_rc = take(4 * (L - 1)), o_sf = take(4 * (L - 1)), o_tb = take(4 * (L - 1)), o_dt = take(4 * (L - 1));
-    size_t o_sg = take(4 * (L - 1)), o_lv = take(8 * L), o_lw = take(8 * L), o_lcn = take(4 * L), o_iv = take(8 * (L - 1)), o_iw = take(8 * (L - 1));
-    size_t o_ic = take(4 * (L - 1)), o_lp = take(4 * L), o_ld = take(4 * L), o_nl = take(16), o_cb = take(32 * (L - 1));
-    size_t o_cl = take(2 * kCatListMax * (L - 1)), o_cn = take(4 * (L - 1));
-    tree_blob_bytes_ = off;
-    tree_blob_.Alloc(off);
-    unsigned char* b = tree_blob_.p;
-    tree_dev_.left_child = reinterpret_cast<int*>(b + o_lc); tree_dev_.right_child = reinterpret_cast<int*>(b + o_rc);
-    tree_dev_.split_feature_inner = reinterpret_cast<int*>(b + o_sf); tree_dev_.threshold_bin = reinterpret_cast<int*>(b + o_tb);
-    tree_dev_.decision_type = reinterpret_cast<int*>(b + o_dt); tree_dev_.split_gain = reinterpret_cast<float*>(b + o_sg);
-    tree_dev_.leaf_value = reinterpret_cast<double*>(b + o_lv); tree_dev_.leaf_weight = reinterpret_cast<double*>(b + o_lw);
-    tree_dev_.leaf_count = reinterpret_cast<int*>(b + o_lcn); tree_dev_.internal_value = reinterpret_cast<double*>(b + o_iv);
-    tree_dev_.internal_weight = reinterpret_cast<double*>(b + o_iw); tree_dev_.internal_count = reinterpret_cast<int*>(b + o_ic);
-    tree_dev_.leaf_parent = reinterpret_cast<int*>(b + o_lp); tree_dev_.leaf_depth = reinterpret_cast<int*>(b + o_ld);
-    tree_dev_.num_leaves = reinterpret_cast<int*>(b + o_nl);
-    tree_dev_.cat_bits = reinterpret_cast<unsigned*>(b + o_cb);
-    tree_dev_.cat_list = reinterpret_cast<unsigned short*>(b + o_cl);
-    tree_dev_.cat_list_len = reinterpret_cast<int*>(b + o_cn);
-    B200_CUDA(cudaMemsetAsync(b, 0, off, stream_));
-    B200_CUDA(cudaMallocHost(reinterpret_cast<void**>(&tree_host_), off));
-    B200_CUDA(cudaMallocHost(reinterpret_cast<void**>(&ctrl_host_), sizeof(TreeCtrl)));
-    B200_CUDA(cudaMallocHost(reinterpret_cast<void**>(&leaves_host_), sizeof(LeafState) * L));
-  }
   // init score from the dataset
   if (!train->init_score.empty()) {
     if (train->init_score.size() != static_cast<size_t>(K) * n) Fatal("Initial score size doesn't match data size");
@@ -1500,23 +1425,7 @@ void Booster::InitTraining() {
   }
   obj_->Init(stream_);
   const_hessian_ = obj_->ConstHessian() && !is_goss_;      // GOSS amplifies hessians [LightGBM goss.hpp GetIsConstHessian -> false]
-  if (obj_->RenewsLeaves()) {      // sort buffers of the renewal pass (renew_kernel.cuh)
-    rn_keys_a_.Alloc(n); rn_keys_b_.Alloc(n); rn_pos_a_.Alloc(n); rn_pos_b_.Alloc(n); rn_leaf_of_pos_.Alloc(n); rn_leaf_a_.Alloc(n); rn_leaf_b_.Alloc(n);
-    rn_res_.Alloc(n); rn_row_.Alloc(n); rn_seg_.Alloc(L + 1); rn_out_.Alloc(2 * static_cast<size_t>(L));
-    if (obj_->RenewWeights()) rn_cdf_.Alloc(n);
-    size_t t1 = 0, t2 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t1, rn_keys_a_.p, rn_keys_b_.p, rn_pos_a_.p, rn_pos_b_.p, n, 0, 64, stream_);
-    cub::DeviceRadixSort::SortPairs(nullptr, t2, rn_leaf_a_.p, rn_leaf_b_.p, rn_pos_b_.p, rn_pos_a_.p, n, 0, 32, stream_);
-    rn_tmp_bytes_ = std::max(t1, t2);
-    rn_tmp_.Alloc(rn_tmp_bytes_ + 16);
-  }
-  // ColSampler: one draw at init, then one per tree ([UPSTREAM] ColSampler::SetTrainingData / ResetByTree)
-  col_rand_ = LcgRandom(cfg.feature_fraction_seed);
-  feature_used_host_.assign(train->nf_pad, 0);
-  for (int u = 0; u < train->nf; ++u) feature_used_host_[u] = 1;
-  feature_used_.Alloc(train->nf_pad);
-  feature_used_.Upload(feature_used_host_.data(), train->nf_pad, stream_);
-  ResetFeaturesByTree();
+  learner_.reset(new TreeLearner(*train, cfg, *obj_, parallel_, same_device_, num_sms_, stream_, timing));      // after Init: renewal weights
   if (bagging_ || is_goss_) {
     bag_blocks_ = (n + kBagBlock - 1) / kBagBlock;
     std::vector<unsigned> st(bag_blocks_);
@@ -1548,14 +1457,6 @@ void Booster::InitTraining() {
 }
 
 // ---- DART [LightGBM src/boosting/dart.hpp]
-TreeDev Booster::RebasedTree(unsigned char* base) const {
-  TreeDev t = tree_dev_;
-  auto mv = [&](auto*& p) { p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + (reinterpret_cast<unsigned char*>(p) - tree_blob_.p)); };
-  mv(t.left_child); mv(t.right_child); mv(t.split_feature_inner); mv(t.threshold_bin); mv(t.decision_type); mv(t.split_gain);
-  mv(t.leaf_value); mv(t.leaf_weight); mv(t.leaf_count); mv(t.internal_value); mv(t.internal_weight); mv(t.internal_count);
-  mv(t.leaf_parent); mv(t.leaf_depth); mv(t.num_leaves); mv(t.cat_bits); mv(t.cat_list); mv(t.cat_list_len);
-  return t;
-}
 // ScoreUpdater::AddScore(models_[tree], class): the tree's CURRENT host leaf values (after the Shrinkage calls) are pushed into
 // its stored device blob and every row walks the tree on its bins.
 void Booster::AddStoredTree(int iter_index, int k, bool to_train, bool to_valid) {
@@ -1572,7 +1473,7 @@ void Booster::AddStoredTree(int iter_index, int k, bool to_train, bool to_valid)
     return;
   }
   DevBuf<unsigned char>& blob = *tree_store_.at(static_cast<size_t>(iter_index) * K + k);
-  TreeDev td = RebasedTree(blob.p);
+  TreeDev td = learner_->TreeAt(blob.p);
   B200_CUDA(cudaMemcpyAsync(td.leaf_value, ht.leaf_value.data(), sizeof(double) * ht.num_leaves, cudaMemcpyHostToDevice, s));
   const int egrid = num_sms_ * 8;
   if (to_train) k_add_tree_binned<<<egrid, 256, 0, s>>>(td, train->meta.p, train->View(), n, score_.p + static_cast<size_t>(k) * n, 1.0);
@@ -1663,17 +1564,6 @@ void Booster::Bagging(int it) {
   use_bag_ = true;
 }
 
-void Booster::ResetFeaturesByTree() {
-  if (cfg.feature_fraction >= 1.0) return;
-  const int total = train->nf;
-  int cnt = std::max(static_cast<int>(total * cfg.feature_fraction + 0.5), std::min(2, total));
-  std::fill(feature_used_host_.begin(), feature_used_host_.end(), 0);
-  for (int i : col_rand_.Sample(total, cnt)) feature_used_host_[train->sample_order[i]] = 1;      // the draw indexes the used features in real-index order
-  // no host sync: the copy is ordered after the previous tree's kernels on the same stream, and a copy from pageable memory is staged
-  // by the driver before the call returns, so the host vector may be rewritten for the next tree
-  feature_used_.Upload(feature_used_host_.data(), train->nf_pad, stream_);
-}
-
 double Booster::BoostFromAverage(int k) {
   if (model.trees.empty() && !has_init_score_ && cfg.boost_from_average) {
     double init = obj_->BoostFromScore(k);
@@ -1695,349 +1585,49 @@ void Booster::ComputeGradientsAt(const double* score_p) {
   timing.launches += 1;
 }
 
-// [LightGBM SerialTreeLearner::RenewTreeOutput] device pass described in renew_kernel.cuh; patches tree_dev_.leaf_value in place
-void Booster::RenewTreeOutput(int k, double rf_pred) {
-  const int n = train->num_data;
-  const int total = use_bag_ ? bag_count_ : n;
-  const int L = cfg.num_leaves;
-  cudaStream_t s = stream_;
-  TreeCtrl* ctrl = ctrl_.p;
-  const int egrid = num_sms_ * 8;
-  const float* wptr = obj_->RenewWeights();      // null: unweighted
-  k_renew_gather<<<egrid, 256, 0, s>>>(ctrl, leaves_.p, idx0_.p, idx1_.p, train->d_label.p, is_rf_ ? nullptr : score_.p + static_cast<size_t>(k) * n, rf_pred,
-                                       rn_keys_a_.p, rn_pos_a_.p, rn_res_.p, rn_leaf_of_pos_.p, rn_row_.p);
-  size_t tb = rn_tmp_bytes_;
-  B200_CUDA(cub::DeviceRadixSort::SortPairs(rn_tmp_.p, tb, rn_keys_a_.p, rn_keys_b_.p, rn_pos_a_.p, rn_pos_b_.p, total, 0, 64, s));
-  k_renew_leaf_keys<<<egrid, 256, 0, s>>>(rn_pos_b_.p, rn_leaf_of_pos_.p, total, rn_leaf_a_.p);
-  int leaf_bits = 1;
-  while ((1 << leaf_bits) < L) ++leaf_bits;
-  tb = rn_tmp_bytes_;
-  B200_CUDA(cub::DeviceRadixSort::SortPairs(rn_tmp_.p, tb, rn_leaf_a_.p, rn_leaf_b_.p, rn_pos_b_.p, rn_pos_a_.p, total, 0, leaf_bits, s));
-  k_renew_offsets<<<1, 32, 0, s>>>(ctrl, leaves_.p, rn_seg_.p);
-  double* out = rn_out_.p;
-  double* has = rn_out_.p + L;
-  const int lgrid = (L + 127) / 128;
-  if (!wptr) {
-    k_renew_unweighted<<<lgrid, 128, 0, s>>>(ctrl, rn_seg_.p, rn_pos_a_.p, rn_res_.p, obj_->RenewAlpha(), out, has);
-  } else {
-    k_renew_cdf<<<L, 1024, 0, s>>>(ctrl, rn_seg_.p, rn_pos_a_.p, rn_row_.p, wptr, rn_cdf_.p);
-    k_renew_weighted<<<lgrid, 128, 0, s>>>(ctrl, rn_seg_.p, rn_pos_a_.p, rn_res_.p, rn_cdf_.p, obj_->RenewAlpha(), out, has);
-  }
-  if (parallel_) Net().AllReduce(out, 2 * static_cast<size_t>(L), ncclDouble, ncclSum, s);
-  k_renew_apply<<<lgrid, 128, 0, s>>>(ctrl, tree_dev_, out, has, parallel_ ? 1 : 0);
-  B200_CUDA(cudaGetLastError());
-  timing.launches += wptr ? 7 : 6;
-}
-
-// k_partition is launched cooperatively: its software grid barriers need every block resident
-// Column-major copies of the training tiles for k_partition, so that its phase 1 reads one byte per row instead of a 32-byte sector —
-// same results either way.  Set up once, before the first tree, after every other buffer of the booster exists, and only within a
-// reserve of device memory (validation scores, metric and prediction scratch come later); B200GBM_COLUMN_COPY=0 disables it.
-//   full copy     every storage column (kernels.cuh: k_tiles_to_columns), if it fits
-//   column cache  otherwise a pool of as many column slots as fit, filled between trees with the columns the trees split on
-//                 (UpdateColumnCache); B200GBM_COLUMN_CACHE_COLUMNS=k forces this mode with at most k slots
-// With R ranks on one device (same-device network) all of them reach this point at their first tree, when every rank's training buffers
-// exist: they measure the free memory before any of them allocates a copy, and each takes at most 1/R of what lies above the reserve.
-void Booster::EnsureColumnCopy() {
-  if (cols_tried_) return;
-  cols_tried_ = true;
-  const Dataset& d = *train;
-  const char* env = std::getenv("B200GBM_COLUMN_COPY");
-  if ((env && std::atoi(env) == 0) || d.nfn == 0) return;      // the same on every rank: the ranks share the bin layout and the process
-  size_t free_b = 0, total_b = 0;
-  const bool mem_ok = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
-  if (!mem_ok) cudaGetLastError();
-  size_t share = 1;
-  if (same_device_) {
-    double arrived = 0.0;
-    AllReduceHost(&arrived, 1, ncclSum, stream_);      // every rank built its buffers
-    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
-    double f = mem_ok ? static_cast<double>(free_b) : 0.0;
-    AllReduceHost(&f, 1, ncclMin, stream_);            // every rank measured before any allocates
-    free_b = static_cast<size_t>(f);
-    share = static_cast<size_t>(Net().world);
-  }
-  if (!mem_ok || d.num_data == 0) return;
-  const char* force = std::getenv("B200GBM_COLUMN_CACHE_COLUMNS");
-  const size_t stride = (static_cast<size_t>(d.num_data) + 255) & ~static_cast<size_t>(255);
-  const int ncols = d.num_tiles * 32;
-  const size_t need = static_cast<size_t>(ncols) * stride;
-  const size_t reserve = std::max<size_t>(static_cast<size_t>(8) << 30, total_b / 10);
-  const size_t spare = free_b > reserve ? (free_b - reserve) / share : 0;
-  const bool full = !force && spare >= need;
-  int slots = ncols;
-  if (!full) {
-    slots = static_cast<int>(std::min<size_t>(d.num_columns, spare / stride));
-    if (force) slots = std::min(slots, std::max(0, std::atoi(force)));
-    if (slots == 0) return;
-  }
-  const size_t bytes = static_cast<size_t>(slots) * stride;
-  uint8_t* p = nullptr;
-  if (cudaMalloc(reinterpret_cast<void**>(&p), bytes) != cudaSuccess) { cudaGetLastError(); return; }
-  bins_cols_.p = p; bins_cols_.n = bytes;
-  cols_stride_ = stride;
-  col_slot_host_.assign(ncols, -1);
-  if (full) {
-    for (int c = 0; c < ncols; ++c) col_slot_host_[c] = c;
-    const long long work = ((static_cast<long long>(d.num_data) + 255) / 256) * d.num_tiles;
-    k_tiles_to_columns<<<static_cast<unsigned>(std::min<long long>(work, static_cast<long long>(num_sms_) * 16)), 256, 0, stream_>>>(
-        d.bins.p, d.rows_stride, d.num_tiles, d.num_data, bins_cols_.p, stride);
-    B200_CUDA(cudaGetLastError());
-  } else {
-    slot_col_.assign(slots, -1);
-    col_splits_.assign(ncols, 0);
-  }
-  col_slot_.Alloc(ncols);
-  col_slot_.Upload(col_slot_host_.data(), ncols, stream_);
-}
-
-// Column cache, after each tree (its host copy is read back, the stream is idle): count the tree's splits per storage column (wide
-// features have their own uint16 columns and are not counted), then copy the most split-on columns that are not cached into free slots.
-// When the pool is full, a candidate replaces the least split-on cached column only if that one has fewer splits, so columns that are
-// split on often stay.  At most kColumnBuildsMax columns (N x 32 bytes read each) are built per tree, in one launch on the stream;
-// the next tree's partitions see the new slot table in stream order, with no host sync inside the tree.
-void Booster::UpdateColumnCache(const HostTree& t) {
-  if (slot_col_.empty()) return;
-  const Dataset& d = *train;
-  for (int i = 0; i + 1 < t.num_leaves; ++i) {
-    const int f = t.split_feature_inner[i];
-    if (f < d.nfn) ++col_splits_[d.meta_host[f].hist_off >> 8];
-  }
-  std::vector<int> cand;
-  for (int c = 0; c < static_cast<int>(col_splits_.size()); ++c)
-    if (col_splits_[c] > 0 && col_slot_host_[c] < 0) cand.push_back(c);
-  std::stable_sort(cand.begin(), cand.end(), [&](int a, int b) { return col_splits_[a] > col_splits_[b]; });
-  ColumnJobs jobs{};
-  for (int c : cand) {
-    if (jobs.n == kColumnBuildsMax) break;
-    int slot = -1, victim = -1;
-    for (int s = 0; s < static_cast<int>(slot_col_.size()) && slot < 0; ++s) {
-      const int held = slot_col_[s];
-      if (held < 0) slot = s;
-      else if (victim < 0 || col_splits_[held] < col_splits_[slot_col_[victim]]) victim = s;
-    }
-    if (slot < 0) {
-      if (col_splits_[slot_col_[victim]] >= col_splits_[c]) break;      // candidates come in descending order: none later wins either
-      slot = victim;
-      col_slot_host_[slot_col_[slot]] = -1;
-      ++cache_evictions_;
-    }
-    slot_col_[slot] = c;
-    col_slot_host_[c] = slot;
-    jobs.col[jobs.n] = c; jobs.slot[jobs.n] = slot; ++jobs.n;
-  }
-  if (jobs.n == 0) return;
-  const long long words = (static_cast<long long>(d.num_data) + 3) / 4;
-  const unsigned gx = static_cast<unsigned>(std::max<long long>(1, std::min<long long>((words + 255) / 256, static_cast<long long>(num_sms_) * 8)));
-  k_tiles_to_column_slots<<<dim3(gx, jobs.n), 256, 0, stream_>>>(d.bins.p, d.rows_stride, d.num_data, jobs, bins_cols_.p, cols_stride_);
-  B200_CUDA(cudaGetLastError());
-  col_slot_.Upload(col_slot_host_.data(), col_slot_host_.size(), stream_);
-  cache_builds_ += jobs.n;
-  timing.launches += 1;
+void Booster::SetProfile(bool profile_hist) {
+  if (learner_) learner_->profile_hist = profile_hist;
 }
 
 void Booster::GetMemoryInfo(int64_t* out2) {
   EnsureDevice();
   size_t free_b = 0, total_b = 0;
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
-  out2[0] = static_cast<int64_t>(bins_cols_.n);
+  out2[0] = learner_ ? static_cast<int64_t>(learner_->ColumnCopyBytes()) : 0;
   out2[1] = static_cast<int64_t>(free_b);
 }
 
 void Booster::GetColumnCacheInfo(int64_t* out4) const {
-  out4[0] = static_cast<int64_t>(slot_col_.size());
-  out4[1] = static_cast<int64_t>(std::count_if(slot_col_.begin(), slot_col_.end(), [](int c) { return c >= 0; }));
-  out4[2] = cache_builds_;
-  out4[3] = cache_evictions_;
+  if (learner_) learner_->GetColumnCacheInfo(out4);
+  else std::fill(out4, out4 + 4, 0);
 }
 
-void Booster::LaunchPartition(int grid, int last) {
-  const Dataset& d = *train;
-  TreeCtrl* ctrl = ctrl_.p;
-  LeafState* leaves = leaves_.p;
-  TreeDev tree = tree_dev_;
-  uint8_t* flags = flags_.p;
-  const FeatMeta* meta = d.meta.p;
-  SplitParams sp = sp_;
-  const uint8_t* bins = d.bins.p;
-  size_t rows_stride = d.rows_stride;
-  int* i0 = idx0_.p; int* i1 = idx1_.p;
-  unsigned* bits = part_bits_.p;
-  int* chunks = part_chunks_.p;
-  const int4* qgh = qgh_.p;
-  int4* qord = qord_.p;
-  long long* H = H_.p;
-  size_t h_elems = slot_elems_;
-  const uint16_t* bins16 = d.bins16.p;
-  static const int tickets = [] { const char* e = std::getenv("B200GBM_PART_TICKETS"); return e ? std::atoi(e) : 8; }();      // 0: one chunk per ticket
-  int tickets_per_block = tickets;
-  const uint8_t* cols = bins_cols_.p;
-  size_t cols_stride = cols_stride_;
-  const int* col_slot = col_slot_.p;
-  int* super_tot = part_chunks_.p + (train->num_data / kPartChunk + 2);
-  const int* bundle_base = d.BundleBase();
-  void* args[] = {&ctrl, &leaves, &tree, &flags, &meta, &sp, &last, &bins, &rows_stride, &i0, &i1, &bits, &chunks, &qgh, &qord, &H, &h_elems, &bins16, &tickets_per_block,
-                  &cols, &cols_stride, &col_slot, &super_tot, &bundle_base};
-  B200_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(k_partition), dim3(grid), dim3(256), args, 0, stream_));
-}
-
-// One tree: the whole leaf-wise growth is enqueued without a host sync; leaf choice, smaller/larger
-// selection, partition sizes all live in TreeCtrl / LeafState on the device.
+// One tree: the learner grows it on class k's (g, h) and renews its leaves; the tree is applied to the training and validation scores
+// on the device, then read back.
 void Booster::TrainOneTree(int k, HostTree* out) {
   NvtxRange nvtx_tree("b200gbm:tree");
-  EnsureColumnCopy();
   const Dataset& d = *train;
   const int n = d.num_data;
-  const int L = cfg.num_leaves;
-  const float* g = grad_.p + static_cast<size_t>(k) * n;
-  const float* h = hess_.p + static_cast<size_t>(k) * n;
-  TreeCtrl* ctrl = ctrl_.p;
+  double* score_k = score_.p + static_cast<size_t>(k) * n;
   cudaStream_t s = stream_;
   const int egrid = num_sms_ * 8;
-  nvtxRangePushA("b200gbm:K3 quantize + C1 root sums");
-  B200_CUDA(cudaMemsetAsync(&ctrl->absmax_bits[0], 0, 8, s));
-  k_absmax<<<egrid, 256, 0, s>>>(g, h, n, ctrl);
-  if (parallel_) Net().AllReduce(&ctrl->absmax_bits[0], 2, ncclUint32, ncclMax, s);
-  k_set_scale<<<1, 1, 0, s>>>(ctrl, const_hessian_ ? 1 : 0, 1.0);
-  k_quantize<<<egrid, 256, 0, s>>>(g, h, n, qgh_.p, ctrl, const_hessian_ ? 1 : 0, use_bag_ ? in_bag_.p : nullptr, bag_count_);
-  if (parallel_) Net().AllReduce(&ctrl->root_q[0], 3, ncclInt64, ncclSum, s);
-  ResetFeaturesByTree();
-  if (use_bag_)      // the root leaf is the ascending in-bag row list (SetBaggingData); partitions then ping-pong idx0/idx1 as usual
-    B200_CUDA(cudaMemcpyAsync(idx0_.p, bag_idx_.p, static_cast<size_t>(bag_count_) * sizeof(int), cudaMemcpyDeviceToDevice, s));
-  k_tree_init<<<1, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, flags_.p, sp_, use_bag_ ? bag_count_ : n, feature_used_.p, use_bag_ ? 1 : 0);
-  nvtxRangePop();
-  timing.launches += 4;
-  const int pgrid = std::max(1, std::min(n / kPartChunk + 1, part_max_blocks_));
-  const dim3 sgrid(std::max(1, d.nfn), 2);      // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates
-  const RowBlockBound bound = d.BlockBound();
-  std::vector<cudaEvent_t> evs;
-  // B200GBM_SPLIT_TIMING=1 (debug): an event after every operation of a split; per-operation averages go to stderr when the booster is freed
-  static const bool split_timing = getenv("B200GBM_SPLIT_TIMING") != nullptr;
-  std::vector<cudaEvent_t> sev;
-  auto mark = [&]() { if (split_timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); sev.push_back(e); } };
-  // round 0's controller is its own launch; every later round's runs in the tail of the previous round's partition kernel
-  k_round_ctl<<<1, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, flags_.p, d.meta.p, sp_, 0);
-  timing.launches += 1;
-  for (int split = 0; split < L - 1; ++split) {
-    mark();
-    if (profile_hist) { cudaEvent_t a, b; B200_CUDA(cudaEventCreate(&a)); B200_CUDA(cudaEventCreate(&b)); evs.push_back(a); evs.push_back(b); B200_CUDA(cudaEventRecord(a, s)); }
-    // leaf order of the (g,h) words: written by the previous split's partition kernel; only a bagged root needs its own pass
-    if (split == 0 && use_bag_) k_gather_q<<<egrid, 256, 0, s>>>(&ctrl->hist_work, idx0_.p, idx1_.p, qgh_.p, qord_.p);
-    mark();
-    // the scratch histogram H is zero here: zeroed at set-up and by every partition kernel after the scan consumed it
-    nvtxRangePushA("b200gbm:K4 histogram");
-    launch_k4(const_hessian_, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-              reinterpret_cast<unsigned long long*>(H_.p), bound, num_sms_, s);
-    if (d.nw > 0) {      // the features with more than 256 bins: own sub-histogram layout (k4_hist_wide)
-      int max_nb = 0;
-      for (const WideMeta& wm : d.wide_host) max_nb = std::max(max_nb, wm.num_bin);
-      const int segs = (max_nb + kWideHistSeg - 1) / kWideHistSeg;      // z: 8192-bin segments of the largest feature
-      // x: row parts, chosen so that the CTAs that have work (a (feature, segment) pair past the feature's last bin exits at once) make
-      // about four waves of one CTA per SM (128 KB of shared memory each)
-      int units = 0;
-      for (const WideMeta& wm : d.wide_host) units += (wm.num_bin + kWideHistSeg - 1) / kWideHistSeg;
-      const dim3 wgrid(static_cast<unsigned>(std::max(1, std::min(64, 4 * num_sms_ / std::max(1, units)))), static_cast<unsigned>(d.nw), static_cast<unsigned>(segs));
-      if (const_hessian_)
-        k4_hist_wide<3><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.wide_meta.p, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-                                                                         reinterpret_cast<unsigned long long*>(H_.p));
-      else
-        k4_hist_wide<4><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.wide_meta.p, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
-                                                                         reinterpret_cast<unsigned long long*>(H_.p));
-      timing.launches += 1;
-    }
-    nvtxRangePop();
-    if (profile_hist) B200_CUDA(cudaEventRecord(evs.back(), s));
-    mark();
-    nvtxRangePushA(parallel_ ? "b200gbm:C2 histogram reduce + K5 scan + pick" : "b200gbm:K5 scan + pick");
-    if (parallel_) Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
-    mark();
-    if (d.nw > 0) {
-      k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
-      timing.launches += 1;
-    }
-    // scan + (last block) pick; the dynamic scratch is only touched by categorical features and bundle members
-    k_scan<<<sgrid, 256, (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase());
-    nvtxRangePop();
-    mark();
-    nvtxRangePushA("b200gbm:K7 partition + controller");
-    LaunchPartition(pgrid, split == L - 2 ? 1 : 0);
-    nvtxRangePop();
-    mark();
-    timing.launches += 3; timing.hist_launches += 1;
-  }
-  if (obj_->RenewsLeaves()) RenewTreeOutput(k, is_rf_ ? rf_init_scores_[k] : 0.0);
+  const TreeLearner::Bag bag{in_bag_.p, bag_idx_.p, bag_count_};
+  learner_->Grow(grad_.p + static_cast<size_t>(k) * n, hess_.p + static_cast<size_t>(k) * n, const_hessian_, use_bag_ ? &bag : nullptr);
+  if (obj_->RenewsLeaves()) learner_->Renew(*obj_, is_rf_ ? nullptr : score_k, is_rf_ ? rf_init_scores_[k] : 0.0);
   // rf keeps scores as the running average of (tree + init score) over the iterations [LightGBM rf.hpp MultiplyScore / UpdateScore]
   const double bias = is_rf_ ? rf_init_scores_[k] : 0.0, pre = is_rf_ ? static_cast<double>(iter + num_init_iteration) : 1.0;
   const double post = is_rf_ ? 1.0 / (iter + num_init_iteration + 1) : 1.0;
+  const TreeDev& tree = learner_->Tree();
   if (use_bag_ || is_rf_)      // out-of-bag rows are scored by walking the tree on the binned data, so walk it for every row
-    k_add_tree_binned<<<egrid, 256, 0, s>>>(tree_dev_, d.meta.p, d.View(), n, score_.p + static_cast<size_t>(k) * n, shrinkage_, bias, pre, post);
+    k_add_tree_binned<<<egrid, 256, 0, s>>>(tree, d.meta.p, d.View(), n, score_k, shrinkage_, bias, pre, post);
   else
-    k_add_score<<<egrid, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, idx0_.p, idx1_.p, score_.p + static_cast<size_t>(k) * n, shrinkage_);
+    learner_->AddScore(score_k, shrinkage_);
   for (auto* v : valids_)
-    k_add_tree_binned<<<egrid, 256, 0, s>>>(tree_dev_, v->ds->meta.p, v->ds->View(), v->ds->num_data,
+    k_add_tree_binned<<<egrid, 256, 0, s>>>(tree, v->ds->meta.p, v->ds->View(), v->ds->num_data,
                                             v->score.p + static_cast<size_t>(k) * v->ds->num_data, shrinkage_, bias, pre, post);
   timing.launches += 2 + static_cast<long long>(valids_.size());
   B200_CUDA(cudaGetLastError());
-  B200_CUDA(cudaMemcpyAsync(tree_host_, tree_blob_.p, tree_blob_bytes_, cudaMemcpyDeviceToHost, s));
-  B200_CUDA(cudaMemcpyAsync(ctrl_host_, ctrl, sizeof(TreeCtrl), cudaMemcpyDeviceToHost, s));
-  B200_CUDA(cudaStreamSynchronize(s));
-  if (split_timing && !sev.empty()) {
-    static const char* kOps[] = {"gather_q(bagged root)", "K4", "allreduce", "scan+pick", "partition+zeroH+ctl"};
-    const int per = 6;       // marks per split
-    for (size_t b0 = 0; b0 + per <= sev.size(); b0 += per)
-      for (int o = 0; o < per - 1; ++o) { float ms = 0; cudaEventElapsedTime(&ms, sev[b0 + o], sev[b0 + o + 1]); split_op_ms_[kOps[o]] += ms; }
-    split_op_trees_ += 1;
-    for (auto e : sev) cudaEventDestroy(e);
-  }
-  if (profile_hist) {
-    for (size_t i = 0; i + 1 < evs.size(); i += 2) { float ms = 0; cudaEventElapsedTime(&ms, evs[i], evs[i + 1]); timing.hist_ms += ms; }
-    for (auto e : evs) cudaEventDestroy(e);
-  }
-  timing.hist_rows += ctrl_host_->trace_rows;
-  // ---- host copy of the tree
-  const unsigned char* hb = tree_host_;
-  auto at = [&](const void* devp) { return hb + (static_cast<const unsigned char*>(devp) - tree_blob_.p); };
-  const int nl = *reinterpret_cast<const int*>(at(tree_dev_.num_leaves));
-  out->Resize(nl);
-  if (nl > 1) {
-    const int* lc = reinterpret_cast<const int*>(at(tree_dev_.left_child));
-    const int* rc = reinterpret_cast<const int*>(at(tree_dev_.right_child));
-    const int* sf = reinterpret_cast<const int*>(at(tree_dev_.split_feature_inner));
-    const int* tb = reinterpret_cast<const int*>(at(tree_dev_.threshold_bin));
-    const int* dt = reinterpret_cast<const int*>(at(tree_dev_.decision_type));
-    const float* sg = reinterpret_cast<const float*>(at(tree_dev_.split_gain));
-    const double* lv = reinterpret_cast<const double*>(at(tree_dev_.leaf_value));
-    const double* lw = reinterpret_cast<const double*>(at(tree_dev_.leaf_weight));
-    const int* lcn = reinterpret_cast<const int*>(at(tree_dev_.leaf_count));
-    const double* iv = reinterpret_cast<const double*>(at(tree_dev_.internal_value));
-    const double* iw = reinterpret_cast<const double*>(at(tree_dev_.internal_weight));
-    const int* ic = reinterpret_cast<const int*>(at(tree_dev_.internal_count));
-    const int* ld = reinterpret_cast<const int*>(at(tree_dev_.leaf_depth));
-    const unsigned* cb = reinterpret_cast<const unsigned*>(at(tree_dev_.cat_bits));
-    const unsigned short* cl = reinterpret_cast<const unsigned short*>(at(tree_dev_.cat_list));
-    const int* cln = reinterpret_cast<const int*>(at(tree_dev_.cat_list_len));
-    for (int i = 0; i < nl - 1; ++i) {
-      out->left_child[i] = lc[i]; out->right_child[i] = rc[i]; out->split_feature_inner[i] = sf[i];
-      out->split_feature[i] = d.used[sf[i]]; out->threshold_in_bin[i] = static_cast<uint32_t>(tb[i]);
-      out->decision_type[i] = static_cast<int8_t>(dt[i]); out->split_gain[i] = sg[i];
-      const FeatureBins& fbm = d.mappers[d.used[sf[i]]];
-      if (dt[i] & 1) {          // categorical node: bins of the inner bitset -> category values ([UPSTREAM] RealThreshold per bin)
-        std::vector<int> cats;
-        if (sf[i] >= d.nfn) { for (int k = 0; k < cln[i]; ++k) cats.push_back(fbm.bin_to_cat[cl[i * kCatListMax + k]]); }
-        else for (int b = 0; b < fbm.num_bin; ++b) if ((cb[i * 8 + (b >> 5)] >> (b & 31)) & 1u) cats.push_back(fbm.bin_to_cat[b]);
-        out->AddCategoricalNode(i, cats);
-      } else {
-        double thr = fbm.upper[tb[i]];
-        if (std::isnan(thr)) thr = 0.0; else if (thr >= 1e300) thr = 1e300; else if (thr <= -1e300) thr = -1e300;
-        out->threshold[i] = thr;
-      }
-      out->internal_value[i] = iv[i]; out->internal_weight[i] = iw[i]; out->internal_count[i] = ic[i];
-    }
-    for (int i = 0; i < nl; ++i) { out->leaf_value[i] = lv[i]; out->leaf_weight[i] = lw[i]; out->leaf_count[i] = lcn[i]; out->leaf_depth[i] = ld[i]; }
-  } else {
-    out->leaf_value[0] = 0.0;
-  }
-  UpdateColumnCache(*out);
+  learner_->ReadTree(out);
 }
 
 bool Booster::TrainTrees(const float* custom_g, const float* custom_h) {
@@ -2084,8 +1674,9 @@ bool Booster::TrainTrees(const float* custom_g, const float* custom_h) {
     model.trees.push_back(std::move(t));
     if (is_dart_) {       // keep the device form of the tree (bin thresholds, inner bitsets) for later drops
       tree_store_.emplace_back(new DevBuf<unsigned char>());
-      tree_store_.back()->Alloc(tree_blob_bytes_);
-      B200_CUDA(cudaMemcpyAsync(tree_store_.back()->p, tree_blob_.p, tree_blob_bytes_, cudaMemcpyDeviceToDevice, s));
+      const DevBuf<unsigned char>& blob = learner_->Blob();
+      tree_store_.back()->Alloc(blob.n);
+      B200_CUDA(cudaMemcpyAsync(tree_store_.back()->p, blob.p, blob.n, cudaMemcpyDeviceToDevice, s));
     }
   }
   const_hessian_ = saved_const;
@@ -2129,8 +1720,7 @@ void Booster::ResetParameter(const char* params) {
   }
   shrinkage_ = is_rf_ ? 1.0 : cfg.learning_rate;
   if (is_dart_) { drop_rand_ = LcgRandom(cfg.drop_seed); sum_weight_ = 0.0; }      // [LightGBM dart.hpp DART::ResetConfig]
-  sp_.l1 = cfg.lambda_l1; sp_.l2 = cfg.lambda_l2; sp_.max_delta_step = cfg.max_delta_step; sp_.min_gain_to_split = cfg.min_gain_to_split;
-  sp_.min_sum_hessian = cfg.min_sum_hessian_in_leaf; sp_.min_data_in_leaf = cfg.min_data_in_leaf; sp_.max_depth = cfg.max_depth;
+  if (learner_) learner_->ResetConfig(cfg);
 }
 
 void Booster::AddValidData(const Dataset* valid) {

@@ -1,4 +1,4 @@
-// b200gbm engine: device dataset, data-parallel network state, booster (GBDT driver + tree learner).
+// b200gbm engine: device dataset, data-parallel network state, booster (the GBDT driver; its tree learner is in tree_learner.h).
 // Everything below the C ABI (include/b200gbm_c_api.h).  One host thread drives one
 // (network, dataset, booster) triple, exactly like one Spark task thread in the reference
 // (SURVEY.md fact 8): network / device / last-error state are thread_local.
@@ -191,6 +191,7 @@ struct ValidSet {
   DevBuf<double> score;   // [K][n]
 };
 class Objective;          // objective.h
+class TreeLearner;        // tree_learner.h
 
 class Booster {
  public:
@@ -228,9 +229,9 @@ class Booster {
   // instrumentation for bench.py / parity tests (B200GBM_* extensions of the C ABI)
   struct Timing { double hist_ms = 0, total_ms = 0; long long hist_rows = 0; long long hist_launches = 0, launches = 0; };
   Timing timing;
-  std::map<std::string, double> split_op_ms_; int split_op_trees_ = 0;      // B200GBM_SPLIT_TIMING debug accounting
-  bool profile_hist = false;                              // time K4 with events on the engine stream
-  std::vector<double> trace;                              // per split records (see B200GBM_BoosterGetTrace)
+  void SetProfile(bool profile_hist);                     // time K4 with events on the engine stream
+  void GetMemoryInfo(int64_t* out2);
+  void GetColumnCacheInfo(int64_t* out4) const;
 
   Config cfg;
   HostModel model;
@@ -243,11 +244,10 @@ class Booster {
   void InitTraining();
   bool TrainTrees(const float* custom_g, const float* custom_h);
   void TrainOneTree(int class_id, HostTree* out);
-  void LaunchPartition(int grid, int last);
-  int part_max_blocks_ = 0;
   double BoostFromAverage(int class_id);
 
   std::unique_ptr<Objective> obj_;      // training boosters only
+  std::unique_ptr<TreeLearner> learner_;      // training boosters only; uses stream_, so it is freed before the stream
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool parallel_ = false;
@@ -255,10 +255,6 @@ class Booster {
   bool const_hessian_ = false;
   bool has_init_score_ = false;
   double shrinkage_ = 0.1;
-  LcgRandom col_rand_{2};               // ColSampler (feature_fraction)
-  std::vector<uint8_t> feature_used_host_;
-  DevBuf<uint8_t> feature_used_;
-  void ResetFeaturesByTree();
   // row subsampling: bagging / GOSS / random forest (SURVEY §8f-3)
   bool is_rf_ = false, is_goss_ = false, bagging_ = false, balanced_bagging_ = false, use_bag_ = false, need_re_bagging_ = false;
   int bag_count_ = 0, bag_blocks_ = 0;
@@ -269,14 +265,6 @@ class Booster {
   std::vector<double> rf_init_scores_;
   void Bagging(int it);
   void ComputeGradientsAt(const double* score);
-  // percentile objectives: regression_l1 / quantile / mape renew the leaf outputs after the tree is grown (renew_kernel.cuh)
-  DevBuf<unsigned long long> rn_keys_a_, rn_keys_b_;
-  DevBuf<unsigned> rn_pos_a_, rn_pos_b_, rn_leaf_of_pos_, rn_leaf_a_, rn_leaf_b_;
-  DevBuf<double> rn_res_, rn_cdf_, rn_out_;      // rn_out_: [2][num_leaves] outputs, has-rows flags
-  DevBuf<int> rn_row_, rn_seg_;
-  DevBuf<unsigned char> rn_tmp_;
-  size_t rn_tmp_bytes_ = 0;
-  void RenewTreeOutput(int class_id, double rf_pred);
   // DART (SURVEY §8f-3): every trained tree keeps its device blob so dropped trees can be re-applied to the binned data
   bool is_dart_ = false, dart_dropped_this_iter_ = false;
   LcgRandom drop_rand_{4};
@@ -287,44 +275,9 @@ class Booster {
   void DroppingTrees();
   void DartNormalize();
   void AddStoredTree(int iter_index, int class_id, bool to_train, bool to_valid);
-  TreeDev RebasedTree(unsigned char* base) const;
-  SplitParams sp_{};
   // device state
   DevBuf<double> score_;        // [K][n]
   DevBuf<float> grad_, hess_;   // [K][n]
-  DevBuf<int4> qgh_, qord_;     // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
-  DevBuf<int> idx0_, idx1_;
-  DevBuf<long long> H_;         // scratch histogram of the current smaller leaf
-  DevBuf<long long> pool_;      // [num_leaves] leaf histograms
-  size_t slot_elems_ = 0;
-  DevBuf<uint8_t> flags_;       // [num_leaves][nf_pad]
-  DevBuf<SplitCand> cands_;     // [2][nf_pad]
-  DevBuf<LeafState> leaves_;
-  DevBuf<TreeCtrl> ctrl_;
-  DevBuf<unsigned char> tree_blob_;
-  TreeDev tree_dev_{};
-  size_t tree_blob_bytes_ = 0;
-  unsigned char* tree_host_ = nullptr;   // pinned mirror of tree_blob_
-  TreeCtrl* ctrl_host_ = nullptr;        // pinned
-  LeafState* leaves_host_ = nullptr;     // pinned
-  // optional [column][row] copies of the uint8 tiles' storage columns for the partition kernel: all of them (full copy), or a pool of
-  // slots that UpdateColumnCache fills with the columns the trees split on (column cache)
-  DevBuf<uint8_t> bins_cols_;
-  size_t cols_stride_ = 0;
-  bool cols_tried_ = false;
-  DevBuf<int> col_slot_;                   // [num_tiles * 32] slot of each storage column in bins_cols_, -1: not copied
-  std::vector<int> col_slot_host_;
-  std::vector<int> slot_col_;              // column cache: storage column held by each slot, -1: free (empty for the full copy)
-  std::vector<long long> col_splits_;      // column cache: splits on each storage column so far
-  long long cache_builds_ = 0, cache_evictions_ = 0;
-  void EnsureColumnCopy();
-  void UpdateColumnCache(const HostTree& t);
- public:
-  void GetMemoryInfo(int64_t* out2);
-  void GetColumnCacheInfo(int64_t* out4) const;
- private:
-  DevBuf<unsigned> part_bits_;
-  DevBuf<int> part_chunks_;
   // flattened forest for PredictBatch
   // PredictBatchCSR's slots (kernels.cuh k_csr_to_slots) for the trees [t0, t1): the U distinct split features in ascending order
   struct SlotBufs { int t0 = 0, t1 = 0, U = 0; DevBuf<int> slot_of_feature, feature_of_slot, split_slot; };

@@ -1120,7 +1120,7 @@ k_tiles_to_columns(const uint8_t* __restrict__ bins, size_t rows_stride, int num
 }
 
 // When the whole copy does not fit, the booster keeps a pool of column slots instead and fills them, between trees, with the storage
-// columns the trees split on (Booster::UpdateColumnCache).  This kernel copies up to kColumnBuildsMax storage columns into given slots:
+// columns the trees split on (TreeLearner::UpdateColumnCache).  This kernel copies up to kColumnBuildsMax storage columns into given slots:
 // blockIdx.y is the job, each thread packs 4 consecutive rows into one 32-bit store.  The 4 bytes lie in 4 sectors of one 128-byte
 // line, so every sector of the column's tile is read from DRAM once per job (32 bytes per row).
 constexpr int kColumnBuildsMax = 8;

@@ -1,0 +1,94 @@
+// Tree learner of a training Booster: grows one tree on the device from (g, h) and hands it back.  It owns everything a tree is
+// built with: the quantised (g,h) words, the histogram slot and pool (K4), the scans (K5), the partition (K7) with its column copy or
+// column cache, the controller state, the device tree blob with its pinned host mirror, the ColSampler and the leaf-renewal buffers.
+// The Booster keeps the scores, the row sampling and the boosting modes, and applies the grown tree to its scores.
+// Part of engine.cu's translation unit (tree_learner.cu is included there).
+#pragma once
+#include "engine.h"
+
+namespace b200gbm {
+
+class TreeLearner {
+ public:
+  // cfg is the booster's, read live (ResetConfig refreshes the split parameters copied from it); stream and timing are the booster's
+  TreeLearner(const Dataset& train, const Config& cfg, const Objective& obj, bool parallel, bool same_device, int num_sms,
+              cudaStream_t stream, Booster::Timing& timing);
+  ~TreeLearner();
+  void ResetConfig(const Config& cfg);      // the split parameters a ResetParameter may change
+
+  // the rows a bagged tree is grown on: the in-bag flags and the ascending in-bag row list
+  struct Bag { const uint8_t* in_bag; const int* rows; int count; };
+  // enqueues the whole leaf-wise growth of one tree on (g, h) without a host sync; bag null: every row
+  void Grow(const float* g, const float* h, bool const_hessian, const Bag* bag);
+  // percentile objectives: patch the grown tree's leaf values (score_k null: residuals against rf_pred)
+  void Renew(const Objective& obj, const double* score_k, double rf_pred);
+  // score_k[row] += shrinkage * leaf value of the row's leaf, walking the leaves' row lists (every row is in a leaf)
+  void AddScore(double* score_k, double shrinkage);
+  const TreeDev& Tree() const { return tree_dev_; }                 // the grown tree on the device
+  const DevBuf<unsigned char>& Blob() const { return tree_blob_; }   // the same tree as one buffer (DART stores copies of it)
+  TreeDev TreeAt(unsigned char* blob) const;                          // the fields of such a buffer or copy
+  // copies the tree to the host (D2H + sync), converts it, and updates the column cache
+  void ReadTree(HostTree* out);
+
+  bool profile_hist = false;                 // time K4 with events on the stream (Timing::hist_ms)
+  size_t ColumnCopyBytes() const { return bins_cols_.n; }
+  void GetColumnCacheInfo(int64_t* out4) const;
+
+ private:
+  void ResetFeaturesByTree();
+  void LaunchPartition(int grid, int last);
+  void EnsureColumnCopy();
+  void UpdateColumnCache(const HostTree& t);
+
+  const Dataset& train_;
+  const Config& cfg_;
+  const bool parallel_, same_device_;
+  const int num_sms_;
+  cudaStream_t stream_;
+  Booster::Timing& timing_;
+  SplitParams sp_{};
+  int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
+  // device state of the tree being grown
+  DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
+  DevBuf<int> idx0_, idx1_;
+  DevBuf<long long> H_;          // scratch histogram of the current smaller leaf
+  DevBuf<long long> pool_;       // [num_leaves] leaf histograms
+  size_t slot_elems_ = 0;
+  DevBuf<uint8_t> flags_;        // [num_leaves][nf_pad]
+  DevBuf<SplitCand> cands_;      // [2][nf_pad]
+  DevBuf<LeafState> leaves_;
+  DevBuf<TreeCtrl> ctrl_;
+  DevBuf<unsigned char> tree_blob_;
+  TreeDev tree_dev_{};
+  unsigned char* tree_host_ = nullptr;   // pinned mirror of tree_blob_
+  TreeCtrl* ctrl_host_ = nullptr;        // pinned
+  DevBuf<unsigned> part_bits_;
+  DevBuf<int> part_chunks_;
+  int part_max_blocks_ = 0;
+  // optional [column][row] copies of the uint8 tiles' storage columns for the partition kernel: all of them (full copy), or a pool of
+  // slots that UpdateColumnCache fills with the columns the trees split on (column cache)
+  DevBuf<uint8_t> bins_cols_;
+  size_t cols_stride_ = 0;
+  bool cols_tried_ = false;
+  DevBuf<int> col_slot_;                   // [num_tiles * 32] slot of each storage column in bins_cols_, -1: not copied
+  std::vector<int> col_slot_host_;
+  std::vector<int> slot_col_;              // column cache: storage column held by each slot, -1: free (empty for the full copy)
+  std::vector<long long> col_splits_;      // column cache: splits on each storage column so far
+  long long cache_builds_ = 0, cache_evictions_ = 0;
+  LcgRandom col_rand_{2};                  // ColSampler (feature_fraction)
+  std::vector<uint8_t> feature_used_host_;
+  DevBuf<uint8_t> feature_used_;
+  // percentile objectives: sort buffers of the renewal pass (renew_kernel.cuh)
+  DevBuf<unsigned long long> rn_keys_a_, rn_keys_b_;
+  DevBuf<unsigned> rn_pos_a_, rn_pos_b_, rn_leaf_of_pos_, rn_leaf_a_, rn_leaf_b_;
+  DevBuf<double> rn_res_, rn_cdf_, rn_out_;      // rn_out_: [2][num_leaves] outputs, has-rows flags
+  DevBuf<int> rn_row_, rn_seg_;
+  DevBuf<unsigned char> rn_tmp_;
+  size_t rn_tmp_bytes_ = 0;
+  // B200GBM_SPLIT_TIMING=1 (debug): events of the tree being grown, per-operation sums reported on stderr at destruction
+  std::vector<cudaEvent_t> split_events_, hist_events_;
+  std::map<std::string, double> split_op_ms_;
+  int split_op_trees_ = 0;
+};
+
+}  // namespace b200gbm
