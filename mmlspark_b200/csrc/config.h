@@ -64,6 +64,7 @@ struct Config {
   bool lambdarank_norm = true;
   std::vector<double> label_gain;
   std::vector<int> eval_at;
+  std::vector<double> auc_mu_weights;       // auc_mu's K x K class-pair weights, row-major; empty = 1 off the diagonal, 0 on it
   // --- network
   int num_machines = 1;
   std::map<std::string, std::string> raw;
@@ -195,6 +196,8 @@ struct Config {
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &label_gain, [](const std::string& x) { return std::atof(x.c_str()); });
       it = raw.find("eval_at");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &eval_at, [](const std::string& x) { return std::atoi(x.c_str()); });
+      it = raw.find("auc_mu_weights");
+      if (it != raw.end() && !it->second.empty()) SplitList(it->second, &auc_mu_weights, [](const std::string& x) { return std::atof(x.c_str()); });
       it = raw.find("categorical_feature");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &categorical_feature, [](const std::string& x) { return std::atoi(x.c_str()); });
     }
@@ -258,7 +261,7 @@ struct Config {
     s << "[reg_sqrt: 0]\n[alpha: " << Num(alpha) << "]\n[fair_c: " << Num(fair_c) << "]\n[poisson_max_delta_step: " << Num(poisson_max_delta_step) << "]\n";
     s << "[tweedie_variance_power: " << Num(tweedie_variance_power) << "]\n[lambdarank_truncation_level: " << lambdarank_truncation_level << "]\n";
     s << "[lambdarank_norm: " << lambdarank_norm << "]\n[label_gain: " << join_d(label_gain) << "]\n[eval_at: " << join_i(eval_at) << "]\n";
-    s << "[multi_error_top_k: 1]\n[auc_mu_weights: ]\n[num_machines: " << num_machines << "]\n[local_listen_port: 12400]\n";
+    s << "[multi_error_top_k: 1]\n[auc_mu_weights: " << join_d(auc_mu_weights) << "]\n[num_machines: " << num_machines << "]\n[local_listen_port: 12400]\n";
     s << "[time_out: 120]\n[machine_list_filename: ]\n[machines: ]\n[gpu_platform_id: -1]\n[gpu_device_id: -1]\n[gpu_use_dp: 0]\n[num_gpu: 1]";
     return s.str();
   }

@@ -300,6 +300,17 @@ class Booster {
   DevBuf<unsigned long long> auc_keys_a_, auc_keys_b_;
   DevBuf<int> auc_rows_a_, auc_rows_b_, auc_head_, auc_start_;
   DevBuf<unsigned char> auc_tmp_;
+  // auc_mu: the class-grouped row order, then one batch of class-pair segments at a time (about 2n items, so O(n) for any K)
+  DevBuf<unsigned> mu_cls_keys_a_, mu_cls_keys_b_;
+  DevBuf<int> mu_cls_rows_a_, mu_cls_rows_b_, mu_cls_start_, mu_off_, mu_end_small_, mu_rows_a_, mu_rows_b_, mu_seg_, mu_head_, mu_start_;
+  DevBuf<int2> mu_pairs_;
+  DevBuf<unsigned long long> mu_keys_a_, mu_keys_b_;
+  DevBuf<double> mu_pv_, mu_wpos_, mu_wneg_, mu_ppos_, mu_pneg_, mu_partial_, mu_pair_auc_;
+  DevBuf<unsigned char> mu_tmp_;
+  // auc's and average_precision's sort by descending score, split weights and prefix sums into auc_* (enqueued on the stream)
+  void RankByScore(const double* score, const float* d_y, const float* d_w, int n);
+  std::vector<double> AucMuWeights() const;      // K x K, row-major, diagonal zeroed
+  double EvalAucMu(const double* score, const float* d_y, const float* d_w, int n);
   int num_sms_ = 0;
   cudaEvent_t ev_a_ = nullptr, ev_b_ = nullptr;
 };

@@ -5,7 +5,15 @@
 //                      k_metric_pointwise -> per-block partial sums -> k_metric_finish (fixed summation order: reproducible)
 //   auc                [UPSTREAM binary_metric.hpp AUCMetric]: radix sort by score (cub, library code off the training path), prefix sums of
 //                      the positive / negative weights, one term per group of tied scores
+//   average_precision  [UPSTREAM binary_metric.hpp AveragePrecisionMetric]: the same sort and prefix sums as auc, one term per tie group
+//                      holding positives: its positive weight times the precision through the group
+//   auc_mu             [UPSTREAM multiclass_metric.hpp AucMuMetric]: rows grouped by class (stable radix sort by label), then batches of
+//                      class pairs of about 2n items: per pair a segment of (key of the pair's distance d, row) for the rows of both
+//                      classes, a segmented sort (a device-wide radix sort for each large segment), segmented prefix sums and the auc
+//                      terms per segment; scratch stays O(n) for any K
 //   ndcg@k / map@k     [UPSTREAM rank_metric.hpp, dcg_calculator.cpp, map_metric.hpp]: one block per query, stable rank by counting
+// Every sum of non-integer terms runs in a fixed order (contiguous row ranges per block, blocks summed in block order), so repeated
+// evaluations are bit-identical.
 #pragma once
 #include <cub/cub.cuh>
 #include <cuda_runtime.h>
@@ -181,6 +189,129 @@ k_auc_terms(const unsigned long long* __restrict__ keys, const int* __restrict__
   }
   d_block_sum2(acc, unused, sm);
   if (threadIdx.x == 0) { partial[2 * blockIdx.x] = acc; partial[2 * blockIdx.x + 1] = 0.0; }
+}
+
+// ---------------------------------------------------------------- average_precision
+// after the auc sort and prefix sums: one term per tie group, at its last position t, pos_g * TP / (TP + FP) with TP / FP the positive /
+// negative weight ranked at or above the group.  A group without positive weight adds nothing (no 0/0 on zero-weight groups).
+__global__ void __launch_bounds__(kMetricBlock)
+k_ap_terms(const unsigned long long* __restrict__ keys, const int* __restrict__ start, const double* __restrict__ ppos, const double* __restrict__ pneg,
+           int n, double* __restrict__ partial) {
+  __shared__ double sm[16];
+  double acc = 0, unused = 0;
+  const long long per = (static_cast<long long>(n) + gridDim.x - 1) / gridDim.x;
+  const long long r0 = per * blockIdx.x, r1 = min(r0 + per, static_cast<long long>(n));
+  for (long long t = r0 + threadIdx.x; t < r1; t += kMetricBlock) {
+    if (t != n - 1 && keys[t] == keys[t + 1]) continue;
+    const int s = start[t];
+    const double tp = ppos[t], fp = pneg[t], pos_g = tp - (s > 0 ? ppos[s - 1] : 0.0);
+    if (pos_g != 0.0) acc += pos_g * __drcp_rn(tp + fp) * tp;      // a reciprocal: the IEEE division's slow path would spill
+  }
+  d_block_sum2(acc, unused, sm);
+  if (threadIdx.x == 0) { partial[2 * blockIdx.x] = acc; partial[2 * blockIdx.x + 1] = 0.0; }
+}
+
+// ---------------------------------------------------------------- auc_mu
+// class-grouped row order: key = the row's class (labels are checked to lie in [0, K)), sorted stably by cub's radix sort
+__global__ void k_class_keys(const float* __restrict__ label, int n, unsigned* __restrict__ keys, int* __restrict__ rows) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    keys[i] = static_cast<unsigned>(static_cast<int>(label[i])); rows[i] = i;
+  }
+}
+// cls_start[c] = first position of class c in the sorted keys, cls_start[K] = n; an absent class gets an empty range.  The host zeroes
+// cls_start first, which is the answer for n = 0.
+__global__ void k_class_bounds(const unsigned* __restrict__ keys, int n, int K, int* __restrict__ cls_start) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int c = static_cast<int>(keys[i]), prev = i == 0 ? -1 : static_cast<int>(keys[i - 1]);
+    for (int k = prev + 1; k <= c; ++k) cls_start[k] = i;
+    if (i == n - 1) for (int k = c + 1; k <= K; ++k) cls_start[k] = n;
+  }
+}
+// the segment g of batch item q: the largest g with off[g] <= q (empty segments share their offset with the next one)
+__device__ __forceinline__ int d_segment_of(const int* __restrict__ off, int P, long long q) {
+  int lo = 0, hi = P - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (off[mid] <= q) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+// One batch of class pairs [p0, p0 + P): segment g holds the rows of pair p0 + g = (i, j), first class i's rows, then class j's, and
+// spans items [off[g], off[g + 1]).  pv[p] = (t1, v[0..K)) for pair p; every row gets d = t1 * sum_c v[c] * s_c over the raw class-major
+// scores (a zero v[c] adds nothing, so the default matrix reads two scores per row).  -0.0 is keyed as +0.0, as in k_auc_keys.
+__global__ void k_aucmu_keys(const double* __restrict__ score, int n, int K, const int* __restrict__ cls_start, const int* __restrict__ cls_rows,
+                             const int2* __restrict__ pairs, const double* __restrict__ pv, int p0, int P, const int* __restrict__ off,
+                             unsigned long long* __restrict__ keys, int* __restrict__ rows, int* __restrict__ seg) {
+  const int N = off[P];
+  for (long long q = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; q < N; q += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int g = d_segment_of(off, P, q);
+    const int2 pr = pairs[p0 + g];
+    const int local = static_cast<int>(q - off[g]), ni = cls_start[pr.x + 1] - cls_start[pr.x];
+    const int r = local < ni ? cls_rows[cls_start[pr.x] + local] : cls_rows[cls_start[pr.y] + local - ni];
+    const double* v = pv + static_cast<size_t>(p0 + g) * (K + 1);
+    double dot = 0.0;
+    for (int c = 0; c < K; ++c) {
+      const double vc = v[1 + c];
+      if (vc != 0.0) dot += vc * score[static_cast<size_t>(c) * n + r];
+    }
+    const double d = v[0] * dot;
+    keys[q] = d_sortable(d == 0.0 ? 0.0 : d); rows[q] = r; seg[q] = g;
+  }
+}
+// sorted batch position q (descending d within its segment): the row's weight as class i ("positive") or class j, and the head marker of
+// its tie group; a segment's first position is always a head, so the max-scan of the heads never reaches into the previous segment
+__global__ void k_aucmu_weights(const unsigned long long* __restrict__ keys, const int* __restrict__ rows, const int* __restrict__ seg,
+                                const int* __restrict__ off, const int2* __restrict__ pairs, int p0, const float* __restrict__ label,
+                                const float* __restrict__ weight, int N, double* __restrict__ wpos, double* __restrict__ wneg, int* __restrict__ head) {
+  for (long long q = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; q < N; q += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int g = seg[q], r = rows[q];
+    const double w = weight ? static_cast<double>(weight[r]) : 1.0;
+    const bool pos = static_cast<int>(label[r]) == pairs[p0 + g].x;
+    wpos[q] = pos ? w : 0.0; wneg[q] = pos ? 0.0 : w;
+    head[q] = (q == off[g] || keys[q] != keys[q - 1]) ? q : 0;
+  }
+}
+// k_auc_terms per segment, over the segmented prefix sums: each block takes a contiguous range of the batch's items and reduces once
+// per segment its range touches into partial[block * P + g] (the host zeroes the rest)
+__global__ void __launch_bounds__(kMetricBlock)
+k_aucmu_terms(const unsigned long long* __restrict__ keys, const int* __restrict__ start, const double* __restrict__ ppos, const double* __restrict__ pneg,
+              const int* __restrict__ off, int P, double* __restrict__ partial) {
+  __shared__ double sm[16];
+  const long long N = off[P];
+  const long long per = (N + gridDim.x - 1) / gridDim.x;
+  const long long r0 = per * blockIdx.x, r1 = min(r0 + per, N);
+  if (r0 >= r1) return;
+  for (int g = d_segment_of(off, P, r0); g < P && off[g] < r1; ++g) {
+    const long long sb = off[g], se = off[g + 1], a = max(r0, sb), b = min(r1, se);
+    double acc = 0, unused = 0;
+    for (long long t = a + threadIdx.x; t < b; t += kMetricBlock) {
+      if (t != se - 1 && keys[t] == keys[t + 1]) continue;
+      const int s = start[t];
+      const double before_p = s > sb ? ppos[s - 1] : 0.0, before_n = s > sb ? pneg[s - 1] : 0.0;
+      const double pos_g = ppos[t] - before_p, neg_g = pneg[t] - before_n;
+      acc += neg_g * (pos_g * 0.5 + before_p);
+    }
+    d_block_sum2(acc, unused, sm);
+    if (threadIdx.x == 0) partial[static_cast<size_t>(blockIdx.x) * P + g] = acc;
+    __syncthreads();      // sm is reused by the next segment
+  }
+}
+// S[p0 + g] = AUC of pair g: its block partials summed in block order, over W_i * W_j (the class weights are the segment's last prefix
+// sums).  A class without rows or weight gives 0 / 0 = NaN, as upstream does not guard that division.
+__global__ void k_aucmu_pair_finish(const double* __restrict__ partial, int blocks, int P, const int* __restrict__ off, const double* __restrict__ ppos,
+                                    const double* __restrict__ pneg, int p0, double* __restrict__ S) {
+  for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < P; g += gridDim.x * blockDim.x) {
+    double s = 0;
+    for (int b = 0; b < blocks; ++b) s += partial[static_cast<size_t>(b) * P + g];
+    const int e = off[g + 1];
+    const bool any = e > off[g];
+    const double wi = any ? ppos[e - 1] : 0.0, wj = any ? pneg[e - 1] : 0.0;
+    S[p0 + g] = s / (wi * wj);
+  }
+}
+// auc_mu = 2 / (K (K - 1)) * sum of the pairs' AUCs, summed in pair order by one thread
+__global__ void k_aucmu_total(const double* __restrict__ S, int npairs, int K, double* __restrict__ out) {
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
+  double s = 0;
+  for (int p = 0; p < npairs; ++p) s += S[p];
+  out[0] = s * (2.0 / (static_cast<double>(K) * (K - 1)));
 }
 
 // ---------------------------------------------------------------- ndcg@k / map@k : one block per query

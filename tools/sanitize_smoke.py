@@ -1,6 +1,6 @@
 """Small end-to-end runs for compute-sanitizer (memcheck / racecheck / synccheck): every hand-synchronised kernel of the engine at shapes a
 sanitizer finishes in minutes — K4 with TMA bulk copies (root) and cp.async gathers (leaves), the ticket-elected pick step of k_scan, the
-software grid barriers of k_partition, the threshold selection + short bitonic sorts of k_scan_wide, the column-major copy (k_tiles_to_columns), k4_hist_wide, bagging, lambdarank and the device metrics."""
+software grid barriers of k_partition, the threshold selection + short bitonic sorts of k_scan_wide, the column-major copy (k_tiles_to_columns), k4_hist_wide, bagging, lambdarank and the device metrics, including the pair batches of auc_mu."""
 import sys
 
 import numpy as np
@@ -41,4 +41,10 @@ Xc[:, 5] = np.floor(3000.0 ** rng.random(30000)) - 1      # a wide categorical c
 Xc[:, 6] = rng.integers(0, 30, 30000)
 yc = (s[:30000] + 0.5 * (Xc[:, 5] % 3) > 0.5).astype(np.float32)
 run("wide categorical", Xc, yc, "objective=binary metric=binary_error", ds_params=DS + " categorical_feature=5,6")
+# average_precision on the auc pipeline; auc_mu with 4 classes: 6 pairs hold 3n items, so several pair batches and segmented sorts run
+run("binary+average_precision", X, (s > 0.5).astype(np.float32), "objective=binary metric=average_precision,auc")
+yk = np.digitize(s[:15000], [-1, 0, 1]).astype(np.float32)
+run("multiclass+auc_mu", X[:15000], yk, "objective=multiclass num_class=4 metric=auc_mu,multi_logloss", iters=1)
+run("multiclassova+auc_mu dense matrix", X[:15000], yk,
+    "objective=multiclassova num_class=4 metric=auc_mu auc_mu_weights=0,1,2,3,1,0,1,2,2,1,0,1,3,2,1,0", iters=1)
 print("sanitize smoke done")
