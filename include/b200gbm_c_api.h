@@ -235,6 +235,10 @@ int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4);
 int B200GBM_BoosterGetMemoryInfo(BoosterHandle handle, int64_t* out2);
 /* out = {slots of the column cache (0 = no cache: full copy or none), slots in use, columns built into slots so far, evictions so far} */
 int B200GBM_BoosterGetColumnCacheInfo(BoosterHandle handle, int64_t* out4);
+/* out = {histogram bytes all-reduced by this rank (data-parallel: the whole histogram slot per split round; voting-parallel: the packed
+ * buffer of 2 * top_k voted storage columns and the two leaves' totals), vote record bytes all-gathered (all ranks' records, voting only),
+ * split rounds enqueued (num_leaves - 1 per tree, also when a tree stops early)}, all since the booster was created; 0 bytes on one rank */
+int B200GBM_BoosterGetCommInfo(BoosterHandle handle, int64_t* out3);
 
 #ifdef __cplusplus
 }

@@ -509,6 +509,12 @@ class Booster:
         check(load().B200GBM_BoosterGetColumnCacheInfo(self.handle, _ptr(out)))
         return dict(slots=int(out[0]), slots_used=int(out[1]), builds=int(out[2]), evictions=int(out[3]))
 
+    def get_comm_info(self):
+        """Bytes this rank sent through the training collectives since the booster was created (B200GBM_BoosterGetCommInfo)."""
+        out = np.zeros(3, dtype=np.int64)
+        check(load().B200GBM_BoosterGetCommInfo(self.handle, _ptr(out)))
+        return dict(hist_bytes=int(out[0]), record_bytes=int(out[1]), splits=int(out[2]))
+
     def get_scores(self, data_idx=0):
         n = C.c_int64(0)
         check(load().LGBM_BoosterGetNumPredict(self.handle, C.c_int(data_idx), C.byref(n)))

@@ -641,6 +641,11 @@ int B200GBM_BoosterGetColumnCacheInfo(BoosterHandle handle, int64_t* out4) {
   BS(handle)->GetColumnCacheInfo(out4);
   API_END();
 }
+int B200GBM_BoosterGetCommInfo(BoosterHandle handle, int64_t* out3) {
+  API_BEGIN();
+  BS(handle)->GetCommInfo(out3);
+  API_END();
+}
 int B200GBM_BoosterGetScores(BoosterHandle handle, int data_idx, double* out) {
   API_BEGIN();
   BS(handle)->GetRawScores(data_idx, out);

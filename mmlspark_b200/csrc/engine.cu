@@ -1379,6 +1379,15 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   parallel_ = Net().active && Net().world > 1;
   same_device_ = parallel_ && Net().same_device != nullptr;
   cfg.num_machines = parallel_ ? Net().world : 1;
+  if (parallel_ && cfg.tree_learner == "voting") {      // identical on every rank: they all fail here, before any collective of training
+    if (cfg.top_k <= 0) Fatal("tree_learner=voting needs top_k > 0, got top_k=" + std::to_string(cfg.top_k));
+    if (train->nw > 0)
+      Fatal("tree_learner=voting does not support features with more than 256 bins (" + std::to_string(train->nw) +
+            " such features); use tree_learner=data_parallel or a max_bin of at most 255");
+    if (static_cast<long long>(Net().world) * std::min(cfg.top_k, std::max(train->nf, 1)) > kVoteMaxRecords)
+      Fatal("tree_learner=voting supports num_machines * top_k <= " + std::to_string(kVoteMaxRecords) + ", got " + std::to_string(Net().world) +
+            " * " + std::to_string(std::min(cfg.top_k, train->nf)));
+  }
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1595,6 +1604,11 @@ void Booster::GetMemoryInfo(int64_t* out2) {
   if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
   out2[0] = learner_ ? static_cast<int64_t>(learner_->ColumnCopyBytes()) : 0;
   out2[1] = static_cast<int64_t>(free_b);
+}
+
+void Booster::GetCommInfo(int64_t* out3) const {
+  out3[0] = out3[1] = out3[2] = 0;
+  if (learner_) learner_->GetCommInfo(out3);
 }
 
 void Booster::GetColumnCacheInfo(int64_t* out4) const {

@@ -232,6 +232,7 @@ class Booster {
   void SetProfile(bool profile_hist);                     // time K4 with events on the engine stream
   void GetMemoryInfo(int64_t* out2);
   void GetColumnCacheInfo(int64_t* out4) const;
+  void GetCommInfo(int64_t* out3) const;
 
   Config cfg;
   HostModel model;

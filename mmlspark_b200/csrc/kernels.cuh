@@ -1924,16 +1924,19 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
 // the column become its bins != mfb; this block alone updates them in the pool (smaller leaf: H, larger: parent - H).  Every column of a leaf
 // sums to the leaf total, so the smaller leaf's total is this column of H summed, and the larger's is its parent's total minus that; the
 // member's mfb is the total minus its other bins.  All exact int64, so `out` equals the unbundled feature's histogram bit for bit.
+// tot != null (the voting learner's global scan): src is the leaf's reduced column and tot its reduced (g,h) total; dst and L are untouched.
+// leaf_tot != null: the leaf total used is also stored there (shared memory, read by the block after the call).
 __device__ __noinline__ void d_unbundle_hist(const long long* __restrict__ src, long long* __restrict__ dst, int num_bin, int mfb, int base, int which,
-                                             LeafState* L, longlong2* out) {
+                                             LeafState* L, longlong2* out, const long long* __restrict__ tot = nullptr,
+                                             longlong2* leaf_tot = nullptr) {
   __shared__ long long s_red[4][8];
   const int b = threadIdx.x, lane = b & 31, warp = b >> 5;
   const longlong2 hv = reinterpret_cast<const longlong2*>(src)[b];
   const bool own = b > base && b < base + num_bin;
   longlong2 sv = hv;
   if (own) {
-    if (which) { const longlong2 pr = reinterpret_cast<const longlong2*>(dst)[b]; sv.x = pr.x - hv.x; sv.y = pr.y - hv.y; }
-    reinterpret_cast<longlong2*>(dst)[b] = sv;
+    if (which && !tot) { const longlong2 pr = reinterpret_cast<const longlong2*>(dst)[b]; sv.x = pr.x - hv.x; sv.y = pr.y - hv.y; }
+    if (!tot) reinterpret_cast<longlong2*>(dst)[b] = sv;
     const int v = b - base - 1;
     out[v < mfb ? v : v + 1] = sv;
   }
@@ -1946,9 +1949,14 @@ __device__ __noinline__ void d_unbundle_hist(const long long* __restrict__ src, 
   if (b == 0) {
     long long t[4] = {0, 0, 0, 0};
     for (int i = 0; i < 4; ++i) for (int w = 0; w < 8; ++w) t[i] += s_red[i][w];
-    const long long tg = which ? L->qpar[0] - t[0] : t[0], th = which ? L->qpar[1] - t[1] : t[1];
-    L->qtot[0] = tg; L->qtot[1] = th;      // every member block of this leaf writes the same value
+    long long tg, th;
+    if (tot) { tg = tot[0]; th = tot[1]; }
+    else {
+      tg = which ? L->qpar[0] - t[0] : t[0]; th = which ? L->qpar[1] - t[1] : t[1];
+      L->qtot[0] = tg; L->qtot[1] = th;      // every member block of this leaf writes the same value
+    }
     out[mfb] = make_longlong2(tg - t[2], th - t[3]);
+    if (leaf_tot) *leaf_tot = make_longlong2(tg, th);
   }
   __syncthreads();
 }
@@ -1960,10 +1968,95 @@ __device__ __noinline__ void d_unbundle_hist(const long long* __restrict__ src, 
 // fp64 divisions per thread is 2 long instead of 16 as in the round-1 warp-per-feature scan, and the code is shared and small (the old
 // kernel was instruction-fetch bound).  Categorical tile features keep the warp-level search (d_scan_feature_cat) on warp 0.  The block that
 // finishes last picks the best candidate per leaf and the next leaf to split.
+//
+// The voting-parallel learner ([UPSTREAM] VotingParallelTreeLearner) runs the same kernel twice per split, with kMode:
+//   kScanLocal   every block writes its column of the LOCAL histograms into the pool whatever the feature's flag (the pool holds local
+//                histograms; the larger child is local parent - local smaller), takes the leaf's exact local (g,h) total from its column
+//                of H (every storage column of a leaf sums to the leaf's total: smaller = H's column, larger = parent total - that; kept in
+//                LeafState::qtot / qpar), and scans flagged features with the local split parameters `p`, the local sums and the leaf's
+//                true local row count.  This scan alone writes the is_splittable flags.  Its last block selects each leaf's local top-k
+//                candidates into the vote records (d_topk_block) instead of picking.
+//   kScanGlobal  a feature voted for the leaf (VoteBufs::voted) is scanned from its column of the reduced buffer (k_vote_pack) with the
+//                global split parameters and leaf sums, whatever its local flag; every other feature yields a -inf candidate.  No flag
+//                is written, and the last block runs the pick step as the data-parallel learner does.
+constexpr int kScanPlain = 0, kScanLocal = 1, kScanGlobal = 2;
+struct VoteRec { int feature, left_count, right_count, pad; double gain; };     // feature: inner index, -1 for no candidate
+// packed (reduced) buffer: [0, 4) the (qg, qh) totals of the smaller and the larger leaf, then 2 * top_k storage columns of 256 (g,h) pairs:
+// column which * top_k + k is the k-th voted feature of leaf `which` (0 smaller, 1 larger), zero when the vote has fewer features
+constexpr int kVoteTotals = 4;
+constexpr int kVoteColumn = 512;
+constexpr int kVoteMaxRecords = 2048;      // records of one leaf over all ranks that k_vote_pack handles (8 per thread)
+struct VoteBufs {
+  VoteRec* recs;              // [2][top_k] this rank's local top-k records (kScanLocal writes them)
+  const int* voted;           // [2][top_k] voted inner features, -1: none (k_vote_pack writes them)
+  const long long* packed;    // reduced packed buffer
+  int top_k;
+};
+
+// this block's leaf's exact (qg, qh) sums of a 256-pair column (thread t = pair t), on every thread
+__device__ __forceinline__ longlong2 d_block_sum_column(const long long* __restrict__ col) {
+  __shared__ long long s_red[2][8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  longlong2 v = reinterpret_cast<const longlong2*>(col)[threadIdx.x];
+  for (int o = 16; o; o >>= 1) { v.x += __shfl_xor_sync(0xffffffffu, v.x, o); v.y += __shfl_xor_sync(0xffffffffu, v.y, o); }
+  if (lane == 0) { s_red[0][warp] = v.x; s_red[1][warp] = v.y; }
+  __syncthreads();
+  longlong2 t = make_longlong2(0, 0);
+  for (int w = 0; w < 8; ++w) { t.x += s_red[0][w]; t.y += s_red[1][w]; }
+  __syncthreads();
+  return t;
+}
+
+// The local top-k of both leaves ([UPSTREAM] VotingParallelTreeLearner::FindBestSplits, ArrayArgs::MaxK on SplitInfo::operator>): round k
+// takes the best candidate after round k-1's in the order (gain desc, real feature index asc), threads 0..127 for the smaller leaf and
+// 128..255 for the larger as in d_pick_block.  A -inf candidate, or no leaf, gives a record with feature -1.
+__device__ __noinline__ void
+d_topk_block(const TreeCtrl* ctrl, const LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p,
+             VoteRec* recs, int top_k) {
+  __shared__ double s_gain[8], s_prev_gain[2];
+  __shared__ int s_feat[8], s_idx[8], s_prev_feat[2];
+  const int which = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int leaf = ctrl->go ? (which ? ctrl->larger : ctrl->smaller) : -1;
+  double pg = __longlong_as_double(0x7ff0000000000000LL);      // +inf: every candidate comes after it
+  int pf = -1;
+  for (int k = 0; k < top_k; ++k) {
+    double bg = kNegInf; int bf = 0x7fffffff, bi = -1;
+    if (leaf >= 0) {
+      for (int u = t; u < p.nf; u += 128) {
+        const double cg = __ldcg(&cands[which * p.nf_pad + u].gain);
+        const int rf = meta[u].real_index;
+        if (!(cg < pg || (cg == pg && rf > pf))) continue;      // taken in an earlier round
+        if (bi < 0 || cg > bg || (cg == bg && rf < bf)) { bg = cg; bf = rf; bi = u; }
+      }
+    }
+    for (int o = 16; o; o >>= 1) {
+      const double og = __shfl_xor_sync(0xffffffffu, bg, o);
+      const int of = __shfl_xor_sync(0xffffffffu, bf, o), oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (oi >= 0 && (bi < 0 || og > bg || (og == bg && of < bf))) { bg = og; bf = of; bi = oi; }
+    }
+    if (lane == 0) { s_gain[warp] = bg; s_feat[warp] = bf; s_idx[warp] = bi; }
+    __syncthreads();
+    if (t == 0) {
+      for (int w = which * 4; w < which * 4 + 4; ++w)
+        if (s_idx[w] >= 0 && (bi < 0 || s_gain[w] > bg || (s_gain[w] == bg && s_feat[w] < bf))) { bg = s_gain[w]; bf = s_feat[w]; bi = s_idx[w]; }
+      VoteRec r{-1, 0, 0, 0, kNegInf};
+      if (bi >= 0 && bg > kNegInf) {
+        const int lc = __ldcg(&cands[which * p.nf_pad + bi].left_count);
+        r.feature = bi; r.gain = bg; r.left_count = lc; r.right_count = leaves[leaf].count - lc;
+      }
+      recs[which * top_k + k] = r;
+      s_prev_gain[which] = bi >= 0 ? bg : kNegInf; s_prev_feat[which] = bi >= 0 ? bf : 0x7fffffff;
+    }
+    __syncthreads();
+    pg = s_prev_gain[which]; pf = s_prev_feat[which];
+  }
+}
+
+template <int kMode>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
@@ -1975,30 +2068,72 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     out.gain = kNegInf; out.left_g = 0; out.left_h = 0; out.threshold = 0; out.left_count = 0; out.default_left = 1; out.feature = u;
     out.l2_extra = 0; out.is_cat = 0; out.cat_list_len = 0;
     for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
-    uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
-    if (*flag) {
-      const LeafState& L = leaves[leaf];
-      const FeatMeta fm = meta[u];
-      long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(fm.hist_off) * 2;
-      const long long* src = H + static_cast<size_t>(fm.hist_off) * 2;
-      if (!bundle_base || bundle_base[u] < 0) {
-        const int b = threadIdx.x;
-        longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
-        if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
-        *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
-        __syncthreads();      // the scan reads bins other threads of this block reduced
-      } else {
-        d_unbundle_hist(src, dst, fm.num_bin, fm.default_bin, bundle_base[u], which, leaves + leaf, reinterpret_cast<longlong2*>(scan_ws));
-        dst = reinterpret_cast<long long*>(scan_ws);
-      }
-      if (!fm.is_categorical) {
-        const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-        d_scan_wide_numeric(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out);
-      } else if (threadIdx.x < 32) {
-        long long qg[8], qh[8];
+    if constexpr (kMode == kScanGlobal) {
+      int col = -1;
+      for (int k = 0; k < vote.top_k; ++k) if (vote.voted[which * vote.top_k + k] == u) col = which * vote.top_k + k;
+      if (col >= 0) {
+        __shared__ uint8_t s_no_flag;      // the global scan writes no is_splittable flag
+        const LeafState& L = leaves[leaf];
+        const FeatMeta fm = meta[u];
+        const long long* hist = vote.packed + kVoteTotals + static_cast<size_t>(col) * kVoteColumn;
+        if (bundle_base && bundle_base[u] >= 0) {
+          d_unbundle_hist(hist, nullptr, fm.num_bin, fm.default_bin, bundle_base[u], which, nullptr, reinterpret_cast<longlong2*>(scan_ws),
+                          vote.packed + 2 * which);
+          hist = reinterpret_cast<const long long*>(scan_ws);
+        }
+        if (!fm.is_categorical) {
+          const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
+          d_scan_wide_numeric(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out);
+        } else if (threadIdx.x < 32) {
+          long long qg[8], qh[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
-        d_scan_feature_cat(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws);
+          for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = hist[b * 2]; qh[j] = hist[b * 2 + 1]; }
+          d_scan_feature_cat(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, scan_ws);
+        }
+      }
+    } else {
+      uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
+      if (kMode == kScanLocal || *flag) {
+        const FeatMeta fm = meta[u];
+        long long* dst = pool + static_cast<size_t>(leaves[leaf].hist_slot) * slot_elems + static_cast<size_t>(fm.hist_off) * 2;
+        const long long* src = H + static_cast<size_t>(fm.hist_off) * 2;
+        const bool bundled = bundle_base && bundle_base[u] >= 0;
+        __shared__ longlong2 s_leaf_tot;      // kScanLocal, bundle member: the leaf's local total from d_unbundle_hist
+        if (!bundled) {
+          const int b = threadIdx.x;
+          longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
+          if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
+          *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
+          __syncthreads();      // the scan reads bins other threads of this block reduced
+        } else {
+          d_unbundle_hist(src, dst, fm.num_bin, fm.default_bin, bundle_base[u], which, leaves + leaf, reinterpret_cast<longlong2*>(scan_ws),
+                          nullptr, kMode == kScanLocal ? &s_leaf_tot : nullptr);
+          dst = reinterpret_cast<long long*>(scan_ws);
+        }
+        LeafState Lloc;      // kScanLocal: the leaf's local sums and true local row count
+        if constexpr (kMode == kScanLocal) {
+          LeafState& Lw = leaves[leaf];
+          longlong2 lt = s_leaf_tot;      // a bundle member's d_unbundle_hist also wrote it to qtot
+          if (!bundled) {
+            const longlong2 t = d_block_sum_column(src);
+            lt = which ? make_longlong2(Lw.qpar[0] - t.x, Lw.qpar[1] - t.y) : t;
+            if (threadIdx.x == 0) { Lw.qtot[0] = lt.x; Lw.qtot[1] = lt.y; }      // every block of this leaf writes the same value
+          }
+          Lloc.sum_g = static_cast<double>(lt.x) * ctrl->inv_g; Lloc.sum_h = static_cast<double>(lt.y) * ctrl->inv_h;
+          Lloc.global_count = Lw.count;
+        }
+        const LeafState& L = kMode == kScanLocal ? Lloc : leaves[leaf];
+        if (*flag) {
+          if (!fm.is_categorical) {
+            const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
+            d_scan_wide_numeric(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out);
+          } else if (threadIdx.x < 32) {
+            long long qg[8], qh[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
+            d_scan_feature_cat(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws);
+          }
+        }
       }
     }
     if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; __threadfence(); }      // visible to the block that runs the pick step
@@ -2013,8 +2148,84 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
   __syncthreads();
   if (s_last) {
     __threadfence();
-    d_pick_block(ctrl, leaves, meta, cands, p);
+    if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
+    else d_pick_block(ctrl, leaves, meta, cands, p);
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
+  }
+}
+
+// The global vote and the packing of the reduced buffer, one block per packed column s = which * top_k + k, after the all-gather of every
+// rank's records recs[R][2][top_k] ([UPSTREAM] VotingParallelTreeLearner::GlobalVoting).  Every block runs its leaf's vote, which is
+// identical on every rank: mean = global count / R (fp32, score_t), a record's weighted gain = gain * (left_count + right_count) / mean,
+// each feature keeps its largest weighted gain (strict >: the first record seen), and the top_k features by (weighted gain desc, real
+// feature index asc) with a finite weighted gain are the leaf's voted features.  Block s then copies its feature's storage column of the
+// leaf's LOCAL histogram (smaller: H, larger: its pool slot) into the packed buffer — of a bundle member only the member's slots, the others
+// zero — and block 0 the leaves' exact local totals (LeafState::qtot).  Dynamic shared memory: 12 bytes per record of one leaf, at most
+// kVoteMaxRecords records (R * top_k, checked when the booster is created).
+__global__ void __launch_bounds__(256)
+k_vote_pack(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const FeatMeta* __restrict__ meta, const int* __restrict__ bundle_base,
+            const VoteRec* __restrict__ recs, int ranks, int top_k, const long long* __restrict__ H, const long long* __restrict__ pool,
+            size_t slot_elems, int* __restrict__ voted, long long* __restrict__ packed) {
+  extern __shared__ double vote_ws[];
+  const int n = ranks * top_k;
+  double* s_wg = vote_ws;                                   // weighted gain of record i of this leaf (-inf: none)
+  int* s_rf = reinterpret_cast<int*>(vote_ws + n);          // its feature, -1 after phase 2 unless it is its feature's representative
+  __shared__ int s_feat;
+  const int s = blockIdx.x, which = s / top_k, k = s % top_k;
+  const int leaf = ctrl->go ? (which ? ctrl->larger : ctrl->smaller) : -1;
+  if (threadIdx.x == 0) s_feat = -1;
+  if (leaf >= 0) {
+    const float mean = static_cast<float>(leaves[leaf].global_count) / static_cast<float>(ranks);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const VoteRec r = recs[(static_cast<size_t>(i / top_k) * 2 + which) * top_k + i % top_k];
+      const double wg = r.gain * static_cast<double>(r.left_count + r.right_count) / static_cast<double>(mean);
+      const bool ok = r.feature >= 0 && wg > kNegInf;       // -inf or NaN never beats the initial kMinScore
+      s_wg[i] = ok ? wg : kNegInf; s_rf[i] = ok ? r.feature : -1;
+    }
+    __syncthreads();
+    int rep[8];       // representative of record i = threadIdx.x + 256 j: its feature's first record with the largest weighted gain
+#pragma unroll
+    for (int j = 0; j < 8; ++j) rep[j] = -1;
+    for (int i = threadIdx.x, j = 0; i < n; i += blockDim.x, ++j) {
+      const int f = s_rf[i];
+      if (f < 0) continue;
+      bool first = true;
+      for (int q = 0; q < n && first; ++q)
+        if (q != i && s_rf[q] == f && (s_wg[q] > s_wg[i] || (s_wg[q] == s_wg[i] && q < i))) first = false;
+      if (j < 8) rep[j] = first ? f : -1;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x, j = 0; i < n; i += blockDim.x, ++j) if (j < 8) s_rf[i] = rep[j];
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const int f = s_rf[i];
+      if (f < 0) continue;
+      const int rf = meta[f].real_index;
+      int rank = 0;
+      for (int q = 0; q < n; ++q) {
+        const int g = s_rf[q];
+        if (g >= 0 && q != i && (s_wg[q] > s_wg[i] || (s_wg[q] == s_wg[i] && meta[g].real_index < rf))) ++rank;
+      }
+      if (rank == k) s_feat = f;
+    }
+  }
+  __syncthreads();
+  const int f = s_feat;
+  if (threadIdx.x == 0) voted[s] = f;
+  longlong2* dst = reinterpret_cast<longlong2*>(packed + kVoteTotals + static_cast<size_t>(s) * kVoteColumn);
+  longlong2 v = make_longlong2(0, 0);
+  if (f >= 0) {
+    const FeatMeta fm = meta[f];
+    const long long* src = (which ? pool + static_cast<size_t>(leaves[leaf].hist_slot) * slot_elems : H) + static_cast<size_t>(fm.hist_off) * 2;
+    const int b = threadIdx.x, base = bundle_base ? bundle_base[f] : -1;
+    if (base < 0 || (b > base && b < base + fm.num_bin)) v = reinterpret_cast<const longlong2*>(src)[b];
+  }
+  dst[threadIdx.x] = v;
+  if (s == 0 && threadIdx.x < 2) {
+    const int l = threadIdx.x ? ctrl->larger : ctrl->smaller;
+    const bool has = ctrl->go && l >= 0;
+    packed[2 * threadIdx.x] = has ? leaves[l].qtot[0] : 0;
+    packed[2 * threadIdx.x + 1] = has ? leaves[l].qtot[1] : 0;
   }
 }
 

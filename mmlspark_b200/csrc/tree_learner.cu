@@ -35,7 +35,8 @@ static TreeDev TreeBlobAt(unsigned char* base, int L) {
 
 TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objective& obj, bool parallel, bool same_device, int num_sms,
                          cudaStream_t stream, Booster::Timing& timing)
-    : train_(train), cfg_(cfg), parallel_(parallel), same_device_(same_device), num_sms_(num_sms), stream_(stream), timing_(timing) {
+    : train_(train), cfg_(cfg), parallel_(parallel), same_device_(same_device), voting_(parallel && cfg.tree_learner == "voting"), num_sms_(num_sms),
+      stream_(stream), timing_(timing) {
   const int n = train.num_data;
   const int L = cfg.num_leaves;
   // leaf passes gather single 32-byte sectors: ask L2 not to fetch the neighbouring sector from DRAM on a miss (default 64 B).
@@ -43,7 +44,7 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   cudaGetLastError();
   B200_CUDA(set_k4_smem_limit());
-  B200_CUDA(cudaFuncSetAttribute(k_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
 
   ResetConfig(cfg);
   sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
@@ -74,6 +75,14 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   }
   flags_.Alloc(static_cast<size_t>(L) * train.nf_pad);
   cands_.Alloc(2 * static_cast<size_t>(train.nf_pad));
+  if (voting_) {      // Booster checked top_k > 0, no feature of more than 256 bins and R * top_k <= kVoteMaxRecords
+    B200_CUDA(cudaFuncSetAttribute(k_scan<kScanLocal>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+    B200_CUDA(cudaFuncSetAttribute(k_scan<kScanGlobal>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+    top_k_ = std::max(1, std::min(cfg.top_k, train.nf));
+    recs_.Alloc(2 * static_cast<size_t>(top_k_)); all_recs_.Alloc(2 * static_cast<size_t>(top_k_) * Net().world);
+    voted_.Alloc(2 * static_cast<size_t>(top_k_));
+    packed_.Alloc(kVoteTotals + 2 * static_cast<size_t>(top_k_) * kVoteColumn); packed_.Zero(stream_);
+  }
   leaves_.Alloc(L); ctrl_.Alloc(1); ctrl_.Zero(stream_);
   const int chunks = n / kPartChunk + 2;
   part_bits_.Alloc(static_cast<size_t>(chunks) * (kPartChunk / 32)); part_chunks_.Alloc(static_cast<size_t>(chunks) + chunks / kPartLocalScan + 8); part_chunks_.Zero(stream_);      // + the super-chunk totals of the two-level scan
@@ -334,6 +343,8 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
   const int pgrid = std::max(1, std::min(n / kPartChunk + 1, part_max_blocks_));
   const dim3 sgrid(std::max(1, d.nfn), 2);      // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates
   const RowBlockBound bound = d.BlockBound();
+  SplitParams sp_local = sp_;      // voting: the local scan's config ([UPSTREAM] VotingParallelTreeLearner::Init local_config_)
+  if (voting_) { sp_local.min_data_in_leaf /= Net().world; sp_local.min_sum_hessian /= Net().world; }
   // B200GBM_SPLIT_TIMING=1 (debug): an event after every operation of a split; per-operation averages go to stderr when the learner is freed
   static const bool split_timing = getenv("B200GBM_SPLIT_TIMING") != nullptr;
   auto mark = [&]() { if (split_timing) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s); split_events_.push_back(e); } };
@@ -370,17 +381,44 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
     nvtxRangePop();
     if (profile_hist) B200_CUDA(cudaEventRecord(hist_events_.back(), s));
     mark();
-    nvtxRangePushA(parallel_ ? "b200gbm:C2 histogram reduce + K5 scan + pick" : "b200gbm:K5 scan + pick");
-    if (parallel_) Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
-    mark();
-    if (d.nw > 0) {
-      k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
-      timing_.launches += 1;
+    // the dynamic scratch of k_scan is only touched by categorical features and bundle members
+    const int scan_smem = (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0;
+    if (voting_) {
+      // local scan + top-k -> all-gather of the records -> vote + pack -> all-reduce of the packed columns -> global scan + pick
+      nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
+      const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
+      k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote);
+      mark();
+      Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
+      mark();
+      const int R = Net().world;
+      k_vote_pack<<<2 * top_k_, 256, static_cast<size_t>(R) * top_k_ * (sizeof(double) + sizeof(int)), s>>>(
+          ctrl, leaves_.p, d.meta.p, d.BundleBase(), all_recs_.p, R, top_k_, H_.p, pool_.p, slot_elems_, voted_.p, packed_.p);
+      mark();
+      Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
+      mark();
+      k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote);
+      nvtxRangePop();
+      comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
+      comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
+      timing_.launches += 2;
+    } else {
+      nvtxRangePushA(parallel_ ? "b200gbm:C2 histogram reduce + K5 scan + pick" : "b200gbm:K5 scan + pick");
+      if (parallel_) {
+        Net().AllReduce(H_.p, slot_elems_, ncclInt64, ncclSum, s);   // C2
+        comm_hist_bytes_ += static_cast<long long>(slot_elems_ * sizeof(long long));
+      }
+      mark();
+      if (d.nw > 0) {
+        k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
+        timing_.launches += 1;
+      }
+      // scan + (last block) pick
+      k_scan<kScanPlain><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{});
+      nvtxRangePop();
     }
-    // scan + (last block) pick; the dynamic scratch is only touched by categorical features and bundle members
-    k_scan<<<sgrid, 256, (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase());
-    nvtxRangePop();
     mark();
+    comm_splits_ += 1;
     nvtxRangePushA("b200gbm:K7 partition + controller");
     LaunchPartition(pgrid, split == L - 2 ? 1 : 0);
     nvtxRangePop();
@@ -401,9 +439,12 @@ void TreeLearner::ReadTree(HostTree* out) {
   B200_CUDA(cudaStreamSynchronize(s));
   if (!split_events_.empty()) {
     static const char* kOps[] = {"gather_q(bagged root)", "K4", "allreduce", "scan+pick", "partition+zeroH+ctl"};
-    const int per = 6;       // marks per split
+    static const char* kVotingOps[] = {"gather_q(bagged root)", "K4", "local scan+top-k", "allgather", "vote+pack", "allreduce", "global scan+pick",
+                                       "partition+zeroH+ctl"};
+    const char* const* ops = voting_ ? kVotingOps : kOps;
+    const int per = voting_ ? 9 : 6;       // marks per split
     for (size_t b0 = 0; b0 + per <= split_events_.size(); b0 += per)
-      for (int o = 0; o < per - 1; ++o) { float ms = 0; cudaEventElapsedTime(&ms, split_events_[b0 + o], split_events_[b0 + o + 1]); split_op_ms_[kOps[o]] += ms; }
+      for (int o = 0; o < per - 1; ++o) { float ms = 0; cudaEventElapsedTime(&ms, split_events_[b0 + o], split_events_[b0 + o + 1]); split_op_ms_[ops[o]] += ms; }
     split_op_trees_ += 1;
     for (auto e : split_events_) cudaEventDestroy(e);
     split_events_.clear();

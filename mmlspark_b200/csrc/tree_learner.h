@@ -33,6 +33,8 @@ class TreeLearner {
   bool profile_hist = false;                 // time K4 with events on the stream (Timing::hist_ms)
   size_t ColumnCopyBytes() const { return bins_cols_.n; }
   void GetColumnCacheInfo(int64_t* out4) const;
+  // {histogram bytes all-reduced, vote record bytes all-gathered (all ranks' records), split rounds enqueued (num_leaves - 1 per tree)}
+  void GetCommInfo(int64_t* out3) const { out3[0] = comm_hist_bytes_; out3[1] = comm_rec_bytes_; out3[2] = comm_splits_; }
 
  private:
   void ResetFeaturesByTree();
@@ -43,6 +45,7 @@ class TreeLearner {
   const Dataset& train_;
   const Config& cfg_;
   const bool parallel_, same_device_;
+  const bool voting_;            // parallel_ and tree_learner=voting: the voting-parallel split chain (kernels.cuh k_scan, k_vote_pack)
   const int num_sms_;
   cudaStream_t stream_;
   Booster::Timing& timing_;
@@ -56,6 +59,13 @@ class TreeLearner {
   size_t slot_elems_ = 0;
   DevBuf<uint8_t> flags_;        // [num_leaves][nf_pad]
   DevBuf<SplitCand> cands_;      // [2][nf_pad]
+  // voting: top_k clamped to the used features; this rank's [2][top_k] records, every rank's [R][2][top_k], the voted features [2][top_k],
+  // and the packed buffer that is all-reduced (kVoteTotals + 2 * top_k storage columns)
+  int top_k_ = 0;
+  DevBuf<VoteRec> recs_, all_recs_;
+  DevBuf<int> voted_;
+  DevBuf<long long> packed_;
+  long long comm_hist_bytes_ = 0, comm_rec_bytes_ = 0, comm_splits_ = 0;
   DevBuf<LeafState> leaves_;
   DevBuf<TreeCtrl> ctrl_;
   DevBuf<unsigned char> tree_blob_;

@@ -1,6 +1,7 @@
 """Small end-to-end runs for compute-sanitizer (memcheck / racecheck / synccheck): every hand-synchronised kernel of the engine at shapes a
 sanitizer finishes in minutes — K4 with TMA bulk copies (root) and cp.async gathers (leaves), the ticket-elected pick step of k_scan, the
-software grid barriers of k_partition, the threshold selection + short bitonic sorts of k_scan_wide, the column-major copy (k_tiles_to_columns), k4_hist_wide, bagging, lambdarank and the device metrics, including the pair batches of auc_mu."""
+software grid barriers of k_partition, the threshold selection + short bitonic sorts of k_scan_wide, the column-major copy (k_tiles_to_columns), k4_hist_wide, bagging, lambdarank, the device metrics, including the pair batches of auc_mu, and the voting-parallel chain (k_scan's local and global
+modes, k_vote_pack) on two rank-threads of one device."""
 import sys
 
 import numpy as np
@@ -47,4 +48,34 @@ yk = np.digitize(s[:15000], [-1, 0, 1]).astype(np.float32)
 run("multiclass+auc_mu", X[:15000], yk, "objective=multiclass num_class=4 metric=auc_mu,multi_logloss", iters=1)
 run("multiclassova+auc_mu dense matrix", X[:15000], yk,
     "objective=multiclassova num_class=4 metric=auc_mu auc_mu_weights=0,1,2,3,1,0,1,2,2,1,0,1,3,2,1,0", iters=1)
+
+
+def run_voting():
+    """tree_learner=voting on 2 rank-threads of this process (same-device collective): k_scan's local and global modes, the ticket-elected
+    top-k step, the all-gather and k_vote_pack"""
+    import threading
+    Xv, yv = X[:20000], s[:20000].astype(np.float32)
+    errs = []
+
+    def task(r):
+        try:
+            capi.set_device(0)
+            capi.network_init("127.0.0.1:31700,127.0.0.1:31701", 31700 + r, 120, 2)
+            ds = capi.Dataset.from_mat(Xv[r * 10000:(r + 1) * 10000], DS).set_field("label", yv[r * 10000:(r + 1) * 10000])
+            b = capi.Booster(ds, BASE + "objective=regression tree_learner=voting top_k=5 num_machines=2")
+            for _ in range(2):
+                b.update_one_iter()
+            b.free(); ds.free()
+            capi.network_free()
+        except Exception as e:   # noqa
+            errs.append(repr(e))
+    ts = [threading.Thread(target=task, args=(r,)) for r in range(2)]
+    for t in ts:
+        t.start()
+    for t in ts:
+        t.join()
+    print("voting(2 ranks, one device)", "ok" if not errs else errs)
+
+
+run_voting()
 print("sanitize smoke done")
