@@ -34,6 +34,8 @@ struct Config {
   int bagging_freq = 0, bagging_seed = 3;
   double feature_fraction = 1.0;
   int feature_fraction_seed = 2;
+  bool extra_trees = false;                 // one random threshold per (leaf, feature) scan (TreeLearner, kernels.cuh K5/K6)
+  int extra_seed = 6;                       // the stream of used feature i starts at extra_seed + i
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -88,7 +90,7 @@ struct Config {
         {"min_child_weight", "min_sum_hessian_in_leaf"}, {"sub_row", "bagging_fraction"},
         {"subsample", "bagging_fraction"}, {"bagging", "bagging_fraction"}, {"subsample_freq", "bagging_freq"},
         {"bagging_fraction_seed", "bagging_seed"}, {"sub_feature", "feature_fraction"},
-        {"colsample_bytree", "feature_fraction"}, {"early_stopping_rounds", "early_stopping_round"},
+        {"colsample_bytree", "feature_fraction"}, {"extra_tree", "extra_trees"}, {"early_stopping_rounds", "early_stopping_round"},
         {"early_stopping", "early_stopping_round"}, {"n_iter_no_change", "early_stopping_round"},
         {"max_tree_output", "max_delta_step"}, {"max_leaf_output", "max_delta_step"}, {"reg_alpha", "lambda_l1"},
         {"reg_lambda", "lambda_l2"}, {"lambda", "lambda_l2"}, {"min_split_gain", "min_gain_to_split"},
@@ -176,6 +178,7 @@ struct Config {
     D("pos_bagging_fraction", &pos_bagging_fraction); D("neg_bagging_fraction", &neg_bagging_fraction);
     I("bagging_freq", &bagging_freq); I("bagging_seed", &bagging_seed); D("feature_fraction", &feature_fraction);
     I("feature_fraction_seed", &feature_fraction_seed); I("early_stopping_round", &early_stopping_round);
+    B("extra_trees", &extra_trees); I("extra_seed", &extra_seed);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -239,7 +242,7 @@ struct Config {
     s << "[bagging_fraction: " << Num(bagging_fraction) << "]\n[pos_bagging_fraction: " << Num(pos_bagging_fraction) << "]\n";
     s << "[neg_bagging_fraction: " << Num(neg_bagging_fraction) << "]\n[bagging_freq: " << bagging_freq << "]\n";
     s << "[bagging_seed: " << bagging_seed << "]\n[feature_fraction: " << Num(feature_fraction) << "]\n";
-    s << "[feature_fraction_bynode: 1]\n[feature_fraction_seed: " << feature_fraction_seed << "]\n[extra_trees: 0]\n[extra_seed: 6]\n";
+    s << "[feature_fraction_bynode: 1]\n[feature_fraction_seed: " << feature_fraction_seed << "]\n[extra_trees: " << extra_trees << "]\n[extra_seed: " << extra_seed << "]\n";
     s << "[early_stopping_round: " << early_stopping_round << "]\n[first_metric_only: 0]\n";
     s << "[max_delta_step: " << Num(max_delta_step) << "]\n[lambda_l1: " << Num(lambda_l1) << "]\n[lambda_l2: " << Num(lambda_l2) << "]\n";
     s << "[linear_lambda: 0]\n[min_gain_to_split: " << Num(min_gain_to_split) << "]\n[drop_rate: " << Num(drop_rate) << "]\n";

@@ -1344,6 +1344,10 @@ void Dataset::SetFeatureNames(const char** names, int n) {
 #include "tree_learner.cu"      // the booster's tree learner, in this translation unit
 namespace b200gbm {
 
+// the voting learner's local and global scans would each need their own draw order of the extra_trees streams; not restated
+static const char* const kVotingExtraTrees = "tree_learner=voting does not support extra_trees with more than one machine; "
+                                             "use tree_learner=data_parallel or extra_trees=false";
+
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1387,6 +1391,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
     if (static_cast<long long>(Net().world) * std::min(cfg.top_k, std::max(train->nf, 1)) > kVoteMaxRecords)
       Fatal("tree_learner=voting supports num_machines * top_k <= " + std::to_string(kVoteMaxRecords) + ", got " + std::to_string(Net().world) +
             " * " + std::to_string(std::min(cfg.top_k, train->nf)));
+    if (cfg.extra_trees) Fatal(kVotingExtraTrees);
   }
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
@@ -1727,6 +1732,7 @@ void Booster::ResetParameter(const char* params) {
     try {
       ValidateMetrics();
       for (auto* v : valids_) CheckMetricData(*v->ds);
+      if (parallel_ && cfg.tree_learner == "voting" && cfg.extra_trees) Fatal(kVotingExtraTrees);
     } catch (...) {
       cfg = before;
       throw;

@@ -69,6 +69,29 @@ struct SplitParams {
   int max_cat_threshold, max_cat_to_onehot, min_data_per_group, pad3;   // 32, 4, 100
 };
 
+// extra_trees (the scans' template parameter kExtra; [UPSTREAM] FeatureHistogram USE_RAND, FeatureMetainfo::rand): every used feature
+// owns one LCG, seeded extra_seed + i with i the feature's position among the used features in real-index order.  Each scan of the
+// feature in a leaf whose draw range is non-empty takes one draw, the smaller leaf's before the larger's: NextInt(0, range) = (x & 0x7fffffff) % range after x = 214013 x + 2531011.
+// An empty range draws nothing and leaves the threshold at 0, as upstream does.  The stream states live in xrand[0, nf_pad); the
+// scan block of (leaf `which`, feature u) writes its number of draws (0 or 1) to xrand[(1 + which) * nf_pad + u], and the block that runs
+// the pick step advances the states by them once every scan block of the round has finished (d_extra_commit).
+__host__ __device__ __forceinline__ unsigned d_lcg_next(unsigned x) { return 214013u * x + 2531011u; }
+__device__ __forceinline__ int d_extra_draw(unsigned* x, int range) {
+  if (range <= 0) return 0;
+  *x = d_lcg_next(*x);
+  return static_cast<int>((*x & 0x7fffffffu) % static_cast<unsigned>(range));
+}
+// seeds every feature's stream: xrand[u] = extra_seed + pos[u], pos[u] = the feature's position among the used features in real-index order
+__global__ void k_extra_seed(unsigned* __restrict__ xrand, const int* __restrict__ pos, int nf, int extra_seed) {
+  for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < nf; u += gridDim.x * blockDim.x) xrand[u] = static_cast<unsigned>(extra_seed + pos[u]);
+}
+// many-vs-many categorical search: the draw range given the number of bins with >= cat_smooth rebuilt rows
+// (max(min(max_num_cat, used_bin) - 1, 0) with max_num_cat = min(max_cat_threshold, (used_bin + 1) / 2))
+__device__ __forceinline__ int d_cat_rand_range(int used_bin, int max_cat_threshold) {
+  const int max_num_cat = min(max_cat_threshold, (used_bin + 1) / 2);
+  return max(min(max_num_cat, used_bin) - 1, 0);
+}
+
 struct SplitCand {         // best threshold of one (leaf, feature)
   double gain;             // best_gain - min_gain_shift, or -inf
   double left_g, left_h;   // best_sum_left_gradient / _hessian (hessian still carries +kEpsilon)
@@ -806,12 +829,34 @@ k_round_ctl(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
 // What k_scan (below) runs besides the numerical scan: the warp-level categorical search, and the pick step of its last block over the
 // candidates of every feature, the wide ones from k_scan_wide included.  All sums are exact int64; gains are fp64.
 
+
+// The larger leaf's block of a many-vs-many categorical feature: did the smaller leaf's scan of it draw?  Counts the smaller leaf's used
+// bins (>= cat_smooth rebuilt rows, bin 0 excluded) in its histogram column `hist` (H), exactly as the smaller leaf's own scan counts
+// them.  Called by every thread of the block; out of line to keep it off the scans' register budget.
+__device__ __noinline__ bool d_smaller_drew_cat(const long long* __restrict__ hist, int num_bin, const LeafState& S, double inv_h,
+                                                const SplitParams& p, int max_cat_threshold) {
+  const double cnt_factor = S.global_count / (S.sum_h + 2 * kEpsD);
+  int used_bin = 0;
+  for (int b0 = 0; b0 < num_bin; b0 += blockDim.x) {      // the same trip count in every thread
+    const int b = b0 + threadIdx.x;
+    bool used = false;
+    if (b >= 1 && b < num_bin) used = static_cast<int>(static_cast<double>(hist[b * 2 + 1]) * inv_h * cnt_factor + 0.5) >= p.cat_smooth;
+    used_bin += __syncthreads_count(used);
+  }
+  return d_cat_rand_range(used_bin, max_cat_threshold) > 0;
+}
+
 // Categorical split search for one feature by one warp (FeatureHistogram::FindBestThresholdCategoricalInner [UPSTREAM]):
 // one-hot when num_bin <= max_cat_to_onehot; otherwise the bins holding >= cat_smooth rows are ranked by g/(h+cat_smooth)
 // (stable, ties by bin) and accumulated from both ends, at most max_cat_threshold bins, lambda_l2 += cat_l2.
 // ws = this warp's shared scratch: g[256], h[256], ctr[256] doubles + order[256] + used[256] bytes.
-__device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const long long (&qh)[8], int lane, const FeatMeta m, const LeafState& L,
-                                                   double inv_g, double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* outp, double* ws) {
+// kExtra (extra_trees): xr is the feature's stream state before this scan's draw.  One-hot draws r over the num_bin - 1 category bins
+// and evaluates only bin r + 1; many-vs-many draws r over d_cat_rand_range and evaluates only the prefixes of r + 1 bins.  Returns the
+// number of draws taken (0 or 1), in every lane.
+template <bool kExtra>
+__device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const long long (&qh)[8], int lane, const FeatMeta m, const LeafState& L,
+                                                  double inv_g, double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* outp, double* ws,
+                                                  unsigned xr) {
   SplitCand& out = *outp;
   double* sg = ws; double* sh = ws + 256; double* sc = ws + 512;
   unsigned char* order = reinterpret_cast<unsigned char*>(ws + 768);
@@ -822,6 +867,8 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
   if (!(p.max_delta_step > 0)) pshift.max_delta_step = 0;
   const double min_gain_shift = d_leaf_gain(sum_g, sum_h, pshift) + p.min_gain_to_split;
   const bool onehot = m.num_bin <= p.max_cat_to_onehot;
+  int drew = 0, rand_t = -1;      // rand_t: the one candidate index evaluated, -1: every candidate
+  if (kExtra && onehot) { rand_t = d_extra_draw(&xr, m.num_bin - 1); drew = m.num_bin > 1 ? 1 : 0; }
   bool any_valid = false;
   double best_gain = kNegInf, best_lg = 0, best_lh = 0;
   int best_t = 0x7fffffff, best_lc = 0;
@@ -837,7 +884,7 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
       if (in_range && !(cnt < p.min_data_in_leaf || h < p.min_sum_hessian)) {
         const int other = num_data - cnt;
         const double oh = sum_h - h - kEpsD;
-        if (other >= p.min_data_in_leaf && oh >= p.min_sum_hessian) {
+        if (other >= p.min_data_in_leaf && oh >= p.min_sum_hessian && (!kExtra || b - 1 == rand_t)) {
           const double gain = d_leaf_gain(sum_g - g, oh, p) + d_leaf_gain(g, h + kEpsD, p);
           if (gain > min_gain_shift) {
             any_valid = true;
@@ -868,7 +915,7 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
         out.cat_bits[best_t >> 5] |= 1u << (best_t & 31);
       }
     }
-    return;
+    return drew;
   }
   // ---- rank the used bins by ctr (stable): rank = #{used j : ctr_j < ctr_i  or (== and j < i)}.
   // Uniform loop over the bins: sc[bj] / usedb[bj] are broadcast loads, the 8 comparisons of a lane are independent.
@@ -882,6 +929,11 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
     usedb[b] = u ? 1 : 0;
     ci[j] = sc[b];
     used_bin += __popc(__ballot_sync(0xffffffffu, u));
+  }
+  if (kExtra) {
+    const int range = d_cat_rand_range(used_bin, p.max_cat_threshold);
+    rand_t = d_extra_draw(&xr, range);
+    drew = range > 0 ? 1 : 0;
   }
   __syncwarp();
   int rank[8];
@@ -920,6 +972,7 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
         if (srh < p.min_sum_hessian) break;
         if (cnt_cur_group < p.min_data_per_group) continue;
         cnt_cur_group = 0;
+        if (kExtra && i != rand_t) continue;
         const double gain = d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
         if (gain <= min_gain_shift) continue;
         any_valid = true;
@@ -936,6 +989,7 @@ __device__ __noinline__ void d_scan_feature_cat(const long long (&qg)[8], const 
       }
     }
   }
+  return drew;
 }
 
 __device__ __forceinline__ void d_choose_leaf(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitParams& p, int lane) {
@@ -1520,8 +1574,11 @@ __device__ __forceinline__ void d_block_excl3(long long& a, long long& b, long l
 // pass, with the bins spread over a 256-thread block — thread t owns the contiguous bins [t*S, (t+1)*S) — exclusive block scans of the per-thread
 // (g, h, count) sums, and a block argmax with the sequential scan's tie-breaks (reverse pass: the highest threshold wins, forward pass: the
 // lowest).  hist = the leaf's reduced histogram of the feature in its pool slot.  Returns through *outp (thread 0) and *flag.
+// kExtra (extra_trees): only the candidate with that threshold is evaluated, in either pass; the count and hessian tests before it
+// still skip and break as they do without it ([UPSTREAM] FindBestThresholdSequentially, USE_RAND: t - 1 + offset resp. t + offset).
+template <bool kExtra>
 __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ hist, const WideMeta m, const LeafState& L, double inv_g, double inv_h,
-                                                  const SplitParams& p, uint8_t* flag, SplitCand* outp) {
+                                                  const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr) {
   __shared__ long long s_sc[24];
   __shared__ double s_bg[8], s_blg[8], s_blh[8];
   __shared__ int s_bt[8], s_blc[8], s_any, s_stop[2];
@@ -1563,6 +1620,7 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       const int left_count = num_data - right_count;
       const double slh = sum_h - srh;
       if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
+      if (kExtra && b - 1 != rand_thr) continue;
       const double slg = sum_g - srg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
@@ -1624,6 +1682,7 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       const int right_count = num_data - left_count;
       const double srh = sum_h - slh;
       if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { f_stop = true; break; }
+      if (kExtra && b != rand_thr) continue;
       const double srg = sum_g - slg;
       const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
@@ -1695,9 +1754,11 @@ __device__ __noinline__ void d_block_bitonic2(double* k, int* id, int stride, in
 // (smaller|larger, feature).  The histogram is reduced into the leaf's pool slot (parent - smaller for the larger child), the
 // max_cat_threshold smallest and largest ctr = g / (h + cat_smooth) among the bins that hold >= cat_smooth rows are selected in the
 // (ctr, bin) order of the reference's stable sort, and thread 0 accumulates from both ends exactly like the sequential code.
+template <bool kExtra>
 __global__ void __launch_bounds__(256)
 k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const WideMeta* __restrict__ wm, const long long* __restrict__ H,
-            long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p) {
+            long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
+            unsigned* __restrict__ xrand) {
   extern __shared__ __align__(16) unsigned char sw_smem[];
   double* s_key = reinterpret_cast<double*>(sw_smem);                          // [num_bin] ctr keys of the used bins, +inf otherwise
   __shared__ int s_used;
@@ -1709,7 +1770,11 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   out.l2_extra = 0; out.is_cat = 1; out.cat_list_len = 0;
   for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
   uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
-  if (!*flag) { if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; __threadfence(); } return; }
+  unsigned* draws = xrand + static_cast<size_t>(1 + which) * p.nf_pad + u;      // extra_trees: this scan's draw count (see d_lcg_next)
+  if (!*flag) {
+    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 0u; __threadfence(); }
+    return;
+  }
   const WideMeta m = wm[w];
   const LeafState& L = leaves[leaf];
   const double inv_g = ctrl->inv_g, inv_h = ctrl->inv_h;
@@ -1718,6 +1783,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
+  unsigned xr = kExtra ? xrand[u] : 0u;      // the stream state before this round's draws of the feature
   if (!m.is_cat) {        // wide numerical feature (max_bin > 255): reduce into the pool slot, then the block-wide two-pass scan
     for (int b = threadIdx.x; b < m.num_bin; b += blockDim.x) {
       longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
@@ -1725,10 +1791,18 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
       *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
     }
     __syncthreads();      // every thread reads bins other threads reduced (same block: visible after the barrier)
-    d_scan_wide_numeric(dst, m, L, inv_g, inv_h, p, flag, &out);
-    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; __threadfence(); }
+    int rand_thr = 0;
+    if (kExtra) {      // more than 256 bins: both leaves draw, the smaller first
+      if (which) xr = d_lcg_next(xr);
+      rand_thr = d_extra_draw(&xr, m.num_bin - 2);
+    }
+    d_scan_wide_numeric<kExtra>(dst, m, L, inv_g, inv_h, p, flag, &out, rand_thr);
+    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 1u; __threadfence(); }
     return;
   }
+  // the larger leaf's draw comes after the smaller's, if that one drew
+  if (kExtra && which && d_smaller_drew_cat(src, m.num_bin, leaves[ctrl->smaller], inv_h, p, min(p.max_cat_threshold, kCatListMax)))
+    xr = d_lcg_next(xr);
   // ---- reduce into the pool slot and build the ctr keys (loads of 4 bins in flight per thread before the dependent stores)
   if (threadIdx.x == 0) s_used = 0;
   __syncthreads();
@@ -1762,6 +1836,12 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   __syncthreads();
   const int used_bin = s_used;
   const int max_num_cat = min(min(p.max_cat_threshold, kCatListMax), (used_bin + 1) / 2);
+  int rand_i = 0, drew = 0;      // extra_trees: the one prefix length - 1 evaluated
+  if (kExtra) {
+    const int range = d_cat_rand_range(used_bin, min(p.max_cat_threshold, kCatListMax));
+    rand_i = d_extra_draw(&xr, range);
+    drew = range > 0 ? 1 : 0;
+  }
   // ---- the reference sorts the used bins by (ctr, bin) and walks max_num_cat bins from either end; only those 2 * max_num_cat order
   // statistics are needed.  Sorting thousands of keys (first version: block-wide bitonic sort, ~600 us per launch) and selecting them
   // one per round (second version: 64 dependent rounds of a strided rescan, ~300 us — the rescan's latency is the same whether one
@@ -1881,6 +1961,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
       if (srh < p.min_sum_hessian) break;
       if (cnt_cur_group < p.min_data_per_group) continue;
       cnt_cur_group = 0;
+      if (kExtra && i != rand_i) continue;
       s_plg[d][i] = slg; s_plh[d][i] = slh; s_plc[d][i] = left_count; s_pgain[d][i] = 0.0;      // 0.0 = "evaluate me"
     }
   }
@@ -1917,6 +1998,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
     for (int i = 0; i <= best_i && i < kCatListMax; ++i) out.cat_list[i] = s_sel[best_dir == 1 ? 0 : 1][i];
   }
   cands[which * p.nf_pad + u] = out;
+  if (kExtra) *draws = static_cast<unsigned>(drew);
   __threadfence();
 }
 
@@ -2052,14 +2134,28 @@ d_topk_block(const TreeCtrl* ctrl, const LeafState* leaves, const FeatMeta* __re
   }
 }
 
-template <int kMode>
+// extra_trees, in the block that runs the pick step once every scan block of the round (k_scan_wide's before them) has finished: advance
+// each feature's stream by the draws of the round's smaller and larger leaf.  Features that were not scanned wrote 0.
+__device__ __noinline__ void d_extra_commit(const TreeCtrl* ctrl, unsigned* xrand, const SplitParams& p) {
+  if (!ctrl->go) return;
+  const bool larger = ctrl->larger >= 0;
+  for (int u = threadIdx.x; u < p.nf; u += blockDim.x) {
+    unsigned n = __ldcg(&xrand[p.nf_pad + u]) + (larger ? __ldcg(&xrand[2 * p.nf_pad + u]) : 0u);
+    unsigned x = xrand[u];
+    for (; n > 0; --n) x = d_lcg_next(x);
+    xrand[u] = x;
+  }
+}
+
+template <int kMode, bool kExtra = false>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
+  static_assert(!kExtra || kMode == kScanPlain, "the voting learner does not train extra trees (Booster fails at create)");
   const int which = blockIdx.y;
   const int leaf = which ? ctrl->larger : ctrl->smaller;
   const int u = blockIdx.x;
@@ -2083,12 +2179,12 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
         }
         if (!fm.is_categorical) {
           const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-          d_scan_wide_numeric(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out);
+          d_scan_wide_numeric<false>(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, 0);
         } else if (threadIdx.x < 32) {
           long long qg[8], qh[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = hist[b * 2]; qh[j] = hist[b * 2 + 1]; }
-          d_scan_feature_cat(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, scan_ws);
+          d_scan_feature_cat<false>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, scan_ws, 0u);
         }
       }
     } else {
@@ -2124,16 +2220,32 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
         }
         const LeafState& L = kMode == kScanLocal ? Lloc : leaves[leaf];
         if (*flag) {
+          // extra_trees: the stream state before this scan's draw — past the smaller leaf's draw for the larger leaf's block.  Both leaves
+          // hold the same pre-scan flag (inherited from their parent), so the smaller one scanned this feature too; it drew unless its range
+          // was empty, which only the many-vs-many categorical search decides from the data: the smaller leaf's used bins, counted in H.
+          unsigned xr = kExtra ? xrand[u] : 0u;
+          if (kExtra && which) {
+            bool smaller_drew = fm.is_categorical ? fm.num_bin > 1 : fm.num_bin > 2;
+            if (fm.is_categorical && fm.num_bin > p.max_cat_to_onehot)
+              smaller_drew = d_smaller_drew_cat(src, fm.num_bin, leaves[ctrl->smaller], ctrl->inv_h, p, p.max_cat_threshold);
+            if (smaller_drew) xr = d_lcg_next(xr);
+          }
+          int drew = 0;
           if (!fm.is_categorical) {
             const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-            d_scan_wide_numeric(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out);
+            const int rand_thr = kExtra ? d_extra_draw(&xr, fm.num_bin - 2) : 0;
+            drew = fm.num_bin > 2 ? 1 : 0;
+            d_scan_wide_numeric<kExtra>(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, rand_thr);
           } else if (threadIdx.x < 32) {
             long long qg[8], qh[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
-            d_scan_feature_cat(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws);
+            drew = d_scan_feature_cat<kExtra>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws, xr);
           }
+          if (kExtra && threadIdx.x == 0) xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = static_cast<unsigned>(drew);
         }
+      } else if (kExtra && threadIdx.x == 0) {      // not scanned: no draw
+        xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = 0u;
       }
     }
     if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; __threadfence(); }      // visible to the block that runs the pick step
@@ -2149,7 +2261,10 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
   if (s_last) {
     __threadfence();
     if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
-    else d_pick_block(ctrl, leaves, meta, cands, p);
+    else {
+      if constexpr (kExtra) d_extra_commit(ctrl, xrand, p);
+      d_pick_block(ctrl, leaves, meta, cands, p);
+    }
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
   }
 }

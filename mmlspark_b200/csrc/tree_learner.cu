@@ -45,6 +45,7 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   cudaGetLastError();
   B200_CUDA(set_k4_smem_limit());
   B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
 
   ResetConfig(cfg);
   sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
@@ -58,7 +59,8 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
       if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
     }
   }
 
@@ -75,6 +77,14 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   }
   flags_.Alloc(static_cast<size_t>(L) * train.nf_pad);
   cands_.Alloc(2 * static_cast<size_t>(train.nf_pad));
+  {   // extra_trees streams, allocated whatever extra_trees says: a ResetParameter may turn it on.  The engine's inner order puts the wide
+      // features last, so feature sample_order[i] is used feature i in real-index order.
+    std::vector<int> pos(train.nf_pad, 0);
+    for (int i = 0; i < train.nf; ++i) pos[train.sample_order[i]] = i;
+    xrand_pos_.Alloc(train.nf_pad); xrand_pos_.Upload(pos.data(), pos.size(), stream_);
+    xrand_.Alloc(3 * static_cast<size_t>(train.nf_pad));
+    SeedExtraStreams(cfg);
+  }
   if (voting_) {      // Booster checked top_k > 0, no feature of more than 256 bins and R * top_k <= kVoteMaxRecords
     B200_CUDA(cudaFuncSetAttribute(k_scan<kScanLocal>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
     B200_CUDA(cudaFuncSetAttribute(k_scan<kScanGlobal>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
@@ -125,6 +135,16 @@ TreeLearner::~TreeLearner() {
 void TreeLearner::ResetConfig(const Config& cfg) {
   sp_.l1 = cfg.lambda_l1; sp_.l2 = cfg.lambda_l2; sp_.max_delta_step = cfg.max_delta_step; sp_.min_gain_to_split = cfg.min_gain_to_split;
   sp_.min_sum_hessian = cfg.min_sum_hessian_in_leaf; sp_.min_data_in_leaf = cfg.min_data_in_leaf; sp_.max_depth = cfg.max_depth;
+  extra_trees_ = cfg.extra_trees;
+  SeedExtraStreams(cfg);      // [UPSTREAM] HistogramPool::ResetConfig re-runs SetFeatureInfo, which re-seeds every feature's Random
+}
+
+// extra_trees streams (kernels.cuh d_lcg_next): used feature i in real-index order starts at extra_seed + i.  One small kernel on the
+// stream, ordered after the trees already enqueued; nothing is copied from the host.  With extra_trees off the states are never read.
+void TreeLearner::SeedExtraStreams(const Config& cfg) {
+  if (!xrand_.p || !cfg.extra_trees) return;      // the constructor's first ResetConfig runs before the buffers exist; it seeds after them
+  k_extra_seed<<<1, 256, 0, stream_>>>(xrand_.p, xrand_pos_.p, train_.nf, cfg.extra_seed);
+  B200_CUDA(cudaGetLastError());
 }
 
 TreeDev TreeLearner::TreeAt(unsigned char* blob) const { return TreeBlobAt(blob, sp_.num_leaves); }
@@ -387,7 +407,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       // local scan + top-k -> all-gather of the records -> vote + pack -> all-reduce of the packed columns -> global scan + pick
       nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
       const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
-      k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote);
+      k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p);
       mark();
       Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
       mark();
@@ -397,7 +417,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       mark();
       Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
       mark();
-      k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote);
+      k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p);
       nvtxRangePop();
       comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
       comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
@@ -410,11 +430,14 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       }
       mark();
       if (d.nw > 0) {
-        k_scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_);
+        auto* scan_wide = extra_trees_ ? k_scan_wide<true> : k_scan_wide<false>;
+        scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p);
         timing_.launches += 1;
       }
       // scan + (last block) pick
-      k_scan<kScanPlain><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{});
+      // extra_trees: the scan's own instantiation, so that the default one compiles to what it was without the feature
+      auto* scan = extra_trees_ ? k_scan<kScanPlain, true> : k_scan<kScanPlain, false>;
+      scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p);
       nvtxRangePop();
     }
     mark();

@@ -38,6 +38,7 @@ class TreeLearner {
 
  private:
   void ResetFeaturesByTree();
+  void SeedExtraStreams(const Config& cfg);
   void LaunchPartition(int grid, int last);
   void EnsureColumnCopy();
   void UpdateColumnCache(const HostTree& t);
@@ -50,6 +51,7 @@ class TreeLearner {
   cudaStream_t stream_;
   Booster::Timing& timing_;
   SplitParams sp_{};
+  bool extra_trees_ = false;     // cfg.extra_trees as of the last ResetConfig: launch the scans' extra_trees instantiations
   int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
@@ -59,6 +61,8 @@ class TreeLearner {
   size_t slot_elems_ = 0;
   DevBuf<uint8_t> flags_;        // [num_leaves][nf_pad]
   DevBuf<SplitCand> cands_;      // [2][nf_pad]
+  DevBuf<unsigned> xrand_;       // extra_trees: [nf_pad] stream state per feature, then [2][nf_pad] draws of the round (kernels.cuh d_lcg_next)
+  DevBuf<int> xrand_pos_;        // [nf_pad] each inner feature's position among the used features in real-index order (its stream's seed offset)
   // voting: top_k clamped to the used features; this rank's [2][top_k] records, every rank's [R][2][top_k], the voted features [2][top_k],
   // and the packed buffer that is all-reduced (kVoteTotals + 2 * top_k storage columns)
   int top_k_ = 0;

@@ -41,6 +41,7 @@ COMMON_DEFAULTS = dict(
     isProvideTrainingMetric=False,      # :402-404
     metric="",                          # :409-438
     minGainToSplit=0.0, maxDeltaStep=0.0, maxBinByFeature=(), minDataInLeaf=20,         # :443-466
+    extraTrees=False, extraSeed=6,      # LightGBM 3.2's extra_trees / extra_seed (not a param of the reference's estimators)
     delegate=None,
     # column params (core/contracts/Params.scala:93-208 + Spark ML)
     featuresCol="features", labelCol="label", predictionCol="prediction", weightCol=None, initScoreCol=None,
@@ -120,6 +121,8 @@ class TrainParams:
             s += ("drop_rate=%s max_drop=%d skip_drop=%s xgboost_dart_mode=%s uniform_drop=%s  " % (
                 scala_double(p["dropRate"]), p["maxDrop"], scala_double(p["skipDrop"]), scala_bool(p["xgboostDartMode"]), scala_bool(p["uniformDrop"])))
         s += "num_threads=%d " % p["numThreads"]
+        if p["extraTrees"]:      # only when set, so every other parameter string stays as the reference builds it
+            s += "extra_trees=true extra_seed=%d " % p["extraSeed"]
         return s
 
     def to_string(self):
