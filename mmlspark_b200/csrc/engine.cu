@@ -3,7 +3,7 @@
 #include "engine.h"
 #include "objective.h"
 #include "renew_kernel.cuh"
-#include "metric_kernels.cuh"
+#include "metrics.h"
 
 #include <nvtx3/nvToolsExt.h>      // header-only NVTX v3: ranges are no-ops unless a profiler injects itself
 
@@ -1377,7 +1377,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
     if (!(bagging_ || ff)) Fatal("Check failed: (config->bagging_freq > 0 && config->bagging_fraction < 1.0f && config->bagging_fraction > 0.0f) || (config->feature_fraction < 1.0f && config->feature_fraction > 0.0f)");
   }
   if (cfg.num_leaves < 2) Fatal("num_leaves should be >= 2");
-  ValidateMetrics();      // an unknown metric must fail LGBM_BoosterCreate, not the first LGBM_BoosterGetEval inside the training loop
+  metrics_.reset(new Metrics(cfg, *obj_, *train));      // an unknown metric must fail LGBM_BoosterCreate, not the first GetEval in training
   if (train->label.empty()) Fatal("label should not be empty for training");
   K = obj_->NumTreePerIteration();
   parallel_ = Net().active && Net().world > 1;
@@ -1730,9 +1730,8 @@ void Booster::ResetParameter(const char* params) {
   cfg.num_machines = keep_machines;
   if (train) {      // metrics named by the reset meet the checks of LGBM_BoosterCreate / AddValidData; a rejected reset changes nothing
     try {
-      ValidateMetrics();
-      for (auto* v : valids_) CheckMetricData(*v->ds);
       if (parallel_ && cfg.tree_learner == "voting" && cfg.extra_trees) Fatal(kVotingExtraTrees);
+      metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;
       throw;
@@ -1747,7 +1746,7 @@ void Booster::AddValidData(const Dataset* valid) {
   EnsureDevice();
   if (!train) Fatal("cannot add validation data to a prediction-only booster");
   if (valid->nf != train->nf) Fatal("validation data must be created with reference=train");
-  CheckMetricData(*valid);
+  metrics_->CheckData(*valid);
   ValidSet* v = new ValidSet();
   v->ds = valid;
   v->score.Alloc(static_cast<size_t>(K) * valid->num_data);
@@ -1828,31 +1827,23 @@ std::string Booster::DumpModelJson(int start_iteration, int num_iteration) const
   return s.str();
 }
 
-// ---- evaluation (host side: metrics are not on the hot path; scores are read back) -------------
-std::vector<std::string> Booster::EvalNames() const {
-  std::vector<std::string> names;
-  for (auto& m : cfg.metric) {
-    if (m == "ndcg" || m == "map") for (int k : cfg.eval_at) names.push_back(m + "@" + std::to_string(k));
-    else names.push_back(m);
-  }
-  return names;
+// ---- the scores of the training / validation data, and their evaluation ------------------------
+std::pair<const Dataset*, const DevBuf<double>*> Booster::ScoredData(int data_idx) const {
+  if (data_idx < 0 || data_idx > static_cast<int>(valids_.size())) Fatal("data_idx out of range");
+  if (data_idx == 0) return {train, &score_};
+  return {valids_[data_idx - 1]->ds, &valids_[data_idx - 1]->score};
 }
 int64_t Booster::NumPredict(int data_idx) const {
   if (!train) Fatal("this booster was loaded from a model string: it holds no training/validation data (use the predict entry points)");
-  if (data_idx == 0) return static_cast<int64_t>(K) * train->num_data;
-  if (data_idx - 1 >= static_cast<int>(valids_.size())) Fatal("data_idx out of range");
-  return static_cast<int64_t>(K) * valids_[data_idx - 1]->ds->num_data;
+  return static_cast<int64_t>(K) * ScoredData(data_idx).first->num_data;
 }
 void Booster::GetPredict(int data_idx, int64_t* out_len, double* out) {
   if (!train) Fatal("this booster was loaded from a model string: it holds no training/validation data (use the predict entry points)");
   EnsureDevice();
   if (is_dart_ && data_idx == 0 && !dart_dropped_this_iter_) DroppingTrees();      // DART::GetTrainingScore
-  const Dataset* ds = data_idx == 0 ? train : valids_.at(data_idx - 1)->ds;
-  const DevBuf<double>& sc = data_idx == 0 ? score_ : valids_[data_idx - 1]->score;
-  const int n = ds->num_data;
+  const int n = ScoredData(data_idx).first->num_data;
   std::vector<double> raw(static_cast<size_t>(K) * n);
-  sc.Download(raw.data(), raw.size(), stream_);
-  B200_CUDA(cudaStreamSynchronize(stream_));
+  GetRawScores(data_idx, raw.data());
   std::vector<double> r(K), o(K);
   for (int i = 0; i < n; ++i) {
     for (int k = 0; k < K; ++k) r[k] = raw[static_cast<size_t>(k) * n + i];
@@ -1861,333 +1852,21 @@ void Booster::GetPredict(int data_idx, int64_t* out_len, double* out) {
   }
   *out_len = static_cast<int64_t>(K) * n;
 }
-
-// ---- evaluation on the device (metric_kernels.cuh): only the reduced sums cross PCIe
-static int MetricKindOf(const std::string& m) {
-  static const std::map<std::string, int> kinds = {
-      {"l2", kMetL2}, {"rmse", kMetL2}, {"l1", kMetL1}, {"huber", kMetHuber}, {"fair", kMetFair}, {"poisson", kMetPoisson}, {"gamma", kMetGamma},
-      {"gamma_deviance", kMetGammaDeviance}, {"tweedie", kMetTweedie}, {"quantile", kMetQuantile}, {"mape", kMetMape},
-      {"binary_logloss", kMetBinLogloss}, {"binary_error", kMetBinError}, {"multi_logloss", kMetMultiLogloss}, {"multi_error", kMetMultiError},
-      {"cross_entropy", kMetXent}, {"cross_entropy_lambda", kMetXentLambda}, {"kullback_leibler", kMetKLDiv}};
-  auto it = kinds.find(m);
-  return it == kinds.end() ? -1 : it->second;
+void Booster::GetRawScores(int data_idx, double* out) {
+  if (!train) Fatal("this booster was loaded from a model string: it holds no training/validation data");
+  EnsureDevice();
+  const auto [ds, sc] = ScoredData(data_idx);
+  sc->Download(out, static_cast<size_t>(K) * ds->num_data, stream_);
+  B200_CUDA(cudaStreamSynchronize(stream_));
 }
-void Booster::ValidateMetrics() const {
-  for (auto& m : cfg.metric)
-    if (MetricKindOf(m) < 0 && m != "auc" && m != "average_precision" && m != "auc_mu" && m != "ndcg" && m != "map")
-      Fatal("Unknown metric type name: " + m);
-  if (cfg.eval_at.size() > static_cast<size_t>(kMaxEvalAt)) Fatal("eval_at: at most " + std::to_string(kMaxEvalAt) + " positions are supported");
-  if (std::find(cfg.metric.begin(), cfg.metric.end(), "auc_mu") != cfg.metric.end()) {
-    const int nc = obj_->NumTreePerIteration();
-    if (nc < 2) Fatal("metric auc_mu needs a multiclass objective");
-    // [UPSTREAM Config::GetAucMuWeights]
-    if (!cfg.auc_mu_weights.empty() && cfg.auc_mu_weights.size() != static_cast<size_t>(nc) * nc)
-      Fatal("auc_mu_weights must have " + std::to_string(nc * nc) + " elements, but found " + std::to_string(cfg.auc_mu_weights.size()));
-  }
-  CheckMetricData(*train);
-}
-// [UPSTREAM CrossEntropyLambdaMetric / KullbackLeiblerDivergence / AucMuMetric ::Init] checks of the labels and weights a metric is
-// evaluated on
-void Booster::CheckMetricData(const Dataset& ds) const {
-  for (auto& m : cfg.metric) {
-    if (m == "auc_mu") {      // the class of a row is its label cast to int, as the multiclass objectives read the training labels
-      const int nc = obj_->NumTreePerIteration();
-      for (float y : ds.label) {
-        const int l = static_cast<int>(y);
-        if (!(y > -1.0f && y < static_cast<float>(nc)) || l < 0 || l >= nc)
-          Fatal("Label must be in [0, " + std::to_string(nc) + "), but found " + std::to_string(l) + " in label");
-      }
-      continue;
-    }
-    const int kind = MetricKindOf(m);
-    if (kind != kMetXentLambda && kind != kMetKLDiv) continue;
-    if (obj_->NumTreePerIteration() > 1) Fatal("metric " + m + " needs a single-output objective");
-    for (float y : ds.label) if (!(y >= 0.0f && y <= 1.0f)) Fatal("[" + m + "]: does not tolerate label " + std::to_string(y) + " outside [0, 1]");
-    if (kind == kMetKLDiv && !ds.weight.empty()) {
-      double sw = 0;
-      for (float w : ds.weight) { if (w < 0) Fatal("[" + m + "]: at least one weight is negative"); sw += w; }
-      if (!(sw > 0)) Fatal("[" + m + "]: sum of weights is zero");
-    }
-  }
-}
-
+std::vector<std::string> Booster::EvalNames() const { return metrics_ ? metrics_->Names() : std::vector<std::string>(); }
 std::vector<double> Booster::GetEval(int data_idx) {
   NvtxRange nvtx("b200gbm:eval metrics (LGBM_BoosterGetEval)");
   if (!train) Fatal("this booster was loaded from a model string: it holds no training/validation data to evaluate");
   EnsureDevice();
   if (is_dart_ && data_idx == 0 && !dart_dropped_this_iter_) DroppingTrees();      // DART::GetTrainingScore
-  const Dataset* ds = data_idx == 0 ? train : valids_.at(data_idx - 1)->ds;
-  const DevBuf<double>& sc = data_idx == 0 ? score_ : valids_[data_idx - 1]->score;
-  const int n = ds->num_data;
-  cudaStream_t s = stream_;
-  if (ds->label.empty()) Fatal("label should not be empty for evaluation");
-  const float* d_y = ds->d_label.p;
-  const float* d_w = ds->weight.empty() ? nullptr : ds->d_weight.p;
-  const int grid = std::max(1, std::min((n + kMetricBlock - 1) / kMetricBlock, num_sms_ * 8));
-  if (met_partial_.n < static_cast<size_t>(grid) * 2 * kMaxEvalAt) met_partial_.Alloc(static_cast<size_t>(grid) * 2 * kMaxEvalAt);
-  if (met_out_.n < 2 * kMaxEvalAt) met_out_.Alloc(2 * kMaxEvalAt);
-  std::vector<double> out;
-  auto avg = [&](double loss, double sw) {
-    double v[2] = {loss, sw};
-    AllReduceHost(v, 2, ncclSum, s);     // averaged metrics are global in distributed mode (B.5)
-    return v[0] / v[1];
-  };
-  auto fetch = [&](int count, double* host) {
-    met_out_.Download(host, count, s);
-    B200_CUDA(cudaStreamSynchronize(s));
-  };
-  bool rank_done = false;
-  std::vector<double> ndcg_vals, map_vals;
-  for (auto& m : cfg.metric) {
-    const int kind = MetricKindOf(m);
-    if (kind >= 0) {
-      HostModel::OutputTransform t;
-      HostModel::ObjectiveTransform(obj_->ToString(), &t);
-      MetricParams mp{kind, K, obj_->kind() == ObjectiveKind::kMulticlassOva ? 1 : 0, t.kind, cfg.alpha, cfg.fair_c, cfg.tweedie_variance_power, cfg.sigmoid, t.sigmoid};
-      if ((kind == kMetMultiLogloss || kind == kMetMultiError) && K < 2) Fatal("metric " + m + " needs a multiclass objective");
-      k_metric_pointwise<<<grid, kMetricBlock, 0, s>>>(sc.p, d_y, d_w, n, mp, met_partial_.p);
-      k_metric_finish<<<1, 32, 0, s>>>(met_partial_.p, grid, 2, met_out_.p);
-      B200_CUDA(cudaGetLastError());
-      double v[2];
-      fetch(2, v);
-      const double a = avg(v[0], v[1]);
-      out.push_back(m == "rmse" ? std::sqrt(a) : a);
-    } else if (m == "auc" || m == "average_precision") {
-      // [UPSTREAM AUCMetric::Eval / AveragePrecisionMetric::Eval] are rank-local (no network sync), like the reference's per-task evaluation
-      RankByScore(sc.p, d_y, d_w, n);
-      if (m == "auc") k_auc_terms<<<grid, kMetricBlock, 0, s>>>(auc_keys_b_.p, auc_start_.p, auc_ppos_.p, auc_pneg_.p, n, met_partial_.p);
-      else k_ap_terms<<<grid, kMetricBlock, 0, s>>>(auc_keys_b_.p, auc_start_.p, auc_ppos_.p, auc_pneg_.p, n, met_partial_.p);
-      k_metric_finish<<<1, 32, 0, s>>>(met_partial_.p, grid, 2, met_out_.p);
-      B200_CUDA(cudaGetLastError());
-      double v[2], tot[2];
-      fetch(2, v);
-      B200_CUDA(cudaMemcpyAsync(&tot[0], auc_ppos_.p + (n - 1), sizeof(double), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaMemcpyAsync(&tot[1], auc_pneg_.p + (n - 1), sizeof(double), cudaMemcpyDeviceToHost, s));
-      B200_CUDA(cudaStreamSynchronize(s));
-      // a single-class set scores 1 ([UPSTREAM] sum_pos > 0 && sum_pos != sum_weights for average_precision)
-      const bool both = tot[0] > 0 && tot[1] > 0;
-      if (m == "auc") out.push_back(both ? v[0] / (tot[0] * tot[1]) : 1.0);
-      else out.push_back(both ? v[0] / tot[0] : 1.0);
-    } else if (m == "auc_mu") {
-      out.push_back(EvalAucMu(sc.p, d_y, d_w, n));      // [UPSTREAM AucMuMetric::Eval] rank-local as well
-    } else if (m == "ndcg" || m == "map") {
-      if (!rank_done) {
-        const int nq = static_cast<int>(ds->query_boundaries.size()) - 1;
-        if (nq <= 0) Fatal("The " + std::string(m == "ndcg" ? "NDCG" : "MAP") + " metric requires query information");
-        const std::vector<double> lg = LabelGain(cfg);
-        int max_q = 1;
-        for (int q = 0; q < nq; ++q) max_q = std::max(max_q, ds->query_boundaries[q + 1] - ds->query_boundaries[q]);
-        const std::vector<double> disc = DcgDiscount(max_q);
-        DevBuf<double> d_lg, d_disc;
-        d_lg.Alloc(lg.size()); d_lg.Upload(lg.data(), lg.size(), s);
-        d_disc.Alloc(disc.size()); d_disc.Upload(disc.data(), disc.size(), s);
-        RankEvalParams rp{};
-        std::vector<int> ks = cfg.eval_at;      // evaluated in ascending order ([UPSTREAM] Config sorts eval_at); reported in the given order
-        std::sort(ks.begin(), ks.end());
-        rp.nk = static_cast<int>(ks.size());
-        for (int e = 0; e < rp.nk; ++e) rp.ks[e] = ks[e];
-        rp.want_ndcg = std::find(cfg.metric.begin(), cfg.metric.end(), "ndcg") != cfg.metric.end();
-        rp.want_map = std::find(cfg.metric.begin(), cfg.metric.end(), "map") != cfg.metric.end();
-        const size_t smem = static_cast<size_t>(max_q) * (8 + 4 + 4);
-        if (smem > 200 * 1024) Fatal("a query group is too large for the ranking metric kernel");
-        B200_CUDA(cudaFuncSetAttribute(k_metric_rank, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(std::max<size_t>(smem, 1024))));
-        const int rgrid = std::max(1, std::min(nq, num_sms_ * 8));
-        if (met_partial_.n < static_cast<size_t>(rgrid) * 2 * kMaxEvalAt) met_partial_.Alloc(static_cast<size_t>(rgrid) * 2 * kMaxEvalAt);
-        k_metric_rank<<<rgrid, 128, std::max<size_t>(smem, 1024), s>>>(sc.p, d_y, ds->d_qb.p, nq, d_lg.p, static_cast<int>(lg.size()), d_disc.p, rp, max_q, met_partial_.p);
-        k_metric_finish<<<1, 32, 0, s>>>(met_partial_.p, rgrid, 2 * kMaxEvalAt, met_out_.p);
-        B200_CUDA(cudaGetLastError());
-        double v[2 * kMaxEvalAt];
-        fetch(2 * kMaxEvalAt, v);
-        for (size_t e = 0; e < cfg.eval_at.size(); ++e) {
-          const size_t pos = std::find(ks.begin(), ks.end(), cfg.eval_at[e]) - ks.begin();
-          ndcg_vals.push_back(avg(v[pos], nq));
-          map_vals.push_back(avg(v[kMaxEvalAt + pos], nq));
-        }
-        rank_done = true;
-      }
-      const std::vector<double>& vals = m == "ndcg" ? ndcg_vals : map_vals;
-      out.insert(out.end(), vals.begin(), vals.end());
-    } else {
-      Fatal("Unknown metric type name: " + m);
-    }
-  }
-  return out;
-}
-
-void Booster::RankByScore(const double* score, const float* d_y, const float* d_w, int n) {
-  cudaStream_t s = stream_;
-  if (auc_keys_a_.n < static_cast<size_t>(n)) {
-    auc_keys_a_.Alloc(n); auc_keys_b_.Alloc(n); auc_rows_a_.Alloc(n); auc_rows_b_.Alloc(n); auc_wpos_.Alloc(n); auc_wneg_.Alloc(n);
-    auc_ppos_.Alloc(n); auc_pneg_.Alloc(n); auc_head_.Alloc(n); auc_start_.Alloc(n);
-    size_t t1 = 0, t2 = 0, t3 = 0;
-    cub::DeviceRadixSort::SortPairsDescending(nullptr, t1, auc_keys_a_.p, auc_keys_b_.p, auc_rows_a_.p, auc_rows_b_.p, n, 0, 64, s);
-    cub::DeviceScan::InclusiveSum(nullptr, t2, auc_wpos_.p, auc_ppos_.p, n, s);
-    cub::DeviceScan::InclusiveScan(nullptr, t3, auc_head_.p, auc_start_.p, cub::Max(), n, s);
-    auc_tmp_.Alloc(std::max(t1, std::max(t2, t3)) + 16);
-  }
-  size_t tb = auc_tmp_.n;
-  const int eg = num_sms_ * 8;
-  k_auc_keys<<<eg, 256, 0, s>>>(score, n, auc_keys_a_.p, auc_rows_a_.p);
-  B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(auc_tmp_.p, tb, auc_keys_a_.p, auc_keys_b_.p, auc_rows_a_.p, auc_rows_b_.p, n, 0, 64, s));
-  k_auc_weights<<<eg, 256, 0, s>>>(auc_keys_b_.p, auc_rows_b_.p, d_y, d_w, n, auc_wpos_.p, auc_wneg_.p, auc_head_.p);
-  tb = auc_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveSum(auc_tmp_.p, tb, auc_wpos_.p, auc_ppos_.p, n, s));
-  tb = auc_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveSum(auc_tmp_.p, tb, auc_wneg_.p, auc_pneg_.p, n, s));
-  tb = auc_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveScan(auc_tmp_.p, tb, auc_head_.p, auc_start_.p, cub::Max(), n, s));
-}
-
-// [UPSTREAM Config::GetAucMuWeights]: the given K x K matrix or 1 off the diagonal; the diagonal is set to 0 either way
-std::vector<double> Booster::AucMuWeights() const {
-  std::vector<double> wm(static_cast<size_t>(K) * K, 1.0);
-  if (!cfg.auc_mu_weights.empty()) wm = cfg.auc_mu_weights;      // length checked by ValidateMetrics
-  for (int c = 0; c < K; ++c) wm[static_cast<size_t>(c) * K + c] = 0.0;
-  return wm;
-}
-
-// [UPSTREAM AucMuMetric::Eval]: for each class pair i < j, the weighted AUC of class i against class j ranked by
-// d = t1 * (Wm[i,:] - Wm[j,:]) . s, t1 = v[i] - v[j]; auc_mu is the mean over the pairs.  Pairs run in batches of consecutive pairs
-// whose segments (the rows of both classes) hold at most about 2n items, so the scratch is O(n) however many classes there are.
-double Booster::EvalAucMu(const double* score, const float* d_y, const float* d_w, int n) {
-  cudaStream_t s = stream_;
-  const int eg = num_sms_ * 8;
-  // the class-grouped row order and the class boundaries
-  const size_t m = static_cast<size_t>(std::max(n, 1));
-  if (mu_cls_keys_a_.n < m) {
-    mu_cls_keys_a_.Alloc(m); mu_cls_keys_b_.Alloc(m); mu_cls_rows_a_.Alloc(m); mu_cls_rows_b_.Alloc(m);
-  }
-  if (mu_cls_start_.n < static_cast<size_t>(K) + 1) mu_cls_start_.Alloc(K + 1);
-  int bits = 1;
-  while ((1 << bits) < K) ++bits;
-  auto ensure_tmp = [&](size_t bytes) { if (mu_tmp_.n < bytes) mu_tmp_.Alloc(bytes + 16); };
-  size_t tb = 0;
-  B200_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, mu_cls_keys_a_.p, mu_cls_keys_b_.p, mu_cls_rows_a_.p, mu_cls_rows_b_.p, n, 0, bits, s));
-  ensure_tmp(tb);
-  mu_cls_start_.Zero(s);
-  if (n > 0) {
-    k_class_keys<<<eg, 256, 0, s>>>(d_y, n, mu_cls_keys_a_.p, mu_cls_rows_a_.p);
-    tb = mu_tmp_.n;
-    B200_CUDA(cub::DeviceRadixSort::SortPairs(mu_tmp_.p, tb, mu_cls_keys_a_.p, mu_cls_keys_b_.p, mu_cls_rows_a_.p, mu_cls_rows_b_.p, n, 0, bits, s));
-    k_class_bounds<<<eg, 256, 0, s>>>(mu_cls_keys_b_.p, n, K, mu_cls_start_.p);
-  }
-  std::vector<int> cls_start(K + 1);
-  mu_cls_start_.Download(cls_start.data(), K + 1, s);
-  B200_CUDA(cudaStreamSynchronize(s));
-
-  // the pairs in order (0,1), (0,2), ..., (K-2,K-1), their (t1, v) rows, and the batches
-  const std::vector<double> wm = AucMuWeights();
-  const int npairs = K * (K - 1) / 2;
-  std::vector<int2> pairs;
-  std::vector<double> pv;
-  pairs.reserve(npairs); pv.reserve(static_cast<size_t>(npairs) * (K + 1));
-  for (int i = 0; i < K; ++i)
-    for (int j = i + 1; j < K; ++j) {
-      pairs.push_back(make_int2(i, j));
-      std::vector<double> v(K);
-      for (int c = 0; c < K; ++c) v[c] = wm[static_cast<size_t>(i) * K + c] - wm[static_cast<size_t>(j) * K + c];
-      pv.push_back(v[i] - v[j]);
-      pv.insert(pv.end(), v.begin(), v.end());
-    }
-  // a batch closes before it passes cap items (one oversized pair still makes a batch of its own) or kMaxPairs pairs, which bounds the
-  // per-block partials; item offsets inside a batch stay below 2^31
-  const long long cap = std::max<long long>(1, std::min<long long>(2LL * n, 1LL << 30));
-  constexpr int kMaxPairs = 1024;
-  std::vector<int> batch_first, off_base, offs;      // batch b: pairs [batch_first[b], batch_first[b + 1]), offsets at offs[off_base[b]]
-  {
-    long long items = 0;
-    for (int p = 0; p < npairs; ++p) {
-      const long long sz = (cls_start[pairs[p].x + 1] - cls_start[pairs[p].x]) + (cls_start[pairs[p].y + 1] - cls_start[pairs[p].y]);
-      const bool open = !batch_first.empty() && p - batch_first.back() < kMaxPairs && items + sz <= cap;
-      if (!open) {
-        if (!batch_first.empty()) offs.push_back(static_cast<int>(items));
-        batch_first.push_back(p); off_base.push_back(static_cast<int>(offs.size())); items = 0;
-      }
-      offs.push_back(static_cast<int>(items));
-      items += sz;
-    }
-    offs.push_back(static_cast<int>(items));
-    batch_first.push_back(npairs);
-  }
-  const int nb = static_cast<int>(off_base.size());
-  // cub's segmented sort gives a large segment one thread block, so a segment of at least kLargeSegment items is sorted by a
-  // device-wide radix sort of its own instead and is left out of the segmented sort (its end offset there equals its begin)
-  constexpr int kLargeSegment = 1 << 16;
-  std::vector<int> ends_small(offs.size(), 0);
-  for (int b = 0; b < nb; ++b)
-    for (int g = 0; g < batch_first[b + 1] - batch_first[b]; ++g) {
-      const int* o = offs.data() + off_base[b];
-      ends_small[off_base[b] + g] = o[g + 1] - o[g] >= kLargeSegment ? o[g] : o[g + 1];
-    }
-  long long max_items = 0;
-  int max_pairs = 0;
-  for (int b = 0; b < nb; ++b) {
-    const int P = batch_first[b + 1] - batch_first[b];
-    max_items = std::max<long long>(max_items, offs[off_base[b] + P]);
-    max_pairs = std::max(max_pairs, P);
-  }
-  const size_t mi = static_cast<size_t>(std::max<long long>(max_items, 1));
-  if (mu_keys_a_.n < mi) {
-    mu_keys_a_.Alloc(mi); mu_keys_b_.Alloc(mi); mu_rows_a_.Alloc(mi); mu_rows_b_.Alloc(mi); mu_seg_.Alloc(mi); mu_head_.Alloc(mi);
-    mu_start_.Alloc(mi); mu_wpos_.Alloc(mi); mu_wneg_.Alloc(mi); mu_ppos_.Alloc(mi); mu_pneg_.Alloc(mi);
-  }
-  if (mu_pairs_.n < pairs.size()) mu_pairs_.Alloc(pairs.size());
-  if (mu_pv_.n < pv.size()) mu_pv_.Alloc(pv.size());
-  if (mu_off_.n < offs.size()) { mu_off_.Alloc(offs.size()); mu_end_small_.Alloc(offs.size()); }
-  if (mu_pair_auc_.n < static_cast<size_t>(npairs)) mu_pair_auc_.Alloc(npairs);
-  const int tgrid = eg;
-  if (mu_partial_.n < static_cast<size_t>(tgrid) * max_pairs) mu_partial_.Alloc(static_cast<size_t>(tgrid) * max_pairs);
-  mu_pairs_.Upload(pairs.data(), pairs.size(), s);
-  mu_pv_.Upload(pv.data(), pv.size(), s);
-  mu_off_.Upload(offs.data(), offs.size(), s);
-  mu_end_small_.Upload(ends_small.data(), ends_small.size(), s);
-
-  for (int b = 0; b < nb; ++b) {
-    const int p0 = batch_first[b], P = batch_first[b + 1] - p0;
-    const int* off = mu_off_.p + off_base[b];
-    const int* end_small = mu_end_small_.p + off_base[b];
-    const int* hoff = offs.data() + off_base[b];
-    const int N = hoff[P];
-    if (N > 0) {
-      k_aucmu_keys<<<eg, 256, 0, s>>>(score, n, K, mu_cls_start_.p, mu_cls_rows_b_.p, mu_pairs_.p, mu_pv_.p, p0, P, off, mu_keys_a_.p, mu_rows_a_.p, mu_seg_.p);
-      size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0;
-      int largest = 0;
-      for (int g = 0; g < P; ++g) largest = std::max(largest, hoff[g + 1] - hoff[g]);
-      B200_CUDA(cub::DeviceSegmentedSort::StableSortPairsDescending(nullptr, t1, mu_keys_a_.p, mu_keys_b_.p, mu_rows_a_.p, mu_rows_b_.p, N, P, off, end_small, s));
-      B200_CUDA(cub::DeviceScan::InclusiveSumByKey(nullptr, t2, mu_seg_.p, mu_wpos_.p, mu_ppos_.p, N, cuda::std::equal_to<>(), s));
-      B200_CUDA(cub::DeviceScan::InclusiveScan(nullptr, t3, mu_head_.p, mu_start_.p, cub::Max(), N, s));
-      B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, t4, mu_keys_a_.p, mu_keys_b_.p, mu_rows_a_.p, mu_rows_b_.p, largest, 0, 64, s));
-      ensure_tmp(std::max(std::max(t1, t2), std::max(t3, t4)));
-      tb = mu_tmp_.n;
-      B200_CUDA(cub::DeviceSegmentedSort::StableSortPairsDescending(mu_tmp_.p, tb, mu_keys_a_.p, mu_keys_b_.p, mu_rows_a_.p, mu_rows_b_.p, N, P, off, end_small, s));
-      for (int g = 0; g < P; ++g) {      // the large segments (radix sorts are stable, as the segmented sort is)
-        const int o = hoff[g], len = hoff[g + 1] - o;
-        if (len < kLargeSegment) continue;
-        tb = mu_tmp_.n;
-        B200_CUDA(cub::DeviceRadixSort::SortPairsDescending(mu_tmp_.p, tb, mu_keys_a_.p + o, mu_keys_b_.p + o, mu_rows_a_.p + o, mu_rows_b_.p + o, len, 0, 64, s));
-      }
-      k_aucmu_weights<<<eg, 256, 0, s>>>(mu_keys_b_.p, mu_rows_b_.p, mu_seg_.p, off, mu_pairs_.p, p0, d_y, d_w, N, mu_wpos_.p, mu_wneg_.p, mu_head_.p);
-      tb = mu_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveSumByKey(mu_tmp_.p, tb, mu_seg_.p, mu_wpos_.p, mu_ppos_.p, N, cuda::std::equal_to<>(), s));
-      tb = mu_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveSumByKey(mu_tmp_.p, tb, mu_seg_.p, mu_wneg_.p, mu_pneg_.p, N, cuda::std::equal_to<>(), s));
-      tb = mu_tmp_.n; B200_CUDA(cub::DeviceScan::InclusiveScan(mu_tmp_.p, tb, mu_head_.p, mu_start_.p, cub::Max(), N, s));
-    }
-    B200_CUDA(cudaMemsetAsync(mu_partial_.p, 0, static_cast<size_t>(tgrid) * P * sizeof(double), s));
-    if (N > 0) k_aucmu_terms<<<tgrid, kMetricBlock, 0, s>>>(mu_keys_b_.p, mu_start_.p, mu_ppos_.p, mu_pneg_.p, off, P, mu_partial_.p);
-    k_aucmu_pair_finish<<<(P + 127) / 128, 128, 0, s>>>(mu_partial_.p, tgrid, P, off, mu_ppos_.p, mu_pneg_.p, p0, mu_pair_auc_.p);
-    B200_CUDA(cudaGetLastError());
-  }
-  k_aucmu_total<<<1, 32, 0, s>>>(mu_pair_auc_.p, npairs, K, met_out_.p);
-  B200_CUDA(cudaGetLastError());
-  double v = 0;
-  met_out_.Download(&v, 1, s);
-  B200_CUDA(cudaStreamSynchronize(s));
-  return v;
-}
-
-void Booster::GetRawScores(int data_idx, double* out) {
-  if (!train) Fatal("this booster was loaded from a model string: it holds no training/validation data");
-  EnsureDevice();
-  const Dataset* ds = data_idx == 0 ? train : valids_.at(data_idx - 1)->ds;
-  const DevBuf<double>& sc = data_idx == 0 ? score_ : valids_[data_idx - 1]->score;
-  sc.Download(out, static_cast<size_t>(K) * ds->num_data, stream_);
-  B200_CUDA(cudaStreamSynchronize(stream_));
+  const auto [ds, sc] = ScoredData(data_idx);
+  return metrics_->Eval(sc->p, *ds, stream_);
 }
 
 void Booster::GetGradients(float* grad, float* hess) {
@@ -2441,3 +2120,4 @@ int64_t Booster::PredictBatchCSR(const void* indptr, int indptr_type, const int3
 }
 
 }  // namespace b200gbm
+#include "metrics.cu"      // the booster's metrics, in this translation unit

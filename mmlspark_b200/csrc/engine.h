@@ -192,6 +192,7 @@ struct ValidSet {
 };
 class Objective;          // objective.h
 class TreeLearner;        // tree_learner.h
+class Metrics;            // metrics.h
 
 class Booster {
  public:
@@ -206,8 +207,6 @@ class Booster {
   void MergeFrom(const Booster* other);
   std::vector<std::string> EvalNames() const;
   std::vector<double> GetEval(int data_idx);
-  void ValidateMetrics() const;
-  void CheckMetricData(const Dataset& ds) const;
   void GetPredict(int data_idx, int64_t* out_len, double* out);
   int64_t NumPredict(int data_idx) const;
   void GetRawScores(int data_idx, double* out);
@@ -249,6 +248,7 @@ class Booster {
 
   std::unique_ptr<Objective> obj_;      // training boosters only
   std::unique_ptr<TreeLearner> learner_;      // training boosters only; uses stream_, so it is freed before the stream
+  std::unique_ptr<Metrics> metrics_;          // training boosters only
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool parallel_ = false;
@@ -296,22 +296,8 @@ class Booster {
                      ShapScratch& shap, double* out);
   void FinishPredict(double* out, int64_t nrow, int predict_type, int t0, int t1) const;      // rf averaging and the objective transform
   std::vector<ValidSet*> valids_;
-  // device-side evaluation scratch (metric_kernels.cuh)
-  DevBuf<double> met_partial_, met_out_, auc_wpos_, auc_wneg_, auc_ppos_, auc_pneg_;
-  DevBuf<unsigned long long> auc_keys_a_, auc_keys_b_;
-  DevBuf<int> auc_rows_a_, auc_rows_b_, auc_head_, auc_start_;
-  DevBuf<unsigned char> auc_tmp_;
-  // auc_mu: the class-grouped row order, then one batch of class-pair segments at a time (about 2n items, so O(n) for any K)
-  DevBuf<unsigned> mu_cls_keys_a_, mu_cls_keys_b_;
-  DevBuf<int> mu_cls_rows_a_, mu_cls_rows_b_, mu_cls_start_, mu_off_, mu_end_small_, mu_rows_a_, mu_rows_b_, mu_seg_, mu_head_, mu_start_;
-  DevBuf<int2> mu_pairs_;
-  DevBuf<unsigned long long> mu_keys_a_, mu_keys_b_;
-  DevBuf<double> mu_pv_, mu_wpos_, mu_wneg_, mu_ppos_, mu_pneg_, mu_partial_, mu_pair_auc_;
-  DevBuf<unsigned char> mu_tmp_;
-  // auc's and average_precision's sort by descending score, split weights and prefix sums into auc_* (enqueued on the stream)
-  void RankByScore(const double* score, const float* d_y, const float* d_w, int n);
-  std::vector<double> AucMuWeights() const;      // K x K, row-major, diagonal zeroed
-  double EvalAucMu(const double* score, const float* d_y, const float* d_w, int n);
+  // data_idx 0: the training data and its scores, i > 0: validation set i - 1; fails for any other data_idx
+  std::pair<const Dataset*, const DevBuf<double>*> ScoredData(int data_idx) const;
   int num_sms_ = 0;
   cudaEvent_t ev_a_ = nullptr, ev_b_ = nullptr;
 };

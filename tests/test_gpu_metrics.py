@@ -294,3 +294,88 @@ def test_unknown_metric_fails_at_booster_create(built):
     ds = capi.Dataset.from_mat(X, DS_PARAMS).set_field("label", X[:, 0].astype(np.float32))
     with pytest.raises(capi.LightGBMError):
         capi.Booster(ds, BASE + "objective=regression metric=l2,not_a_metric")
+
+
+def _error_data(n=2000, seed=6):
+    rng = np.random.default_rng(seed)
+    X = rng.standard_normal((n, 4))
+    return X, (X[:, 0] > 0).astype(np.float32)
+
+
+def test_metric_errors_are_raised_by_the_call_that_meets_them(built):
+    """Each metric error at the call that raises it: LGBM_BoosterCreate and LGBM_BoosterResetParameter reject the metric list, GetEval
+    what it finds in the data it evaluates; a rejected reset leaves the names and values of every evaluation as they were."""
+    from mmlspark_b200 import capi
+    X, y = _error_data()
+    ds = capi.Dataset.from_mat(X, DS_PARAMS).set_field("label", y)
+    many = "eval_at=" + ",".join(str(k) for k in range(1, 18))
+    for params, match in (("objective=regression metric=l2,not_a_metric", "Unknown metric type name: not_a_metric"),
+                          ("objective=regression metric=ndcg " + many, "eval_at: at most 16 positions are supported"),
+                          ("objective=multiclass num_class=2 metric=kldiv", "metric kullback_leibler needs a single-output objective")):
+        with pytest.raises(capi.LightGBMError, match=match):
+            capi.Booster(ds, BASE + params)
+
+    # create succeeds; the evaluation fails
+    b, _, _ = _fit(X, y, "objective=binary metric=multi_logloss", X[:500], y[:500], iters=1)
+    for idx in (0, 1):
+        with pytest.raises(capi.LightGBMError, match="metric multi_logloss needs a multiclass objective"):
+            b.get_eval(idx)
+    for metric, name in (("ndcg", "NDCG"), ("map", "MAP")):
+        b, _, _ = _fit(X, y, "objective=regression metric=" + metric, X[:500], y[:500], iters=1)
+        assert b.eval_names() == [metric + "@%d" % k for k in range(1, 6)]
+        for idx in (0, 1):
+            with pytest.raises(capi.LightGBMError, match="The %s metric requires query information" % name):
+                b.get_eval(idx)
+    Xb, yb = _error_data(13_000, seed=7)      # one query of 13000 documents: more shared memory than the rank kernel may take
+    b, _, _ = _fit(Xb, yb, "objective=regression metric=map", group=np.array([13_000], np.int32), iters=1)
+    with pytest.raises(capi.LightGBMError, match="a query group is too large for the ranking metric kernel"):
+        b.get_eval(0)
+
+    # resets that fail every check of create and of the validation data
+    b, _, _ = _fit(X, y, "objective=binary metric=binary_logloss,auc,l2", X[:500], y[:500], iters=2)
+    names, evals = b.eval_names(), [b.get_eval(idx).tobytes() for idx in (0, 1)]
+    yv_bad = y[:500].copy()
+    yv_bad[3] = 2.0
+    b2, _, _ = _fit(X, y, "objective=binary metric=binary_logloss", X[:500], yv_bad, iters=2)
+    names2, evals2 = b2.eval_names(), [b2.get_eval(idx).tobytes() for idx in (0, 1)]
+    for booster, params, match in ((b, "metric=l2,auc,bogus_metric", "Unknown metric type name: bogus_metric"),
+                                   (b, "metric=ndcg " + many, "eval_at: at most 16 positions are supported"),
+                                   (b, "metric=auc_mu", "metric auc_mu needs a multiclass objective"),
+                                   (b2, "metric=binary_logloss,cross_entropy_lambda", r"\[cross_entropy_lambda\]: does not tolerate label 2")):
+        with pytest.raises(capi.LightGBMError, match=match):
+            booster.reset_parameter(params)
+    assert b.eval_names() == names and [b.get_eval(idx).tobytes() for idx in (0, 1)] == evals
+    assert b2.eval_names() == names2 and [b2.get_eval(idx).tobytes() for idx in (0, 1)] == evals2
+
+
+def test_data_idx_out_of_range_is_rejected(built):
+    """GetEval, GetNumPredict, GetPredict and the raw scores accept data_idx 0 (training) up to the number of validation sets"""
+    import ctypes as C
+    from mmlspark_b200 import capi
+    X, y = _error_data()
+    b, _, _ = _fit(X, y, "objective=binary metric=binary_logloss,auc", X[:500], y[:500], iters=2)
+    before = [(b.get_eval(idx).tobytes(), b.get_predict(idx).tobytes(), b.get_scores(idx).tobytes()) for idx in (0, 1)]
+    L, out, n = capi.load(), np.zeros(len(X), np.float64), C.c_int64(0)
+    for idx in (-1, 2):
+        # get_predict / get_scores call GetNumPredict first, so GetPredict and GetScores are also called on their own
+        for call in (b.get_eval, b.get_predict, b.get_scores,
+                     lambda i: capi.check(L.LGBM_BoosterGetPredict(b.handle, C.c_int(i), C.byref(n), capi._ptr(out))),
+                     lambda i: capi.check(L.B200GBM_BoosterGetScores(b.handle, C.c_int(i), capi._ptr(out)))):
+            with pytest.raises(capi.LightGBMError, match="data_idx out of range"):
+                call(idx)
+    assert not out.any()
+    assert [(b.get_eval(idx).tobytes(), b.get_predict(idx).tobytes(), b.get_scores(idx).tobytes()) for idx in (0, 1)] == before
+
+
+def test_booster_from_model_string_has_no_metrics(built):
+    """A booster loaded from a model string evaluates nothing, so it lists no metric names, also after a parameter reset (LightGBM's
+    GetEvalCounts of a loaded model is 0)"""
+    from mmlspark_b200 import capi
+    X, y = _error_data()
+    b, _, _ = _fit(X, y, "objective=binary metric=binary_logloss,auc", iters=2)
+    loaded = capi.Booster(model_str=b.save_model_to_string())
+    assert loaded.eval_names() == []
+    loaded.reset_parameter("metric=auc,l2")
+    assert loaded.eval_names() == []
+    with pytest.raises(capi.LightGBMError, match="loaded from a model string"):
+        loaded.get_eval(0)
