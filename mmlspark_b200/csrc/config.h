@@ -36,6 +36,9 @@ struct Config {
   int feature_fraction_seed = 2;
   bool extra_trees = false;                 // one random threshold per (leaf, feature) scan (TreeLearner, kernels.cuh K5/K6)
   int extra_seed = 6;                       // the stream of used feature i starts at extra_seed + i
+  std::vector<int> monotone_constraints;    // per real feature -1, 0 or +1; non-empty: the constrained scans (TreeLearner, kernels.cuh kMono)
+  std::string monotone_constraints_method = "basic";      // only "basic" trains (Booster checks at create)
+  double monotone_penalty = 0.0;            // scales a monotone split's gain down near the root (kernels.cuh d_mono_penalty)
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -91,6 +94,9 @@ struct Config {
         {"subsample", "bagging_fraction"}, {"bagging", "bagging_fraction"}, {"subsample_freq", "bagging_freq"},
         {"bagging_fraction_seed", "bagging_seed"}, {"sub_feature", "feature_fraction"},
         {"colsample_bytree", "feature_fraction"}, {"extra_tree", "extra_trees"}, {"early_stopping_rounds", "early_stopping_round"},
+        {"mc", "monotone_constraints"}, {"monotone_constraint", "monotone_constraints"},
+        {"monotone_constraining_method", "monotone_constraints_method"}, {"mc_method", "monotone_constraints_method"},
+        {"monotone_splits_penalty", "monotone_penalty"}, {"ms_penalty", "monotone_penalty"}, {"mc_penalty", "monotone_penalty"},
         {"early_stopping", "early_stopping_round"}, {"n_iter_no_change", "early_stopping_round"},
         {"max_tree_output", "max_delta_step"}, {"max_leaf_output", "max_delta_step"}, {"reg_alpha", "lambda_l1"},
         {"reg_lambda", "lambda_l2"}, {"lambda", "lambda_l2"}, {"min_split_gain", "min_gain_to_split"},
@@ -179,6 +185,7 @@ struct Config {
     I("bagging_freq", &bagging_freq); I("bagging_seed", &bagging_seed); D("feature_fraction", &feature_fraction);
     I("feature_fraction_seed", &feature_fraction_seed); I("early_stopping_round", &early_stopping_round);
     B("extra_trees", &extra_trees); I("extra_seed", &extra_seed);
+    S("monotone_constraints_method", &monotone_constraints_method); D("monotone_penalty", &monotone_penalty);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -201,6 +208,8 @@ struct Config {
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &eval_at, [](const std::string& x) { return std::atoi(x.c_str()); });
       it = raw.find("auc_mu_weights");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &auc_mu_weights, [](const std::string& x) { return std::atof(x.c_str()); });
+      it = raw.find("monotone_constraints");      // an empty value clears the list
+      if (it != raw.end()) SplitList(it->second, &monotone_constraints, [](const std::string& x) { return std::atoi(x.c_str()); });
       it = raw.find("categorical_feature");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &categorical_feature, [](const std::string& x) { return std::atoi(x.c_str()); });
     }
@@ -250,7 +259,8 @@ struct Config {
     s << "[uniform_drop: " << uniform_drop << "]\n[drop_seed: " << drop_seed << "]\n[top_rate: " << Num(top_rate) << "]\n[other_rate: " << Num(other_rate) << "]\n";
     s << "[min_data_per_group: " << min_data_per_group << "]\n[max_cat_threshold: " << max_cat_threshold << "]\n[cat_l2: " << Num(cat_l2) << "]\n";
     s << "[cat_smooth: " << Num(cat_smooth) << "]\n[max_cat_to_onehot: " << max_cat_to_onehot << "]\n";
-    s << "[top_k: " << top_k << "]\n[monotone_constraints: ]\n[monotone_constraints_method: basic]\n[monotone_penalty: 0]\n";
+    s << "[top_k: " << top_k << "]\n[monotone_constraints: " << join_i(monotone_constraints) << "]\n";
+    s << "[monotone_constraints_method: " << monotone_constraints_method << "]\n[monotone_penalty: " << Num(monotone_penalty) << "]\n";
     s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
     s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: 0]\n[interaction_constraints: ]\n";
     s << "[verbosity: " << verbosity << "]\n[saved_feature_importance_type: 0]\n[linear_tree: 0]\n[max_bin: " << max_bin << "]\n";

@@ -1347,6 +1347,27 @@ namespace b200gbm {
 // the voting learner's local and global scans would each need their own draw order of the extra_trees streams; not restated
 static const char* const kVotingExtraTrees = "tree_learner=voting does not support extra_trees with more than one machine; "
                                              "use tree_learner=data_parallel or extra_trees=false";
+// the voting learner's local scan and vote would need the leaf bounds of every rank's candidates; not restated
+static const char* const kVotingMonotone = "tree_learner=voting does not support monotone_constraints with more than one machine; "
+                                           "use tree_learner=data_parallel or no monotone_constraints";
+
+// monotone constraints (basic method only): the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+static void CheckMonotone(const Config& cfg, const Dataset& train, bool voting_parallel) {
+  if (!(cfg.monotone_penalty >= 0.0)) Fatal("monotone_penalty should be >= 0, got " + Config::Num(cfg.monotone_penalty));
+  const std::vector<int>& mc = cfg.monotone_constraints;
+  if (mc.empty()) return;
+  if (cfg.monotone_constraints_method != "basic")
+    Fatal("monotone_constraints_method=" + cfg.monotone_constraints_method + " is not supported; use monotone_constraints_method=basic");
+  if (static_cast<int>(mc.size()) != train.num_total_features)
+    Fatal("monotone_constraints has " + std::to_string(mc.size()) + " entries, but the dataset has " + std::to_string(train.num_total_features) +
+          " features");
+  for (int f = 0; f < train.num_total_features; ++f) {
+    if (mc[f] < -1 || mc[f] > 1) Fatal("monotone_constraints entries should be -1, 0 or 1, got " + std::to_string(mc[f]) + " for feature " + std::to_string(f));
+    if (mc[f] != 0 && train.mappers[f].categorical)
+      Fatal("monotone_constraints: feature " + std::to_string(f) + " is categorical and cannot carry a monotone constraint");
+  }
+  if (voting_parallel) Fatal(kVotingMonotone);
+}
 
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
@@ -1393,6 +1414,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
             " * " + std::to_string(std::min(cfg.top_k, train->nf)));
     if (cfg.extra_trees) Fatal(kVotingExtraTrees);
   }
+  CheckMonotone(cfg, *train, parallel_ && cfg.tree_learner == "voting");
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1410,6 +1432,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   model.max_feature_idx = train->num_total_features - 1;
   model.feature_names = train->feature_names;
   for (int f = 0; f < train->num_total_features; ++f) model.feature_infos.push_back(train->mappers[f].InfoString());
+  model.monotone_constraints = cfg.monotone_constraints;
   InitTraining();
   model.objective_str = obj_->ToString();
 }
@@ -1731,6 +1754,7 @@ void Booster::ResetParameter(const char* params) {
   if (train) {      // metrics named by the reset meet the checks of LGBM_BoosterCreate / AddValidData; a rejected reset changes nothing
     try {
       if (parallel_ && cfg.tree_learner == "voting" && cfg.extra_trees) Fatal(kVotingExtraTrees);
+      CheckMonotone(cfg, *train, parallel_ && cfg.tree_learner == "voting");
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;
@@ -1739,6 +1763,7 @@ void Booster::ResetParameter(const char* params) {
   }
   shrinkage_ = is_rf_ ? 1.0 : cfg.learning_rate;
   if (is_dart_) { drop_rand_ = LcgRandom(cfg.drop_seed); sum_weight_ = 0.0; }      // [LightGBM dart.hpp DART::ResetConfig]
+  if (train) model.monotone_constraints = cfg.monotone_constraints;
   if (learner_) learner_->ResetConfig(cfg);
 }
 

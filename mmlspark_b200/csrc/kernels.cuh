@@ -108,7 +108,7 @@ struct LeafBest {
   double left_out, right_out;
   int feature, threshold, default_left, left_count, right_count, is_cat;
   unsigned cat_bits[8];
-  int cat_list_len, pad;
+  int cat_list_len, monotone_type;           // monotone_type: the split feature's constraint (0 without monotone constraints)
   unsigned short cat_list[kCatListMax];
 };
 
@@ -120,7 +120,14 @@ struct LeafState {
   // exact fixed-point (g,h) totals, kept only for datasets with feature bundles: qtot = this leaf's (written by k_scan), qpar = its
   // parent's (written by the round controller); a bundle member's most frequent bin is the leaf total minus its other bins
   long long qtot[2], qpar[2];
+  // monotone constraints (basic method): the bounds [mono_min, mono_max] of this leaf's output; the root's are (-inf, +inf), children
+  // inherit their parent's and a numerical split on a monotone feature narrows them at the mid-point of the two outputs (d_round_ctl)
+  double mono_min, mono_max;
 };
+
+// monotone constraints ([UPSTREAM] monotone_constraints.hpp BasicLeafConstraints, FeatureHistogram USE_MC): the scans' template parameter
+// kMono.  type: per inner feature -1, 0 or +1 (the real feature's monotone_constraints entry); penalty: monotone_penalty.
+struct MonoArgs { const signed char* type; double penalty; };
 
 struct TreeCtrl {
   int num_leaves, left_leaf, right_leaf, smaller, larger, go, finished, split_leaf;
@@ -174,6 +181,30 @@ __device__ __noinline__ double d_leaf_gain(double g, double h, const SplitParams
   double out = d_calc_output(g, h, p);
   double sg = (p.l1 > 0) ? d_threshold_l1(g, p.l1) : g;
   return -(2.0 * sg * out + (h + p.l2) * out * out);
+}
+// monotone constraints: a child's output, CalculateSplittedLeafOutput clamped to the leaf's bounds after max_delta_step
+__device__ __forceinline__ double d_mono_output(double g, double h, const SplitParams& p, double lo, double hi) {
+  double ret = d_calc_output(g, h, p);
+  if (ret < lo) ret = lo;
+  else if (ret > hi) ret = hi;
+  return ret;
+}
+// The kMono scans' split gain ([UPSTREAM] GetSplitGains<USE_MC>): both children's outputs clamped to the leaf's bounds [lo, hi], then
+// GetLeafGainGivenOutput(left) + GetLeafGainGivenOutput(right) = -(2 ThresholdL1(g) out + (h + l2) out^2) at those outputs; 0 when the
+// outputs break the split feature's direction `mono` (left > right for +1, left < right for -1).  Out of line for d_leaf_gain's reason.
+__device__ __noinline__ double d_mono_split_gain(double lg, double lh, double rg, double rh, const SplitParams& p, double lo, double hi, int mono) {
+  const double lo_out = d_mono_output(lg, lh, p, lo, hi), ro_out = d_mono_output(rg, rh, p, lo, hi);
+  if ((mono > 0 && lo_out > ro_out) || (mono < 0 && lo_out < ro_out)) return 0.0;
+  const double slg = (p.l1 > 0) ? d_threshold_l1(lg, p.l1) : lg, srg = (p.l1 > 0) ? d_threshold_l1(rg, p.l1) : rg;
+  return -(2.0 * slg * lo_out + (lh + p.l2) * lo_out * lo_out) + -(2.0 * srg * ro_out + (rh + p.l2) * ro_out * ro_out);
+}
+// monotone_penalty: the factor on a monotone feature's shifted gain in a leaf of depth d ([UPSTREAM] ComputeMonotoneSplitGainPenalty,
+// kEpsilon = 1e-15f)
+__device__ __forceinline__ double d_mono_penalty(int depth, double penalty) {
+  const double eps = static_cast<double>(1e-15f);
+  if (penalty >= depth + 1.0) return eps;
+  if (penalty <= 1.0) return 1.0 - penalty / exp2(static_cast<double>(depth)) + eps;
+  return 1.0 - exp2(penalty - 1.0 - depth) + eps;
 }
 
 // ---------------------------------------------------------------- binning (dataset creation)
@@ -716,12 +747,25 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
   if (threadIdx.x == 0) {
     LeafState& r = leaves[0];
     r.begin = 0; r.count = n_local; r.buf = 0; r.depth = 0; r.identity = root_is_bag ? 0 : 1; r.hist_slot = 0; r.parent_node = -1;
+    r.mono_min = kNegInf; r.mono_max = -kNegInf;
     r.global_count = static_cast<int>(ctrl->root_q[2]);
     r.sum_g = static_cast<double>(ctrl->root_q[0]) * ctrl->inv_g;
     r.sum_h = static_cast<double>(ctrl->root_q[1]) * ctrl->inv_h;
     ctrl->num_leaves = 1; ctrl->left_leaf = 0; ctrl->right_leaf = -1; ctrl->smaller = 0; ctrl->larger = -1;
     ctrl->go = 0; ctrl->finished = 0; ctrl->split_leaf = -1; ctrl->pending = 0; ctrl->round = 0; ctrl->trace_rows = 0;
     *tree.num_leaves = 1;
+  }
+}
+
+// monotone constraints ([UPSTREAM] BasicLeafConstraints::Update), when the round controller applies a split of leaf L into L and R: both
+// children inherit the parent's bounds; a numerical split on a monotone feature narrows them at mid = (left_out + right_out) / 2 — the
+// left child's max and the right child's min for +1, the mirror for -1.  Out of line to keep it off the partition kernel's registers.
+__device__ __noinline__ void d_mono_children(LeafState& L, LeafState& R, int monotone_type, int is_cat, double left_out, double right_out) {
+  R.mono_min = L.mono_min; R.mono_max = L.mono_max;
+  if (monotone_type != 0 && !is_cat) {
+    const double mid = (left_out + right_out) / 2.0;
+    if (monotone_type > 0) { L.mono_max = fmin(L.mono_max, mid); R.mono_min = fmax(R.mono_min, mid); }
+    else { L.mono_min = fmax(L.mono_min, mid); R.mono_max = fmin(R.mono_max, mid); }
   }
 }
 
@@ -781,6 +825,7 @@ d_round_ctl(TreeCtrl* ctrl, LeafState* leaves, const TreeDev& tree, uint8_t* fla
       L.count = true_left; L.buf = dst_buf; L.identity = 0; L.depth += 1;
       L.global_count = b.left_count; R.global_count = b.right_count;
       L.sum_g = b.left_g; L.sum_h = b.left_h; R.sum_g = b.right_g; R.sum_h = b.right_h;
+      d_mono_children(L, R, b.monotone_type, b.is_cat, b.left_out, b.right_out);
       R.hist_slot = nl;
       L.best.gain = kNegInf; L.best.feature = -1; R.best.gain = kNegInf; R.best.feature = -1;
       ctrl->left_leaf = leaf; ctrl->right_leaf = nl;
@@ -853,7 +898,9 @@ __device__ __noinline__ bool d_smaller_drew_cat(const long long* __restrict__ hi
 // kExtra (extra_trees): xr is the feature's stream state before this scan's draw.  One-hot draws r over the num_bin - 1 category bins
 // and evaluates only bin r + 1; many-vs-many draws r over d_cat_rand_range and evaluates only the prefixes of r + 1 bins.  Returns the
 // number of draws taken (0 or 1), in every lane.
-template <bool kExtra>
+// kMono (monotone constraints): every gain is d_mono_split_gain's at outputs clamped to the leaf's bounds; categorical features carry no
+// constraint of their own.
+template <bool kExtra, bool kMono>
 __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const long long (&qh)[8], int lane, const FeatMeta m, const LeafState& L,
                                                   double inv_g, double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* outp, double* ws,
                                                   unsigned xr) {
@@ -885,7 +932,8 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
         const int other = num_data - cnt;
         const double oh = sum_h - h - kEpsD;
         if (other >= p.min_data_in_leaf && oh >= p.min_sum_hessian && (!kExtra || b - 1 == rand_t)) {
-          const double gain = d_leaf_gain(sum_g - g, oh, p) + d_leaf_gain(g, h + kEpsD, p);
+          const double gain = kMono ? d_mono_split_gain(sum_g - g, oh, g, h + kEpsD, p, L.mono_min, L.mono_max, 0)
+                                    : d_leaf_gain(sum_g - g, oh, p) + d_leaf_gain(g, h + kEpsD, p);
           if (gain > min_gain_shift) {
             any_valid = true;
             if (gain > best_gain) { best_gain = gain; best_t = b; best_lg = g; best_lh = h + kEpsD; best_lc = cnt; }
@@ -973,7 +1021,8 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
         if (cnt_cur_group < p.min_data_per_group) continue;
         cnt_cur_group = 0;
         if (kExtra && i != rand_t) continue;
-        const double gain = d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
+        const double gain = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, srh, pc, L.mono_min, L.mono_max, 0)
+                                  : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
         if (gain <= min_gain_shift) continue;
         any_valid = true;
         if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_lc = left_count; best_i = i; best_dir = dir; }
@@ -1041,8 +1090,12 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
 // The two leaves of the round are handled side by side (threads 0..127: smaller, 128..255: larger) with warp-shuffle argmaxes — the
 // first version looped over the two leaves with an 8-step shared-memory tree each (18 block barriers) and ncu showed this serial tail
 // taking longer than the scan itself.  The order (gain desc, real feature index asc) is total, so any reduction shape picks the same winner.
+// kMono (monotone constraints): the outputs are clamped to the leaf's bounds ([UPSTREAM] CalculateSplittedLeafOutput<USE_MC>) and the
+// split feature's constraint (mono_type, per inner feature) is kept for the round controller's bound update.
+template <bool kMono>
 __device__ __noinline__ void
-d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p) {
+d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p,
+             const signed char* __restrict__ mono_type) {
   __shared__ double s_gain[8];
   __shared__ int s_feat[8], s_idx[8];
   const int which = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1068,7 +1121,7 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
     LeafState& L = leaves[leaf];
     LeafBest b;
     b.gain = kNegInf; b.feature = -1; b.threshold = 0; b.default_left = 1; b.left_count = 0; b.right_count = 0;
-    b.left_g = b.left_h = b.right_g = b.right_h = b.left_out = b.right_out = 0; b.is_cat = 0; b.cat_list_len = 0; b.pad = 0;
+    b.left_g = b.left_h = b.right_g = b.right_h = b.left_out = b.right_out = 0; b.is_cat = 0; b.cat_list_len = 0; b.monotone_type = 0;
     for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = 0u;
     if (bi >= 0 && bg > kNegInf) {
       const SplitCand c = d_load_cand(&cands[which * p.nf_pad + bi]);
@@ -1081,8 +1134,14 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
       b.right_g = L.sum_g - c.left_g; b.right_h = sum_h - c.left_h - kEpsD;
       SplitParams pc = p;
       pc.l2 += c.l2_extra;
-      b.left_out = d_calc_output(c.left_g, c.left_h, pc);
-      b.right_out = d_calc_output(L.sum_g - c.left_g, sum_h - c.left_h, pc);
+      if constexpr (kMono) {
+        b.left_out = d_mono_output(c.left_g, c.left_h, pc, L.mono_min, L.mono_max);
+        b.right_out = d_mono_output(L.sum_g - c.left_g, sum_h - c.left_h, pc, L.mono_min, L.mono_max);
+        b.monotone_type = mono_type[c.feature];
+      } else {
+        b.left_out = d_calc_output(c.left_g, c.left_h, pc);
+        b.right_out = d_calc_output(L.sum_g - c.left_g, sum_h - c.left_h, pc);
+      }
       b.is_cat = c.is_cat;
       for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = c.cat_bits[wd];
     }
@@ -1576,9 +1635,11 @@ __device__ __forceinline__ void d_block_excl3(long long& a, long long& b, long l
 // lowest).  hist = the leaf's reduced histogram of the feature in its pool slot.  Returns through *outp (thread 0) and *flag.
 // kExtra (extra_trees): only the candidate with that threshold is evaluated, in either pass; the count and hessian tests before it
 // still skip and break as they do without it ([UPSTREAM] FindBestThresholdSequentially, USE_RAND: t - 1 + offset resp. t + offset).
-template <bool kExtra>
+// kMono (monotone constraints): every gain, in both passes, is d_mono_split_gain's at outputs clamped to the leaf's bounds, 0 when they
+// break the feature's direction `mono`; min_gain_shift stays the leaf's unconstrained gain.
+template <bool kExtra, bool kMono>
 __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ hist, const WideMeta m, const LeafState& L, double inv_g, double inv_h,
-                                                  const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr) {
+                                                  const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr, int mono) {
   __shared__ long long s_sc[24];
   __shared__ double s_bg[8], s_blg[8], s_blh[8];
   __shared__ int s_bt[8], s_blc[8], s_any, s_stop[2];
@@ -1622,7 +1683,8 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
       if (kExtra && b - 1 != rand_thr) continue;
       const double slg = sum_g - srg;
-      const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
+      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, p, L.mono_min, L.mono_max, mono)
+                                : d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       any_valid = true;
       if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_thr = b - 1; best_lc = left_count; }
@@ -1684,7 +1746,8 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
       if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { f_stop = true; break; }
       if (kExtra && b != rand_thr) continue;
       const double srg = sum_g - slg;
-      const double gain = d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
+      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, p, L.mono_min, L.mono_max, mono)
+                                : d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       f_valid = true;
       if (gain > f_gain) { f_gain = gain; f_lg = slg; f_lh = slh; f_thr = b; f_lc = left_count; }
@@ -1754,11 +1817,13 @@ __device__ __noinline__ void d_block_bitonic2(double* k, int* id, int stride, in
 // (smaller|larger, feature).  The histogram is reduced into the leaf's pool slot (parent - smaller for the larger child), the
 // max_cat_threshold smallest and largest ctr = g / (h + cat_smooth) among the bins that hold >= cat_smooth rows are selected in the
 // (ctr, bin) order of the reference's stable sort, and thread 0 accumulates from both ends exactly like the sequential code.
-template <bool kExtra>
+// kMono (monotone constraints): constrained gains as in d_scan_wide_numeric / d_scan_feature_cat, and a monotone numerical feature's
+// candidate gain times d_mono_penalty at the leaf's depth.
+template <bool kExtra, bool kMono>
 __global__ void __launch_bounds__(256)
 k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const WideMeta* __restrict__ wm, const long long* __restrict__ H,
             long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
-            unsigned* __restrict__ xrand) {
+            unsigned* __restrict__ xrand, MonoArgs mono) {
   extern __shared__ __align__(16) unsigned char sw_smem[];
   double* s_key = reinterpret_cast<double*>(sw_smem);                          // [num_bin] ctr keys of the used bins, +inf otherwise
   __shared__ int s_used;
@@ -1796,8 +1861,12 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
       if (which) xr = d_lcg_next(xr);
       rand_thr = d_extra_draw(&xr, m.num_bin - 2);
     }
-    d_scan_wide_numeric<kExtra>(dst, m, L, inv_g, inv_h, p, flag, &out, rand_thr);
-    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 1u; __threadfence(); }
+    const int mt = kMono ? mono.type[u] : 0;
+    d_scan_wide_numeric<kExtra, kMono>(dst, m, L, inv_g, inv_h, p, flag, &out, rand_thr, mt);
+    if (threadIdx.x == 0) {
+      if (kMono && mt != 0) out.gain *= d_mono_penalty(L.depth, mono.penalty);
+      cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 1u; __threadfence();
+    }
     return;
   }
   // the larger leaf's draw comes after the smaller's, if that one drew
@@ -1975,7 +2044,8 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
       SplitParams pc = p;
       pc.l2 += p.cat_l2;
       const double slg = s_plg[d][i], slh = s_plh[d][i];
-      s_pgain[d][i] = d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, sum_h - slh, pc);
+      s_pgain[d][i] = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, sum_h - slh, pc, L.mono_min, L.mono_max, 0)
+                            : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, sum_h - slh, pc);
     }
   }
   __syncthreads();
@@ -2147,15 +2217,18 @@ __device__ __noinline__ void d_extra_commit(const TreeCtrl* ctrl, unsigned* xran
   }
 }
 
-template <int kMode, bool kExtra = false>
+// kMono (monotone constraints): the constrained scans (d_scan_wide_numeric, d_scan_feature_cat), a monotone feature's candidate gain
+// times d_mono_penalty at the leaf's depth, and outputs clamped to the leaf's bounds in the pick step.
+template <int kMode, bool kExtra = false, bool kMono = false>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, MonoArgs mono) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
   static_assert(!kExtra || kMode == kScanPlain, "the voting learner does not train extra trees (Booster fails at create)");
+  static_assert(!kMono || kMode == kScanPlain, "the voting learner does not train monotone constraints (Booster fails at create)");
   const int which = blockIdx.y;
   const int leaf = which ? ctrl->larger : ctrl->smaller;
   const int u = blockIdx.x;
@@ -2179,12 +2252,12 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
         }
         if (!fm.is_categorical) {
           const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-          d_scan_wide_numeric<false>(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, 0);
+          d_scan_wide_numeric<false, false>(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, 0, 0);
         } else if (threadIdx.x < 32) {
           long long qg[8], qh[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = hist[b * 2]; qh[j] = hist[b * 2 + 1]; }
-          d_scan_feature_cat<false>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, scan_ws, 0u);
+          d_scan_feature_cat<false, false>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, scan_ws, 0u);
         }
       }
     } else {
@@ -2235,12 +2308,14 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
             const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
             const int rand_thr = kExtra ? d_extra_draw(&xr, fm.num_bin - 2) : 0;
             drew = fm.num_bin > 2 ? 1 : 0;
-            d_scan_wide_numeric<kExtra>(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, rand_thr);
+            const int mt = kMono ? mono.type[u] : 0;
+            d_scan_wide_numeric<kExtra, kMono>(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, rand_thr, mt);
+            if (kMono && mt != 0 && threadIdx.x == 0) out.gain *= d_mono_penalty(L.depth, mono.penalty);
           } else if (threadIdx.x < 32) {
             long long qg[8], qh[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
-            drew = d_scan_feature_cat<kExtra>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws, xr);
+            drew = d_scan_feature_cat<kExtra, kMono>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws, xr);
           }
           if (kExtra && threadIdx.x == 0) xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = static_cast<unsigned>(drew);
         }
@@ -2263,7 +2338,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
     else {
       if constexpr (kExtra) d_extra_commit(ctrl, xrand, p);
-      d_pick_block(ctrl, leaves, meta, cands, p);
+      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, mono.type);
     }
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
   }

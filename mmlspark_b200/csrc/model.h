@@ -289,6 +289,7 @@ struct HostModel {
   bool average_output = false;
   std::vector<std::string> feature_names;
   std::vector<std::string> feature_infos;
+  std::vector<int> monotone_constraints;     // the header's monotone_constraints= line, only when non-empty ([UPSTREAM] GBDT::SaveModelToString)
   std::vector<std::unique_ptr<HostTree>> trees;
   std::string loaded_parameters;
 
@@ -313,6 +314,10 @@ struct HostModel {
     if (average_output) ss << "average_output\n";
     ss << "feature_names=";
     for (size_t i = 0; i < feature_names.size(); ++i) ss << (i ? " " : "") << feature_names[i];
+    if (!monotone_constraints.empty()) {
+      ss << "\nmonotone_constraints=";
+      for (size_t i = 0; i < monotone_constraints.size(); ++i) ss << (i ? " " : "") << monotone_constraints[i];
+    }
     ss << "\nfeature_infos=";
     for (size_t i = 0; i < feature_infos.size(); ++i) ss << (i ? " " : "") << feature_infos[i];
     ss << '\n';
@@ -381,6 +386,11 @@ struct HostModel {
       std::string x;
       while (is >> x) m->feature_names.push_back(x);
       if (static_cast<int>(m->feature_names.size()) != m->max_feature_idx + 1) throw std::runtime_error("Wrong size of feature_names");
+    }
+    if (head.count("monotone_constraints")) {
+      std::istringstream is(head["monotone_constraints"]);
+      int x;
+      while (is >> x) m->monotone_constraints.push_back(x);
     }
     if (head.count("feature_infos")) {
       std::istringstream is(head["feature_infos"]);

@@ -46,6 +46,9 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   B200_CUDA(set_k4_smem_limit());
   B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
   B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  mono_.Alloc(train.nf_pad);      // allocated whatever monotone_constraints says: a ResetParameter may set them
 
   ResetConfig(cfg);
   sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
@@ -59,8 +62,10 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
       if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
     }
   }
 
@@ -137,6 +142,18 @@ void TreeLearner::ResetConfig(const Config& cfg) {
   sp_.min_sum_hessian = cfg.min_sum_hessian_in_leaf; sp_.min_data_in_leaf = cfg.min_data_in_leaf; sp_.max_depth = cfg.max_depth;
   extra_trees_ = cfg.extra_trees;
   SeedExtraStreams(cfg);      // [UPSTREAM] HistogramPool::ResetConfig re-runs SetFeatureInfo, which re-seeds every feature's Random
+  // monotone constraints: a non-empty list runs the constrained scans for every feature, even when every entry is 0 ([UPSTREAM] USE_MC).
+  // The list is indexed by real feature (Booster checked its length and entries); the device copy by inner feature.  Uploaded here when
+  // it changes, ordered after the trees already enqueued (a learning-rate delegate resets every iteration and uploads nothing).
+  monotone_ = !cfg.monotone_constraints.empty();
+  monotone_penalty_ = cfg.monotone_penalty;
+  std::vector<signed char> types(train_.nf_pad, 0);
+  if (monotone_)
+    for (int u = 0; u < train_.nf; ++u) types[u] = static_cast<signed char>(cfg.monotone_constraints[train_.used[u]]);
+  if (types != mono_host_) {
+    mono_host_ = std::move(types);
+    mono_.Upload(mono_host_.data(), mono_host_.size(), stream_);
+  }
 }
 
 // extra_trees streams (kernels.cuh d_lcg_next): used feature i in real-index order starts at extra_seed + i.  One small kernel on the
@@ -407,7 +424,8 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       // local scan + top-k -> all-gather of the records -> vote + pack -> all-reduce of the packed columns -> global scan + pick
       nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
       const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
-      k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p);
+      k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p,
+                                                        MonoArgs{});
       mark();
       Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
       mark();
@@ -417,7 +435,8 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       mark();
       Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
       mark();
-      k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p);
+      k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p,
+                                                         MonoArgs{});
       nvtxRangePop();
       comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
       comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
@@ -429,15 +448,20 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
         comm_hist_bytes_ += static_cast<long long>(slot_elems_ * sizeof(long long));
       }
       mark();
+      const MonoArgs mono{mono_.p, monotone_penalty_};
       if (d.nw > 0) {
-        auto* scan_wide = extra_trees_ ? k_scan_wide<true> : k_scan_wide<false>;
-        scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p);
+        auto* scan_wide = monotone_ ? (extra_trees_ ? k_scan_wide<true, true> : k_scan_wide<false, true>)
+                                    : (extra_trees_ ? k_scan_wide<true, false> : k_scan_wide<false, false>);
+        scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
+                                                               mono);
         timing_.launches += 1;
       }
       // scan + (last block) pick
-      // extra_trees: the scan's own instantiation, so that the default one compiles to what it was without the feature
-      auto* scan = extra_trees_ ? k_scan<kScanPlain, true> : k_scan<kScanPlain, false>;
-      scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p);
+      // extra_trees, monotone constraints: the scan's own instantiations, so that the default one compiles to what it was without them
+      auto* scan = monotone_ ? (extra_trees_ ? k_scan<kScanPlain, true, true> : k_scan<kScanPlain, false, true>)
+                             : (extra_trees_ ? k_scan<kScanPlain, true, false> : k_scan<kScanPlain, false, false>);
+      scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
+                                         mono);
       nvtxRangePop();
     }
     mark();

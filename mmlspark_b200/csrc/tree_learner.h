@@ -52,6 +52,10 @@ class TreeLearner {
   Booster::Timing& timing_;
   SplitParams sp_{};
   bool extra_trees_ = false;     // cfg.extra_trees as of the last ResetConfig: launch the scans' extra_trees instantiations
+  bool monotone_ = false;        // cfg.monotone_constraints non-empty as of the last ResetConfig: launch the scans' kMono instantiations
+  double monotone_penalty_ = 0.0;
+  std::vector<signed char> mono_host_;      // [nf_pad] each inner feature's monotone constraint, as uploaded to mono_
+  DevBuf<signed char> mono_;
   int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
