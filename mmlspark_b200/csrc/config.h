@@ -6,6 +6,7 @@
 // and LightGBMBase.getDatasetParams (lightgbm/src/main/scala/com/microsoft/ml/spark/lightgbm/LightGBMBase.scala:265-272).
 // Keys the reference never sets keep the native LightGBM 3.2.x defaults (SURVEY.md Appendix B.2).
 #pragma once
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <map>
@@ -39,6 +40,9 @@ struct Config {
   std::vector<int> monotone_constraints;    // per real feature -1, 0 or +1; non-empty: the constrained scans (TreeLearner, kernels.cuh kMono)
   std::string monotone_constraints_method = "basic";      // only "basic" trains (Booster checks at create)
   double monotone_penalty = 0.0;            // scales a monotone split's gain down near the root (kernels.cuh d_mono_penalty)
+  // sets of real feature indices; a branch's split features stay inside one set (TreeLearner sets_of_, kernels.cuh d_pick_block)
+  std::vector<std::vector<int>> interaction_constraints;
+  std::string interaction_constraints_malformed;      // the value given when it does not parse (Booster fails at create)
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -159,6 +163,30 @@ struct Config {
     }
     Refresh();
   }
+  // "[0,1,2],[2,3]" -> {{0,1,2},{2,3}} ([UPSTREAM] Common::StringToArrayofArrays); false unless the value is a comma-separated list of
+  // bracketed, comma-separated integer lists with no empty item.  An empty value is the empty list; "[]" is an empty set.
+  static bool ParseSets(const std::string& s, std::vector<std::vector<int>>* out) {
+    out->clear();
+    for (size_t i = 0; i < s.size();) {
+      const size_t close = s.find(']', i);
+      if (s[i] != '[' || close == std::string::npos) return false;
+      std::vector<int> set;
+      const std::string inner = s.substr(i + 1, close - i - 1);
+      if (!inner.empty() && inner.back() == ',') return false;      // getline would drop the empty last item
+      std::stringstream ss(inner);
+      std::string x;
+      while (std::getline(ss, x, ',')) {
+        char* end = nullptr;
+        const long long v = std::strtoll(x.c_str(), &end, 10);
+        if (x.empty() || *end != '\0' || v < INT_MIN || v > INT_MAX) return false;
+        set.push_back(static_cast<int>(v));
+      }
+      out->push_back(std::move(set));
+      i = close + 1;
+      if (i < s.size() && (s[i] != ',' || ++i == s.size())) return false;
+    }
+    return true;
+  }
   template <typename T, typename F>
   static void SplitList(const std::string& s, std::vector<T>* out, F conv) {
     out->clear();
@@ -210,6 +238,11 @@ struct Config {
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &auc_mu_weights, [](const std::string& x) { return std::atof(x.c_str()); });
       it = raw.find("monotone_constraints");      // an empty value clears the list
       if (it != raw.end()) SplitList(it->second, &monotone_constraints, [](const std::string& x) { return std::atoi(x.c_str()); });
+      it = raw.find("interaction_constraints");   // an empty value clears the list
+      if (it != raw.end()) {
+        interaction_constraints_malformed.clear();
+        if (!ParseSets(it->second, &interaction_constraints)) { interaction_constraints.clear(); interaction_constraints_malformed = it->second; }
+      }
       it = raw.find("categorical_feature");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &categorical_feature, [](const std::string& x) { return std::atoi(x.c_str()); });
     }
@@ -240,6 +273,7 @@ struct Config {
     std::ostringstream s;
     auto join_i = [](const std::vector<int>& v) { std::string r; for (size_t i = 0; i < v.size(); ++i) r += (i ? "," : "") + std::to_string(v[i]); return r; };
     auto join_d = [](const std::vector<double>& v) { std::string r; for (size_t i = 0; i < v.size(); ++i) r += (i ? "," : "") + Num(v[i]); return r; };
+    auto join_sets = [&](const std::vector<std::vector<int>>& v) { std::string r; for (size_t i = 0; i < v.size(); ++i) r += (i ? ",[" : "[") + join_i(v[i]) + "]"; return r; };
     auto join_s = [](const std::vector<std::string>& v) { std::string r; for (size_t i = 0; i < v.size(); ++i) r += (i ? "," : "") + v[i]; return r; };
     std::string tl = tree_learner == "data" ? "data" : tree_learner;
     s << "[boosting: " << boosting << "]\n[objective: " << objective << "]\n[metric: " << join_s(metric) << "]\n";
@@ -262,7 +296,8 @@ struct Config {
     s << "[top_k: " << top_k << "]\n[monotone_constraints: " << join_i(monotone_constraints) << "]\n";
     s << "[monotone_constraints_method: " << monotone_constraints_method << "]\n[monotone_penalty: " << Num(monotone_penalty) << "]\n";
     s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
-    s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: 0]\n[interaction_constraints: ]\n";
+    s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: 0]\n";
+    s << "[interaction_constraints: " << join_sets(interaction_constraints) << "]\n";
     s << "[verbosity: " << verbosity << "]\n[saved_feature_importance_type: 0]\n[linear_tree: 0]\n[max_bin: " << max_bin << "]\n";
     s << "[max_bin_by_feature: " << max_bin_by_feature << "]\n[min_data_in_bin: " << min_data_in_bin << "]\n";
     s << "[bin_construct_sample_cnt: " << bin_construct_sample_cnt << "]\n[data_random_seed: " << data_random_seed << "]\n";

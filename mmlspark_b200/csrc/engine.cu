@@ -1369,6 +1369,29 @@ static void CheckMonotone(const Config& cfg, const Dataset& train, bool voting_p
   if (voting_parallel) Fatal(kVotingMonotone);
 }
 
+// the voting learner's local top-k and vote would need every rank's candidates filtered by the leaves' set masks; not restated
+static const char* const kVotingInteraction = "tree_learner=voting does not support interaction_constraints with more than one machine; "
+                                              "use tree_learner=data_parallel or no interaction_constraints";
+constexpr size_t kMaxInteractionSets = 64;      // one 64-bit set mask per leaf (kernels.cuh LeafState::inter_mask)
+
+// interaction constraints: the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+static void CheckInteraction(const Config& cfg, const Dataset& train, bool voting_parallel) {
+  if (!cfg.interaction_constraints_malformed.empty())
+    Fatal("interaction_constraints should be bracketed lists of feature indices like [0,1,2],[2,3], got '" +
+          cfg.interaction_constraints_malformed + "'");
+  const std::vector<std::vector<int>>& ic = cfg.interaction_constraints;
+  if (ic.empty()) return;
+  if (ic.size() > kMaxInteractionSets)
+    Fatal("interaction_constraints supports at most " + std::to_string(kMaxInteractionSets) + " sets (one 64-bit mask per leaf), got " +
+          std::to_string(ic.size()));
+  for (size_t s = 0; s < ic.size(); ++s)
+    for (int f : ic[s])
+      if (f < 0 || f >= train.num_total_features)
+        Fatal("interaction_constraints: feature index " + std::to_string(f) + " in set " + std::to_string(s) + " is outside [0, " +
+              std::to_string(train.num_total_features) + ")");
+  if (voting_parallel) Fatal(kVotingInteraction);
+}
+
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1404,7 +1427,8 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   parallel_ = Net().active && Net().world > 1;
   same_device_ = parallel_ && Net().same_device != nullptr;
   cfg.num_machines = parallel_ ? Net().world : 1;
-  if (parallel_ && cfg.tree_learner == "voting") {      // identical on every rank: they all fail here, before any collective of training
+  voting_ = parallel_ && cfg.tree_learner == "voting";
+  if (voting_) {      // identical on every rank: they all fail here, before any collective of training
     if (cfg.top_k <= 0) Fatal("tree_learner=voting needs top_k > 0, got top_k=" + std::to_string(cfg.top_k));
     if (train->nw > 0)
       Fatal("tree_learner=voting does not support features with more than 256 bins (" + std::to_string(train->nw) +
@@ -1414,7 +1438,8 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
             " * " + std::to_string(std::min(cfg.top_k, train->nf)));
     if (cfg.extra_trees) Fatal(kVotingExtraTrees);
   }
-  CheckMonotone(cfg, *train, parallel_ && cfg.tree_learner == "voting");
+  CheckMonotone(cfg, *train, voting_);
+  CheckInteraction(cfg, *train, voting_);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1753,8 +1778,10 @@ void Booster::ResetParameter(const char* params) {
   cfg.num_machines = keep_machines;
   if (train) {      // metrics named by the reset meet the checks of LGBM_BoosterCreate / AddValidData; a rejected reset changes nothing
     try {
-      if (parallel_ && cfg.tree_learner == "voting" && cfg.extra_trees) Fatal(kVotingExtraTrees);
-      CheckMonotone(cfg, *train, parallel_ && cfg.tree_learner == "voting");
+      // the voting checks follow the learner built at create: a reset's tree_learner does not change it
+      if (voting_ && cfg.extra_trees) Fatal(kVotingExtraTrees);
+      CheckMonotone(cfg, *train, voting_);
+      CheckInteraction(cfg, *train, voting_);
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;

@@ -252,6 +252,7 @@ class Booster {
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   bool parallel_ = false;
+  bool voting_ = false;                 // parallel_ and tree_learner=voting at create: the learner's split chain, which ResetParameter keeps
   bool same_device_ = false;            // parallel_ over the same-device communicator: all ranks are threads of this process on this device
   bool const_hessian_ = false;
   bool has_init_score_ = false;

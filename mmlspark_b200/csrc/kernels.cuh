@@ -66,7 +66,8 @@ struct SplitParams {
   int min_data_in_leaf, max_depth, num_leaves, parallel;
   int nf, nf_pad, num_tiles, nfn;                              // nfn: features stored in uint8 tiles; [nfn, nf) are wide
   double cat_l2, cat_smooth;                                   // categorical split search ([UPSTREAM] defaults 10, 10)
-  int max_cat_threshold, max_cat_to_onehot, min_data_per_group, pad3;   // 32, 4, 100
+  int max_cat_threshold, max_cat_to_onehot, min_data_per_group;         // 32, 4, 100
+  int interaction;                                             // 1 when interaction_constraints is non-empty (d_pick_block, d_round_ctl)
 };
 
 // extra_trees (the scans' template parameter kExtra; [UPSTREAM] FeatureHistogram USE_RAND, FeatureMetainfo::rand): every used feature
@@ -110,6 +111,7 @@ struct LeafBest {
   unsigned cat_bits[8];
   int cat_list_len, monotone_type;           // monotone_type: the split feature's constraint (0 without monotone constraints)
   unsigned short cat_list[kCatListMax];
+  unsigned long long inter_sets;             // interaction constraints: the split feature's sets_of word (0 without them)
 };
 
 struct LeafState {
@@ -123,11 +125,17 @@ struct LeafState {
   // monotone constraints (basic method): the bounds [mono_min, mono_max] of this leaf's output; the root's are (-inf, +inf), children
   // inherit their parent's and a numerical split on a monotone feature narrows them at the mid-point of the two outputs (d_round_ctl)
   double mono_min, mono_max;
+  // interaction constraints: bit s is set when constraint set s holds every split feature on the path from the root to this leaf.  The
+  // root's has every bit; a split on feature u gives both children parent & sets_of[u] (d_round_ctl).  Read only when p.interaction.
+  unsigned long long inter_mask;
 };
 
-// monotone constraints ([UPSTREAM] monotone_constraints.hpp BasicLeafConstraints, FeatureHistogram USE_MC): the scans' template parameter
+// The scans' constraint arguments.
+// Monotone constraints ([UPSTREAM] monotone_constraints.hpp BasicLeafConstraints, FeatureHistogram USE_MC): the scans' template parameter
 // kMono.  type: per inner feature -1, 0 or +1 (the real feature's monotone_constraints entry); penalty: monotone_penalty.
-struct MonoArgs { const signed char* type; double penalty; };
+// Interaction constraints ([UPSTREAM] ColSampler::GetByNode): sets_of[u], per inner feature, has bit s set when constraint set s holds
+// the feature's real index; feature u may split a leaf iff sets_of[u] & inter_mask != 0.  Read by the pick step only when p.interaction.
+struct ConstraintArgs { const signed char* type; double penalty; const unsigned long long* sets_of; };
 
 struct TreeCtrl {
   int num_leaves, left_leaf, right_leaf, smaller, larger, go, finished, split_leaf;
@@ -747,7 +755,7 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
   if (threadIdx.x == 0) {
     LeafState& r = leaves[0];
     r.begin = 0; r.count = n_local; r.buf = 0; r.depth = 0; r.identity = root_is_bag ? 0 : 1; r.hist_slot = 0; r.parent_node = -1;
-    r.mono_min = kNegInf; r.mono_max = -kNegInf;
+    r.mono_min = kNegInf; r.mono_max = -kNegInf; r.inter_mask = ~0ull;
     r.global_count = static_cast<int>(ctrl->root_q[2]);
     r.sum_g = static_cast<double>(ctrl->root_q[0]) * ctrl->inv_g;
     r.sum_h = static_cast<double>(ctrl->root_q[1]) * ctrl->inv_h;
@@ -757,16 +765,21 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
   }
 }
 
-// monotone constraints ([UPSTREAM] BasicLeafConstraints::Update), when the round controller applies a split of leaf L into L and R: both
-// children inherit the parent's bounds; a numerical split on a monotone feature narrows them at mid = (left_out + right_out) / 2 — the
-// left child's max and the right child's min for +1, the mirror for -1.  Out of line to keep it off the partition kernel's registers.
-__device__ __noinline__ void d_mono_children(LeafState& L, LeafState& R, int monotone_type, int is_cat, double left_out, double right_out) {
+// The constraints of the two children when the round controller applies a split of leaf L into L and R.  Out of line to keep it off the
+// partition kernel's registers.
+// Monotone constraints ([UPSTREAM] BasicLeafConstraints::Update): both children inherit the parent's bounds; a numerical split on a
+// monotone feature narrows them at mid = (left_out + right_out) / 2 — the left child's max and the right child's min for +1, the mirror
+// for -1.
+// Interaction constraints (interaction != 0): both children's set mask is the parent's & the split feature's sets_of word.
+__device__ __noinline__ void d_constrain_children(LeafState& L, LeafState& R, int monotone_type, int is_cat, double left_out, double right_out,
+                                                  int interaction, const unsigned long long& inter_sets) {
   R.mono_min = L.mono_min; R.mono_max = L.mono_max;
   if (monotone_type != 0 && !is_cat) {
     const double mid = (left_out + right_out) / 2.0;
     if (monotone_type > 0) { L.mono_max = fmin(L.mono_max, mid); R.mono_min = fmax(R.mono_min, mid); }
     else { L.mono_min = fmax(L.mono_min, mid); R.mono_max = fmin(R.mono_max, mid); }
   }
+  if (interaction) { const unsigned long long m = L.inter_mask & inter_sets; L.inter_mask = m; R.inter_mask = m; }
 }
 
 // Applies the split chosen in the previous round (Tree::Split + leaf bookkeeping, using the TRUE row
@@ -825,7 +838,7 @@ d_round_ctl(TreeCtrl* ctrl, LeafState* leaves, const TreeDev& tree, uint8_t* fla
       L.count = true_left; L.buf = dst_buf; L.identity = 0; L.depth += 1;
       L.global_count = b.left_count; R.global_count = b.right_count;
       L.sum_g = b.left_g; L.sum_h = b.left_h; R.sum_g = b.right_g; R.sum_h = b.right_h;
-      d_mono_children(L, R, b.monotone_type, b.is_cat, b.left_out, b.right_out);
+      d_constrain_children(L, R, b.monotone_type, b.is_cat, b.left_out, b.right_out, p.interaction, L.best.inter_sets);
       R.hist_slot = nl;
       L.best.gain = kNegInf; L.best.feature = -1; R.best.gain = kNegInf; R.best.feature = -1;
       ctrl->left_leaf = leaf; ctrl->right_leaf = nl;
@@ -1092,17 +1105,23 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
 // taking longer than the scan itself.  The order (gain desc, real feature index asc) is total, so any reduction shape picks the same winner.
 // kMono (monotone constraints): the outputs are clamped to the leaf's bounds ([UPSTREAM] CalculateSplittedLeafOutput<USE_MC>) and the
 // split feature's constraint (mono_type, per inner feature) is kept for the round controller's bound update.
+// p.interaction (interaction constraints): a feature that may not split the leaf (sets_of[u] & the leaf's inter_mask == 0) is passed
+// over here and only here, after the scans, so the scans, their is_splittable flags and the extra_trees draws are what they are
+// without constraints ([UPSTREAM] SerialTreeLearner::ComputeBestSplitForFeature filters after FindBestThreshold).  The chosen
+// feature's sets_of word is kept for the round controller's mask update.
 template <bool kMono>
 __device__ __noinline__ void
 d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p,
-             const signed char* __restrict__ mono_type) {
+             const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of) {
   __shared__ double s_gain[8];
   __shared__ int s_feat[8], s_idx[8];
   const int which = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int leaf = ctrl->go ? (which ? ctrl->larger : ctrl->smaller) : -1;
   double bg = kNegInf; int bf = 0x7fffffff, bi = -1;
   if (leaf >= 0) {
+    const unsigned long long mask = p.interaction ? leaves[leaf].inter_mask : 0ull;
     for (int u = t; u < p.nf; u += 128) {
+      if (p.interaction && !(sets_of[u] & mask)) continue;
       const double cg = __ldcg(&cands[which * p.nf_pad + u].gain);
       const int rf = meta[u].real_index;
       if (cg > bg || (cg == bg && rf < bf)) { bg = cg; bf = rf; bi = u; }
@@ -1122,6 +1141,7 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
     LeafBest b;
     b.gain = kNegInf; b.feature = -1; b.threshold = 0; b.default_left = 1; b.left_count = 0; b.right_count = 0;
     b.left_g = b.left_h = b.right_g = b.right_h = b.left_out = b.right_out = 0; b.is_cat = 0; b.cat_list_len = 0; b.monotone_type = 0;
+    b.inter_sets = 0ull;
     for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = 0u;
     if (bi >= 0 && bg > kNegInf) {
       const SplitCand c = d_load_cand(&cands[which * p.nf_pad + bi]);
@@ -1142,6 +1162,7 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
         b.left_out = d_calc_output(c.left_g, c.left_h, pc);
         b.right_out = d_calc_output(L.sum_g - c.left_g, sum_h - c.left_h, pc);
       }
+      if (p.interaction) b.inter_sets = sets_of[c.feature];
       b.is_cat = c.is_cat;
       for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = c.cat_bits[wd];
     }
@@ -1823,7 +1844,7 @@ template <bool kExtra, bool kMono>
 __global__ void __launch_bounds__(256)
 k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const WideMeta* __restrict__ wm, const long long* __restrict__ H,
             long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
-            unsigned* __restrict__ xrand, MonoArgs mono) {
+            unsigned* __restrict__ xrand, ConstraintArgs cons) {
   extern __shared__ __align__(16) unsigned char sw_smem[];
   double* s_key = reinterpret_cast<double*>(sw_smem);                          // [num_bin] ctr keys of the used bins, +inf otherwise
   __shared__ int s_used;
@@ -1861,10 +1882,10 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
       if (which) xr = d_lcg_next(xr);
       rand_thr = d_extra_draw(&xr, m.num_bin - 2);
     }
-    const int mt = kMono ? mono.type[u] : 0;
+    const int mt = kMono ? cons.type[u] : 0;
     d_scan_wide_numeric<kExtra, kMono>(dst, m, L, inv_g, inv_h, p, flag, &out, rand_thr, mt);
     if (threadIdx.x == 0) {
-      if (kMono && mt != 0) out.gain *= d_mono_penalty(L.depth, mono.penalty);
+      if (kMono && mt != 0) out.gain *= d_mono_penalty(L.depth, cons.penalty);
       cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 1u; __threadfence();
     }
     return;
@@ -2223,7 +2244,7 @@ template <int kMode, bool kExtra = false, bool kMono = false>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, MonoArgs mono) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, ConstraintArgs cons) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
@@ -2308,9 +2329,9 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
             const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
             const int rand_thr = kExtra ? d_extra_draw(&xr, fm.num_bin - 2) : 0;
             drew = fm.num_bin > 2 ? 1 : 0;
-            const int mt = kMono ? mono.type[u] : 0;
+            const int mt = kMono ? cons.type[u] : 0;
             d_scan_wide_numeric<kExtra, kMono>(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, rand_thr, mt);
-            if (kMono && mt != 0 && threadIdx.x == 0) out.gain *= d_mono_penalty(L.depth, mono.penalty);
+            if (kMono && mt != 0 && threadIdx.x == 0) out.gain *= d_mono_penalty(L.depth, cons.penalty);
           } else if (threadIdx.x < 32) {
             long long qg[8], qh[8];
 #pragma unroll
@@ -2338,7 +2359,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
     else {
       if constexpr (kExtra) d_extra_commit(ctrl, xrand, p);
-      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, mono.type);
+      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, cons.type, cons.sets_of);
     }
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
   }

@@ -49,6 +49,7 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
   B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
   mono_.Alloc(train.nf_pad);      // allocated whatever monotone_constraints says: a ResetParameter may set them
+  sets_of_.Alloc(train.nf_pad);   // and whatever interaction_constraints says
 
   ResetConfig(cfg);
   sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
@@ -56,7 +57,7 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   {   // categorical split search parameters (Config keeps the native defaults unless given, SURVEY.md B.2)
     sp_.cat_l2 = cfg.cat_l2; sp_.cat_smooth = cfg.cat_smooth;
     sp_.max_cat_threshold = cfg.max_cat_threshold; sp_.max_cat_to_onehot = cfg.max_cat_to_onehot;
-    sp_.min_data_per_group = cfg.min_data_per_group; sp_.pad3 = 0;
+    sp_.min_data_per_group = cfg.min_data_per_group;
     if (train.nw > 0) {
       if (sp_.max_cat_threshold > kCatListMax) Fatal("max_cat_threshold > " + std::to_string(kCatListMax) + " is not supported together with categorical features of more than 256 bins");
       if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");
@@ -153,6 +154,18 @@ void TreeLearner::ResetConfig(const Config& cfg) {
   if (types != mono_host_) {
     mono_host_ = std::move(types);
     mono_.Upload(mono_host_.data(), mono_host_.size(), stream_);
+  }
+  // interaction constraints: sets_of[u] has bit s set when set s holds inner feature u's real index (Booster checked the indices and
+  // that there are at most 64 sets).  Uploaded when it changes, as the monotone types are.
+  // never on for the voting learner, whose scans do not apply the masks (Booster rejects a list for it)
+  sp_.interaction = (voting_ || cfg.interaction_constraints.empty()) ? 0 : 1;
+  std::vector<unsigned long long> by_real(train_.num_total_features, 0ull), sets(train_.nf_pad, 0ull);
+  for (size_t s = 0; s < cfg.interaction_constraints.size(); ++s)
+    for (int f : cfg.interaction_constraints[s]) by_real[f] |= 1ull << s;
+  for (int u = 0; u < train_.nf; ++u) sets[u] = by_real[train_.used[u]];
+  if (sets != sets_of_host_) {
+    sets_of_host_ = std::move(sets);
+    sets_of_.Upload(sets_of_host_.data(), sets_of_host_.size(), stream_);
   }
 }
 
@@ -420,12 +433,14 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
     mark();
     // the dynamic scratch of k_scan is only touched by categorical features and bundle members
     const int scan_smem = (d.has_categorical || !d.bundles.empty()) ? kScanSmem : 0;
+    // every scan gets the device constraint arrays, so no instantiation can read through a null pointer
+    const ConstraintArgs cons{mono_.p, monotone_penalty_, sets_of_.p};
     if (voting_) {
       // local scan + top-k -> all-gather of the records -> vote + pack -> all-reduce of the packed columns -> global scan + pick
       nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
       const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
       k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p,
-                                                        MonoArgs{});
+                                                        cons);
       mark();
       Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
       mark();
@@ -436,7 +451,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
       mark();
       k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p,
-                                                         MonoArgs{});
+                                                         cons);
       nvtxRangePop();
       comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
       comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
@@ -448,12 +463,11 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
         comm_hist_bytes_ += static_cast<long long>(slot_elems_ * sizeof(long long));
       }
       mark();
-      const MonoArgs mono{mono_.p, monotone_penalty_};
       if (d.nw > 0) {
         auto* scan_wide = monotone_ ? (extra_trees_ ? k_scan_wide<true, true> : k_scan_wide<false, true>)
                                     : (extra_trees_ ? k_scan_wide<true, false> : k_scan_wide<false, false>);
         scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
-                                                               mono);
+                                                               cons);
         timing_.launches += 1;
       }
       // scan + (last block) pick
@@ -461,7 +475,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       auto* scan = monotone_ ? (extra_trees_ ? k_scan<kScanPlain, true, true> : k_scan<kScanPlain, false, true>)
                              : (extra_trees_ ? k_scan<kScanPlain, true, false> : k_scan<kScanPlain, false, false>);
       scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
-                                         mono);
+                                         cons);
       nvtxRangePop();
     }
     mark();

@@ -56,6 +56,8 @@ class TreeLearner {
   double monotone_penalty_ = 0.0;
   std::vector<signed char> mono_host_;      // [nf_pad] each inner feature's monotone constraint, as uploaded to mono_
   DevBuf<signed char> mono_;
+  std::vector<unsigned long long> sets_of_host_;      // [nf_pad] each inner feature's interaction-constraint sets, as uploaded to sets_of_
+  DevBuf<unsigned long long> sets_of_;
   int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built

@@ -43,6 +43,7 @@ COMMON_DEFAULTS = dict(
     minGainToSplit=0.0, maxDeltaStep=0.0, maxBinByFeature=(), minDataInLeaf=20,         # :443-466
     extraTrees=False, extraSeed=6,      # LightGBM 3.2's extra_trees / extra_seed (not a param of the reference's estimators)
     monotoneConstraints=(), monotoneConstraintsMethod="basic", monotonePenalty=0.0,      # monotone_constraints (per feature -1/0/1) etc.
+    interactionConstraints=(),          # interaction_constraints: lists of feature indices; a branch splits on features of one list only
     delegate=None,
     # column params (core/contracts/Params.scala:93-208 + Spark ML)
     featuresCol="features", labelCol="label", predictionCol="prediction", weightCol=None, initScoreCol=None,
@@ -124,9 +125,11 @@ class TrainParams:
         s += "num_threads=%d " % p["numThreads"]
         if p["extraTrees"]:      # only when set, so every other parameter string stays as the reference builds it
             s += "extra_trees=true extra_seed=%d " % p["extraSeed"]
-        if p["monotoneConstraints"]:      # only when given, so every other parameter string stays as the reference builds it
+        if len(p["monotoneConstraints"]) > 0:      # only when given, so every other parameter string stays as the reference builds it
             s += "monotone_constraints=%s monotone_constraints_method=%s monotone_penalty=%s " % (
                 ",".join(str(int(c)) for c in p["monotoneConstraints"]), p["monotoneConstraintsMethod"], scala_double(p["monotonePenalty"]))
+        if len(p["interactionConstraints"]) > 0:      # only when given, so every other parameter string stays as the reference builds it
+            s += "interaction_constraints=%s " % ",".join("[%s]" % ",".join(str(int(f)) for f in c) for c in p["interactionConstraints"])
         return s
 
     def to_string(self):
