@@ -680,41 +680,34 @@ void Dataset::UploadMeta() {
   for (int u = 0; u < nfn; ++u) if (base_of[u] < 0) col_feat[col_of[u]] = u;
   const int nft = std::max(1, (nfn + 31) / 32) * 32;      // inner slots of the tile features
   nf_pad = nft + nw;
-  meta_host.assign(nf_pad, FeatMeta{1, 0, 0, 0, 0, 0, 0, 0});
+  meta_host.assign(nf_pad, FeatMeta{1, 0, 0, 0, 0, 0, 0, 0, 0});
   bundle_base.assign(nf_pad, -1);
   for (int u = 0; u < nfn; ++u) bundle_base[u] = base_of[u];
+  // bin tables: tile slot u's row at u * 256 (k_bin_rows stages a tile's rows in shared memory), then one row per wide feature
   std::vector<double> ubh(static_cast<size_t>(nft) * 256, 0.0);
-  std::vector<uint8_t> cbh(static_cast<size_t>(nft) * 256, 0);
+  std::vector<uint16_t> cbh(ubh.size(), 0);
   has_categorical = false;
   hist_pairs = static_cast<size_t>(num_tiles) * 32 * 256;
-  wide_host.clear();
-  std::vector<int> wcats;
-  std::vector<unsigned short> wbins;
-  std::vector<double> wub;
   for (int u = 0; u < nf; ++u) {
     const FeatureBins& fb = mappers[used[u]];
+    const size_t row_len = fb.categorical ? fb.sorted_cats.size() : static_cast<size_t>(fb.num_bin);
     int hist_off = u < nfn ? col_of[u] * 256 : 0;
+    size_t table_off = static_cast<size_t>(u) * 256;
     if (u >= nfn) {
       hist_off = static_cast<int>(hist_pairs);
-      WideMeta wm{fb.num_bin, hist_off, static_cast<int>(fb.categorical ? wcats.size() : wub.size()), static_cast<int>(fb.sorted_cats.size()),
-                  static_cast<int>(fb.default_bin), fb.missing_type, used[u], fb.categorical ? 1 : 0, fb.most_freq_bin == 0 ? 1 : 0, 0, 0, 0};
-      wide_host.push_back(wm);
-      if (fb.categorical) for (size_t i = 0; i < fb.sorted_cats.size(); ++i) { wcats.push_back(fb.sorted_cats[i]); wbins.push_back(static_cast<unsigned short>(fb.sorted_bins[i])); }
-      else wub.insert(wub.end(), fb.upper.begin(), fb.upper.end());
       hist_pairs += (static_cast<size_t>(fb.num_bin) + 255) / 256 * 256;
       if (hist_pairs > (1u << 30)) Fatal("histogram of the wide features is too large");
+      table_off = ubh.size();
+      ubh.resize(table_off + row_len, 0.0);
+      cbh.resize(table_off + row_len, 0);
     }
     meta_host[u] = FeatMeta{fb.num_bin, fb.missing_type, static_cast<int>(fb.default_bin), fb.most_freq_bin == 0 ? 1 : 0, used[u],
-                            fb.categorical ? 1 : 0, static_cast<int>(fb.sorted_cats.size()), hist_off};
-    if (fb.categorical) has_categorical = true;
-    if (u >= nfn) continue;
+                            fb.categorical ? 1 : 0, static_cast<int>(fb.sorted_cats.size()), hist_off, static_cast<int>(table_off)};
     if (fb.categorical) {
-      for (size_t i = 0; i < fb.sorted_cats.size(); ++i) {
-        ubh[static_cast<size_t>(u) * 256 + i] = fb.sorted_cats[i];
-        cbh[static_cast<size_t>(u) * 256 + i] = static_cast<uint8_t>(fb.sorted_bins[i]);
-      }
+      has_categorical = true;
+      for (size_t i = 0; i < row_len; ++i) { ubh[table_off + i] = fb.sorted_cats[i]; cbh[table_off + i] = static_cast<uint16_t>(fb.sorted_bins[i]); }
     } else {
-      for (int b = 0; b < fb.num_bin; ++b) ubh[static_cast<size_t>(u) * 256 + b] = fb.upper[b];
+      for (size_t b = 0; b < row_len; ++b) ubh[table_off + b] = fb.upper[b];
     }
   }
   meta.Alloc(nf_pad); ub.Alloc(ubh.size()); catbin.Alloc(cbh.size());
@@ -724,13 +717,6 @@ void Dataset::UploadMeta() {
   if (!bundles.empty()) UploadBundleMembers();
   ub.Upload(ubh.data(), ubh.size(), stream);
   catbin.Upload(cbh.data(), cbh.size(), stream);
-  if (nw > 0) {
-    wide_meta.Alloc(nw); wide_meta.Upload(wide_host.data(), nw, stream);
-    wide_cats.Alloc(std::max<size_t>(wcats.size(), 1)); wide_catbin.Alloc(std::max<size_t>(wbins.size(), 1));
-    if (!wcats.empty()) { wide_cats.Upload(wcats.data(), wcats.size(), stream); wide_catbin.Upload(wbins.data(), wbins.size(), stream); }
-    wide_ub.Alloc(std::max<size_t>(wub.size(), 1));
-    if (!wub.empty()) wide_ub.Upload(wub.data(), wub.size(), stream);
-  }
   B200_CUDA(cudaStreamSynchronize(stream));
 }
 
@@ -754,7 +740,7 @@ static void LaunchBin(const T* X, long long nrow, int ncol, int row_major, long 
     k_bin_bundles<T><<<sms * 8, 256, 0, s>>>(X, nrow, row_major, ld, d.d_members.p, d.d_bundle_start.p, d.d_bundle_col.p, static_cast<int>(d.bundles.size()),
                                              d.meta.p, d.ub.p, d.bins.p, static_cast<long long>(d.rows_stride), row_offset);
   if (d.nw > 0)
-    k_bin_wide<T><<<sms * 8, 256, 0, s>>>(X, nrow, row_major, ld, d.wide_meta.p, d.nw, d.wide_cats.p, d.wide_catbin.p, d.wide_ub.p, d.bins16.p, d.rows_stride, row_offset);
+    k_bin_wide<T><<<sms * 8, 256, 0, s>>>(X, nrow, row_major, ld, d.meta.p + d.nfn, d.nw, d.ub.p, d.catbin.p, d.bins16.p, d.rows_stride, row_offset);
   B200_CUDA(cudaGetLastError());
 }
 
@@ -1082,10 +1068,11 @@ Dataset* Dataset::CreateFromMats(int nmat, const void* const* data, int data_typ
 // ---- CSR ingestion without densifying (replaces LGBM_DatasetCreateFromCSR, reference call site DatasetAggregator.scala:438-459).
 // Bin finding walks the nonzeros of the sampled rows only; binning fills every row of a tile with the features' zero bins and then
 // scatters one thread per stored element.  Memory: O(nnz) + the uint8 bins, never nrow x num_col doubles.
-__global__ void k_fill_default_wide(const WideMeta* __restrict__ wm, int nw, uint16_t* __restrict__ bins16, size_t rows_stride, long long nrow) {
+// every wide column's default bin; wmeta = meta + nfn
+__global__ void k_fill_default_wide(const FeatMeta* __restrict__ wmeta, int nw, uint16_t* __restrict__ bins16, size_t rows_stride, long long nrow) {
   for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < nrow * nw; e += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int w = static_cast<int>(e / nrow);
-    bins16[static_cast<size_t>(w) * rows_stride + (e - static_cast<long long>(w) * nrow)] = static_cast<uint16_t>(wm[w].default_bin);
+    bins16[static_cast<size_t>(w) * rows_stride + (e - static_cast<long long>(w) * nrow)] = static_cast<uint16_t>(wmeta[w].default_bin);
   }
 }
 // every column's default: a plain feature's default bin, slot 0 of a bundle column (all members at their default bin), 0 for padding
@@ -1103,10 +1090,8 @@ __global__ void k_fill_default_bins(const FeatMeta* __restrict__ meta, const int
 }
 template <typename TI, typename TV>
 __global__ void k_bin_csr(const TI* __restrict__ indptr, const int* __restrict__ indices, const TV* __restrict__ vals, long long nrow, const int* __restrict__ inner_of,
-                          const FeatMeta* __restrict__ meta, const double* __restrict__ ub, const uint8_t* __restrict__ catbin, uint8_t* __restrict__ bins,
-                          size_t rows_stride, long long elem_base, int nfn, const WideMeta* __restrict__ wm, const int* __restrict__ wcats,
-                          const unsigned short* __restrict__ wcatbin, const double* __restrict__ wub, uint16_t* __restrict__ bins16,
-                          const int* __restrict__ bundle_base) {
+                          const FeatMeta* __restrict__ meta, const double* __restrict__ ub, const uint16_t* __restrict__ catbin, uint8_t* __restrict__ bins,
+                          size_t rows_stride, long long elem_base, int nfn, uint16_t* __restrict__ bins16, const int* __restrict__ bundle_base) {
   const int lane = threadIdx.x & 31;
   const long long warp = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) >> 5, nwarps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
   for (long long r = warp; r < nrow; r += nwarps) {
@@ -1115,29 +1100,10 @@ __global__ void k_bin_csr(const TI* __restrict__ indptr, const int* __restrict__
       const int u = inner_of[indices[k]];
       if (u < 0) continue;
       const FeatMeta m = meta[u];
-      double v = static_cast<double>(vals[k]);
+      unsigned bin = d_value_to_bin(static_cast<double>(vals[k]), m, ub + m.table_off, 1, catbin + m.table_off);
       if (u >= nfn) {           // wide column (categorical with > 256 bins, or numerical with max_bin > 255)
-        bins16[static_cast<size_t>(u - nfn) * rows_stride + r] = static_cast<uint16_t>(d_wide_bin(v, wm[u - nfn], wcats, wcatbin, wub));
+        bins16[static_cast<size_t>(u - nfn) * rows_stride + r] = static_cast<uint16_t>(bin);
         continue;
-      }
-      const double* myub = ub + static_cast<size_t>(u) * 256;
-      unsigned bin = 0;
-      if (m.is_categorical) {
-        if (!isnan(v)) {
-          const int iv = static_cast<int>(v);
-          if (iv >= 0) {
-            int lo = 0, hi = m.num_sorted_cats;
-            while (lo < hi) { int mid = (lo + hi) >> 1; if (static_cast<int>(myub[mid]) < iv) lo = mid + 1; else hi = mid; }
-            if (lo < m.num_sorted_cats && static_cast<int>(myub[lo]) == iv) bin = catbin[static_cast<size_t>(u) * 256 + lo];
-          }
-        }
-      } else {
-        if (isnan(v)) { if (m.missing_type == 2) bin = m.num_bin - 1; else v = 0.0; }
-        if (!isnan(v)) {
-          int lo = 0, hi = m.num_bin - 1 - (m.missing_type == 2 ? 1 : 0);
-          while (lo < hi) { int mid = (hi + lo - 1) / 2; if (v <= myub[mid]) hi = mid; else lo = mid + 1; }
-          bin = lo;
-        }
       }
       const int base = bundle_base[u], c = m.hist_off >> 8;
       if (base >= 0) {      // a bundle member: its default bin is the column's slot 0, already filled
@@ -1255,7 +1221,7 @@ Dataset* Dataset::CreateFromCSRs(int nparts, const void* const* indptr, int indp
   });
   d->AllocBins();
   k_fill_default_bins<<<sms * 8, 256, 0, d->stream>>>(d->meta.p, d->d_col_feat.p, d->bins.p, d->rows_stride, nrow, d->num_tiles);
-  if (d->nw > 0) k_fill_default_wide<<<sms * 8, 256, 0, d->stream>>>(d->wide_meta.p, d->nw, d->bins16.p, d->rows_stride, nrow);
+  if (d->nw > 0) k_fill_default_wide<<<sms * 8, 256, 0, d->stream>>>(d->meta.p + d->nfn, d->nw, d->bins16.p, d->rows_stride, nrow);
   B200_CUDA(cudaGetLastError());
   if (d->nf > 0) {
     DevBuf<int> d_inner; d_inner.Alloc(F); d_inner.Upload(d->inner_of.data(), F, d->stream);
@@ -1266,8 +1232,7 @@ Dataset* Dataset::CreateFromCSRs(int nparts, const void* const* indptr, int indp
       uint8_t* base = d->bins.p + static_cast<size_t>(r0) * 32;       // row offset inside every tile
       k_bin_csr<TI, TV><<<grid, 256, 0, d->stream>>>(reinterpret_cast<const TI*>(d_ip.p), reinterpret_cast<const int*>(d_ix.p),
                                                     reinterpret_cast<const TV*>(d_v.p), nr, d_inner.p, d->meta.p, d->ub.p, d->catbin.p, base,
-                                                    d->rows_stride, e0k, d->nfn, d->wide_meta.p, d->wide_cats.p, d->wide_catbin.p, d->wide_ub.p,
-                                                    d->bins16.p ? d->bins16.p + r0 : nullptr, d->d_bundle_base.p);
+                                                    d->rows_stride, e0k, d->nfn, d->bins16.p ? d->bins16.p + r0 : nullptr, d->d_bundle_base.p);
     });
   }
   d->ingest_ms = timer.Ms();

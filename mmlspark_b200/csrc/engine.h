@@ -138,16 +138,12 @@ class Dataset {
   size_t rows_stride = 0;
   DevBuf<uint8_t> bins;                      // [num_tiles][rows_stride][32]
   DevBuf<uint16_t> bins16;                   // [nw][rows_stride]
-  std::vector<WideMeta> wide_host;
-  DevBuf<WideMeta> wide_meta;
-  DevBuf<int> wide_cats;                     // sorted category values of all wide features (slices per WideMeta)
-  DevBuf<unsigned short> wide_catbin;        // ... and their bins
-  DevBuf<double> wide_ub;                    // bin upper bounds of the wide numerical features (max_bin > 255)
   const int* BundleBase() const { return bundles.empty() ? nullptr : d_bundle_base.p; }      // null: no feature bundle, no decode
   BinView View() const { return BinView{bins.p, rows_stride, bins16.p, nfn, meta.p, BundleBase()}; }
-  DevBuf<FeatMeta> meta;
-  DevBuf<double> ub;                         // [nf][256] bin upper bounds (categorical: sorted category values)
-  DevBuf<uint8_t> catbin;                    // [nf][256] categorical: bin of the i-th sorted category
+  DevBuf<FeatMeta> meta;                     // [nf_pad] every inner feature, tile and wide; the wide ones at [nfn, nf)
+  // bin tables, one row per feature at its FeatMeta::table_off: [nft][256] for the tile slots, then one row per wide feature
+  DevBuf<double> ub;                         // bin upper bounds (categorical: sorted category values)
+  DevBuf<uint16_t> catbin;                   // categorical: bin of the i-th sorted category
   bool has_categorical = false;
   std::vector<float> label, weight;
   std::vector<double> init_score;

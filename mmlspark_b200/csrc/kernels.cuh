@@ -21,6 +21,8 @@ struct FeatMeta {          // per inner (used) feature
   int num_sorted_cats;     // categorical: entries of the sorted category table (ub row = categories, catbin row = their bins)
   int hist_off;            // first (g,h) pair of the feature's storage column in a histogram slot: col * 256 for a tile feature (col = u
                            // without feature bundles), beyond the tiles for a wide one
+  int table_off;           // first entry of the feature's row in the bin tables ub / catbin: u * 256 for a tile feature, beyond the
+                           // tile rows for a wide one
 };
 
 // Exclusive feature bundles (bundle.h): a bundle column holds several features of which at most one is away from its most frequent bin
@@ -40,16 +42,11 @@ __host__ __device__ __forceinline__ unsigned d_bundle_slot(unsigned bin, int bas
 // "Wide" features: more than 256 bins.  LightGBM does not cap a categorical feature at max_bin — it keeps categories until 99 % of the
 // sampled mass is covered (BinMapper::FindBin) — so a 10^3..10^5-cardinality column (BASELINE.json configs[4]) needs thousands of bins.
 // They live outside the uint8 feature tiles: one uint16 column per feature, their own histogram kernel (k4_hist_wide) and scan
-// (k_scan_wide); inner index = nfn + w.  A categorical split on one sends at most max_cat_threshold bins left, carried as a bin list.
+// (k_scan_wide); inner index = nfn + w, described by meta[nfn + w] like every other feature.  A categorical split on one sends at most
+// max_cat_threshold bins left, carried as a bin list.
 constexpr int kWideHistSeg = 8192;       // bins one k4_hist_wide CTA accumulates: 4 planes x 8192 x 4 B = 128 KB of shared memory
 constexpr int kWideMaxBins = 16384;      // per feature (k_scan_wide sorts (ctr, bin) keys in 160 KB of shared memory); more fails loudly
 constexpr int kCatListMax = 64;          // >= max_cat_threshold (default 32) when wide features exist
-struct WideMeta {
-  int num_bin, hist_off, cat_off, num_cats;      // hist_off in (g,h) pairs; categorical: slice of the sorted category table (cat_off, num_cats);
-                                                 // numerical (max_bin > 255): cat_off = first entry of the feature's upper bounds in the wide ub table
-  int default_bin, missing_type, real_index, is_cat;
-  int offset, pad0, pad1, pad2;                  // offset: 1 iff most_freq_bin == 0 (as FeatMeta::offset)
-};
 struct BinView {                         // where a row's bin of inner feature u is stored
   const uint8_t* bins; size_t rows_stride; const uint16_t* bins16; int nfn;
   const FeatMeta* meta; const int* bundle_base;      // bundle_base null: no feature bundle, column = feature, no decode
@@ -229,6 +226,19 @@ __device__ __forceinline__ unsigned d_num_bin(double v, const FeatMeta& m, const
   }
   return static_cast<unsigned>(lo);
 }
+// value -> bin of any feature, tile or wide.  row = the feature's ub row (entry i at row[i * stride]), catbin_row = its catbin row.
+// Categorical: binary search of the category int(v) in the sorted category values; NaN, negative or unseen -> bin 0.  The values are
+// integers stored as doubles, which hold them exactly, so the probes compare doubles and convert nothing.
+__device__ __forceinline__ unsigned d_value_to_bin(double v, const FeatMeta& m, const double* row, int stride, const uint16_t* catbin_row) {
+  if (!m.is_categorical) return d_num_bin(v, m, row, stride);
+  if (isnan(v)) return 0;
+  const int iv = static_cast<int>(v);
+  if (iv < 0) return 0;
+  const double cat = iv;
+  int lo = 0, hi = m.num_sorted_cats;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (row[mid * stride] < cat) lo = mid + 1; else hi = mid; }
+  return lo < m.num_sorted_cats && row[lo * stride] == cat ? catbin_row[lo] : 0u;
+}
 
 // One warp per row-of-a-tile: lane = storage column of the tile.  Upper bounds of the tile's (at most 32) plain features sit
 // in shared memory ([32][256] doubles = 64 KB).  col_feat[column] = the plain feature of the column, or -1: a bundle column (left at
@@ -236,7 +246,7 @@ __device__ __forceinline__ unsigned d_num_bin(double v, const FeatMeta& m, const
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_bin_rows(const T* __restrict__ X, long long nrow, int ncol, int row_major, long long ld, const FeatMeta* __restrict__ meta,
-           const double* __restrict__ ub, const uint8_t* __restrict__ catbin, const int* __restrict__ col_feat, uint8_t* __restrict__ bins,
+           const double* __restrict__ ub, const uint16_t* __restrict__ catbin, const int* __restrict__ col_feat, uint8_t* __restrict__ bins,
            long long rows_stride, long long row_offset) {
   extern __shared__ double s_ub[];   // [256 bins][32 lanes]: lane l always hits bank pair 2l -> no conflicts beyond the 64-bit 2-phase
   const int tile = blockIdx.y;
@@ -254,19 +264,8 @@ k_bin_rows(const T* __restrict__ X, long long nrow, int ncol, int row_major, lon
   for (long long r = blockIdx.x * 8LL + warp; r < nrow; r += gridDim.x * 8LL) {
     unsigned bin = 0;
     if (u >= 0) {
-      double v = row_major ? static_cast<double>(X[r * ld + m.real_index]) : static_cast<double>(X[static_cast<long long>(m.real_index) * ld + r]);
-      if (m.is_categorical) {     // category -> bin: binary search in the sorted category table; NaN / negative / unseen -> bin 0
-        if (!isnan(v)) {
-          const int iv = static_cast<int>(v);
-          if (iv >= 0) {
-            int lo = 0, hi = m.num_sorted_cats;
-            while (lo < hi) { int mid = (lo + hi) >> 1; if (static_cast<int>(myub[mid * 32]) < iv) lo = mid + 1; else hi = mid; }
-            if (lo < m.num_sorted_cats && static_cast<int>(myub[lo * 32]) == iv) bin = catbin[static_cast<size_t>(u) * 256 + lo];
-          }
-        }
-      } else {
-        bin = d_num_bin(v, m, myub, 32);
-      }
+      const double v = row_major ? static_cast<double>(X[r * ld + m.real_index]) : static_cast<double>(X[static_cast<long long>(m.real_index) * ld + r]);
+      bin = d_value_to_bin(v, m, myub, 32, catbin + m.table_off);
     }
     bins[(static_cast<size_t>(tile) * rows_stride + row_offset + r) * 32 + lane] = static_cast<uint8_t>(bin);
   }
@@ -903,6 +902,41 @@ __device__ __noinline__ bool d_smaller_drew_cat(const long long* __restrict__ hi
   }
   return d_cat_rand_range(used_bin, max_cat_threshold) > 0;
 }
+// extra_trees, the larger leaf's block of feature m: did the smaller leaf's scan of it draw?  Both leaves hold the same pre-scan flag
+// (inherited from their parent), so the smaller one scanned the feature too; it drew unless its range was empty, which only the
+// many-vs-many categorical search decides from the data: the smaller leaf's used bins, counted in its histogram column `hist` (H).
+// max_cat_threshold: the calling scan's.  Called by every thread of the block.
+__device__ __forceinline__ bool d_smaller_drew(const long long* __restrict__ hist, const FeatMeta& m, const TreeCtrl* ctrl, const LeafState* leaves,
+                                               const SplitParams& p, int max_cat_threshold) {
+  if (!m.is_categorical) return m.num_bin > 2;
+  if (m.num_bin <= p.max_cat_to_onehot) return m.num_bin > 1;
+  return d_smaller_drew_cat(hist, m.num_bin, leaves[ctrl->smaller], ctrl->inv_h, p, max_cat_threshold);
+}
+
+// The many-vs-many walk of FindBestThresholdCategoricalInner [UPSTREAM] from one end of the ranked used bins: at most max_num_cat bins
+// are added to the left side, with the sequential code's skip (continue) and stop (break) rules.  next(&g, &h) gives the next bin's sums
+// in walk order; visit(i, slg, slh, srh, left_count) is called for every prefix (i + 1 bins) whose gain the reference evaluates.
+template <bool kExtra, typename Next, typename Visit>
+__device__ __forceinline__ void d_cat_walk(int used_bin, int max_num_cat, int num_data, double sum_h, double cnt_factor, const SplitParams& p,
+                                           int rand_i, Next next, Visit visit) {
+  int cnt_cur_group = 0, left_count = 0;
+  double slg = 0.0, slh = kEpsD;
+  for (int i = 0; i < used_bin && i < max_num_cat; ++i) {
+    double g, h;
+    next(&g, &h);
+    const int cnt = static_cast<int>(h * cnt_factor + 0.5);
+    slg += g; slh += h; left_count += cnt; cnt_cur_group += cnt;
+    if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
+    const int right_count = num_data - left_count;
+    if (right_count < p.min_data_in_leaf || right_count < p.min_data_per_group) break;
+    const double srh = sum_h - slh;
+    if (srh < p.min_sum_hessian) break;
+    if (cnt_cur_group < p.min_data_per_group) continue;
+    cnt_cur_group = 0;
+    if (kExtra && i != rand_i) continue;
+    visit(i, slg, slh, srh, left_count);
+  }
+}
 
 // Categorical split search for one feature by one warp (FeatureHistogram::FindBestThresholdCategoricalInner [UPSTREAM]):
 // one-hot when num_bin <= max_cat_to_onehot; otherwise the bins holding >= cat_smooth rows are ranked by g/(h+cat_smooth)
@@ -923,9 +957,7 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
-  SplitParams pshift = p;
-  if (!(p.max_delta_step > 0)) pshift.max_delta_step = 0;
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, pshift) + p.min_gain_to_split;
+  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
   const bool onehot = m.num_bin <= p.max_cat_to_onehot;
   int drew = 0, rand_t = -1;      // rand_t: the one candidate index evaluated, -1: every candidate
   if (kExtra && onehot) { rand_t = d_extra_draw(&xr, m.num_bin - 1); drew = m.num_bin > 1 ? 1 : 0; }
@@ -1018,28 +1050,15 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
     for (int d = 0; d < 2; ++d) {
       const int dir = d == 0 ? 1 : -1;
       int pos = d == 0 ? 0 : used_bin - 1;
-      int cnt_cur_group = 0, left_count = 0;
-      double slg = 0.0, slh = kEpsD;
-      for (int i = 0; i < used_bin && i < max_num_cat; ++i) {
-        const int t = order[pos];
-        pos += dir;
-        const double g = sg[t], h = sh[t];
-        const int cnt = static_cast<int>(h * cnt_factor + 0.5);
-        slg += g; slh += h; left_count += cnt; cnt_cur_group += cnt;
-        if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
-        const int right_count = num_data - left_count;
-        if (right_count < p.min_data_in_leaf || right_count < p.min_data_per_group) break;
-        const double srh = sum_h - slh;
-        if (srh < p.min_sum_hessian) break;
-        if (cnt_cur_group < p.min_data_per_group) continue;
-        cnt_cur_group = 0;
-        if (kExtra && i != rand_t) continue;
-        const double gain = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, srh, pc, L.mono_min, L.mono_max, 0)
-                                  : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
-        if (gain <= min_gain_shift) continue;
-        any_valid = true;
-        if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_lc = left_count; best_i = i; best_dir = dir; }
-      }
+      d_cat_walk<kExtra>(used_bin, max_num_cat, num_data, sum_h, cnt_factor, p, rand_t,
+                         [&](double* g, double* h) { const int t = order[pos]; pos += dir; *g = sg[t]; *h = sh[t]; },
+                         [&](int i, double slg, double slh, double srh, int left_count) {
+                           const double gain = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, srh, pc, L.mono_min, L.mono_max, 0)
+                                                     : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
+                           if (gain <= min_gain_shift) return;
+                           any_valid = true;
+                           if (gain > best_gain) { best_gain = gain; best_lg = slg; best_lh = slh; best_lc = left_count; best_i = i; best_dir = dir; }
+                         });
     }
     *flag = any_valid ? 1 : 0;
     if (any_valid) {
@@ -1527,40 +1546,18 @@ k_partition(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, con
 }
 
 // ---------------------------------------------------------------- wide features (> 256 bins): binning, histogram, categorical scan
-// value -> bin of the wide columns of a row block (categorical lookup: binary search in the feature's sorted category table)
-// value -> bin of one wide feature (shared by the dense and CSR ingestion kernels)
-__device__ __forceinline__ unsigned d_wide_bin(double v, const WideMeta& m, const int* __restrict__ cats, const unsigned short* __restrict__ catbin,
-                                               const double* __restrict__ wub) {
-  unsigned bin = 0;
-  if (m.is_cat) {
-    if (!isnan(v)) {
-      const int iv = static_cast<int>(v);
-      if (iv >= 0) {
-        const int* c = cats + m.cat_off;
-        int lo = 0, hi = m.num_cats;
-        while (lo < hi) { const int mid = (lo + hi) >> 1; if (c[mid] < iv) lo = mid + 1; else hi = mid; }
-        if (lo < m.num_cats && c[lo] == iv) bin = catbin[m.cat_off + lo];
-      }
-    }
-    return bin;
-  }
-  if (isnan(v)) { if (m.missing_type == 2) return static_cast<unsigned>(m.num_bin - 1); v = 0.0; }
-  const double* ub = wub + m.cat_off;
-  int lo = 0, hi = m.num_bin - 1 - (m.missing_type == 2 ? 1 : 0);
-  while (lo < hi) { const int mid = (hi + lo - 1) / 2; if (v <= ub[mid]) hi = mid; else lo = mid + 1; }
-  return static_cast<unsigned>(lo);
-}
+// value -> bin of the wide columns of a row block; wmeta = meta + nfn, the wide features' descriptions
 template <typename T>
-__global__ void k_bin_wide(const T* __restrict__ X, long long nrow, int row_major, long long ld, const WideMeta* __restrict__ wm, int nw,
-                           const int* __restrict__ cats, const unsigned short* __restrict__ catbin, const double* __restrict__ wub,
-                           uint16_t* __restrict__ bins16, size_t rows_stride, long long row_offset) {
+__global__ void k_bin_wide(const T* __restrict__ X, long long nrow, int row_major, long long ld, const FeatMeta* __restrict__ wmeta, int nw,
+                           const double* __restrict__ ub, const uint16_t* __restrict__ catbin, uint16_t* __restrict__ bins16, size_t rows_stride,
+                           long long row_offset) {
   const long long total = nrow * nw;
   for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total; e += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int w = static_cast<int>(e / nrow);
     const long long r = e - static_cast<long long>(w) * nrow;
-    const WideMeta m = wm[w];
+    const FeatMeta m = wmeta[w];
     const double v = row_major ? static_cast<double>(X[r * ld + m.real_index]) : static_cast<double>(X[static_cast<long long>(m.real_index) * ld + r]);
-    bins16[static_cast<size_t>(w) * rows_stride + row_offset + r] = static_cast<uint16_t>(d_wide_bin(v, m, cats, catbin, wub));
+    bins16[static_cast<size_t>(w) * rows_stride + row_offset + r] = static_cast<uint16_t>(d_value_to_bin(v, m, ub + m.table_off, 1, catbin + m.table_off));
   }
 }
 
@@ -1571,7 +1568,7 @@ __global__ void k_bin_wide(const T* __restrict__ X, long long nrow, int row_majo
 constexpr int kWideThreads = 1024;     // one CTA per SM (128 KB of planes): the loop is latency-bound, so as many rows in flight as the SM allows
 template <int NATOM>
 __global__ void __launch_bounds__(kWideThreads, 1)
-k4_hist_wide(const uint16_t* __restrict__ bins16, size_t rows_stride, const WideMeta* __restrict__ wm, const int4* __restrict__ qgh,
+k4_hist_wide(const uint16_t* __restrict__ bins16, size_t rows_stride, const FeatMeta* __restrict__ wmeta, const int4* __restrict__ qgh,
              const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1, const HistWork* __restrict__ work,
              unsigned long long* __restrict__ hist) {
   extern __shared__ __align__(16) unsigned wplane[];        // [NATOM][nb_pad]
@@ -1580,8 +1577,8 @@ k4_hist_wide(const uint16_t* __restrict__ bins16, size_t rows_stride, const Wide
   if (n <= 0) return;
   const int active = min(static_cast<int>(gridDim.x), (n + 4095) / 4096);
   if (static_cast<int>(blockIdx.x) >= active) return;
-  const WideMeta m = wm[blockIdx.y];
-  const unsigned lo = blockIdx.z * kWideHistSeg;              // this CTA accumulates bins [lo, lo + nb) of the feature
+  const FeatMeta m = wmeta[blockIdx.y];      // wmeta = meta + nfn
+  const unsigned lo = blockIdx.z * kWideHistSeg;             // this CTA accumulates bins [lo, lo + nb) of the feature
   if (static_cast<int>(lo) >= m.num_bin) return;
   const int nb = min(kWideHistSeg, m.num_bin - static_cast<int>(lo));
   const int p0 = static_cast<int>(static_cast<long long>(n) * blockIdx.x / active), p1 = static_cast<int>(static_cast<long long>(n) * (blockIdx.x + 1) / active);
@@ -1659,8 +1656,8 @@ __device__ __forceinline__ void d_block_excl3(long long& a, long long& b, long l
 // kMono (monotone constraints): every gain, in both passes, is d_mono_split_gain's at outputs clamped to the leaf's bounds, 0 when they
 // break the feature's direction `mono`; min_gain_shift stays the leaf's unconstrained gain.
 template <bool kExtra, bool kMono>
-__device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ hist, const WideMeta m, const LeafState& L, double inv_g, double inv_h,
-                                                  const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr, int mono) {
+__device__ __noinline__ void d_scan_numeric(const long long* __restrict__ hist, const FeatMeta m, const LeafState& L, double inv_g, double inv_h,
+                                            const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr, int mono) {
   __shared__ long long s_sc[24];
   __shared__ double s_bg[8], s_blg[8], s_blh[8];
   __shared__ int s_bt[8], s_blc[8], s_any, s_stop[2];
@@ -1806,6 +1803,48 @@ __device__ __noinline__ void d_scan_wide_numeric(const long long* __restrict__ h
   }
 }
 
+// ---- steps shared by the split scans k_scan and k_scan_wide (one block per (smaller|larger leaf, feature))
+// the candidate of a feature that is not scanned, or before its scan found a split
+__device__ __forceinline__ SplitCand d_empty_cand(int u) {
+  SplitCand out;
+  out.gain = kNegInf; out.left_g = 0; out.left_h = 0; out.threshold = 0; out.left_count = 0; out.default_left = 1; out.feature = u;
+  out.l2_extra = 0; out.is_cat = 0; out.cat_list_len = 0;
+  for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
+  return out;
+}
+// one thread: the candidate of (leaf `which`, feature u) and, for extra_trees, the scan's number of draws (see d_lcg_next), then a fence
+// that makes both visible to the block that runs the pick step
+template <bool kExtra>
+__device__ __forceinline__ void d_publish_cand(SplitCand* cands, unsigned* xrand, const SplitParams& p, int which, int u, const SplitCand& out,
+                                               int drew) {
+  cands[which * p.nf_pad + u] = out;
+  if (kExtra) xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = static_cast<unsigned>(drew);
+  __threadfence();
+}
+// a feature's histogram column of n (g,h) pairs reduced into the leaf's pool slot: the smaller leaf's (which = 0) is H's, the larger's is
+// parent - H (exact int64).  Ends with a barrier: the scan reads pairs other threads of the block reduced.
+__device__ __forceinline__ void d_reduce_column(const long long* __restrict__ src, long long* __restrict__ dst, int n, int which) {
+  for (int b = threadIdx.x; b < n; b += blockDim.x) {
+    longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
+    if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
+    *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
+  }
+  __syncthreads();
+}
+// a numerical feature u scanned by this block: extra_trees' draw from the feature's stream state xr (for the larger leaf already past the
+// smaller leaf's draw, d_smaller_drew), the two-pass scan of its reduced histogram, and a monotone feature's candidate gain times
+// d_mono_penalty at the leaf's depth.  Returns the number of draws taken.
+template <bool kExtra, bool kMono>
+__device__ __forceinline__ int d_scan_numeric_feature(const long long* __restrict__ hist, const FeatMeta& m, int u, const LeafState& L, double inv_g,
+                                                      double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* out, unsigned xr,
+                                                      const ConstraintArgs& cons) {
+  const int rand_thr = kExtra ? d_extra_draw(&xr, m.num_bin - 2) : 0;
+  const int mono = kMono ? cons.type[u] : 0;
+  d_scan_numeric<kExtra, kMono>(hist, m, L, inv_g, inv_h, p, flag, out, rand_thr, mono);
+  if (kMono && mono != 0 && threadIdx.x == 0) out->gain *= d_mono_penalty(L.depth, cons.penalty);
+  return m.num_bin > 2 ? 1 : 0;
+}
+
 // order of the wide categorical selection: side 0 ascending (key, bin), side 1 descending
 __device__ __forceinline__ bool d_sel_prec(int side, double k, int b, double rk, int rb) {
   return side == 0 ? (k < rk || (k == rk && b < rb)) : (k > rk || (k == rk && b > rb));
@@ -1838,30 +1877,26 @@ __device__ __noinline__ void d_block_bitonic2(double* k, int* id, int stride, in
 // (smaller|larger, feature).  The histogram is reduced into the leaf's pool slot (parent - smaller for the larger child), the
 // max_cat_threshold smallest and largest ctr = g / (h + cat_smooth) among the bins that hold >= cat_smooth rows are selected in the
 // (ctr, bin) order of the reference's stable sort, and thread 0 accumulates from both ends exactly like the sequential code.
-// kMono (monotone constraints): constrained gains as in d_scan_wide_numeric / d_scan_feature_cat, and a monotone numerical feature's
+// kMono (monotone constraints): constrained gains as in d_scan_numeric / d_scan_feature_cat, and a monotone numerical feature's
 // candidate gain times d_mono_penalty at the leaf's depth.
 template <bool kExtra, bool kMono>
 __global__ void __launch_bounds__(256)
-k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const WideMeta* __restrict__ wm, const long long* __restrict__ H,
+k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const FeatMeta* __restrict__ meta, const long long* __restrict__ H,
             long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
             unsigned* __restrict__ xrand, ConstraintArgs cons) {
   extern __shared__ __align__(16) unsigned char sw_smem[];
   double* s_key = reinterpret_cast<double*>(sw_smem);                          // [num_bin] ctr keys of the used bins, +inf otherwise
   __shared__ int s_used;
-  const int which = blockIdx.y, w = blockIdx.x, u = p.nfn + w;
+  const int which = blockIdx.y, u = p.nfn + blockIdx.x;
   const int leaf = which ? ctrl->larger : ctrl->smaller;
   if (!ctrl->go || leaf < 0) return;
-  SplitCand out;
-  out.gain = kNegInf; out.left_g = 0; out.left_h = 0; out.threshold = 0; out.left_count = 0; out.default_left = 0; out.feature = u;
-  out.l2_extra = 0; out.is_cat = 1; out.cat_list_len = 0;
-  for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
+  SplitCand out = d_empty_cand(u);
   uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
-  unsigned* draws = xrand + static_cast<size_t>(1 + which) * p.nf_pad + u;      // extra_trees: this scan's draw count (see d_lcg_next)
   if (!*flag) {
-    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 0u; __threadfence(); }
+    if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, 0);
     return;
   }
-  const WideMeta m = wm[w];
+  const FeatMeta m = meta[u];
   const LeafState& L = leaves[leaf];
   const double inv_g = ctrl->inv_g, inv_h = ctrl->inv_h;
   long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(m.hist_off) * 2;
@@ -1869,30 +1904,15 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
-  unsigned xr = kExtra ? xrand[u] : 0u;      // the stream state before this round's draws of the feature
-  if (!m.is_cat) {        // wide numerical feature (max_bin > 255): reduce into the pool slot, then the block-wide two-pass scan
-    for (int b = threadIdx.x; b < m.num_bin; b += blockDim.x) {
-      longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
-      if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
-      *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
-    }
-    __syncthreads();      // every thread reads bins other threads reduced (same block: visible after the barrier)
-    int rand_thr = 0;
-    if (kExtra) {      // more than 256 bins: both leaves draw, the smaller first
-      if (which) xr = d_lcg_next(xr);
-      rand_thr = d_extra_draw(&xr, m.num_bin - 2);
-    }
-    const int mt = kMono ? cons.type[u] : 0;
-    d_scan_wide_numeric<kExtra, kMono>(dst, m, L, inv_g, inv_h, p, flag, &out, rand_thr, mt);
-    if (threadIdx.x == 0) {
-      if (kMono && mt != 0) out.gain *= d_mono_penalty(L.depth, cons.penalty);
-      cands[which * p.nf_pad + u] = out; if (kExtra) *draws = 1u; __threadfence();
-    }
+  // extra_trees: the stream state before this scan's draw (see d_smaller_drew); every categorical feature here is many-vs-many
+  unsigned xr = kExtra ? xrand[u] : 0u;
+  if (kExtra && which && d_smaller_drew(src, m, ctrl, leaves, p, min(p.max_cat_threshold, kCatListMax))) xr = d_lcg_next(xr);
+  if (!m.is_categorical) {        // wide numerical feature (max_bin > 255): reduce into the pool slot, then the block-wide two-pass scan
+    d_reduce_column(src, dst, m.num_bin, which);
+    const int drew = d_scan_numeric_feature<kExtra, kMono>(dst, m, u, L, inv_g, inv_h, p, flag, &out, xr, cons);
+    if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, drew);
     return;
   }
-  // the larger leaf's draw comes after the smaller's, if that one drew
-  if (kExtra && which && d_smaller_drew_cat(src, m.num_bin, leaves[ctrl->smaller], inv_h, p, min(p.max_cat_threshold, kCatListMax)))
-    xr = d_lcg_next(xr);
   // ---- reduce into the pool slot and build the ctr keys (loads of 4 bins in flight per thread before the dependent stores)
   if (threadIdx.x == 0) s_used = 0;
   __syncthreads();
@@ -2038,27 +2058,15 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   __syncthreads();
   if (lane == 0 && warp < 2) {
     const int d = warp;
-    int cnt_cur_group = 0, left_count = 0;
-    double slg = 0.0, slh = kEpsD;
-    for (int i = 0; i < used_bin && i < max_num_cat; ++i) {
-      const double g = s_selg[d][i], h = s_selh[d][i];
-      const int cnt = static_cast<int>(h * cnt_factor + 0.5);
-      slg += g; slh += h; left_count += cnt; cnt_cur_group += cnt;
-      if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) continue;
-      const int right_count = num_data - left_count;
-      if (right_count < p.min_data_in_leaf || right_count < p.min_data_per_group) break;
-      const double srh = sum_h - slh;
-      if (srh < p.min_sum_hessian) break;
-      if (cnt_cur_group < p.min_data_per_group) continue;
-      cnt_cur_group = 0;
-      if (kExtra && i != rand_i) continue;
-      s_plg[d][i] = slg; s_plh[d][i] = slh; s_plc[d][i] = left_count; s_pgain[d][i] = 0.0;      // 0.0 = "evaluate me"
-    }
+    int i = 0;
+    d_cat_walk<kExtra>(used_bin, max_num_cat, num_data, sum_h, cnt_factor, p, rand_i,
+                       [&](double* g, double* h) { *g = s_selg[d][i]; *h = s_selh[d][i]; ++i; },
+                       [&](int j, double slg, double slh, double, int left_count) {
+                         s_plg[d][j] = slg; s_plh[d][j] = slh; s_plc[d][j] = left_count; s_pgain[d][j] = 0.0;      // 0.0 = "evaluate me"
+                       });
   }
   __syncthreads();
-  SplitParams pshift = p;
-  if (!(p.max_delta_step > 0)) pshift.max_delta_step = 0;
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, pshift) + p.min_gain_to_split;
+  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
   if (threadIdx.x < 2 * kCatListMax) {
     const int d = threadIdx.x / kCatListMax, i = threadIdx.x % kCatListMax;
     if (s_pgain[d][i] == 0.0) {
@@ -2088,9 +2096,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
     out.cat_list_len = best_i + 1;
     for (int i = 0; i <= best_i && i < kCatListMax; ++i) out.cat_list[i] = s_sel[best_dir == 1 ? 0 : 1][i];
   }
-  cands[which * p.nf_pad + u] = out;
-  if (kExtra) *draws = static_cast<unsigned>(drew);
-  __threadfence();
+  d_publish_cand<kExtra>(cands, xrand, p, which, u, out, drew);
 }
 
 // A bundle member's histogram out of its bundle column, by the member's k_scan block (thread t = column slot t).  The member's slots of
@@ -2136,7 +2142,7 @@ __device__ __noinline__ void d_unbundle_hist(const long long* __restrict__ src, 
 
 // ---------------------------------------------------------------- K5/K6 for the tile features: one BLOCK per (smaller|larger, feature)
 // Thread t = bin t.  The block reduces the feature into the leaf's pool slot (larger child: parent - smaller, exact int64), then runs the
-// same block-wide two-pass scan as the wide numerical features (d_scan_wide_numeric with one bin per thread: exclusive block scans of
+// same block-wide two-pass scan as the wide numerical features (d_scan_numeric with one bin per thread: exclusive block scans of
 // (g, h, count), one candidate per thread and direction, block argmax with the sequential tie-breaks) — the dependent chain of software
 // fp64 divisions per thread is 2 long instead of 16 as in the round-1 warp-per-feature scan, and the code is shared and small (the old
 // kernel was instruction-fetch bound).  Categorical tile features keep the warp-level search (d_scan_feature_cat) on warp 0.  The block that
@@ -2238,7 +2244,7 @@ __device__ __noinline__ void d_extra_commit(const TreeCtrl* ctrl, unsigned* xran
   }
 }
 
-// kMono (monotone constraints): the constrained scans (d_scan_wide_numeric, d_scan_feature_cat), a monotone feature's candidate gain
+// kMono (monotone constraints): the constrained scans (d_scan_numeric, d_scan_feature_cat), a monotone feature's candidate gain
 // times d_mono_penalty at the leaf's depth, and outputs clamped to the leaf's bounds in the pick step.
 template <int kMode, bool kExtra = false, bool kMono = false>
 __global__ void __launch_bounds__(256, 4)
@@ -2254,10 +2260,8 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
   const int leaf = which ? ctrl->larger : ctrl->smaller;
   const int u = blockIdx.x;
   if (ctrl->go && leaf >= 0 && u < p.nfn) {
-    SplitCand out;
-    out.gain = kNegInf; out.left_g = 0; out.left_h = 0; out.threshold = 0; out.left_count = 0; out.default_left = 1; out.feature = u;
-    out.l2_extra = 0; out.is_cat = 0; out.cat_list_len = 0;
-    for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
+    SplitCand out = d_empty_cand(u);
+    int drew = 0;      // extra_trees: this scan's number of draws (0 when the feature is not scanned)
     if constexpr (kMode == kScanGlobal) {
       int col = -1;
       for (int k = 0; k < vote.top_k; ++k) if (vote.voted[which * vote.top_k + k] == u) col = which * vote.top_k + k;
@@ -2272,8 +2276,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
           hist = reinterpret_cast<const long long*>(scan_ws);
         }
         if (!fm.is_categorical) {
-          const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-          d_scan_wide_numeric<false, false>(hist, wm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, 0, 0);
+          d_scan_numeric<false, false>(hist, fm, L, ctrl->inv_g, ctrl->inv_h, p, &s_no_flag, &out, 0, 0);
         } else if (threadIdx.x < 32) {
           long long qg[8], qh[8];
 #pragma unroll
@@ -2290,11 +2293,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
         const bool bundled = bundle_base && bundle_base[u] >= 0;
         __shared__ longlong2 s_leaf_tot;      // kScanLocal, bundle member: the leaf's local total from d_unbundle_hist
         if (!bundled) {
-          const int b = threadIdx.x;
-          longlong2 sv = *reinterpret_cast<const longlong2*>(src + b * 2);
-          if (which) { const longlong2 pr = *reinterpret_cast<const longlong2*>(dst + b * 2); sv.x = pr.x - sv.x; sv.y = pr.y - sv.y; }
-          *reinterpret_cast<longlong2*>(dst + b * 2) = sv;
-          __syncthreads();      // the scan reads bins other threads of this block reduced
+          d_reduce_column(src, dst, 256, which);      // the whole storage column: k_vote_pack reads whole columns of the pool
         } else {
           d_unbundle_hist(src, dst, fm.num_bin, fm.default_bin, bundle_base[u], which, leaves + leaf, reinterpret_cast<longlong2*>(scan_ws),
                           nullptr, kMode == kScanLocal ? &s_leaf_tot : nullptr);
@@ -2314,37 +2313,21 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
         }
         const LeafState& L = kMode == kScanLocal ? Lloc : leaves[leaf];
         if (*flag) {
-          // extra_trees: the stream state before this scan's draw — past the smaller leaf's draw for the larger leaf's block.  Both leaves
-          // hold the same pre-scan flag (inherited from their parent), so the smaller one scanned this feature too; it drew unless its range
-          // was empty, which only the many-vs-many categorical search decides from the data: the smaller leaf's used bins, counted in H.
+          // extra_trees: the stream state before this scan's draw (see d_smaller_drew)
           unsigned xr = kExtra ? xrand[u] : 0u;
-          if (kExtra && which) {
-            bool smaller_drew = fm.is_categorical ? fm.num_bin > 1 : fm.num_bin > 2;
-            if (fm.is_categorical && fm.num_bin > p.max_cat_to_onehot)
-              smaller_drew = d_smaller_drew_cat(src, fm.num_bin, leaves[ctrl->smaller], ctrl->inv_h, p, p.max_cat_threshold);
-            if (smaller_drew) xr = d_lcg_next(xr);
-          }
-          int drew = 0;
+          if (kExtra && which && d_smaller_drew(src, fm, ctrl, leaves, p, p.max_cat_threshold)) xr = d_lcg_next(xr);
           if (!fm.is_categorical) {
-            const WideMeta wm{fm.num_bin, 0, 0, 0, fm.default_bin, fm.missing_type, fm.real_index, 0, fm.offset, 0, 0, 0};
-            const int rand_thr = kExtra ? d_extra_draw(&xr, fm.num_bin - 2) : 0;
-            drew = fm.num_bin > 2 ? 1 : 0;
-            const int mt = kMono ? cons.type[u] : 0;
-            d_scan_wide_numeric<kExtra, kMono>(dst, wm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, rand_thr, mt);
-            if (kMono && mt != 0 && threadIdx.x == 0) out.gain *= d_mono_penalty(L.depth, cons.penalty);
+            drew = d_scan_numeric_feature<kExtra, kMono>(dst, fm, u, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, xr, cons);
           } else if (threadIdx.x < 32) {
             long long qg[8], qh[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) { const int b = threadIdx.x * 8 + j; qg[j] = dst[b * 2]; qh[j] = dst[b * 2 + 1]; }
             drew = d_scan_feature_cat<kExtra, kMono>(qg, qh, threadIdx.x, fm, L, ctrl->inv_g, ctrl->inv_h, p, flag, &out, scan_ws, xr);
           }
-          if (kExtra && threadIdx.x == 0) xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = static_cast<unsigned>(drew);
         }
-      } else if (kExtra && threadIdx.x == 0) {      // not scanned: no draw
-        xrand[static_cast<size_t>(1 + which) * p.nf_pad + u] = 0u;
       }
     }
-    if (threadIdx.x == 0) { cands[which * p.nf_pad + u] = out; __threadfence(); }      // visible to the block that runs the pick step
+    if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, drew);
   }
   __shared__ int s_last;
   __syncthreads();

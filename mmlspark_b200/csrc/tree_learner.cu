@@ -7,6 +7,16 @@ static size_t Align16(size_t x) { return (x + 15) & ~static_cast<size_t>(15); }
 constexpr int kScanSmem = (768 + 64) * 8;         // k_scan: scratch of the categorical split search (one warp per block runs it)
 constexpr int kPartTickets = 8;                   // k_partition: chunks a block takes per ticket (0: one chunk per ticket)
 
+// The split scans of one (extra_trees, monotone constraints) pair, indexed [extra_trees][monotone].  Each pair has its own instantiations,
+// so that the default one compiles to what it was without either.
+struct ScanKernels {
+  decltype(&k_scan<kScanPlain>) scan;
+  decltype(&k_scan_wide<false, false>) scan_wide;
+};
+static const ScanKernels kScanKernels[2][2] = {
+    {{k_scan<kScanPlain, false, false>, k_scan_wide<false, false>}, {k_scan<kScanPlain, false, true>, k_scan_wide<false, true>}},
+    {{k_scan<kScanPlain, true, false>, k_scan_wide<true, false>}, {k_scan<kScanPlain, true, true>, k_scan_wide<true, true>}}};
+
 // The device tree blob: the TreeDev fields one after another in this order, each 16-byte aligned, with its element count for L
 // leaves.  The allocation, a stored copy (DART) and the pinned host mirror all take their field pointers from this one list.
 template <typename Fn>
@@ -44,10 +54,11 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   cudaGetLastError();
   B200_CUDA(set_k4_smem_limit());
-  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
-  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
-  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
-  B200_CUDA(cudaFuncSetAttribute(k_scan<kScanPlain, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+  for (const auto& by_mono : kScanKernels)
+    for (const ScanKernels& k : by_mono) {
+      B200_CUDA(cudaFuncSetAttribute(k.scan, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmem));
+      if (train.nw > 0) B200_CUDA(cudaFuncSetAttribute(k.scan_wide, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
+    }
   mono_.Alloc(train.nf_pad);      // allocated whatever monotone_constraints says: a ResetParameter may set them
   sets_of_.Alloc(train.nf_pad);   // and whatever interaction_constraints says
 
@@ -63,10 +74,6 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
       if (sp_.max_cat_to_onehot > 256) Fatal("max_cat_to_onehot > 256 is not supported together with categorical features of more than 256 bins");
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
       B200_CUDA(cudaFuncSetAttribute(k4_hist_wide<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kWideHistSeg * 4));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
-      B200_CUDA(cudaFuncSetAttribute(k_scan_wide<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWideMaxBins * 8));
     }
   }
 
@@ -412,19 +419,20 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
     launch_k4(const_hessian, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
               reinterpret_cast<unsigned long long*>(H_.p), bound, num_sms_, s);
     if (d.nw > 0) {      // the features with more than 256 bins: own sub-histogram layout (k4_hist_wide)
-      int max_nb = 0;
-      for (const WideMeta& wm : d.wide_host) max_nb = std::max(max_nb, wm.num_bin);
+      int max_nb = 0, units = 0;
+      for (int u = d.nfn; u < d.nf; ++u) {
+        max_nb = std::max(max_nb, d.meta_host[u].num_bin);
+        units += (d.meta_host[u].num_bin + kWideHistSeg - 1) / kWideHistSeg;
+      }
       const int segs = (max_nb + kWideHistSeg - 1) / kWideHistSeg;      // z: 8192-bin segments of the largest feature
       // x: row parts, chosen so that the CTAs that have work (a (feature, segment) pair past the feature's last bin exits at once) make
       // about four waves of one CTA per SM (128 KB of shared memory each)
-      int units = 0;
-      for (const WideMeta& wm : d.wide_host) units += (wm.num_bin + kWideHistSeg - 1) / kWideHistSeg;
       const dim3 wgrid(static_cast<unsigned>(std::max(1, std::min(64, 4 * num_sms_ / std::max(1, units)))), static_cast<unsigned>(d.nw), static_cast<unsigned>(segs));
       if (const_hessian)
-        k4_hist_wide<3><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.wide_meta.p, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
+        k4_hist_wide<3><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.meta.p + d.nfn, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
                                                                          reinterpret_cast<unsigned long long*>(H_.p));
       else
-        k4_hist_wide<4><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.wide_meta.p, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
+        k4_hist_wide<4><<<wgrid, kWideThreads, 4 * kWideHistSeg * 4, s>>>(d.bins16.p, d.rows_stride, d.meta.p + d.nfn, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
                                                                          reinterpret_cast<unsigned long long*>(H_.p));
       timing_.launches += 1;
     }
@@ -463,19 +471,15 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
         comm_hist_bytes_ += static_cast<long long>(slot_elems_ * sizeof(long long));
       }
       mark();
+      const ScanKernels& k = kScanKernels[extra_trees_][monotone_];
       if (d.nw > 0) {
-        auto* scan_wide = monotone_ ? (extra_trees_ ? k_scan_wide<true, true> : k_scan_wide<false, true>)
-                                    : (extra_trees_ ? k_scan_wide<true, false> : k_scan_wide<false, false>);
-        scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.wide_meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
-                                                               cons);
+        k.scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
+                                                                 cons);
         timing_.launches += 1;
       }
       // scan + (last block) pick
-      // extra_trees, monotone constraints: the scan's own instantiations, so that the default one compiles to what it was without them
-      auto* scan = monotone_ ? (extra_trees_ ? k_scan<kScanPlain, true, true> : k_scan<kScanPlain, false, true>)
-                             : (extra_trees_ ? k_scan<kScanPlain, true, false> : k_scan<kScanPlain, false, false>);
-      scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
-                                         cons);
+      k.scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
+                                           cons);
       nvtxRangePop();
     }
     mark();

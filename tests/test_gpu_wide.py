@@ -201,7 +201,18 @@ def test_numerical_max_bin_above_255(built, max_bin):
     for f in range(8):
         assert infos[f] == ods.feature_info(f)
         assert ds.upper_bounds(f).tobytes() == ods.upper_bounds(f).tobytes()
-    assert np.array_equal(ds.get_bins16(), ods.bins16())
+    want = ods.bins16()
+    assert np.array_equal(ds.get_bins16(), want)
+    # the same bins from the streamed (sampled columns + pushed rows) and the CSR ingestion paths, NaN and mostly-zero columns included
+    rows = capi.sample_indices(n, 200000, 1)
+    dp = capi.Dataset.from_sampled_columns(X[rows], n, dsp)
+    for off in range(0, n, 64_000):
+        dp.push_rows(X[off:off + 64_000], off)
+    assert np.array_equal(dp.get_bins16(), want)
+    stored = (X != 0) | np.isnan(X)
+    indptr = np.concatenate([[0], np.cumsum(stored.sum(axis=1))]).astype(np.int32)
+    dc = capi.Dataset.from_csr(indptr, np.nonzero(stored)[1].astype(np.int32), X[stored], X.shape[1], dsp)
+    assert np.array_equal(dc.get_bins16(), want)
     params = ("objective=binary boosting_type=gbdt num_leaves=31 learning_rate=0.1 min_data_in_leaf=20 min_sum_hessian_in_leaf=0.001 verbosity=-1 "
               "max_bin=%d is_unbalance=false" % max_bin)
     b = capi.Booster(ds, params)
