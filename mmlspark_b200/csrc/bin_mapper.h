@@ -50,6 +50,9 @@ class LcgRandom {
     return out;
   }
   float NextFloat() { return static_cast<float>((Step() >> 16) & 0x7FFF) / 32768.0f; }
+  // the stream position, so that the device can continue the stream within a tree (TreeLearner, per-node sampling)
+  unsigned state() const { return x_; }
+  void set_state(unsigned x) { x_ = x; }
 
  private:
   unsigned Step() { x_ = 214013u * x_ + 2531011u; return x_; }

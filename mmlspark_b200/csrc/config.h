@@ -35,6 +35,7 @@ struct Config {
   int bagging_freq = 0, bagging_seed = 3;
   double feature_fraction = 1.0;
   int feature_fraction_seed = 2;
+  double feature_fraction_bynode = 1.0;     // < 1: each leaf's split is chosen among a sample of the tree's features (kernels.cuh d_bynode_sample)
   bool extra_trees = false;                 // one random threshold per (leaf, feature) scan (TreeLearner, kernels.cuh K5/K6)
   int extra_seed = 6;                       // the stream of used feature i starts at extra_seed + i
   std::vector<int> monotone_constraints;    // per real feature -1, 0 or +1; non-empty: the constrained scans (TreeLearner, kernels.cuh kMono)
@@ -97,7 +98,8 @@ struct Config {
         {"min_child_weight", "min_sum_hessian_in_leaf"}, {"sub_row", "bagging_fraction"},
         {"subsample", "bagging_fraction"}, {"bagging", "bagging_fraction"}, {"subsample_freq", "bagging_freq"},
         {"bagging_fraction_seed", "bagging_seed"}, {"sub_feature", "feature_fraction"},
-        {"colsample_bytree", "feature_fraction"}, {"extra_tree", "extra_trees"}, {"early_stopping_rounds", "early_stopping_round"},
+        {"colsample_bytree", "feature_fraction"}, {"sub_feature_bynode", "feature_fraction_bynode"},
+        {"colsample_bynode", "feature_fraction_bynode"}, {"extra_tree", "extra_trees"}, {"early_stopping_rounds", "early_stopping_round"},
         {"mc", "monotone_constraints"}, {"monotone_constraint", "monotone_constraints"},
         {"monotone_constraining_method", "monotone_constraints_method"}, {"mc_method", "monotone_constraints_method"},
         {"monotone_splits_penalty", "monotone_penalty"}, {"ms_penalty", "monotone_penalty"}, {"mc_penalty", "monotone_penalty"},
@@ -211,7 +213,8 @@ struct Config {
     D("min_sum_hessian_in_leaf", &min_sum_hessian_in_leaf); D("bagging_fraction", &bagging_fraction);
     D("pos_bagging_fraction", &pos_bagging_fraction); D("neg_bagging_fraction", &neg_bagging_fraction);
     I("bagging_freq", &bagging_freq); I("bagging_seed", &bagging_seed); D("feature_fraction", &feature_fraction);
-    I("feature_fraction_seed", &feature_fraction_seed); I("early_stopping_round", &early_stopping_round);
+    I("feature_fraction_seed", &feature_fraction_seed); D("feature_fraction_bynode", &feature_fraction_bynode);
+    I("early_stopping_round", &early_stopping_round);
     B("extra_trees", &extra_trees); I("extra_seed", &extra_seed);
     S("monotone_constraints_method", &monotone_constraints_method); D("monotone_penalty", &monotone_penalty);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
@@ -285,7 +288,7 @@ struct Config {
     s << "[bagging_fraction: " << Num(bagging_fraction) << "]\n[pos_bagging_fraction: " << Num(pos_bagging_fraction) << "]\n";
     s << "[neg_bagging_fraction: " << Num(neg_bagging_fraction) << "]\n[bagging_freq: " << bagging_freq << "]\n";
     s << "[bagging_seed: " << bagging_seed << "]\n[feature_fraction: " << Num(feature_fraction) << "]\n";
-    s << "[feature_fraction_bynode: 1]\n[feature_fraction_seed: " << feature_fraction_seed << "]\n[extra_trees: " << extra_trees << "]\n[extra_seed: " << extra_seed << "]\n";
+    s << "[feature_fraction_bynode: " << Num(feature_fraction_bynode) << "]\n[feature_fraction_seed: " << feature_fraction_seed << "]\n[extra_trees: " << extra_trees << "]\n[extra_seed: " << extra_seed << "]\n";
     s << "[early_stopping_round: " << early_stopping_round << "]\n[first_metric_only: 0]\n";
     s << "[max_delta_step: " << Num(max_delta_step) << "]\n[lambda_l1: " << Num(lambda_l1) << "]\n[lambda_l2: " << Num(lambda_l2) << "]\n";
     s << "[linear_lambda: 0]\n[min_gain_to_split: " << Num(min_gain_to_split) << "]\n[drop_rate: " << Num(drop_rate) << "]\n";

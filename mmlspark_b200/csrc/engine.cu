@@ -1357,6 +1357,17 @@ static void CheckInteraction(const Config& cfg, const Dataset& train, bool votin
   if (voting_parallel) Fatal(kVotingInteraction);
 }
 
+// the voting learner's local top-k would need every rank's candidates restricted to the leaves' samples; not restated
+static const char* const kVotingByNode = "tree_learner=voting does not support feature_fraction_bynode < 1 with more than one machine; "
+                                         "use tree_learner=data_parallel or feature_fraction_bynode=1";
+
+// per-node feature sampling: the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+static void CheckByNode(const Config& cfg, bool voting_parallel) {
+  const double f = cfg.feature_fraction_bynode;
+  if (!(f > 0.0 && f <= 1.0)) Fatal("feature_fraction_bynode should be in (0, 1], got " + Config::Num(f));
+  if (f < 1.0 && voting_parallel) Fatal(kVotingByNode);
+}
+
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1405,6 +1416,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   }
   CheckMonotone(cfg, *train, voting_);
   CheckInteraction(cfg, *train, voting_);
+  CheckByNode(cfg, voting_);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1747,6 +1759,7 @@ void Booster::ResetParameter(const char* params) {
       if (voting_ && cfg.extra_trees) Fatal(kVotingExtraTrees);
       CheckMonotone(cfg, *train, voting_);
       CheckInteraction(cfg, *train, voting_);
+      CheckByNode(cfg, voting_);
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;

@@ -2,6 +2,7 @@
 // Kernel numbering follows SURVEY.md §2.5.  Everything a tree needs lives in device memory
 // (leaf table, control block, tree arrays) so the host enqueues a whole tree without a sync.
 #pragma once
+#include <climits>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "hist_kernel.cuh"
@@ -133,6 +134,11 @@ struct LeafState {
 // Interaction constraints ([UPSTREAM] ColSampler::GetByNode): sets_of[u], per inner feature, has bit s set when constraint set s holds
 // the feature's real index; feature u may split a leaf iff sets_of[u] & inter_mask != 0.  Read by the pick step only when p.interaction.
 struct ConstraintArgs { const signed char* type; double penalty; const unsigned long long* sets_of; };
+// Per-node feature sampling ([UPSTREAM] ColSampler::GetByNode with feature_fraction_bynode < 1), k_scan's argument: d_bynode_sample
+// writes mask[which][u] = 1 for the features the leaf of the round samples, and the pick step passes over the others.  mask is null
+// without per-node sampling (nothing is read then).  k = GetCnt(|tree sample|, feature_fraction_bynode); order: the used features in
+// real-index order (Dataset::sample_order); tree_used: the tree's feature_fraction sample; work: [2][4][nf_pad] ints of scratch.
+struct NodeSampleArgs { uint8_t* mask; int* work; const int* order; const uint8_t* tree_used; int k; };
 
 struct TreeCtrl {
   int num_leaves, left_leaf, right_leaf, smaller, larger, go, finished, split_leaf;
@@ -153,6 +159,9 @@ struct TreeCtrl {
   int split_wide;              // wide index (inner feature - nfn) of the split feature, or -1
   int split_cat_list_len;
   unsigned short split_cat_list[kCatListMax];
+  // per-node feature sampling: the ColSampler stream's state.  k_tree_init takes it from the host after the tree's feature_fraction
+  // draw, the pick step advances it to col_next (written by d_bynode_sample) each round, and ReadTree hands it back to the host.
+  unsigned col_state, col_next;
 };
 
 struct TreeDev {               // SoA tree under construction (sizes: num_leaves / num_leaves-1)
@@ -745,7 +754,7 @@ k_quantize(const float* __restrict__ g, const float* __restrict__ h, int n, int4
 // ---------------------------------------------------------------- tree init / round controller
 __global__ void __launch_bounds__(256)
 k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, SplitParams p, int n_local, const uint8_t* feature_used,
-            int root_is_bag) {
+            int root_is_bag, unsigned col_state) {
   for (int u = threadIdx.x; u < p.nf_pad; u += blockDim.x) flags[u] = (u < p.nf && (!feature_used || feature_used[u])) ? 1 : 0;
   for (int l = threadIdx.x; l < p.num_leaves; l += blockDim.x) {
     leaves[l].best.gain = kNegInf; leaves[l].best.feature = -1;
@@ -760,6 +769,7 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
     r.sum_h = static_cast<double>(ctrl->root_q[1]) * ctrl->inv_h;
     ctrl->num_leaves = 1; ctrl->left_leaf = 0; ctrl->right_leaf = -1; ctrl->smaller = 0; ctrl->larger = -1;
     ctrl->go = 0; ctrl->finished = 0; ctrl->split_leaf = -1; ctrl->pending = 0; ctrl->round = 0; ctrl->trace_rows = 0;
+    ctrl->col_state = col_state;
     *tree.num_leaves = 1;
   }
 }
@@ -1128,10 +1138,12 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
 // over here and only here, after the scans, so the scans, their is_splittable flags and the extra_trees draws are what they are
 // without constraints ([UPSTREAM] SerialTreeLearner::ComputeBestSplitForFeature filters after FindBestThreshold).  The chosen
 // feature's sets_of word is kept for the round controller's mask update.
+// node_mask non-null (per-node feature sampling): likewise a feature the leaf did not sample (written by d_bynode_sample in this kernel)
+// is passed over, and the ColSampler stream moves past the round's draws.
 template <bool kMono>
 __device__ __noinline__ void
 d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p,
-             const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of) {
+             const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of, const uint8_t* node_mask) {
   __shared__ double s_gain[8];
   __shared__ int s_feat[8], s_idx[8];
   const int which = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1141,6 +1153,7 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
     const unsigned long long mask = p.interaction ? leaves[leaf].inter_mask : 0ull;
     for (int u = t; u < p.nf; u += 128) {
       if (p.interaction && !(sets_of[u] & mask)) continue;
+      if (node_mask && !__ldcg(&node_mask[which * p.nf_pad + u])) continue;
       const double cg = __ldcg(&cands[which * p.nf_pad + u].gain);
       const int rf = meta[u].real_index;
       if (cg > bg || (cg == bg && rf < bf)) { bg = cg; bf = rf; bi = u; }
@@ -1187,6 +1200,7 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
     }
     L.best = b;
   }
+  if (node_mask && threadIdx.x == 0 && ctrl->go) ctrl->col_state = __ldcg(&ctrl->col_next);
   __syncthreads();
   if (threadIdx.x < 32 && !ctrl->finished) d_choose_leaf(ctrl, leaves, meta, p, threadIdx.x);
 }
@@ -2244,13 +2258,139 @@ __device__ __noinline__ void d_extra_commit(const TreeCtrl* ctrl, unsigned* xran
   }
 }
 
+// ---------------------------------------------------------------- per-node feature sampling
+// The LCG of Random (d_lcg_next) advanced d steps at once: x -> A x + C, composed from the one-step map by squaring.
+__device__ __forceinline__ void d_lcg_jump_map(unsigned d, unsigned* A, unsigned* C) {
+  unsigned a = 214013u, c = 2531011u, ra = 1u, rc = 0u;
+  for (; d; d >>= 1) {
+    if (d & 1u) { ra = a * ra; rc = a * rc + c; }
+    c = a * c + c; a = a * a;
+  }
+  *A = ra; *C = rc;
+}
+__device__ __forceinline__ unsigned d_lcg_jump(unsigned x, unsigned d) { unsigned A, C; d_lcg_jump_map(d, &A, &C); return A * x + C; }
+// Random::Sample(n, k) (bin_mapper.h LcgRandom::Sample): whether it takes the selection branch, and how many draws it takes
+__device__ __forceinline__ bool d_sample_selects(int n, int k) { return k > 1 && k > (n / log2(static_cast<double>(k))); }
+__device__ __forceinline__ unsigned d_sample_draws(int n, int k) { return (k <= 0 || k >= n) ? 0u : (d_sample_selects(n, k) ? n : k); }
+
+// The node sample of the round's leaf `which` ([UPSTREAM] ColSampler::GetByNode with feature_fraction_bynode < 1), run by one extra
+// block per leaf in the k_scan grid, alongside the scan blocks; the pick step in the kernel's last block reads the masks.
+// - pool: the tree's feature_fraction sample in real-index order, filtered to the features the leaf's interaction mask allows; n = |pool|.
+// - k = min(a.k, n), with a.k = GetCnt(|tree sample|, feature_fraction_bynode) from the host.
+// - the sample is Random::Sample(n, k) on the ColSampler stream: the smaller leaf's from the round's state, the larger leaf's from that
+//   state advanced by the smaller leaf's draws (which depend only on its (n, k)), so both blocks draw at once.  The larger leaf's block
+//   (or the smaller's, when the round has one leaf) writes the state after the round to col_next; the pick step commits it.
+// - selection branch (n draws): warp 0 makes 32 draws at a time, one per lane, from jumps of the stream.  Position i is taken iff
+//   NextFloat() < (k - c) / (n - i), c = positions taken so far.  NextFloat() = m / 32768 with m < 2^15, and a rational a / b with
+//   b < 2^31 that differs from m / 32768 differs by at least 2^-15 / b, more than half an ulp of m / 32768, so the fp64 quotient is
+//   below m / 32768 exactly when a / b is: the test is c < k - floor(m (n - i) / 2^15), a threshold each lane computes on its own.
+//   The lanes' thresholds then pass through the dependent chain c += (c < t) in registers, 32 steps per warp shuffle round.
+// - Floyd's branch (k draws): step s draws v_s in [0, r_s), r_s = n - k + s, and takes v_s unless it is taken already, else r_s.  v_s is
+//   taken before step s iff an earlier step drew the same value (first[v] = the earliest step that drew v), or v_s = r_s' of an earlier
+//   step s' that took its r.  Every thread resolves its steps from those two facts, repeating while any step changes (the chains of
+//   the second kind are short), so no step waits on the one before it.
+__device__ __noinline__ void d_bynode_sample(TreeCtrl* ctrl, const LeafState* leaves, const SplitParams& p,
+                                             const unsigned long long* __restrict__ sets_of, NodeSampleArgs a) {
+  const int which = blockIdx.y;
+  const int leaf = which ? ctrl->larger : ctrl->smaller;
+  if (!ctrl->go || leaf < 0) return;
+  __shared__ int s_warp[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint8_t* mask = a.mask + static_cast<size_t>(which) * p.nf_pad;
+  int* pool = a.work + static_cast<size_t>(which) * 4 * p.nf_pad;
+  int* first = pool + p.nf_pad;
+  int* vs = first + p.nf_pad;
+  int* col = vs + p.nf_pad;
+  const unsigned long long im = p.interaction ? leaves[leaf].inter_mask : ~0ull;
+  const unsigned long long sm = p.interaction ? leaves[ctrl->smaller].inter_mask : ~0ull;
+  int n = 0, n_smaller = 0;
+  for (int i0 = 0; i0 < p.nf; i0 += blockDim.x) {      // ordered compaction of the pool; the same trip count in every thread
+    const int i = i0 + threadIdx.x;
+    bool in = false, in_smaller = false;
+    int u = 0;
+    if (i < p.nf) {
+      u = a.order[i];
+      mask[u] = 0;
+      const bool used = a.tree_used[u] != 0;
+      in = used && (!p.interaction || (sets_of[u] & im));
+      in_smaller = used && (!p.interaction || (sets_of[u] & sm));
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    n_smaller += __syncthreads_count(in_smaller);
+    int at = n + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < warp; ++w) at += s_warp[w];
+    if (in) pool[at] = u;
+    n += __syncthreads_count(in);
+  }
+  const int k = min(a.k, n);
+  unsigned x0 = ctrl->col_state;
+  if (which) x0 = d_lcg_jump(x0, d_sample_draws(n_smaller, min(a.k, n_smaller)));
+  if (threadIdx.x == 0 && (which || ctrl->larger < 0)) ctrl->col_next = d_lcg_jump(x0, d_sample_draws(n, k));
+  if (k <= 0) {
+  } else if (k == n) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) mask[pool[i]] = 1;
+  } else if (d_sample_selects(n, k)) {
+    if (warp == 0) {
+      unsigned Aj, Cj, A32, C32;
+      d_lcg_jump_map(lane + 1, &Aj, &Cj);
+      d_lcg_jump_map(32, &A32, &C32);
+      unsigned base = x0;
+      int c = 0;
+      for (int i0 = 0; i0 < n; i0 += 32) {
+        const int i = i0 + lane;
+        const unsigned m = ((Aj * base + Cj) >> 16) & 0x7fffu;
+        base = A32 * base + C32;
+        const int t = i < n ? k - static_cast<int>((static_cast<unsigned long long>(m) * static_cast<unsigned>(n - i)) >> 15) : INT_MIN;
+        const int u = i < n ? pool[i] : 0;
+        unsigned taken = 0u;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int tj = __shfl_sync(0xffffffffu, t, j);
+          const int s = c < tj ? 1 : 0;
+          taken |= static_cast<unsigned>(s) << j;
+          c += s;
+        }
+        if ((taken >> lane) & 1u) mask[u] = 1;
+      }
+    }
+  } else {
+    const int r0 = n - k;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) first[i] = INT_MAX;
+    __syncthreads();
+    unsigned A, C;
+    d_lcg_jump_map(blockDim.x, &A, &C);
+    unsigned x = d_lcg_jump(x0, threadIdx.x + 1);
+    for (int s = threadIdx.x; s < k; s += blockDim.x) {
+      const int v = static_cast<int>((x & 0x7fffffffu) % static_cast<unsigned>(r0 + s));
+      vs[s] = v;
+      atomicMin(&first[v], s);
+      x = A * x + C;
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < k; s += blockDim.x) col[s] = first[vs[s]] < s ? 1 : 0;
+    for (;;) {
+      __syncthreads();
+      int changed = 0;
+      for (int s = threadIdx.x; s < k; s += blockDim.x) {
+        const int v = vs[s];
+        if (!col[s] && v >= r0 && *reinterpret_cast<volatile int*>(&col[v - r0])) { col[s] = 1; changed = 1; }
+      }
+      if (!__syncthreads_or(changed)) break;
+    }
+    for (int s = threadIdx.x; s < k; s += blockDim.x) mask[pool[col[s] ? r0 + s : vs[s]]] = 1;
+  }
+  __threadfence();      // every thread's mask bytes, before thread 0 takes the kernel's scan ticket
+}
+
 // kMono (monotone constraints): the constrained scans (d_scan_numeric, d_scan_feature_cat), a monotone feature's candidate gain
 // times d_mono_penalty at the leaf's depth, and outputs clamped to the leaf's bounds in the pick step.
 template <int kMode, bool kExtra = false, bool kMono = false>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
-       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, ConstraintArgs cons) {
+       SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, ConstraintArgs cons,
+       NodeSampleArgs node) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
@@ -2328,6 +2468,8 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
       }
     }
     if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, drew);
+  } else if constexpr (kMode == kScanPlain) {
+    if (node.mask && u == static_cast<int>(gridDim.x) - 1) d_bynode_sample(ctrl, leaves, p, cons.sets_of, node);      // the grid's extra column
   }
   __shared__ int s_last;
   __syncthreads();
@@ -2342,7 +2484,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
     else {
       if constexpr (kExtra) d_extra_commit(ctrl, xrand, p);
-      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, cons.type, cons.sets_of);
+      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, cons.type, cons.sets_of, node.mask);
     }
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
   }

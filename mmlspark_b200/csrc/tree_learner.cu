@@ -7,6 +7,9 @@ static size_t Align16(size_t x) { return (x + 15) & ~static_cast<size_t>(15); }
 constexpr int kScanSmem = (768 + 64) * 8;         // k_scan: scratch of the categorical split search (one warp per block runs it)
 constexpr int kPartTickets = 8;                   // k_partition: chunks a block takes per ticket (0: one chunk per ticket)
 
+// ColSampler's GetCnt: the size of a feature sample ([UPSTREAM] ColSampler::GetCnt)
+static int SampleCount(int total, double fraction) { return std::max(static_cast<int>(total * fraction + 0.5), std::min(2, total)); }
+
 // The split scans of one (extra_trees, monotone constraints) pair, indexed [extra_trees][monotone].  Each pair has its own instantiations,
 // so that the default one compiles to what it was without either.
 struct ScanKernels {
@@ -61,6 +64,9 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
     }
   mono_.Alloc(train.nf_pad);      // allocated whatever monotone_constraints says: a ResetParameter may set them
   sets_of_.Alloc(train.nf_pad);   // and whatever interaction_constraints says
+  // and whatever feature_fraction_bynode says: the node masks, the sampler's scratch and the used features in real-index order
+  node_mask_.Alloc(2 * static_cast<size_t>(train.nf_pad)); node_work_.Alloc(8 * static_cast<size_t>(train.nf_pad));
+  real_order_.Alloc(train.nf_pad); real_order_.Upload(train.sample_order.data(), train.nf, stream_);
 
   ResetConfig(cfg);
   sp_.num_leaves = L; sp_.parallel = parallel_ ? 1 : 0;
@@ -174,6 +180,11 @@ void TreeLearner::ResetConfig(const Config& cfg) {
     sets_of_host_ = std::move(sets);
     sets_of_.Upload(sets_of_host_.data(), sets_of_host_.size(), stream_);
   }
+  // per-node feature sampling: K from the size of the tree's sample, which is fixed by feature_fraction.  Never on for the voting
+  // learner (Booster rejects feature_fraction_bynode < 1 for it).
+  bynode_ = !voting_ && cfg.feature_fraction_bynode < 1.0;
+  const int pool = cfg.feature_fraction < 1.0 ? SampleCount(train_.nf, cfg.feature_fraction) : train_.nf;
+  bynode_k_ = bynode_ ? SampleCount(pool, cfg.feature_fraction_bynode) : 0;
 }
 
 // extra_trees streams (kernels.cuh d_lcg_next): used feature i in real-index order starts at extra_seed + i.  One small kernel on the
@@ -189,7 +200,7 @@ TreeDev TreeLearner::TreeAt(unsigned char* blob) const { return TreeBlobAt(blob,
 void TreeLearner::ResetFeaturesByTree() {
   if (cfg_.feature_fraction >= 1.0) return;
   const int total = train_.nf;
-  int cnt = std::max(static_cast<int>(total * cfg_.feature_fraction + 0.5), std::min(2, total));
+  const int cnt = SampleCount(total, cfg_.feature_fraction);
   std::fill(feature_used_host_.begin(), feature_used_host_.end(), 0);
   for (int i : col_rand_.Sample(total, cnt)) feature_used_host_[train_.sample_order[i]] = 1;      // the draw indexes the used features in real-index order
   // no host sync: the copy is ordered after the previous tree's kernels on the same stream, and a copy from pageable memory is staged
@@ -394,11 +405,14 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
   ResetFeaturesByTree();
   if (bag)      // the root leaf is the ascending in-bag row list (SetBaggingData); partitions then ping-pong idx0/idx1 as usual
     B200_CUDA(cudaMemcpyAsync(idx0_.p, bag->rows, static_cast<size_t>(bag->count) * sizeof(int), cudaMemcpyDeviceToDevice, s));
-  k_tree_init<<<1, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, flags_.p, sp_, rows_, feature_used_.p, bag ? 1 : 0);
+  // the ColSampler stream passes to the device after the tree's feature_fraction draw (ReadTree takes it back)
+  k_tree_init<<<1, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, flags_.p, sp_, rows_, feature_used_.p, bag ? 1 : 0, col_rand_.state());
   nvtxRangePop();
   timing_.launches += 4;
   const int pgrid = std::max(1, std::min(n / kPartChunk + 1, part_max_blocks_));
-  const dim3 sgrid(std::max(1, d.nfn), 2);      // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates
+  // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates.  Per-node feature
+  // sampling adds one column: each leaf's d_bynode_sample block
+  const dim3 sgrid(std::max(1, d.nfn) + (bynode_ ? 1 : 0), 2);
   const RowBlockBound bound = d.BlockBound();
   SplitParams sp_local = sp_;      // voting: the local scan's config ([UPSTREAM] VotingParallelTreeLearner::Init local_config_)
   if (voting_) { sp_local.min_data_in_leaf /= Net().world; sp_local.min_sum_hessian /= Net().world; }
@@ -448,7 +462,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
       const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
       k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p,
-                                                        cons);
+                                                        cons, NodeSampleArgs{});
       mark();
       Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
       mark();
@@ -459,7 +473,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
       mark();
       k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p,
-                                                         cons);
+                                                         cons, NodeSampleArgs{});
       nvtxRangePop();
       comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
       comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
@@ -478,8 +492,9 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
         timing_.launches += 1;
       }
       // scan + (last block) pick
+      const NodeSampleArgs node = bynode_ ? NodeSampleArgs{node_mask_.p, node_work_.p, real_order_.p, feature_used_.p, bynode_k_} : NodeSampleArgs{};
       k.scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
-                                           cons);
+                                           cons, node);
       nvtxRangePop();
     }
     mark();
@@ -520,6 +535,7 @@ void TreeLearner::ReadTree(HostTree* out) {
     hist_events_.clear();
   }
   timing_.hist_rows += ctrl_host_->trace_rows;
+  col_rand_.set_state(ctrl_host_->col_state);      // the ColSampler stream after the tree's per-node draws (none without them)
   // ---- host copy of the tree
   const TreeDev t = TreeAt(tree_host_);
   const int nl = *t.num_leaves;

@@ -58,6 +58,11 @@ class TreeLearner {
   DevBuf<signed char> mono_;
   std::vector<unsigned long long> sets_of_host_;      // [nf_pad] each inner feature's interaction-constraint sets, as uploaded to sets_of_
   DevBuf<unsigned long long> sets_of_;
+  bool bynode_ = false;            // feature_fraction_bynode < 1 as of the last ResetConfig: the k_scan grid's sampler column
+  int bynode_k_ = 0;               // its sample size K
+  DevBuf<uint8_t> node_mask_;      // per-node feature sampling: [2][nf_pad] the round's leaf samples (kernels.cuh d_bynode_sample)
+  DevBuf<int> node_work_;          // [2][4][nf_pad] the sampler's scratch
+  DevBuf<int> real_order_;         // [nf_pad] Dataset::sample_order: the used features in real-index order
   int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
@@ -95,7 +100,7 @@ class TreeLearner {
   std::vector<int> slot_col_;              // column cache: storage column held by each slot, -1: free (empty for the full copy)
   std::vector<long long> col_splits_;      // column cache: splits on each storage column so far
   long long cache_builds_ = 0, cache_evictions_ = 0;
-  LcgRandom col_rand_{2};                  // ColSampler (feature_fraction)
+  LcgRandom col_rand_{2};                  // ColSampler (feature_fraction; the device continues it within a tree for feature_fraction_bynode)
   std::vector<uint8_t> feature_used_host_;
   DevBuf<uint8_t> feature_used_;
   // percentile objectives: sort buffers of the renewal pass (renew_kernel.cuh)

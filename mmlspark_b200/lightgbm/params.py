@@ -44,6 +44,7 @@ COMMON_DEFAULTS = dict(
     extraTrees=False, extraSeed=6,      # LightGBM 3.2's extra_trees / extra_seed (not a param of the reference's estimators)
     monotoneConstraints=(), monotoneConstraintsMethod="basic", monotonePenalty=0.0,      # monotone_constraints (per feature -1/0/1) etc.
     interactionConstraints=(),          # interaction_constraints: lists of feature indices; a branch splits on features of one list only
+    featureFractionByNode=1.0,          # feature_fraction_bynode: the share of the tree's features each leaf's split is chosen from
     delegate=None,
     # column params (core/contracts/Params.scala:93-208 + Spark ML)
     featuresCol="features", labelCol="label", predictionCol="prediction", weightCol=None, initScoreCol=None,
@@ -130,6 +131,8 @@ class TrainParams:
                 ",".join(str(int(c)) for c in p["monotoneConstraints"]), p["monotoneConstraintsMethod"], scala_double(p["monotonePenalty"]))
         if len(p["interactionConstraints"]) > 0:      # only when given, so every other parameter string stays as the reference builds it
             s += "interaction_constraints=%s " % ",".join("[%s]" % ",".join(str(int(f)) for f in c) for c in p["interactionConstraints"])
+        if p["featureFractionByNode"] != 1.0:      # only when set, so every other parameter string stays as the reference builds it
+            s += "feature_fraction_bynode=%s " % scala_double(p["featureFractionByNode"])
         return s
 
     def to_string(self):
