@@ -1,5 +1,6 @@
-"""NumPy restatement of LightGBM 3.2's extremely randomised trees (`extra_trees`, `extra_seed`) on top of split_scan_ref.py, used to pin the
-engine's scans (k_scan, k_scan_wide with kExtra) tree by tree and tree after tree.
+"""NumPy restatement of LightGBM 3.2's extremely randomised trees (`extra_trees`, `extra_seed`) on top of split_scan_ref.py, the rule
+tree_ref.grow_tree applies with `streams`, used to pin the engine's scans (k_scan, k_scan_wide with kExtra) tree by tree and tree after
+tree.
 
 Restated from LightGBM 3.2 (FeatureHistogram's USE_RAND branch, HistogramPool::SetFeatureInfo); not checked against the native library:
 - Used feature i (its position among the used features in real-index order) owns Random(extra_seed + i): x = 214013 x + 2531011,
@@ -16,8 +17,6 @@ Restated from LightGBM 3.2 (FeatureHistogram's USE_RAND branch, HistogramPool::S
 The filtered scans are taken from split_scan_ref's full scans: those record every candidate that passed the count and hessian tests
 before the pass ended, which is exactly the set the random threshold is tested against."""
 import math
-
-import numpy as np
 
 import split_scan_ref as ref
 
@@ -149,112 +148,10 @@ def find_best_categorical(hg, hh, num_bin, sum_g, sum_h_in, num_data, p, feature
 
 
 class Streams:
-    """the per-feature Random of every used feature; `features` in real-index order"""
+    """the per-feature Random of every used feature, numbered in real-index order"""
 
     def __init__(self, features, extra_seed):
-        self.rand = {f.real_index: Random(extra_seed + i) for i, f in enumerate(features)}
+        self.rand = {f.real_index: Random(extra_seed + i) for i, f in enumerate(sorted(features, key=lambda f: f.real_index))}
 
     def draw(self, f, rng):
         return self.rand[f.real_index].next_int(0, rng) if rng > 0 else 0
-
-
-def scan_leaf(bins, g, h, rows, sum_g, sum_h, num_data, features, flags, p, streams, used):
-    """split_scan_ref.scan_leaf with one draw per scanned feature"""
-    out = {}
-    for f in features:
-        if f.real_index not in used or not flags[f.real_index]:
-            continue
-        col = bins[rows, f.real_index].astype(np.int64)
-        hg = np.bincount(col, weights=g[rows], minlength=f.num_bin)
-        hh = np.bincount(col, weights=h[rows], minlength=f.num_bin)
-        if f.is_cat:
-            t = streams.draw(f, categorical_range(hh, f.num_bin, sum_h, num_data, p))
-            out[f.real_index] = find_best_categorical(hg, hh, f.num_bin, sum_g, sum_h, num_data, p, f.real_index, t)
-        else:
-            t = streams.draw(f, numerical_range(f.num_bin))
-            out[f.real_index] = find_best_numerical(hg, hh, f.num_bin, f.missing_type, f.offset, sum_g, sum_h, num_data, p, f.real_index, t)
-    return out
-
-
-def grow_tree(bins, g, h, features, p, num_leaves, extra_trees=False, extra_seed=6, streams=None, used=None):
-    """split_scan_ref.grow_tree with extra_trees: pass `streams` (a Streams) to carry the feature streams from tree to tree; `used`: the
-    real indices the tree's feature_fraction sample holds (None: every feature).  The smaller leaf of a round (fewer rows; the right
-    one on a tie) is scanned first."""
-    if not extra_trees:
-        return ref.grow_tree(bins, g, h, features, p, num_leaves)
-    features = sorted(features, key=lambda f: f.real_index)
-    if streams is None:
-        streams = Streams(features, extra_seed)
-    used = {f.real_index for f in features} if used is None else set(used)
-    n = len(g)
-    by_real = {f.real_index: f for f in features}
-    leaves = [dict(rows=np.arange(n), sum_g=math.fsum(g), sum_h=math.fsum(h), count=n, best=None, value=0.0, weight=0.0,
-                   flags={f.real_index: f.real_index in used for f in features})]
-    T = dict(split_feature=[], threshold_bin=[], default_left=[], is_cat=[], cat_bins=[], split_gain=[], left_child=[], right_child=[],
-             internal_value=[], internal_weight=[], internal_count=[])
-    parent_of = [-1]
-    rounds, picks = [], []
-    new_leaves = [0]
-    while True:
-        counts = [leaves[l]["count"] for l in new_leaves]
-        go = len(leaves) < num_leaves and not all(c < p.min_data_in_leaf * 2 for c in counts)
-        if go:
-            if len(new_leaves) == 2 and not counts[0] < counts[1]:
-                new_leaves = new_leaves[::-1]            # smaller first
-            rnd = []
-            for l in new_leaves:
-                L = leaves[l]
-                scans = scan_leaf(bins, g, h, L["rows"], L["sum_g"], L["sum_h"], L["count"], features, L["flags"], p, streams, used)
-                for fi, s in scans.items():
-                    L["flags"][fi] = s.splittable
-                L["best"] = ref.best_of_leaf(scans)
-                rnd.append((l, L, scans))
-            rounds.append(rnd)
-        else:
-            for l in new_leaves:
-                leaves[l]["best"] = None
-        if len(leaves) >= num_leaves:
-            break
-        picks.append([(li, L["best"]) for li, L in enumerate(leaves) if L["best"] is not None])
-        pick = None
-        for li, L in enumerate(leaves):
-            b = L["best"]
-            if b is not None and (pick is None or ref.better_split(b.gain, b.feature, leaves[pick]["best"].gain, leaves[pick]["best"].feature)):
-                pick = li
-        if pick is None or not leaves[pick]["best"].gain > 0.0:
-            break
-        L, s = leaves[pick], leaves[pick]["best"]
-        f = by_real[s.feature]
-        left = ref.goes_left(bins[L["rows"], f.real_index].astype(np.int64), f, s)
-        sum_h2 = L["sum_h"] + 2 * ref.K_EPS
-        left_out = ref.calc_output(s.left_g, s.left_h, p, s.l2)
-        right_out = ref.calc_output(L["sum_g"] - s.left_g, sum_h2 - s.left_h, p, s.l2)
-        node, nl = len(leaves) - 1, len(leaves)
-        par = parent_of[pick]
-        if par >= 0:
-            if T["left_child"][par] == ~pick:
-                T["left_child"][par] = node
-            else:
-                T["right_child"][par] = node
-        T["split_feature"].append(s.feature); T["threshold_bin"].append(0 if s.is_cat else s.threshold)
-        T["default_left"].append(bool(s.default_left)); T["is_cat"].append(s.is_cat); T["cat_bins"].append(s.cat_bins)
-        T["split_gain"].append(float(np.float32(s.gain + p.min_gain_to_split)))
-        T["left_child"].append(~pick); T["right_child"].append(~nl)
-        T["internal_value"].append(L["value"]); T["internal_weight"].append(L["weight"]); T["internal_count"].append(L["count"])
-        lrows, rrows = L["rows"][left], L["rows"][~left]
-        flags = dict(L["flags"])
-        R = dict(rows=rrows, sum_g=L["sum_g"] - s.left_g, sum_h=sum_h2 - s.left_h - ref.K_EPS, count=len(rrows), best=None,
-                 value=0.0 if math.isnan(right_out) else right_out, weight=sum_h2 - s.left_h - ref.K_EPS, flags=dict(flags))
-        L.update(rows=lrows, sum_g=s.left_g, sum_h=s.left_h - ref.K_EPS, count=len(lrows), best=None,
-                 value=0.0 if math.isnan(left_out) else left_out, weight=s.left_h - ref.K_EPS, flags=flags)
-        leaves.append(R)
-        parent_of[pick] = node
-        parent_of.append(node)
-        new_leaves = [pick, nl]
-    T["num_leaves"] = len(leaves)
-    T["leaf_value"] = [L["value"] if abs(L["value"]) > ref.K_ZERO else 0.0 for L in leaves]
-    T["leaf_weight"] = [L["weight"] for L in leaves]
-    T["leaf_count"] = [L["count"] for L in leaves]
-    T["internal_value"] = [v if abs(v) > ref.K_ZERO else 0.0 for v in T["internal_value"]]
-    T["rounds"], T["picks"], T["scanned_counts"] = rounds, picks, []
-    return T

@@ -8,8 +8,8 @@ Restated from LightGBM 3.2 (FeatureHistogram, SerialTreeLearner):
 - GetLeafGain / CalculateSplittedLeafOutput: L1 soft threshold, L2, max_delta_step; min_gain_shift.
 - FindBestThresholdCategorical: one-hot, and many-vs-many over the bins with >= cat_smooth rebuilt rows, stably sorted by
   g / (h + cat_smooth) and walked from both ends; cat_l2 enters the gains and leaf outputs but not min_gain_shift.
-- The feature choice per leaf (gain, then smaller real feature index), the leaf choice (SplitInfo::operator>, then the first leaf),
-  child sums taken from the split, and is_splittable inheritance (a feature with no valid split in a leaf is skipped in its children).
+- The feature choice per leaf (gain, then smaller real feature index) and the row partition of a split; tree_ref.py grows the trees
+  from them (the leaf choice, child sums taken from the split, is_splittable inheritance).
 
 Histograms are sums of values on a fixed-point grid, so every bin and prefix sum is exact in fp64 and kEpsilon is added once to an exact
 sum, as the engine's int64 histograms do.  (Upstream accumulates kEpsilon + h_1 + h_2 + ... in fp64; that differs only in the rounding of
@@ -244,22 +244,6 @@ class Feature:
         self.real_index, self.num_bin, self.missing_type, self.offset, self.is_cat = real_index, num_bin, missing_type, offset, is_cat
 
 
-def scan_leaf(bins, g, h, rows, sum_g, sum_h, num_data, features, flags, p):
-    """All (feature) searches of one leaf over its rows.  Returns {real_index: Scan} for the features whose flag is set."""
-    out = {}
-    for f in features:
-        if not flags[f.real_index]:
-            continue
-        col = bins[rows, f.real_index].astype(np.int64)
-        hg = np.bincount(col, weights=g[rows], minlength=f.num_bin)
-        hh = np.bincount(col, weights=h[rows], minlength=f.num_bin)
-        if f.is_cat:
-            out[f.real_index] = find_best_categorical(hg, hh, f.num_bin, sum_g, sum_h, num_data, p, f.real_index)
-        else:
-            out[f.real_index] = find_best_numerical(hg, hh, f.num_bin, f.missing_type, f.offset, sum_g, sum_h, num_data, p, f.real_index)
-    return out
-
-
 def best_of_leaf(scans):
     best = None
     for fi in sorted(scans):
@@ -279,89 +263,6 @@ def goes_left(col, f, s):
     if f.missing_type == 2:
         left = np.where(col == f.num_bin - 1, s.default_left, left)
     return left
-
-
-def grow_tree(bins, g, h, features, p, num_leaves):
-    """SerialTreeLearner::Train with learning_rate 1 and no bias: leaves grow best-first; in every round the two new leaves are scanned.
-    bins: [rows][real features] bin indices; g/h: fp64 values on an exact grid.  Returns the tree arrays as the model text prints them
-    (bins instead of threshold values, bin sets instead of categories) plus `rounds`: the scans of every round for the decided check,
-    and `scanned_counts`: the (leaf, row count) pairs each round scanned."""
-    n = len(g)
-    by_real = {f.real_index: f for f in features}
-    all_rows = np.arange(n)
-    leaves = [dict(rows=all_rows, sum_g=math.fsum(g), sum_h=math.fsum(h), count=n, best=None, value=0.0, weight=0.0,
-                   flags={f.real_index: True for f in features})]
-    T = dict(split_feature=[], threshold_bin=[], default_left=[], is_cat=[], cat_bins=[], split_gain=[], left_child=[], right_child=[],
-             internal_value=[], internal_weight=[], internal_count=[])
-    parent_of = [-1]
-    rounds, picks, scanned_counts = [], [], []
-    new_leaves = [0]
-    while True:
-        counts = [leaves[l]["count"] for l in new_leaves]
-        go = len(leaves) < num_leaves and not all(c < p.min_data_in_leaf * 2 for c in counts)
-        if go:
-            rnd = []
-            for l in new_leaves:
-                L = leaves[l]
-                scans = scan_leaf(bins, g, h, L["rows"], L["sum_g"], L["sum_h"], L["count"], features, L["flags"], p)
-                for fi, s in scans.items():
-                    L["flags"][fi] = s.splittable
-                L["best"] = best_of_leaf(scans)
-                rnd.append((l, L, scans))
-            rounds.append(rnd)
-            scanned_counts.append([(l, leaves[l]["count"]) for l in new_leaves])
-        else:
-            for l in new_leaves:
-                leaves[l]["best"] = None
-        if len(leaves) >= num_leaves:
-            break
-        pick = None
-        picks.append([(li, L["best"]) for li, L in enumerate(leaves) if L["best"] is not None])
-        for li, L in enumerate(leaves):
-            b = L["best"]
-            if b is None:
-                continue
-            if pick is None or better_split(b.gain, b.feature, leaves[pick]["best"].gain, leaves[pick]["best"].feature):
-                pick = li
-        if pick is None or not leaves[pick]["best"].gain > 0.0:
-            break
-        L, s = leaves[pick], leaves[pick]["best"]
-        f = by_real[s.feature]
-        col = bins[L["rows"], f.real_index].astype(np.int64)
-        left = goes_left(col, f, s)
-        sum_h2 = L["sum_h"] + 2 * K_EPS
-        left_out = calc_output(s.left_g, s.left_h, p, s.l2)
-        right_out = calc_output(L["sum_g"] - s.left_g, sum_h2 - s.left_h, p, s.l2)
-        node, nl = len(leaves) - 1, len(leaves)
-        par = parent_of[pick]
-        if par >= 0:
-            if T["left_child"][par] == ~pick:
-                T["left_child"][par] = node
-            else:
-                T["right_child"][par] = node
-        T["split_feature"].append(s.feature); T["threshold_bin"].append(0 if s.is_cat else s.threshold)
-        T["default_left"].append(bool(s.default_left)); T["is_cat"].append(s.is_cat); T["cat_bins"].append(s.cat_bins)
-        T["split_gain"].append(float(np.float32(s.gain + p.min_gain_to_split)))
-        T["left_child"].append(~pick); T["right_child"].append(~nl)
-        T["internal_value"].append(L["value"]); T["internal_weight"].append(L["weight"])
-        T["internal_count"].append(L["count"])
-        lrows, rrows = L["rows"][left], L["rows"][~left]
-        flags = dict(L["flags"])
-        R = dict(rows=rrows, sum_g=L["sum_g"] - s.left_g, sum_h=sum_h2 - s.left_h - K_EPS, count=len(rrows), best=None,
-                 value=0.0 if math.isnan(right_out) else right_out, weight=sum_h2 - s.left_h - K_EPS, flags=dict(flags))
-        L.update(rows=lrows, sum_g=s.left_g, sum_h=s.left_h - K_EPS, count=len(lrows), best=None,
-                 value=0.0 if math.isnan(left_out) else left_out, weight=s.left_h - K_EPS, flags=flags)
-        leaves.append(R)
-        parent_of[pick] = node
-        parent_of.append(node)
-        new_leaves = [pick, nl]
-    T["num_leaves"] = len(leaves)
-    T["leaf_value"] = [L["value"] if abs(L["value"]) > K_ZERO else 0.0 for L in leaves]
-    T["leaf_weight"] = [L["weight"] for L in leaves]
-    T["leaf_count"] = [L["count"] for L in leaves]
-    T["internal_value"] = [v if abs(v) > K_ZERO else 0.0 for v in T["internal_value"]]
-    T["rounds"], T["picks"], T["scanned_counts"] = rounds, picks, scanned_counts
-    return T
 
 
 def undecided(T, rel=1e-12, count_margin=1e-9):

@@ -1,4 +1,4 @@
-"""The per-node sampling restatement (bynode_ref.py) on its own: which draws GetByNode takes and when, the sample size rule, both branches
+"""The per-node sampling restatement (bynode_ref.py, grown by tree_ref.py) on its own: which draws GetByNode takes and when, the sample size rule, both branches
 of Random::Sample, the pool with a tree sample and under interaction constraints, the stream position across trees, the exact integer
 form of the selection test the device uses, and the estimators' parameter string."""
 import math
@@ -10,6 +10,7 @@ import bynode_ref as B
 import extra_trees_ref as X3
 import interaction_ref as I
 import split_scan_ref as ref
+import tree_ref
 
 
 def _data(seed, n=4000, nf=6):
@@ -29,9 +30,9 @@ def test_bynode_one_draws_nothing():
     bins, g, h, feats = _data(1)
     p = ref.Params(min_data_in_leaf=20)
     s = B.ColSampler(feats, 1.0, 1.0)
-    T = B.grow_tree(bins, g, h, feats, p, 12, s)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 12, sampler=s)
     assert T["draws"] == 0 and s.rnd.x == 2
-    plain = ref.grow_tree(bins, g, h, feats, p, 12)
+    plain = tree_ref.grow_tree(bins, g, h, feats, p, 12)
     for k in _SHAPE:
         assert T[k] == plain[k], k
     assert all(samp == set(range(6)) for rnd in T["node_rounds"] for _, samp in rnd)
@@ -61,7 +62,7 @@ def test_each_round_samples_from_the_stream():
     bins, g, h, feats = _data(2)
     p = ref.Params(min_data_in_leaf=20)
     s = B.ColSampler(feats, 1.0, 0.5)
-    T = B.grow_tree(bins, g, h, feats, p, 12, s)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 12, sampler=s)
     rounds = T["node_rounds"]
     assert len(rounds) == len(T["rounds"]) and [len(r) for r in rounds] == [len(r) for r in T["rounds"]]
     assert len(rounds[0]) == 1 and all(len(r) == 2 for r in rounds[1:])
@@ -86,7 +87,7 @@ def test_tree_sample_is_the_pool():
     cnt = B.get_cnt(8, 0.6)
     replay.sample(8, cnt)
     for _ in range(3):
-        T = B.grow_tree(bins, g, h, feats, p, 8, s)
+        T = tree_ref.grow_tree(bins, g, h, feats, p, 8, sampler=s)
         tree = replay.sample(8, cnt)
         assert set(tree) == set(s.tree)
         for r in T["node_rounds"]:
@@ -102,7 +103,7 @@ def test_interaction_filters_the_pool_and_caps_k():
     p = ref.Params(min_data_in_leaf=20)
     cons = [[0, 1, 2, 3, 4, 5, 6, 7], [0, 5]]
     s = B.ColSampler(feats, 1.0, 0.5)
-    T = B.grow_tree(bins, g, h, feats, p, 12, s, cons)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 12, sampler=s, constraints=cons)
     sets = I.sets_of(cons, 8)
     saw_capped = False
     replay = X3.Random(2)
@@ -125,13 +126,13 @@ def test_stream_after_an_early_stop_and_depth_gated_rounds():
     bins, g, h, feats = _data(5)
     p = ref.Params(min_data_in_leaf=20, min_gain_to_split=40.0)
     s = B.ColSampler(feats, 1.0, 0.5)
-    T = B.grow_tree(bins, g, h, feats, p, 31, s)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 31, sampler=s)
     assert T["num_leaves"] < 31, "the case must stop early"
     assert T["draws"] == sum(len(r) for r in T["node_rounds"]) * B.sample_draws(6, 3)
     assert len(T["node_rounds"]) == T["num_leaves"], "one round per split, plus the round that found no gain"
     p = ref.Params(min_data_in_leaf=20)
     s = B.ColSampler(feats, 1.0, 0.5)
-    T = B.grow_tree(bins, g, h, feats, p, 31, s, max_depth=2)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 31, sampler=s, max_depth=2)
     assert T["num_leaves"] == 4
     assert len(T["node_rounds"]) == 2 and T["draws"] == 3 * B.sample_draws(6, 3)
 
@@ -189,12 +190,13 @@ def test_estimator_parameter_string():
 
 
 @pytest.mark.parametrize("extra", [False, True])
-def test_growth_equals_interaction_ref_at_one(extra):
-    """with feature_fraction_bynode = 1 the growth here is interaction_ref.grow_tree's, with and without constraints and extra trees"""
+def test_sampler_at_one_grows_the_unsampled_tree(extra):
+    """a sampler at feature_fraction_bynode = 1 grows the tree of no sampler, with and without constraints and extra trees"""
     bins, g, h, feats = _data(6)
     p = ref.Params(min_data_in_leaf=20)
     for cons in (None, [[0, 1, 2], [2, 3, 4, 5]]):
-        T = B.grow_tree(bins, g, h, feats, p, 12, B.ColSampler(feats, 1.0, 1.0), cons, extra, 7)
-        want = I.grow_tree(bins, g, h, feats, p, 12, cons or [list(range(6))], extra, 7)
+        streams = (lambda: X3.Streams(feats, 7)) if extra else (lambda: None)
+        T = tree_ref.grow_tree(bins, g, h, feats, p, 12, sampler=B.ColSampler(feats, 1.0, 1.0), constraints=cons, streams=streams())
+        want = tree_ref.grow_tree(bins, g, h, feats, p, 12, constraints=cons, streams=streams())
         for k in _SHAPE + ("masks", "branches"):
             assert T[k] == want[k], (cons, k)

@@ -4,6 +4,7 @@ import numpy as np
 
 import extra_trees_ref as X3
 import split_scan_ref as ref
+import tree_ref
 
 
 def test_stream_matches_a_published_sequence():
@@ -69,8 +70,8 @@ def test_categorical_scans_evaluate_only_the_drawn_candidate():
 
 
 def test_grow_tree_draw_order_and_seeds():
-    """trees differ by seed, repeat with the same seed, and extra_trees=False is split_scan_ref's tree; the root split's threshold is
-    the first draw of its feature's stream"""
+    """trees differ by seed, repeat with the same seed, and without streams the root splits where the full scans put it; the root
+    split's threshold is the first draw of its feature's stream"""
     rng = np.random.default_rng(3)
     n = 4000
     bins = np.stack([rng.integers(0, 40, n), rng.integers(0, 25, n), rng.integers(0, 4, n)], axis=1)
@@ -78,11 +79,15 @@ def test_grow_tree_draw_order_and_seeds():
     h = np.ones(n)
     feats = [ref.Feature(0, 40), ref.Feature(1, 25), ref.Feature(2, 4, is_cat=True)]
     p = ref.Params(min_data_in_leaf=20)
-    T6 = X3.grow_tree(bins, g, h, feats, p, 8, True, 6)
-    assert T6["split_feature"] == X3.grow_tree(bins, g, h, feats, p, 8, True, 6)["split_feature"]
-    assert X3.grow_tree(bins, g, h, feats, p, 8, False)["split_feature"] == ref.grow_tree(bins, g, h, feats, p, 8)["split_feature"]
-    shapes = {tuple(zip(X3.grow_tree(bins, g, h, feats, p, 8, True, s)["split_feature"],
-                        X3.grow_tree(bins, g, h, feats, p, 8, True, s)["threshold_bin"])) for s in range(6, 12)}
+    def grow(seed):
+        return tree_ref.grow_tree(bins, g, h, feats, p, 8, streams=None if seed is None else X3.Streams(feats, seed))
+
+    T6 = grow(6)
+    assert T6["split_feature"] == grow(6)["split_feature"]
+    root = ref.best_of_leaf(tree_ref.scan_leaf(bins, g, h, np.arange(n), g.sum(), h.sum(), n, feats, {0: True, 1: True, 2: True}, p))
+    plain = grow(None)
+    assert (plain["split_feature"][0], plain["threshold_bin"][0]) == (root.feature, root.threshold)
+    shapes = {tuple(zip(grow(s)["split_feature"], grow(s)["threshold_bin"])) for s in range(6, 12)}
     assert len(shapes) > 1
     f = T6["split_feature"][0]
     if f != 2:

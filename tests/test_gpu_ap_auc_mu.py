@@ -304,7 +304,7 @@ def test_two_ranks_on_one_device_are_rank_local(built):
     """data-parallel with both ranks on device 0 (the same-device collective): each rank reports average_precision and auc_mu on its
     own shard, nothing is all-reduced"""
     import test_gpu_multi as M
-    from test_gpu_shared_device import _on_ranks
+    from tree_check import on_ranks
     from mmlspark_b200 import capi
     from sklearn.metrics import average_precision_score
     rng = np.random.default_rng(260)
@@ -328,7 +328,7 @@ def test_two_ranks_on_one_device_are_rank_local(built):
             b.free(); ds.free()
         return out
 
-    res, errs = _on_ranks(2, 26800, body)
+    res, errs = on_ranks(2, 26800, body)
     assert not errs, errs
     for r in range(2):
         sl = slice(int(offs[r]), int(offs[r + 1]))

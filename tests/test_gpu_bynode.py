@@ -1,61 +1,17 @@
 """Per-node feature sampling (feature_fraction_bynode): the device sampler (d_bynode_sample), the pick step's node filter and the
-ColSampler stream the host and the device share, tree by tree against the NumPy restatement in bynode_ref.py, and whole models on the
-engine's own gradients.
-
-As in test_gpu_interaction.py, gradients and hessians lie on a 2^-10 grid with few enough rows that K4's fixed-point histograms equal
-NumPy's fp64 ones bit for bit, so only the scans, the samples and the pick are under test.  Every tree of a run is grown from the same
-custom (g, h): the trees differ only by the stream's position, which carries from tree to tree.  Bar: identical structure, leaf values
-within 4 fp64 ulps, split gains as printed, and every tree decided on the reference side (split_scan_ref.undecided)."""
+ColSampler stream the host and the device share, tree by tree against the NumPy restatement in bynode_ref.py (grown by tree_ref.py) on
+grid gradients and at the bar tree_check.py describes, and whole models on the engine's own gradients.  Every tree of a run is grown
+from the same custom (g, h): the trees differ only by the stream's position, which carries from tree to tree."""
 import numpy as np
 import pytest
 
 import bynode_ref as B
-import extra_trees_ref as X3
 import interaction_ref as I
 import split_scan_ref as ref
-import test_gpu_extra_trees as ET
-import test_gpu_interaction as TI
-import test_gpu_monotone as MT
+import tree_check as tc
+import tree_ref
 
 pytestmark = pytest.mark.gpu
-
-
-def _check_run(X, g, h, cats, num_leaves, iters, bynode, cons=None, max_bin=255, extra="", extra_seed=None, fraction=1.0, mono=None,
-               max_depth=-1):
-    """`iters` iterations on the same custom (g, h) against bynode_ref.grow_tree; returns the model text and the restated trees.  A
-    restated tree of one leaf is not in the model (GBDT::TrainOneIter drops it)."""
-    from mmlspark_b200.modeltext import parse_model
-    dsp = ET._ds_params(cats, max_bin)
-    opts = "feature_fraction_bynode=%r %s" % (bynode, extra)
-    if cons is not None:
-        opts += " " + TI._ic(cons)
-    if extra_seed is not None:
-        opts += " extra_trees=true extra_seed=%d" % extra_seed
-    if fraction < 1.0:
-        opts += " feature_fraction=%r" % fraction
-    if mono is not None:
-        opts += " " + MT._mc(mono)
-    if max_depth > 0:
-        opts += " max_depth=%d" % max_depth
-    model = ET._run(X, g, h, ET._params(num_leaves, opts, cats, max_bin), iters, dsp)
-    feats, bins, ub, b2c = TI._reference(X, cats, max_bin)
-    kv = dict(tok.split("=", 1) for tok in extra.split())
-    p = ref.Params(min_data_in_leaf=20, **{k: v for k, v in kv.items() if k in ref.Params.DEFAULTS})
-    trees = parse_model(model)["trees"] if "Tree=" in model else []
-    kept = iter(trees)
-    sampler = B.ColSampler(feats, fraction, bynode)
-    streams = X3.Streams(feats, extra_seed) if extra_seed is not None else None
-    Ts = []
-    for k in range(iters):
-        T = B.grow_tree(bins, g, h, feats, p, num_leaves, sampler, cons, extra_seed is not None, extra_seed or 6, streams, mono,
-                        max_depth=max_depth)
-        why = ref.undecided(T)
-        assert not why, "tree %d does not discriminate:\n%s" % (k, "\n".join(why[:10]))
-        Ts.append(T)
-        if T["num_leaves"] > 1:
-            ET._compare(next(kept), T, ub, b2c)
-    assert next(kept, None) is None
-    return model, Ts
 
 
 def _sampled_out(Ts):
@@ -73,34 +29,34 @@ def _sampled_out(Ts):
 # ---------------------------------------------------------------- tree by tree against the restatement
 @pytest.mark.parametrize("bynode", [0.5, 0.8])      # 5 features: K = 3 (Floyd's branch) and K = 4 (the selection branch)
 def test_numerical_with_nan(built, bynode):
-    X, g, h, cats = ET._data(1, cat=True)
-    _, Ts = _check_run(X, g, h, cats, 12, 4, bynode, extra="min_data_per_group=20 cat_smooth=5")
+    X, g, h, cats = tc.data(1, cat=True)
+    _, Ts = tc.check_run(X, g, h, cats, 12, 4, bynode=bynode, extra="min_data_per_group=20 cat_smooth=5")
     assert _sampled_out(Ts), "the samples must change some leaf's choice"
 
 
 def test_categoricals(built):
     """one-hot (3) and many-vs-many (4) categoricals that the gradients follow, so both split"""
-    X, _, h, cats = ET._data(2, cat=True)
+    X, _, h, cats = tc.data(2, cat=True)
     rng = np.random.default_rng(21)
     y = 0.8 * (X[:, 3] == 1) + 0.6 * (X[:, 4] % 7 < 3) + 0.1 * np.nan_to_num(X[:, 1])
-    g = np.round((-y + 0.3 * rng.standard_normal(len(X))) / ET.GRID) * ET.GRID
-    model, Ts = _check_run(X, g, h, cats, 16, 3, 0.6, extra="min_data_per_group=20 cat_smooth=5")
-    assert ET._split_features(model) >= {3, 4}
+    g = np.round((-y + 0.3 * rng.standard_normal(len(X))) / tc.GRID) * tc.GRID
+    model, Ts = tc.check_run(X, g, h, cats, 16, 3, bynode=0.6, extra="min_data_per_group=20 cat_smooth=5")
+    assert tc.split_features(model) >= {3, 4}
     assert _sampled_out(Ts)
 
 
 def test_wide_features(built):
     """max_bin=511: wide numerical and wide categorical features are sampled like any other"""
-    X, g, h, cats = ET._data(4, n=9000, wide=True)
-    model, Ts = _check_run(X, g, h, cats, 12, 3, 0.5, max_bin=511, extra="min_data_per_group=20 cat_smooth=5")
-    assert ET._split_features(model) & {3, 5}
+    X, g, h, cats = tc.data(4, n=9000, wide=True)
+    model, Ts = tc.check_run(X, g, h, cats, 12, 3, bynode=0.5, max_bin=511, extra="min_data_per_group=20 cat_smooth=5")
+    assert tc.split_features(model) & {3, 5}
     assert _sampled_out(Ts)
 
 
 def test_feature_fraction_carries_the_stream(built):
     """the pool is the tree's feature_fraction sample, and the by-tree draws continue after the previous tree's by-node draws"""
-    X, g, h, cats = ET._data(5, cat=True)
-    model, Ts = _check_run(X, g, h, cats, 8, 6, 0.7, extra="min_data_per_group=20 cat_smooth=5", fraction=0.6)
+    X, g, h, cats = tc.data(5, cat=True)
+    model, Ts = tc.check_run(X, g, h, cats, 8, 6, bynode=0.7, extra="min_data_per_group=20 cat_smooth=5", fraction=0.6)
     assert all(T["draws"] > 0 for T in Ts)
     assert len({tuple(T["split_feature"]) for T in Ts}) > 1
 
@@ -108,44 +64,44 @@ def test_feature_fraction_carries_the_stream(built):
 def test_interaction_constraints(built):
     """K = 3 of 5; the gradients follow feature 4, which is only in the set [3, 4], so the leaves below a split on it have a pool of
     2 < K, which they sample whole"""
-    X, _, h, cats = ET._data(3, cat=True)
+    X, _, h, cats = tc.data(3, cat=True)
     X[:, 4] = X[:, 4] % 9
     rng = np.random.default_rng(31)
     y = 1.5 * (X[:, 4] < 4) + 0.8 * (X[:, 3] == 1) + 0.1 * np.nan_to_num(X[:, 1])
-    g = np.round((-y + 0.3 * rng.standard_normal(len(X))) / ET.GRID) * ET.GRID
+    g = np.round((-y + 0.3 * rng.standard_normal(len(X))) / tc.GRID) * tc.GRID
     cons = [[0, 1, 2, 3], [3, 4]]
-    model, Ts = _check_run(X, g, h, cats, 12, 4, 0.5, cons=cons, extra="min_data_per_group=20 cat_smooth=5")
+    model, Ts = tc.check_run(X, g, h, cats, 12, 4, bynode=0.5, cons=cons, extra="min_data_per_group=20 cat_smooth=5")
     sets = I.sets_of(cons, X.shape[1])
     capped = [samp for T in Ts for rnd in T["node_rounds"] for mask, samp in rnd if sum(1 for f in range(5) if sets[f] & mask) < 3]
     assert capped and all(samp <= {3, 4} for samp in capped)
-    assert TI._paths_inside(model, cons) == 0
+    assert tc.paths_inside(model, cons) == 0
 
 
 def test_extra_trees_draws_of_unsampled_features(built):
     """every scanned feature draws, sampled or not; the case has a feature drawn at a leaf that did not sample it, scanned again later"""
-    X, g, h, cats = ET._data(13, cat=True)
-    _, Ts = _check_run(X, g, h, cats, 12, 4, 0.5, extra="min_data_per_group=20 cat_smooth=5", extra_seed=9)
+    X, g, h, cats = tc.data(13, cat=True)
+    _, Ts = tc.check_run(X, g, h, cats, 12, 4, bynode=0.5, extra="min_data_per_group=20 cat_smooth=5", extra_seed=9)
     events = [(fi, fi in samp) for T in Ts for rnd, samples in zip(T["rounds"], T["node_rounds"])
               for (_, _, scans), (_, samp) in zip(rnd, samples) for fi in sorted(scans)]
     assert any(not ok and any(f2 == fi and ok2 for f2, ok2 in events[k + 1:]) for k, (fi, ok) in enumerate(events))
 
 
 def test_monotone_constraints(built):
-    X, g, h, cats = ET._data(1, cat=True)
+    X, g, h, cats = tc.data(1, cat=True)
     X[:, 2] = -X[:, 2]
-    _check_run(X, g, h, cats, 12, 3, 0.6, mono=[1, 0, -1, 0, 0], extra="min_data_per_group=20 cat_smooth=5")
+    tc.check_run(X, g, h, cats, 12, 3, bynode=0.6, mono=[1, 0, -1, 0, 0], extra="min_data_per_group=20 cat_smooth=5")
 
 
 def test_early_stop_and_max_depth(built):
     """trees that stop early (min_gain_to_split above some gains, then max_depth) take no draws after their last round, so the trees
     after them start from the exact stream position"""
-    X, g, h, cats = ET._data(7, cat=True)
-    feats, bins, _, _ = TI._reference(X, cats, 255)
-    T0 = B.grow_tree(bins, g, h, feats, ref.Params(min_data_in_leaf=20), 31, B.ColSampler(feats, 1.0, 0.5))
+    X, g, h, cats = tc.data(7, cat=True)
+    feats, bins, _, _ = tc.dataset(X, cats, 255)
+    T0 = tree_ref.grow_tree(bins, g, h, feats, ref.Params(min_data_in_leaf=20), 31, sampler=B.ColSampler(feats, 1.0, 0.5))
     thr = float(np.median(T0["split_gain"]))
-    _, Ts = _check_run(X, g, h, cats, 31, 4, 0.5, extra="min_gain_to_split=%r" % thr)
+    _, Ts = tc.check_run(X, g, h, cats, 31, 4, bynode=0.5, extra="min_gain_to_split=%r" % thr)
     assert all(1 < T["num_leaves"] < 31 for T in Ts)
-    _, Ts = _check_run(X, g, h, cats, 31, 4, 0.8, max_depth=3)
+    _, Ts = tc.check_run(X, g, h, cats, 31, 4, bynode=0.8, max_depth=3)
     assert all(T["num_leaves"] <= 8 for T in Ts) and all(len(T["node_rounds"]) < T["num_leaves"] for T in Ts)
 
 
@@ -153,8 +109,8 @@ def _many(seed, n=2000, nf=320):
     rng = np.random.default_rng(seed)
     X = rng.integers(0, 8, (n, nf)).astype(np.float64)
     y = X[:, :40] @ rng.standard_normal(40) * 0.1
-    g = np.round((-y + 0.2 * rng.standard_normal(n)) / ET.GRID) * ET.GRID
-    return X, g, ET._grid(rng, 0.5, 1.5, n)
+    g = np.round((-y + 0.2 * rng.standard_normal(n)) / tc.GRID) * tc.GRID
+    return X, g, tc.grid(rng, 0.5, 1.5, n)
 
 
 @pytest.mark.parametrize("bynode", [0.5, 0.05])      # 320 features: K = 160 (selection branch) and K = 16 (Floyd's branch)
@@ -162,41 +118,41 @@ def test_more_features_than_a_block(built, bynode):
     X, g, h = _many(30)
     n, k = 320, B.get_cnt(320, bynode)
     assert B.selection_branch(n, k) == (bynode == 0.5)
-    _, Ts = _check_run(X, g, h, [], 6, 2, bynode)
+    _, Ts = tc.check_run(X, g, h, [], 6, 2, bynode=bynode)
     assert _sampled_out(Ts)
 
 
 # ---------------------------------------------------------------- whole models on the engine's own gradients
 def _base(case, extra=""):
-    obj = MT.CASES[case][0]
-    return "%s num_leaves=15 learning_rate=0.3 min_data_in_leaf=20 verbosity=-1 metric= %s max_bin=255 %s" % (obj, ET.DS, extra)
+    obj = tc.CASES[case][0]
+    return "%s num_leaves=15 learning_rate=0.3 min_data_in_leaf=20 verbosity=-1 metric= %s max_bin=255 %s" % (obj, tc.DS, extra)
 
 
 def _case_data(case, n=8000):
-    X, z = MT._monotone_data(n, 90)
-    return X, MT.CASES[case][2](z)
+    X, z = tc.monotone_data(n, 90)
+    return X, tc.CASES[case][2](z)
 
 
 @pytest.mark.parametrize("case", ["regression", "binary", "multiclass", "goss", "dart", "rf", "bagging"])
 def test_boosting_modes(built, case):
     """1.0 is the model of no key; 0.5 changes the trees and repeats with its seed; another feature_fraction_seed changes them"""
     X, y = _case_data(case)
-    dsp = ET.DS + " max_bin=255"
-    plain = MT._boosted(X, y, _base(case), 5, dsp)
-    assert ET._trees(MT._boosted(X, y, _base(case, "feature_fraction_bynode=1.0"), 5, dsp)) == ET._trees(plain)
-    a = MT._boosted(X, y, _base(case, "feature_fraction_bynode=0.5"), 5, dsp)
-    assert ET._trees(a) != ET._trees(plain)
-    assert ET._trees(MT._boosted(X, y, _base(case, "colsample_bynode=0.5"), 5, dsp)) == ET._trees(a)
-    assert ET._trees(MT._boosted(X, y, _base(case, "sub_feature_bynode=0.5 feature_fraction_seed=7"), 5, dsp)) != ET._trees(a)
+    dsp = tc.DS + " max_bin=255"
+    plain = tc.boost(X, y, _base(case), 5, dsp)
+    assert tc.trees(tc.boost(X, y, _base(case, "feature_fraction_bynode=1.0"), 5, dsp)) == tc.trees(plain)
+    a = tc.boost(X, y, _base(case, "feature_fraction_bynode=0.5"), 5, dsp)
+    assert tc.trees(a) != tc.trees(plain)
+    assert tc.trees(tc.boost(X, y, _base(case, "colsample_bynode=0.5"), 5, dsp)) == tc.trees(a)
+    assert tc.trees(tc.boost(X, y, _base(case, "sub_feature_bynode=0.5 feature_fraction_seed=7"), 5, dsp)) != tc.trees(a)
 
 
 def test_two_ranks_on_one_device(built):
     X, y = _case_data("regression")
-    dsp = ET.DS + " max_bin=255"
+    dsp = tc.DS + " max_bin=255"
     params = _base("regression", "feature_fraction_bynode=0.4 feature_fraction=0.8")
-    one = MT._boosted(X, y, params, 5, dsp)
-    two = MT._boosted(X, y, params + " tree_learner=data num_machines=2", 5, dsp, rank_rows=[4000, 4000], port=29900)
-    assert ET._trees(one) == ET._trees(two)
+    one = tc.boost(X, y, params, 5, dsp)
+    two = tc.boost(X, y, params + " tree_learner=data num_machines=2", 5, dsp, rank_rows=[4000, 4000], port=29900)
+    assert tc.trees(one) == tc.trees(two)
 
 
 def test_two_ranks_nccl(built):
@@ -206,9 +162,9 @@ def test_two_ranks_nccl(built):
     if len([l for l in out.splitlines() if l.startswith("GPU ")]) < 2:
         pytest.skip("needs 2 GPUs")
     X, y = _case_data("regression")
-    dsp = ET.DS + " max_bin=255"
+    dsp = tc.DS + " max_bin=255"
     params = _base("regression", "feature_fraction_bynode=0.4")
-    one = MT._boosted(X, y, params, 5, dsp)
+    one = tc.boost(X, y, params, 5, dsp)
     rows = [4000, 4000]
     offs = [0, 4000, 8000]
 
@@ -224,9 +180,9 @@ def test_two_ranks_nccl(built):
         finally:
             b.free(); ds.free(); full.free()
 
-    res, errs = ET._on_ranks(len(rows), 29920, body, device_of=lambda r: r)
+    res, errs = tc.on_ranks(len(rows), 29920, body, device_of=lambda r: r)
     assert not errs, errs
-    assert ET._trees(res[0]) == ET._trees(res[1]) == ET._trees(one)
+    assert tc.trees(res[0]) == tc.trees(res[1]) == tc.trees(one)
 
 
 def test_bundles_equal_unbundled(built):
@@ -239,13 +195,13 @@ def test_bundles_equal_unbundled(built):
         X[on, j] = rng.integers(1, 12, on.sum())
     X[:, 6] = rng.standard_normal(n)
     X[:, 7] = rng.integers(0, 30, n)
-    g = np.round((-(X[:, 0] * 0.2 + X[:, 3] * 0.1 - X[:, 1] * 0.15 + X[:, 6]) + 0.2 * rng.standard_normal(n)) / ET.GRID) * ET.GRID
-    h = ET._grid(rng, 0.5, 1.5, n)
+    g = np.round((-(X[:, 0] * 0.2 + X[:, 3] * 0.1 - X[:, 1] * 0.15 + X[:, 6]) + 0.2 * rng.standard_normal(n)) / tc.GRID) * tc.GRID
+    h = tc.grid(rng, 0.5, 1.5, n)
     models = []
     for bundle in ("true", "false"):
-        dsp = ET.DS + " max_bin=255 enable_bundle=" + bundle
-        models.append(ET._run(X, g, h, ET._params(12, "feature_fraction_bynode=0.5 enable_bundle=" + bundle), 4, dsp))
-    assert ET._trees(models[0]) == ET._trees(models[1])
+        dsp = tc.DS + " max_bin=255 enable_bundle=" + bundle
+        models.append(tc.run(X, g, h, tc.params(12, "feature_fraction_bynode=0.5 enable_bundle=" + bundle), 4, dsp))
+    assert tc.trees(models[0]) == tc.trees(models[1])
 
 
 def test_reset_parameter(built):
@@ -253,11 +209,11 @@ def test_reset_parameter(built):
     place after tree 1, and a reset back to 1.0 grows the plain tree"""
     from mmlspark_b200 import capi
     from mmlspark_b200.modeltext import parse_model
-    X, g, h, cats = ET._data(15, cat=True)
-    dsp = ET._ds_params(cats, 255)
+    X, g, h, cats = tc.data(15, cat=True)
+    dsp = tc.ds_params(cats, 255)
     plan = [0.5, 0.5, 0.8, 1.0, 0.5]
     ds = capi.Dataset.from_mat(X, dsp).set_field("label", np.zeros(len(X), np.float32))
-    b = capi.Booster(ds, ET._params(12, "feature_fraction_bynode=0.5 min_data_per_group=20 cat_smooth=5", cats))
+    b = capi.Booster(ds, tc.params(12, "feature_fraction_bynode=0.5 min_data_per_group=20 cat_smooth=5", cats))
     try:
         for k, f in enumerate(plan):
             if k and f != plan[k - 1]:
@@ -266,15 +222,15 @@ def test_reset_parameter(built):
         model = b.save_model_to_string()
     finally:
         b.free(); ds.free()
-    feats, bins, ub, b2c = TI._reference(X, cats, 255)
+    feats, bins, ub, b2c = tc.dataset(X, cats, 255)
     p = ref.Params(min_data_in_leaf=20, min_data_per_group=20, cat_smooth=5)
     trees = parse_model(model)["trees"]
     s = B.ColSampler(feats, 1.0, 0.5)
     for k, f in enumerate(plan):
         s.bynode = f
-        T = B.grow_tree(bins, g, h, feats, p, 12, s)
+        T = tree_ref.grow_tree(bins, g, h, feats, p, 12, sampler=s)
         assert not ref.undecided(T)
-        ET._compare(trees[k], T, ub, b2c)
+        tc.compare_tree(trees[k], T, ub, b2c)
     assert "[feature_fraction_bynode: 0.5]" in model
 
 
@@ -289,13 +245,13 @@ ERRORS = [
 @pytest.mark.parametrize("opts,msg", ERRORS)
 def test_create_and_reset_errors(built, opts, msg):
     from mmlspark_b200 import capi
-    X, g, h, cats = ET._data(7, cat=True)
-    ds = capi.Dataset.from_mat(X, ET._ds_params(cats, 255)).set_field("label", np.asarray(-g, np.float32))
+    X, g, h, cats = tc.data(7, cat=True)
+    ds = capi.Dataset.from_mat(X, tc.ds_params(cats, 255)).set_field("label", np.asarray(-g, np.float32))
     try:
         with pytest.raises(Exception) as e:
-            capi.Booster(ds, ET._params(8, opts, cats))
+            capi.Booster(ds, tc.params(8, opts, cats))
         assert msg in str(e.value), str(e.value)
-        b = capi.Booster(ds, ET._params(8, "feature_fraction_bynode=0.5", cats))
+        b = capi.Booster(ds, tc.params(8, "feature_fraction_bynode=0.5", cats))
         try:
             b.update_one_iter()
             before = b.save_model_to_string()
@@ -314,21 +270,21 @@ def test_create_and_reset_errors(built, opts, msg):
 def test_errors_fire_on_every_rank(built):
     """each range error and the voting rejection at create on both ranks, and the voting rejection at ResetParameter"""
     from mmlspark_b200 import capi
-    X, g, h, cats = ET._data(25, cat=True)
+    X, g, h, cats = tc.data(25, cat=True)
     half = len(X) // 2
     cases = [(o + " tree_learner=data num_machines=2", m) for o, m in ERRORS] + \
             [("feature_fraction_bynode=0.5 tree_learner=voting top_k=2 num_machines=2", "does not support feature_fraction_bynode")]
 
     def body(r):
         sl = slice(r * half, (r + 1) * half)
-        ds = capi.Dataset.from_mat(X[sl], ET._ds_params(cats, 255)).set_field("label", np.asarray(-g[sl], np.float32))
+        ds = capi.Dataset.from_mat(X[sl], tc.ds_params(cats, 255)).set_field("label", np.asarray(-g[sl], np.float32))
         try:
             msgs = []
             for opts, _ in cases:
                 with pytest.raises(Exception) as e:
-                    capi.Booster(ds, ET._params(8, opts, cats))
+                    capi.Booster(ds, tc.params(8, opts, cats))
                 msgs.append(str(e.value))
-            b = capi.Booster(ds, ET._params(8, "tree_learner=voting top_k=2 num_machines=2", cats))
+            b = capi.Booster(ds, tc.params(8, "tree_learner=voting top_k=2 num_machines=2", cats))
             try:
                 b.update_one_iter()
                 before = b.save_model_to_string()
@@ -343,28 +299,28 @@ def test_errors_fire_on_every_rank(built):
         finally:
             ds.free()
 
-    res, errs = ET._on_ranks(2, 29940, body)
+    res, errs = tc.on_ranks(2, 29940, body)
     assert not errs, errs
     for msgs, unchanged, model in res:
         for (_, want), got in zip(cases + [(None, "does not support feature_fraction_bynode")], msgs):
             assert want in got, (want, got)
         assert unchanged
         assert "[feature_fraction_bynode: 1]" in model
-    assert ET._trees(res[0][2]) == ET._trees(res[1][2])
+    assert tc.trees(res[0][2]) == tc.trees(res[1][2])
 
 
 def test_model_text_round_trips(built):
     from mmlspark_b200 import capi
-    X, g, h, cats = ET._data(8)
-    dsp = ET._ds_params(cats, 255)
-    model = ET._run(X, g, h, ET._params(8, "feature_fraction_bynode=0.35", cats), 2, dsp)
+    X, g, h, cats = tc.data(8)
+    dsp = tc.ds_params(cats, 255)
+    model = tc.run(X, g, h, tc.params(8, "feature_fraction_bynode=0.35", cats), 2, dsp)
     assert "[feature_fraction_bynode: 0.35]" in model
     b = capi.Booster(model_str=model)
     try:
         assert b.save_model_to_string() == model
     finally:
         b.free()
-    assert "[feature_fraction_bynode: 1]" in ET._run(X, g, h, ET._params(8, "", cats), 2, dsp)
+    assert "[feature_fraction_bynode: 1]" in tc.run(X, g, h, tc.params(8, "", cats), 2, dsp)
 
 
 def test_estimator(built):
@@ -372,7 +328,7 @@ def test_estimator(built):
     from mmlspark_b200 import capi
     from mmlspark_b200.lightgbm import Frame, LightGBMRegressor
     from mmlspark_b200.lightgbm.params import dataset_params
-    X, z = MT._monotone_data(5000, 10)
+    X, z = tc.monotone_data(5000, 10)
     X = np.nan_to_num(X)
     df = Frame({"features": X, "label": z})
     est = LightGBMRegressor(featureFractionByNode=0.4, numIterations=5, numTasks=1)
@@ -388,6 +344,6 @@ def test_estimator(built):
         low = b.save_model_to_string()
     finally:
         b.free(); ds.free()
-    assert ET._trees(model) == ET._trees(low)
+    assert tc.trees(model) == tc.trees(low)
     plain = LightGBMRegressor(numIterations=5, numTasks=1).fit(df).getNativeModel()
-    assert ET._trees(plain) != ET._trees(model)
+    assert tc.trees(plain) != tc.trees(model)

@@ -8,7 +8,6 @@ emulation, ranks agreeing).  The tests are called through their module objects s
 import os
 import subprocess
 import sys
-import threading
 import time
 
 import numpy as np
@@ -20,6 +19,7 @@ import test_gpu_multi as M
 import test_gpu_sparse_estimators as S
 import test_gpu_wide as W
 import test_gpu_xendcg_xentlambda as X
+import tree_check as tc
 
 pytestmark = pytest.mark.gpu
 
@@ -82,33 +82,6 @@ def test_sparse_estimator_two_tasks(built, one_device):
 
 
 # ------------------------------------------------------------------------------------------------ helpers
-def _on_ranks(R, base_port, body, device_of=lambda r: 0, timeout=120):
-    """body(r) on R rank-threads of this process, rank r on device_of(r), between network_init and network_free (in finally).
-    Returns the bodies' results and the (rank, error) pairs."""
-    from mmlspark_b200 import capi
-    machines = ",".join("127.0.0.1:%d" % (base_port + r) for r in range(R))
-    out, errs = [None] * R, []
-
-    def task(r):
-        try:
-            capi.set_device(device_of(r))
-            capi.network_init(machines, base_port + r, timeout, R)
-            try:
-                out[r] = body(r)
-            finally:
-                capi.network_free()
-        except Exception as e:   # noqa
-            errs.append((r, str(e)))
-
-    ts = [threading.Thread(target=task, args=(r,)) for r in range(R)]
-    for t in ts:
-        t.start()
-    for t in ts:
-        t.join(300)
-    assert not any(t.is_alive() for t in ts), "a rank-thread did not finish"
-    return out, errs
-
-
 def _regression_data(seed, n, F=20):
     rng = np.random.default_rng(seed)
     X_ = rng.standard_normal((n, F))
@@ -117,7 +90,7 @@ def _regression_data(seed, n, F=20):
 
 
 def _train_shards(X_, y, rank_rows, params, iters):
-    """body for _on_ranks: rank r trains on its contiguous shard and returns its model, scores, GetInfo and memory info"""
+    """body for tree_check.on_ranks: rank r trains on its contiguous shard and returns its model, scores, GetInfo and memory info"""
     from mmlspark_b200 import capi
     offs = np.concatenate([[0], np.cumsum(rank_rows)])
 
@@ -159,7 +132,7 @@ def test_wide_categorical_two_ranks_on_one_device(built):
         b.free(); ds.free()
         return res
 
-    res, errs = _on_ranks(2, 26000, body)
+    res, errs = tc.on_ranks(2, 26000, body)
     assert not errs, errs
     ods = O.OracleDataset(X_, W.DS, rank_rows=rank_rows).set_field("label", y)
     ob = O.OracleBooster(ods, params)
@@ -200,7 +173,7 @@ def test_reduce_mode_is_same_device(built):
     X_, y = _regression_data(41, n)
     rank_rows = [n // 2 + 99, n - n // 2 - 99]
     params = M._params("regression", 2)
-    res, errs = _on_ranks(2, 26200, _train_shards(X_, y, rank_rows, params, 8))
+    res, errs = tc.on_ranks(2, 26200, _train_shards(X_, y, rank_rows, params, 8))
     assert not errs, errs
     for r in range(2):
         assert res[r]["info"]["num_machines"] == 2 and res[r]["info"]["rank"] == r and res[r]["info"]["reduce_mode"] == 3
@@ -213,10 +186,10 @@ def test_column_copy_with_four_ranks_on_one_device(built, monkeypatch):
     X_, y = _regression_data(51, n)
     rank_rows = [n // 4] * 4
     params = M._params("regression", 4)
-    res, errs = _on_ranks(4, 26300, _train_shards(X_, y, rank_rows, params, 6))
+    res, errs = tc.on_ranks(4, 26300, _train_shards(X_, y, rank_rows, params, 6))
     assert not errs, errs
     monkeypatch.setenv("B200GBM_COLUMN_COPY", "0")
-    off, errs = _on_ranks(4, 26310, _train_shards(X_, y, rank_rows, params, 6))
+    off, errs = tc.on_ranks(4, 26310, _train_shards(X_, y, rank_rows, params, 6))
     assert not errs, errs
     for r in range(4):
         assert res[r]["model"] == res[0]["model"] and off[r]["model"] == res[0]["model"]
@@ -268,7 +241,7 @@ def test_a_rank_that_fails_releases_the_others(built):
     y[n - 5] = 1.5
     params = M._params("cross_entropy", 2)
     t0 = time.time()
-    _, errs = _on_ranks(2, 26500, _train_shards(X_, y, [n // 2, n - n // 2], params, 5), timeout=100)
+    _, errs = tc.on_ranks(2, 26500, _train_shards(X_, y, [n // 2, n - n // 2], params, 5), timeout=100)
     elapsed = time.time() - t0
     by_rank = dict(errs)
     assert "outside [0, 1]" in by_rank.get(1, ""), errs
@@ -290,9 +263,9 @@ def test_same_device_model_equals_nccl_model(built):
     X_, y = _regression_data(71, n)
     rank_rows = [n // 2 + 5, n - n // 2 - 5]
     params = M._params("regression", 2)
-    same, errs = _on_ranks(2, 26600, _train_shards(X_, y, rank_rows, params, 10))
+    same, errs = tc.on_ranks(2, 26600, _train_shards(X_, y, rank_rows, params, 10))
     assert not errs, errs
-    nccl, errs = _on_ranks(2, 26610, _train_shards(X_, y, rank_rows, params, 10), device_of=lambda r: r)
+    nccl, errs = tc.on_ranks(2, 26610, _train_shards(X_, y, rank_rows, params, 10), device_of=lambda r: r)
     assert not errs, errs
     assert same[0]["info"]["reduce_mode"] == 3 and nccl[0]["info"]["reduce_mode"] == 0
     assert same[0]["model"] == nccl[0]["model"]
@@ -301,7 +274,7 @@ def test_same_device_model_equals_nccl_model(built):
 def test_three_ranks_on_two_devices_are_rejected(built):
     if REAL_NGPU() < 2:
         pytest.skip("needs 2 GPUs")
-    _, errs = _on_ranks(3, 26700, lambda r: None, device_of=lambda r: r % 2, timeout=60)
+    _, errs = tc.on_ranks(3, 26700, lambda r: None, device_of=lambda r: r % 2, timeout=60)
     assert sorted(r for r, _ in errs) == [0, 1, 2], errs
     for _, e in errs:
         assert "ranks 0,2 share CUDA device" in e and "supported layouts" in e, e

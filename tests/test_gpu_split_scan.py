@@ -13,15 +13,12 @@ import numpy as np
 import pytest
 
 import split_scan_ref as ref
+import tree_check as tc
+import tree_ref
 
 pytestmark = pytest.mark.gpu
 
-GRID = 1.0 / 1024
-
-
-def _grid(rng, lo, hi, n):
-    """values on the 2^-10 grid in [lo, hi]"""
-    return rng.integers(int(lo * 1024), int(hi * 1024) + 1, n) * GRID
+GRID = tc.GRID
 
 
 def _on_grid(x):
@@ -55,10 +52,6 @@ def _train(X, g, h, params, ds_params="", cat=(), label=None):
     return parse_model(text), text, feats, bins, side
 
 
-def _ulps(a, b):
-    return np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)) / np.spacing(np.maximum(np.abs(a), np.abs(b)) + 1e-300)
-
-
 def _check(X, g, h, params, num_leaves, ds_params="", cat=(), label=None, expect_leaves=None):
     """train, restate, assert decided, compare; returns (reference tree, model text)"""
     p = ref.Params(**params)
@@ -73,38 +66,13 @@ def _check(X, g, h, params, num_leaves, ds_params="", cat=(), label=None, expect
         if len(nz):
             step = 2.0 ** (np.floor(np.log2(nz.max())) - 23)
             assert np.array_equal(np.round(v / step) * step, v)
-    T = ref.grow_tree(bins, np.asarray(g, np.float64), np.asarray(h, np.float64), feats, p, num_leaves)
+    T = tree_ref.grow_tree(bins, np.asarray(g, np.float64), np.asarray(h, np.float64), feats, p, num_leaves)
     T["features"] = {f.real_index: f for f in feats}
     why = ref.undecided(T)
     assert not why, "the case does not discriminate:\n" + "\n".join(why[:10])
     if expect_leaves is not None:
         assert T["num_leaves"] == expect_leaves, "the case was built to grow %d leaves, the reference grows %d" % (expect_leaves, T["num_leaves"])
-    t = m["trees"][0]
-    assert t["num_leaves"] == T["num_leaves"], "num_leaves %d vs reference %d" % (t["num_leaves"], T["num_leaves"])
-    nl = T["num_leaves"]
-    if nl > 1:
-        assert t["split_feature"].tolist() == T["split_feature"], (t["split_feature"], T["split_feature"])
-        assert t["left_child"].tolist() == T["left_child"] and t["right_child"].tolist() == T["right_child"]
-        for i in range(nl - 1):
-            f, dt = T["split_feature"][i], int(t["decision_type"][i])
-            assert bool(dt & 1) == T["is_cat"][i], "node %d: categorical flag" % i
-            if T["is_cat"][i]:
-                k = int(t["threshold"][i])
-                words = t["cat_threshold"][t["cat_boundaries"][k]:t["cat_boundaries"][k + 1]]
-                cats = {32 * w + j for w, word in enumerate(words) for j in range(32) if (int(word) >> j) & 1}
-                got = {b for b, c in enumerate(side["b2c"][f]) if b > 0 and c in cats}
-                assert got == set(T["cat_bins"][i]), "node %d: category bins %s vs reference %s" % (i, sorted(got), sorted(T["cat_bins"][i]))
-            else:
-                hit = np.nonzero(side["ub"][f] == t["threshold"][i])[0]
-                assert len(hit) == 1, "node %d: threshold %r is not exactly one upper bound" % (i, t["threshold"][i])
-                assert hit[0] == T["threshold_bin"][i], "node %d: threshold bin %d vs reference %d" % (i, hit[0], T["threshold_bin"][i])
-                assert bool(dt & 2) == T["default_left"][i], "node %d: default_left" % i
-            assert t["split_gain"][i] == float("%g" % T["split_gain"][i]), "node %d: split_gain %r vs %g" % (i, t["split_gain"][i], T["split_gain"][i])
-        assert t["leaf_count"].tolist() == T["leaf_count"] and t["internal_count"].tolist() == T["internal_count"]
-        assert (_ulps(t["leaf_weight"], T["leaf_weight"]) <= 4).all(), (t["leaf_weight"], T["leaf_weight"])
-        for k in ("internal_value", "internal_weight"):
-            assert t[k].tolist() == [float("%g" % v) for v in T[k]], (k, t[k], T[k])
-    assert (_ulps(t["leaf_value"], T["leaf_value"]) <= 4).all(), (t["leaf_value"], T["leaf_value"])
+    tc.compare_tree(m["trees"][0], T, side["ub"], side["b2c"])
     return T, text
 
 
@@ -117,10 +85,10 @@ def _step_case(num_bin, split_at, seed, rows_per_bin=24, nan_rows=0, scale=1.0):
         v = np.concatenate([v, np.full(nan_rows, np.nan)])
     n = len(v)
     w = rng.integers(0, 13, n).astype(np.float64)
-    g = np.where(v <= split_at, -2.0, 1.5) + 0.25 * (w - 6) / 6 + _grid(rng, -0.5, 0.5, n)
+    g = np.where(v <= split_at, -2.0, 1.5) + 0.25 * (w - 6) / 6 + tc.grid(rng, -0.5, 0.5, n)
     if nan_rows:
-        g[np.isnan(v)] = -3.0 + _grid(rng, -0.25, 0.25, nan_rows)
-    h = _grid(rng, 0.5, 1.5, n)
+        g[np.isnan(v)] = -3.0 + tc.grid(rng, -0.25, 0.25, nan_rows)
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([v, w], axis=1)
     perm = rng.permutation(n)
     return X[perm], np.round(g[perm] / GRID) * GRID * scale, h[perm] * scale
@@ -164,9 +132,9 @@ def test_nan_offset_zero(built, sign):
     n = 8000
     v = rng.integers(-10, 11, n).astype(np.float64)
     v[rng.random(n) < 0.1] = np.nan
-    g = np.where(v <= 2, -1.0, 1.0) + _grid(rng, -0.5, 0.5, n)
-    g[np.isnan(v)] = sign * 1.25 + _grid(rng, -0.25, 0.25, int(np.isnan(v).sum()))
-    h = _grid(rng, 0.5, 1.5, n)
+    g = np.where(v <= 2, -1.0, 1.0) + tc.grid(rng, -0.5, 0.5, n)
+    g[np.isnan(v)] = sign * 1.25 + tc.grid(rng, -0.25, 0.25, int(np.isnan(v).sum()))
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([v, rng.integers(0, 5, n).astype(np.float64)], axis=1)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 3)
     f0 = T["features"][0]
@@ -181,8 +149,8 @@ def test_nan_offset_one_forward_pass(built):
     n = 6000
     v = np.where(rng.random(n) < 0.6, 0.0, rng.integers(1, 20, n).astype(np.float64))
     v[rng.random(n) < 0.1] = np.nan
-    g = np.where(np.isnan(v) | (v > 9), 1.0, -1.0) + _grid(rng, -0.5, 0.5, n)
-    h = _grid(rng, 0.5, 1.5, n)
+    g = np.where(np.isnan(v) | (v > 9), 1.0, -1.0) + tc.grid(rng, -0.5, 0.5, n)
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([v, rng.integers(0, 5, n).astype(np.float64)], axis=1)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 2, expect_leaves=2)
     assert T["features"][0].offset == 1 and T["default_left"][0] is False
@@ -248,7 +216,7 @@ def test_min_gain_to_split_equal_to_best_gain_is_rejected(built):
     X, g, h = _blocks([64, 64, 64, 64], [-1, -0.5, 0.5, 1], [1, 1, 1, 1])
     feats = [ref.Feature(0, 4), ref.Feature(1, 7)]
     p0 = ref.Params(min_data_in_leaf=5)
-    scans = ref.scan_leaf(X.astype(np.int64), g, h, np.arange(len(g)), float(g.sum()), float(h.sum()), len(g), feats, {0: True, 1: True}, p0)
+    scans = tree_ref.scan_leaf(X.astype(np.int64), g, h, np.arange(len(g)), float(g.sum()), float(h.sum()), len(g), feats, {0: True, 1: True}, p0)
     best, base = max(c[0] for sc in scans.values() for c in sc.candidates), scans[0].shift
     mg = best - base
     while base + mg < best:
@@ -259,7 +227,7 @@ def test_min_gain_to_split_equal_to_best_gain_is_rejected(built):
     for mgs, leaves in ((float(mg), 1), (float(np.nextafter(mg, -np.inf)), 2)):
         p = dict(min_data_in_leaf=5, min_gain_to_split=mgs)
         m, _, feats, bins, _ = _train(X, g, h, "num_leaves=2 " + ref.Params(**p).as_string())
-        T = ref.grow_tree(bins, g, h, feats, ref.Params(**p), 2)
+        T = tree_ref.grow_tree(bins, g, h, feats, ref.Params(**p), 2)
         assert T["num_leaves"] == leaves and m["trees"][0]["num_leaves"] == leaves
 
 
@@ -287,7 +255,7 @@ def test_negative_hessians_break_hides_a_better_threshold(built):
     v = np.repeat(np.arange(10, dtype=np.float64), 100)
     h = np.where(v == 8, -8.0, np.where(v == 9, 10.0, 1.0))
     w = rng.integers(0, 4, len(v)).astype(np.float64)
-    g = np.where(v <= 7, -1.0, 2.0) + np.where(w >= 2, 0.5, -0.5) + _grid(rng, -0.125, 0.125, len(v))
+    g = np.where(v <= 7, -1.0, 2.0) + np.where(w >= 2, 0.5, -0.5) + tc.grid(rng, -0.125, 0.125, len(v))
     X = np.stack([v, w], axis=1)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 2, expect_leaves=2)
     assert T["split_feature"][0] == 1
@@ -301,8 +269,8 @@ def test_empty_bins_in_children_reverse_keeps_the_higher_threshold(built):
     rng = np.random.default_rng(8)
     v = np.concatenate([rng.integers(0, 4, 3000), rng.integers(6, 10, 3000), np.full(500, -1)]).astype(np.float64)
     v[v < 0] = np.nan
-    g = np.where(np.isnan(v), 2.0, np.where(v < 5, -1.0, 1.0)) + _grid(rng, -0.25, 0.25, len(v))
-    h = _grid(rng, 0.5, 1.5, len(v))
+    g = np.where(np.isnan(v), 2.0, np.where(v < 5, -1.0, 1.0)) + tc.grid(rng, -0.25, 0.25, len(v))
+    h = tc.grid(rng, 0.5, 1.5, len(v))
     X = np.stack([v, rng.integers(0, 3, len(v)).astype(np.float64)], axis=1)
     _check(X, g, h, dict(min_data_in_leaf=20), 3, ds_params="max_bin=12")
 
@@ -317,8 +285,8 @@ def test_empty_bins_in_a_child_forward_keeps_the_lower_threshold(built):
     v = np.where(a == 0, rng.choice([0, 1, 2, 7, 8, 9], n), rng.integers(0, 10, n)).astype(np.float64)
     v[rng.random(n) < 0.1] = np.nan
     hi = np.isnan(v) | (v >= 7)
-    g = np.where(a == 0, np.where(hi, 1.0, -1.0) - 2.0, 2.0 + 0.25 * np.where(v > 4, 1, -1)) + _grid(rng, -0.125, 0.125, n)
-    h = _grid(rng, 0.5, 1.5, n)
+    g = np.where(a == 0, np.where(hi, 1.0, -1.0) - 2.0, 2.0 + 0.25 * np.where(v > 4, 1, -1)) + tc.grid(rng, -0.125, 0.125, n)
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([a, v], axis=1)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 3, expect_leaves=3)
     assert T["split_feature"] == [0, 1] and T["left_child"][0] == 1           # the second split is in the child a == 0
@@ -332,8 +300,8 @@ def test_duplicate_columns_smaller_real_index_wins(built):
     n = 9000
     a = rng.integers(0, 20, n).astype(np.float64)
     wide = rng.integers(0, 300, n).astype(np.float64)
-    g = np.where(wide < 120, -1.0, 1.0) + 0.5 * np.where(a < 7, -1.0, 1.0) + _grid(rng, -0.25, 0.25, n)
-    h = _grid(rng, 0.5, 1.5, n)
+    g = np.where(wide < 120, -1.0, 1.0) + 0.5 * np.where(a < 7, -1.0, 1.0) + tc.grid(rng, -0.25, 0.25, n)
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([a, rng.integers(0, 5, n).astype(np.float64), a, wide, np.minimum(wide, 119.0) + (wide >= 120) * 120], axis=1)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 4, ds_params="max_bin=300")
     assert 3 in T["split_feature"] and 0 in T["split_feature"] and 2 not in T["split_feature"]
@@ -358,7 +326,7 @@ def test_constant_hessian_regression(built, num_leaves):
     rng = np.random.default_rng(20 + num_leaves)
     n = 20000
     X = np.stack([rng.integers(0, 50, n), rng.integers(0, 7, n), rng.integers(0, 200, n)], axis=1).astype(np.float64)
-    y = (np.where(X[:, 0] < 17, -1.0, 1.0) + np.where(X[:, 2] < 150, 0.75, -0.5) + _grid(rng, -0.5, 0.5, n)).astype(np.float32)
+    y = (np.where(X[:, 0] < 17, -1.0, 1.0) + np.where(X[:, 2] < 150, 0.75, -0.5) + tc.grid(rng, -0.5, 0.5, n)).astype(np.float32)
     _check(X, None, None, dict(min_data_in_leaf=20), num_leaves, label=y, expect_leaves=num_leaves)
 
 
@@ -370,8 +338,8 @@ def test_second_round_larger_child_from_subtraction(built, larger):
     v = rng.integers(0, 40, n).astype(np.float64)
     cut = 29 if larger == "left" else 10
     X = np.stack([v, rng.integers(0, 30, n).astype(np.float64), rng.integers(0, 9, n).astype(np.float64)], axis=1)
-    g = np.where(v <= cut, -1.5, 1.5) + np.where(X[:, 1] < 12, -0.5, 0.5) + 0.25 * np.where(X[:, 2] < 4, -1, 1) + _grid(rng, -0.25, 0.25, n)
-    h = _grid(rng, 0.5, 1.5, n)
+    g = np.where(v <= cut, -1.5, 1.5) + np.where(X[:, 1] < 12, -0.5, 0.5) + 0.25 * np.where(X[:, 2] < 4, -1, 1) + tc.grid(rng, -0.25, 0.25, n)
+    h = tc.grid(rng, 0.5, 1.5, n)
     T, _ = _check(X, g, h, dict(min_data_in_leaf=20), 4, expect_leaves=4)
     (l_leaf, l_cnt), (r_leaf, r_cnt) = T["scanned_counts"][1]
     assert T["split_feature"][0] == 0 and l_leaf == 0 and r_leaf == 1
@@ -385,8 +353,8 @@ def test_equal_gain_leaves_smaller_leaf_index_wins(built):
     rng = np.random.default_rng(12)
     m = 3000
     a = rng.integers(0, 10, m).astype(np.float64)
-    ga = np.where(a < 4, -1.0, 1.0) + 0.5 + _grid(rng, -0.25, 0.25, m)
-    ha = _grid(rng, 0.5, 1.5, m)
+    ga = np.where(a < 4, -1.0, 1.0) + 0.5 + tc.grid(rng, -0.25, 0.25, m)
+    ha = tc.grid(rng, 0.5, 1.5, m)
     X = np.stack([np.concatenate([np.zeros(m), np.ones(m)]), np.concatenate([a, a + 10])], axis=1)
     T, _ = _check(X, np.concatenate([ga, -ga]), np.concatenate([ha, ha]), dict(min_data_in_leaf=20), 3, expect_leaves=3)
     assert T["left_child"][0] == 1 and T["right_child"][0] == ~1      # the second split (node 1) took leaf 0, not leaf 1
@@ -400,8 +368,8 @@ def test_categorical_one_hot_boundary(built, ncat, onehot):
     n = 4000
     c = rng.integers(0, ncat, n).astype(np.float64)
     eff = np.array([-1.0, 1.5, 0.3125, -0.625, 0.8125])[:ncat]
-    g = eff[c.astype(int)] + _grid(rng, -0.25, 0.25, n)
-    h = _grid(rng, 0.5, 1.5, n)
+    g = eff[c.astype(int)] + tc.grid(rng, -0.25, 0.25, n)
+    h = tc.grid(rng, 0.5, 1.5, n)
     X = np.stack([c, rng.integers(0, 5, n).astype(np.float64)], axis=1)
     _check(X, g, h, dict(min_data_in_leaf=20, max_cat_to_onehot=onehot, min_data_per_group=20, cat_smooth=5.0), 3, cat=(0,))
 
@@ -417,7 +385,7 @@ def test_categorical_many_vs_many(built, params):
     sizes[5] = 30
     c = np.repeat(np.arange(20, dtype=np.float64), sizes)
     eff = _on_grid(rng.permutation(np.linspace(-2, 2, 20)))
-    g = eff[c.astype(int)] + _grid(rng, -0.5, 0.5, len(c))
+    g = eff[c.astype(int)] + tc.grid(rng, -0.5, 0.5, len(c))
     h = np.ones(len(c))
     X = np.stack([c, rng.integers(0, 5, len(c)).astype(np.float64)], axis=1)
     p = dict(min_data_in_leaf=20)
@@ -441,9 +409,9 @@ def test_wide_categorical(built):
     ncat = 600
     c = np.repeat(np.arange(ncat, dtype=np.float64), rng.integers(10, 40, ncat))
     eff = _on_grid(rng.permutation(np.linspace(-2, 2, ncat)))
-    g = eff[c.astype(int)] + _grid(rng, -0.25, 0.25, len(c))
+    g = eff[c.astype(int)] + tc.grid(rng, -0.25, 0.25, len(c))
     X = np.stack([c, rng.integers(0, 5, len(c)).astype(np.float64)], axis=1)
-    _check(X, g, _grid(rng, 0.75, 1.25, len(c)), dict(min_data_in_leaf=20, min_data_per_group=30), 3, ds_params="min_data_in_bin=1", cat=(0,))
+    _check(X, g, tc.grid(rng, 0.75, 1.25, len(c)), dict(min_data_in_leaf=20, min_data_per_group=30), 3, ds_params="min_data_in_bin=1", cat=(0,))
 
 
 def test_wide_categorical_selection_list_overflow(built):
@@ -463,7 +431,7 @@ def test_wide_categorical_selection_list_overflow(built):
     low = ((bins % 256) < 31) & ((bins // 256) < 20) & (bins > 0)
     assert len(np.unique(bins[low])) > 512
     noise = _on_grid(rng.standard_normal(int(bins.max()) + 1) * 0.05)       # distinct-ish ctr per category; equal keys sort by bin
-    g = np.where(low, -5.0, 5.0) + noise[bins] + _grid(rng, -0.01, 0.01, len(cat))
+    g = np.where(low, -5.0, 5.0) + noise[bins] + tc.grid(rng, -0.01, 0.01, len(cat))
     T, _ = _check(X, g, np.ones(len(cat)), dict(min_data_in_leaf=5, min_data_per_group=10, cat_smooth=10.0), 3,
                   ds_params="min_data_in_bin=1", cat=(0,))
     assert T["is_cat"][0]
@@ -486,7 +454,7 @@ def test_feature_without_root_split_is_not_split_in_children(built):
     n = 6000
     a = np.repeat([0.0, 1.0], n // 2)
     b = np.tile(np.where(np.arange(n // 2) < 300, 1.0, 0.0), 2)
-    g = np.where(a == 0, -1.0, 1.0) * np.where(b == 1, 2.0, 1.0) + _grid(rng, -0.125, 0.125, n)
+    g = np.where(a == 0, -1.0, 1.0) * np.where(b == 1, 2.0, 1.0) + tc.grid(rng, -0.125, 0.125, n)
     X = np.stack([a, b], axis=1)
     T, _ = _check(X, g, np.ones(n), dict(min_data_in_leaf=20, min_gain_to_split=100.0), 3, expect_leaves=2)
     assert not T["rounds"][0][0][2][1].splittable

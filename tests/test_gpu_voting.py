@@ -2,17 +2,17 @@
 local histograms, the ranks vote on top_k features per leaf, and only the voted features' histograms are all-reduced and scanned globally.
 
 All ranks are rank-threads of this process on device 0 (the same-device communicator), so every test runs on one GPU; the NCCL variant
-runs one rank per GPU and is skipped with fewer than two.  Trees are pinned against the NumPy restatement in voting_ref.py on custom
-gradients and hessians on a 2^-10 grid (as test_gpu_split_scan.py does for the serial scan): K4's fixed-point quantisation is exact there,
+runs one rank per GPU and is skipped with fewer than two.  Trees are pinned against the NumPy restatement in voting_ref.py (grown by
+tree_ref.py, compared at the bar tree_check.py describes) on custom gradients and hessians on a 2^-10 grid (as test_gpu_split_scan.py does for the serial scan): K4's fixed-point quantisation is exact there,
 so the local and the reduced int64 histograms equal NumPy's fp64 ones bit for bit and only the scans, the vote and the pick are under test."""
 import subprocess
-import threading
 
 import numpy as np
 import pytest
 
 import split_scan_ref as ref
-import voting_ref as V
+import tree_check as tc
+import tree_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -26,35 +26,6 @@ def _ngpu():
         return len([l for l in out.splitlines() if l.startswith("GPU ")])
     except Exception:
         return 0
-
-
-def _on_ranks(R, base_port, body, device_of=lambda r: 0):
-    """body(r) on R rank-threads, rank r on device_of(r), between network_init and network_free; returns (results, errors)"""
-    from mmlspark_b200 import capi
-    machines = ",".join("127.0.0.1:%d" % (base_port + r) for r in range(R))
-    out, errs = [None] * R, []
-
-    def task(r):
-        try:
-            capi.set_device(device_of(r))
-            if R == 1:
-                out[r] = body(r)
-                return
-            capi.network_init(machines, base_port + r, 120, R)
-            try:
-                out[r] = body(r)
-            finally:
-                capi.network_free()
-        except Exception as e:   # noqa
-            errs.append((r, str(e)))
-
-    ts = [threading.Thread(target=task, args=(r,)) for r in range(R)]
-    for t in ts:
-        t.start()
-    for t in ts:
-        t.join(300)
-    assert not any(t.is_alive() for t in ts), "a rank-thread did not finish"
-    return out, errs
 
 
 def _skewed(seed, rank_rows, F=30, per_rank=5, nan_feature=29):
@@ -103,17 +74,13 @@ def _train(X, y, rank_rows, params, iters, port, device_of=lambda r: 0, grads=No
         finally:
             b.free(); ds.free()
 
-    res, errs = _on_ranks(len(rank_rows), port, body, device_of)
+    res, errs = tc.on_ranks(len(rank_rows), port, body, device_of)
     assert not errs, errs
     return res
 
 
 def _categorical(ds_params):
     return [int(c) for tok in ds_params.split() if tok.startswith("categorical_feature=") for c in tok.split("=")[1].split(",")]
-
-
-def _trees(model):
-    return model.split("\nparameters:")[0]
 
 
 def _grid_gradients(y, seed):
@@ -129,70 +96,20 @@ def _features(res, F, cat=()):
             for f in range(F) if not infos[f]["is_trivial"]]
 
 
-def _compare_tree(t, T, side, lr=1.0):
-    """the engine's tree t (parse_model) against voting_ref's T: structure, thresholds, default directions, category sets and counts
-    exact, split_gain equal to the reference's float32 gain as printed (%g), leaf values within 1e-12 relative"""
-    assert t["num_leaves"] == T["num_leaves"]
-    nl = T["num_leaves"]
-    if nl > 1:
-        assert t["split_feature"].tolist() == T["split_feature"]
-        assert t["left_child"].tolist() == T["left_child"] and t["right_child"].tolist() == T["right_child"]
-        assert t["leaf_count"].tolist() == T["leaf_count"] and t["internal_count"].tolist() == T["internal_count"]
-        for i in range(nl - 1):
-            f, dt = T["split_feature"][i], int(t["decision_type"][i])
-            assert bool(dt & 1) == T["is_cat"][i], "node %d: categorical flag" % i
-            if T["is_cat"][i]:
-                k = int(t["threshold"][i])
-                words = t["cat_threshold"][t["cat_boundaries"][k]:t["cat_boundaries"][k + 1]]
-                cats = {32 * w + j for w, word in enumerate(words) for j in range(32) if (int(word) >> j) & 1}
-                got = {b for b, c in enumerate(side["b2c"][f]) if b > 0 and c in cats}
-                assert got == set(T["cat_bins"][i]), "node %d: category bins" % i
-            else:
-                hit = np.nonzero(side["ub"][f] == t["threshold"][i])[0]
-                assert len(hit) == 1 and hit[0] == T["threshold_bin"][i], "node %d: threshold %r" % (i, t["threshold"][i])
-                assert bool(dt & 2) == T["default_left"][i], "node %d: default_left" % i
-            assert t["split_gain"][i] == float("%g" % T["split_gain"][i]), "node %d: split_gain %r vs %g" % (i, t["split_gain"][i], T["split_gain"][i])
-    np.testing.assert_allclose(t["leaf_value"], np.asarray(T["leaf_value"]) * lr, rtol=1e-12, atol=1e-300)
-
-
 def _check_against_reference(res, X, g, h, rank_of_row, R, top_k, num_leaves, cat=()):
-    """every rank holds the same model; its tree equals voting_ref.grow_voting_tree on the same (g, h)"""
+    """every rank holds the same model; its tree equals tree_ref.grow_tree's voting tree on the same (g, h)"""
     from mmlspark_b200.modeltext import parse_model
     bins = np.concatenate([r["bins"] for r in res])
-    T = V.grow_voting_tree(bins, g, h, _features(res, X.shape[1], cat), ref.Params(min_data_in_leaf=20), num_leaves, rank_of_row, R, top_k)
+    T = tree_ref.grow_tree(bins, g, h, _features(res, X.shape[1], cat), ref.Params(min_data_in_leaf=20), num_leaves,
+                           voting=(rank_of_row, R, top_k))
     for r in range(R):
         assert res[r]["model"] == res[0]["model"]
-    _compare_tree(parse_model(res[0]["model"])["trees"][0], T, res[0])
+    tc.compare_tree(parse_model(res[0]["model"])["trees"][0], T, res[0]["ub"], res[0]["b2c"])
     return T
 
 
-def _quantized(v):
-    """K3's fixed-point grid: q = rint(v * 2^e), e = 34 - ilogb(max |v|) over every rank's rows; the histograms are exact sums of q, so
-    NumPy's fp64 sums of q * 2^-e equal the engine's int64 ones"""
-    m = np.float32(np.max(np.abs(v)))
-    e = 34 - (int(np.frexp(m)[1]) - 1) if m > 0 and np.isfinite(m) else 0
-    return np.rint(v.astype(np.float64) * 2.0 ** e) * 2.0 ** -e
-
-
-def _bags(n, iters, fraction, seed):
-    """GBDT::Bagging with bagging_freq = 1 on one rank: per 1024-row block an LCG seeded seed + block, row j of a block takes the next
-    draw ((x >> 16) & 0x7fff) / 32768 < fraction; the states carry over to the next iteration's draw"""
-    blocks = (n + 1023) // 1024
-    x = np.arange(blocks, dtype=np.uint64) + np.uint64(seed)
-    out = []
-    for _ in range(iters):
-        take = np.zeros(blocks * 1024, bool)
-        for j in range(1024):
-            live = j < n - np.arange(blocks) * 1024
-            nx = (x * np.uint64(214013) + np.uint64(2531011)) & np.uint64(0xFFFFFFFF)
-            x = np.where(live, nx, x)
-            take[np.arange(blocks) * 1024 + j] = live & (((x >> np.uint64(16)) & np.uint64(0x7FFF)).astype(np.float64) / 32768.0 < fraction)
-        out.append(take[:n])
-    return out
-
-
 def _check_boosting(res, X, rank_rows, R, top_k, K, lr, num_leaves, bag=None):
-    """every tree of a boosting run equals voting_ref.grow_voting_tree on the gradients the engine trained it on (read back before each
+    """every tree of a boosting run equals tree_ref.grow_tree's voting tree on the gradients the engine trained it on (read back before each
     iteration, quantised as K3 does) over the rows it was grown on (bag: (fraction, seed) of plain bagging)"""
     from mmlspark_b200.modeltext import parse_model
     trees = parse_model(res[0]["model"])["trees"]
@@ -204,17 +121,18 @@ def _check_boosting(res, X, rank_rows, R, top_k, K, lr, num_leaves, bag=None):
     const_h = res[0]["info"]["constant_hessian"]
     bags = None
     if bag is not None:
-        per_rank = [_bags(n_r, iters, bag[0], bag[1]) for n_r in rank_rows]
+        per_rank = [tc.bags(n_r, iters, bag[0], bag[1]) for n_r in rank_rows]
         bags = [np.concatenate([per_rank[r][it] for r in range(R)]) for it in range(iters)]
     for it in range(iters):
         for k in range(K):
             g = np.concatenate([r["grads"][it][0].reshape(K, -1)[k] for r in res])
             h = np.concatenate([r["grads"][it][1].reshape(K, -1)[k] for r in res])
-            gq = _quantized(g)
-            hq = np.ones(len(h)) if const_h else _quantized(h)
+            gq = tc.quantized(g)
+            hq = np.ones(len(h)) if const_h else tc.quantized(h)
             rows = np.arange(len(g)) if bags is None else np.nonzero(bags[it])[0]
-            T = V.grow_voting_tree(bins[rows], gq[rows], hq[rows], feats, ref.Params(min_data_in_leaf=20), num_leaves, rank_of_row[rows], R, top_k)
-            _compare_tree(trees[it * K + k], T, res[0], lr)
+            T = tree_ref.grow_tree(bins[rows], gq[rows], hq[rows], feats, ref.Params(min_data_in_leaf=20), num_leaves,
+                                   voting=(rank_of_row[rows], R, top_k))
+            tc.compare_tree(trees[it * K + k], T, res[0]["ub"], res[0]["b2c"], lr)
 
 
 def _custom_params(R, top_k, learner="voting", extra=""):
@@ -233,7 +151,7 @@ def test_voting_tree_matches_reference(built, R, top_k):
     assert all(len(v[0]) <= top_k for v in T["voted"])
     # the data-parallel learner on the same gradients splits the root on the shared feature, which no rank votes for at top_k <= 5
     dp = _train(X, y, rank_rows, _custom_params(R, top_k, "data_parallel"), 1, 27300 + 20 * R + top_k, grads=(g, h))
-    assert _trees(dp[0]["model"]) != _trees(res[0]["model"])
+    assert tc.trees(dp[0]["model"]) != tc.trees(res[0]["model"])
     assert R * 5 not in T["voted"][0][0]
 
 
@@ -256,7 +174,7 @@ def test_one_rank_equals_data_parallel(built):
     X, y, _ = _skewed(5, [20000], per_rank=5)
     a = _train(X, y, [20000], _params("regression", 1, "voting", 2), 10, 27600)
     b = _train(X, y, [20000], _params("regression", 1, "data_parallel", 2), 10, 27610)
-    assert _trees(a[0]["model"]) == _trees(b[0]["model"])
+    assert tc.trees(a[0]["model"]) == tc.trees(b[0]["model"])
     assert a[0]["comm"] == dict(hist_bytes=0, record_bytes=0, splits=10 * 14)
 
 
@@ -285,7 +203,7 @@ def test_voting_boosting(built, objective, R, top_k):
     for r in range(R):
         assert vt[r]["model"] == vt[0]["model"]
     _check_boosting(vt, X, rank_rows, R, top_k, 1, lr, 15)
-    assert _trees(vt[0]["model"]) != _trees(dp[0]["model"])
+    assert tc.trees(vt[0]["model"]) != tc.trees(dp[0]["model"])
     splits = iters * 14
     assert vt[0]["comm"]["splits"] == splits and dp[0]["comm"]["splits"] == splits
     col = 256 * 16
@@ -340,7 +258,7 @@ def test_voting_bundles_equal_unbundled(built):
     p = "objective=binary num_leaves=15 tree_learner=voting top_k=4 num_machines=2 verbosity=-1 metric= " + ds
     a = _train(X, y, rank_rows, p, 8, 29100, ds_params=ds)
     b = _train(X, y, rank_rows, p + " enable_bundle=false", 8, 29110, ds_params=ds + " enable_bundle=false")
-    assert _trees(a[0]["model"]) == _trees(b[0]["model"])
+    assert tc.trees(a[0]["model"]) == tc.trees(b[0]["model"])
     for r in range(2):
         assert np.array_equal(a[r]["scores"], b[r]["scores"])
 
@@ -380,7 +298,7 @@ def test_voting_rejects_at_create(built, case):
         finally:
             ds.free()
 
-    res, errs = _on_ranks(2, 29300 + (0 if case == "top_k" else 10), body)
+    res, errs = tc.on_ranks(2, 29300 + (0 if case == "top_k" else 10), body)
     assert not errs, errs
     want = "top_k > 0" if case == "top_k" else "more than 256 bins"
     assert all(want in m for m in res), res
@@ -399,10 +317,10 @@ def test_estimator_voting_parallel(built):
     est = LightGBMRegressor(parallelism="voting_parallel", topK=3, numTasks=2, numIterations=5, defaultListenPort=29400)
     mv = est.fit(df)
     md = LightGBMRegressor(parallelism="data_parallel", topK=3, numTasks=2, numIterations=5, defaultListenPort=29420).fit(df)
-    assert _trees(mv.getNativeModel()) != _trees(md.getNativeModel())
+    assert tc.trees(mv.getNativeModel()) != tc.trees(md.getNativeModel())
     params = est.getTrainParams(2, df).to_string()
     assert "tree_learner=voting_parallel" in params and "top_k=3" in params
     ds = dataset_params(est.get("maxBin"), est.get("binSampleCount"), est.get("numThreads"), [])
     swap = np.r_[10000:20000, 0:10000]
     low = [_train(X, y, rank_rows, params, 5, 29440, ds_params=ds), _train(X[swap], y[swap], rank_rows, params, 5, 29450, ds_params=ds)]
-    assert _trees(mv.getNativeModel()) in [_trees(r[0]["model"]) for r in low]
+    assert tc.trees(mv.getNativeModel()) in [tc.trees(r[0]["model"]) for r in low]

@@ -1,12 +1,13 @@
-"""The interaction-constraints restatement (interaction_ref.py) on its own: the engine's set masks equal LightGBM's branch rule, a single
-set of every feature grows the unconstrained tree, and constrained trees keep every path inside one set while scanning as without
-constraints."""
+"""The interaction-constraints restatement (interaction_ref.py, grown by tree_ref.py) on its own: the engine's set masks equal LightGBM's
+branch rule, a single set of every feature grows the unconstrained tree, and constrained trees keep every path inside one set while
+scanning as without constraints."""
 import numpy as np
 import pytest
 
 import extra_trees_ref as X3
 import interaction_ref as I
 import split_scan_ref as ref
+import tree_ref
 
 
 def _random_constraints(rng, nf):
@@ -57,13 +58,13 @@ _SHAPE = ("split_feature", "threshold_bin", "default_left", "left_child", "right
 def test_one_set_of_every_feature_is_unconstrained():
     bins, g, h, feats = _data(3)
     p = ref.Params(min_data_in_leaf=20)
-    T = I.grow_tree(bins, g, h, feats, p, 16, [[0, 1, 2, 3]])
-    U = ref.grow_tree(bins, g, h, feats, p, 16)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 16, constraints=[[0, 1, 2, 3]])
+    U = tree_ref.grow_tree(bins, g, h, feats, p, 16)
     assert T["num_leaves"] == U["num_leaves"] > 8
     for k in _SHAPE:
         assert T[k] == U[k], k
-    E = I.grow_tree(bins, g, h, feats, p, 16, [[3, 2, 1, 0]], extra_trees=True, extra_seed=5)
-    V = X3.grow_tree(bins, g, h, feats, p, 16, True, 5)
+    E = tree_ref.grow_tree(bins, g, h, feats, p, 16, constraints=[[3, 2, 1, 0]], streams=X3.Streams(feats, 5))
+    V = tree_ref.grow_tree(bins, g, h, feats, p, 16, streams=X3.Streams(feats, 5))
     for k in _SHAPE:
         assert E[k] == V[k], k
 
@@ -71,7 +72,7 @@ def test_one_set_of_every_feature_is_unconstrained():
 @pytest.mark.parametrize("cons", [[[0, 1], [2, 3]], [[0], [1], [2, 3]], [[0, 1, 2], [2, 3]], [[1, 2]]])
 def test_paths_stay_inside_one_set(cons):
     bins, g, h, feats = _data(4)
-    T = I.grow_tree(bins, g, h, feats, ref.Params(min_data_in_leaf=20), 16, cons)
+    T = tree_ref.grow_tree(bins, g, h, feats, ref.Params(min_data_in_leaf=20), 16, constraints=cons)
     assert T["num_leaves"] > 2
     sets = I.sets_of(cons, 4)
     for branch, mask in zip(T["branches"], T["masks"]):
@@ -88,7 +89,7 @@ def test_scans_and_flags_run_as_without_constraints():
     bins, g, h, feats = _data(5)
     p = ref.Params(min_data_in_leaf=20)
     s1 = X3.Streams(feats, 7)
-    T = I.grow_tree(bins, g, h, feats, p, 8, [[0]], extra_trees=True, extra_seed=7, streams=s1)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 8, constraints=[[0]], streams=s1)
     assert set(T["split_feature"]) == {0}
     root_scans = T["rounds"][0][0][2]
     assert set(root_scans) == {0, 1, 2, 3}

@@ -7,6 +7,7 @@ import pytest
 
 import monotone_ref as M
 import split_scan_ref as ref
+import tree_ref
 
 INF = math.inf
 
@@ -157,7 +158,7 @@ def test_grow_tree_is_monotone():
     h = np.ones(n)
     feats = [ref.Feature(0, 20), ref.Feature(1, 20), ref.Feature(2, 8)]
     p = ref.Params(min_data_in_leaf=20)
-    T = M.grow_tree(bins, g, h, feats, p, 16, [1, -1, 0], penalty=0.0)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 16, mono=[1, -1, 0], penalty=0.0)
     assert T["num_leaves"] > 4
 
     def leaf_of(row):

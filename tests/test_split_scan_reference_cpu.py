@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import split_scan_ref as ref
+import tree_ref
 
 GRID = 1.0 / 1024
 
@@ -210,8 +211,8 @@ def test_max_delta_step_clipping_changes_the_winner():
 def test_undecided_flags_a_near_tie_and_a_count_at_half():
     p = ref.Params(min_data_in_leaf=1)
     bins = np.array([[0], [1], [2], [3]])
-    T = ref.grow_tree(bins, np.array([-1.0, 1.0, 1.0, -1.0 - GRID]), np.ones(4), [ref.Feature(0, 4)], p, 2)
+    T = tree_ref.grow_tree(bins, np.array([-1.0, 1.0, 1.0, -1.0 - GRID]), np.ones(4), [ref.Feature(0, 4)], p, 2)
     assert ref.undecided(T) == []
     bins2 = np.array([[0], [1]])
-    T = ref.grow_tree(bins2, np.array([-1.0, 1.0]), np.array([1.0, 3.0]), [ref.Feature(0, 2)], ref.Params(min_data_in_leaf=0), 2)
+    T = tree_ref.grow_tree(bins2, np.array([-1.0, 1.0]), np.array([1.0, 3.0]), [ref.Feature(0, 2)], ref.Params(min_data_in_leaf=0), 2)
     assert any(".5 boundary" in w for w in ref.undecided(T))   # 2 rows, h = 1 and 3: rebuilt counts 0.5 and 1.5

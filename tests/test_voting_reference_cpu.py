@@ -1,4 +1,4 @@
-"""The NumPy restatement of the voting-parallel learner (voting_ref.py) on its own: the vote rule on hand-made records, the local top-k
+"""The NumPy restatement of the voting-parallel learner (voting_ref.py, grown by tree_ref.py) on its own: the vote rule on hand-made records, the local top-k
 order, one rank as the serial learner, and shard-skewed data on which the vote decides the tree.  No GPU."""
 import math
 
@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import split_scan_ref as ref
+import tree_ref
 import voting_ref as V
 
 GRID = 1.0 / 1024
@@ -59,8 +60,8 @@ def _skewed_bins(seed, rank_rows, F=12, nbin=16):
 def test_one_rank_is_the_serial_learner():
     bins, g, h, feats, rank_of_row = _skewed_bins(1, [3000])
     p = ref.Params(min_data_in_leaf=20)
-    T = V.grow_voting_tree(bins, g, h, feats, p, 8, rank_of_row, 1, 1)
-    S = ref.grow_tree(bins, g, h, feats, p, 8)
+    T = tree_ref.grow_tree(bins, g, h, feats, p, 8, voting=(rank_of_row, 1, 1))
+    S = tree_ref.grow_tree(bins, g, h, feats, p, 8)
     for k in ("split_feature", "threshold_bin", "left_child", "right_child", "leaf_count", "leaf_value"):
         assert T[k] == S[k]
 
@@ -74,16 +75,16 @@ def test_skewed_shards_vote_for_their_own_features(R):
     bins, g, h, feats, rank_of_row = _skewed_bins(10 + R, rank_rows)
     F = len(feats)
     p = ref.Params(min_data_in_leaf=20)
-    S = ref.grow_tree(bins, g, h, feats, p, 8)
+    S = tree_ref.grow_tree(bins, g, h, feats, p, 8)
     assert S["split_feature"][0] == F - 1
-    T1 = V.grow_voting_tree(bins, g, h, feats, p, 8, rank_of_row, R, 1)
+    T1 = tree_ref.grow_tree(bins, g, h, feats, p, 8, voting=(rank_of_row, R, 1))
     assert T1["voted"][0][1] is None and T1["voted"][0][0][0] in range(R)
     assert T1["split_feature"][0] in range(R) and T1["split_feature"] != S["split_feature"]
     for smaller, larger in T1["voted"]:
         assert len(smaller) <= 1 and (larger is None or len(larger) <= 1)
-    T3 = V.grow_voting_tree(bins, g, h, feats, p, 8, rank_of_row, R, R + 1)
+    T3 = tree_ref.grow_tree(bins, g, h, feats, p, 8, voting=(rank_of_row, R, R + 1))
     assert F - 1 in T3["voted"][0][0] and T3["split_feature"][0] == F - 1      # every rank's second best: the shared feature
-    TF = V.grow_voting_tree(bins, g, h, feats, p, 8, rank_of_row, R, F)
+    TF = tree_ref.grow_tree(bins, g, h, feats, p, 8, voting=(rank_of_row, R, F))
     assert TF["split_feature"][0] == S["split_feature"][0] and TF["threshold_bin"][0] == S["threshold_bin"][0]
     # counts of a voting tree are the hessian-rebuilt global counts of its splits, and they add up at every node
     for T in (T1, T3, TF):
