@@ -17,6 +17,9 @@
 
 namespace b200gbm {
 
+// LightGBM's kEpsilon (1e-15f): path smoothing is on when path_smooth exceeds it
+constexpr double kPathSmoothEps = static_cast<double>(1e-15f);
+
 struct Config {
   // --- core
   std::string objective = "regression";
@@ -41,6 +44,8 @@ struct Config {
   std::vector<int> monotone_constraints;    // per real feature -1, 0 or +1; non-empty: the constrained scans (TreeLearner, kernels.cuh kMono)
   std::string monotone_constraints_method = "basic";      // only "basic" trains (Booster checks at create)
   double monotone_penalty = 0.0;            // scales a monotone split's gain down near the root (kernels.cuh d_mono_penalty)
+  // > kPathSmoothEps: every split gain and leaf output is smoothed toward the parent leaf's output (kernels.cuh d_smooth_output)
+  double path_smooth = 0.0;
   // sets of real feature indices; a branch's split features stay inside one set (TreeLearner sets_of_, kernels.cuh d_pick_block)
   std::vector<std::vector<int>> interaction_constraints;
   std::string interaction_constraints_malformed;      // the value given when it does not parse (Booster fails at create)
@@ -217,6 +222,7 @@ struct Config {
     I("early_stopping_round", &early_stopping_round);
     B("extra_trees", &extra_trees); I("extra_seed", &extra_seed);
     S("monotone_constraints_method", &monotone_constraints_method); D("monotone_penalty", &monotone_penalty);
+    D("path_smooth", &path_smooth);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -250,6 +256,9 @@ struct Config {
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &categorical_feature, [](const std::string& x) { return std::atoi(x.c_str()); });
     }
     if (eval_at.empty()) eval_at = {1, 2, 3, 4, 5};
+    // [UPSTREAM] Config::CheckParamConflict: a smoothed leaf needs at least two rows.  min_data_in_leaf is re-read from raw above, so a
+    // reset that turns smoothing off gives back the value the caller set.
+    if (path_smooth > kPathSmoothEps && min_data_in_leaf < 2) min_data_in_leaf = 2;
     // metric resolution: empty => the objective's default metric (SURVEY.md B.5)
     metric.clear();
     auto it = raw.find("metric");
@@ -299,7 +308,7 @@ struct Config {
     s << "[top_k: " << top_k << "]\n[monotone_constraints: " << join_i(monotone_constraints) << "]\n";
     s << "[monotone_constraints_method: " << monotone_constraints_method << "]\n[monotone_penalty: " << Num(monotone_penalty) << "]\n";
     s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
-    s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: 0]\n";
+    s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: " << Num(path_smooth) << "]\n";
     s << "[interaction_constraints: " << join_sets(interaction_constraints) << "]\n";
     s << "[verbosity: " << verbosity << "]\n[saved_feature_importance_type: 0]\n[linear_tree: 0]\n[max_bin: " << max_bin << "]\n";
     s << "[max_bin_by_feature: " << max_bin_by_feature << "]\n[min_data_in_bin: " << min_data_in_bin << "]\n";

@@ -1368,6 +1368,16 @@ static void CheckByNode(const Config& cfg, bool voting_parallel) {
   if (f < 1.0 && voting_parallel) Fatal(kVotingByNode);
 }
 
+// the voting learner's local scans and vote would need every leaf's output on every rank to smooth toward; not restated
+static const char* const kVotingPathSmooth = "tree_learner=voting does not support path_smooth with more than one machine; "
+                                             "use tree_learner=data_parallel or path_smooth=0";
+
+// path smoothing: the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+static void CheckPathSmooth(const Config& cfg, bool voting_parallel) {
+  if (!(cfg.path_smooth >= 0.0)) Fatal("path_smooth should be >= 0, got " + Config::Num(cfg.path_smooth));
+  if (cfg.path_smooth > kPathSmoothEps && voting_parallel) Fatal(kVotingPathSmooth);
+}
+
 Booster::Booster(const std::string& model_text) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1417,6 +1427,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
   CheckMonotone(cfg, *train, voting_);
   CheckInteraction(cfg, *train, voting_);
   CheckByNode(cfg, voting_);
+  CheckPathSmooth(cfg, voting_);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1760,6 +1771,7 @@ void Booster::ResetParameter(const char* params) {
       CheckMonotone(cfg, *train, voting_);
       CheckInteraction(cfg, *train, voting_);
       CheckByNode(cfg, voting_);
+      CheckPathSmooth(cfg, voting_);
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;

@@ -5,6 +5,7 @@
 #include <climits>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "config.h"
 #include "hist_kernel.cuh"
 
 namespace b200gbm {
@@ -66,6 +67,7 @@ struct SplitParams {
   double cat_l2, cat_smooth;                                   // categorical split search ([UPSTREAM] defaults 10, 10)
   int max_cat_threshold, max_cat_to_onehot, min_data_per_group;         // 32, 4, 100
   int interaction;                                             // 1 when interaction_constraints is non-empty (d_pick_block, d_round_ctl)
+  double path_smooth;                                          // > kPathSmoothEps: outputs and gains smoothed (d_smooth_output)
 };
 
 // extra_trees (the scans' template parameter kExtra; [UPSTREAM] FeatureHistogram USE_RAND, FeatureMetainfo::rand): every used feature
@@ -123,6 +125,9 @@ struct LeafState {
   // monotone constraints (basic method): the bounds [mono_min, mono_max] of this leaf's output; the root's are (-inf, +inf), children
   // inherit their parent's and a numerical split on a monotone feature narrows them at the mid-point of the two outputs (d_round_ctl)
   double mono_min, mono_max;
+  // path smoothing: this leaf's output, the parent_output its scans smooth toward ([UPSTREAM] LeafSplits::weight).  A child's is the
+  // smoothed (and clamped) output the pick step gave it; the root's is its own unsmoothed output (k_tree_init).
+  double output;
   // interaction constraints: bit s is set when constraint set s holds every split feature on the path from the root to this leaf.  The
   // root's has every bit; a split on feature u gives both children parent & sets_of[u] (d_round_ctl).  Read only when p.interaction.
   unsigned long long inter_mask;
@@ -130,7 +135,8 @@ struct LeafState {
 
 // The scans' constraint arguments.
 // Monotone constraints ([UPSTREAM] monotone_constraints.hpp BasicLeafConstraints, FeatureHistogram USE_MC): the scans' template parameter
-// kMono.  type: per inner feature -1, 0 or +1 (the real feature's monotone_constraints entry); penalty: monotone_penalty.
+// kMono, which path smoothing (USE_SMOOTHING) turns on too.  type: per inner feature -1, 0 or +1 (the real feature's
+// monotone_constraints entry, all 0 without a list); penalty: monotone_penalty.
 // Interaction constraints ([UPSTREAM] ColSampler::GetByNode): sets_of[u], per inner feature, has bit s set when constraint set s holds
 // the feature's real index; feature u may split a leaf iff sets_of[u] & inter_mask != 0.  Read by the pick step only when p.interaction.
 struct ConstraintArgs { const signed char* type; double penalty; const unsigned long long* sets_of; };
@@ -196,18 +202,41 @@ __device__ __noinline__ double d_leaf_gain(double g, double h, const SplitParams
   double sg = (p.l1 > 0) ? d_threshold_l1(g, p.l1) : g;
   return -(2.0 * sg * out + (h + p.l2) * out * out);
 }
-// monotone constraints: a child's output, CalculateSplittedLeafOutput clamped to the leaf's bounds after max_delta_step
-__device__ __forceinline__ double d_mono_output(double g, double h, const SplitParams& p, double lo, double hi) {
+// path smoothing ([UPSTREAM] CalculateSplittedLeafOutput<USE_SMOOTHING>): the output of a leaf of n rows (L1, l2, max_delta_step as
+// d_calc_output), then, when p.path_smooth > kPathSmoothEps, ret * (n/s) / (n/s + 1) + parent_output / (n/s + 1) in that order.
+// Out of line for d_leaf_gain's reason.
+__device__ __noinline__ double d_smooth_output(double g, double h, int n, double parent_output, const SplitParams& p) {
   double ret = d_calc_output(g, h, p);
+  if (p.path_smooth > kPathSmoothEps) {
+    const double w = n / p.path_smooth;
+    ret = ret * w / (w + 1) + parent_output / (w + 1);
+  }
+  return ret;
+}
+// path smoothing: a leaf's gain at its smoothed output ([UPSTREAM] GetLeafGain<USE_SMOOTHING>, never clamped to monotone bounds), the
+// scans' min_gain_shift; d_leaf_gain's when smoothing is off.  Out of line for d_leaf_gain's reason.
+__device__ __noinline__ double d_smooth_leaf_gain(double g, double h, int n, double parent_output, const SplitParams& p) {
+  if (!(p.path_smooth > kPathSmoothEps)) return d_leaf_gain(g, h, p);
+  const double out = d_smooth_output(g, h, n, parent_output, p);
+  const double sg = (p.l1 > 0) ? d_threshold_l1(g, p.l1) : g;
+  return -(2.0 * sg * out + (h + p.l2) * out * out);
+}
+// monotone constraints: a child's output of n rows, CalculateSplittedLeafOutput (smoothed toward parent_output when path smoothing is
+// on) clamped to the leaf's bounds
+__device__ __forceinline__ double d_mono_output(double g, double h, int n, double parent_output, const SplitParams& p, double lo, double hi) {
+  double ret = d_smooth_output(g, h, n, parent_output, p);
   if (ret < lo) ret = lo;
   else if (ret > hi) ret = hi;
   return ret;
 }
-// The kMono scans' split gain ([UPSTREAM] GetSplitGains<USE_MC>): both children's outputs clamped to the leaf's bounds [lo, hi], then
+// The kMono scans' split gain ([UPSTREAM] GetSplitGains<USE_MC, USE_SMOOTHING>): both children's outputs (of lc and rc rows, smoothed
+// toward the leaf's output `parent_output` when path smoothing is on) clamped to the leaf's bounds [lo, hi], then
 // GetLeafGainGivenOutput(left) + GetLeafGainGivenOutput(right) = -(2 ThresholdL1(g) out + (h + l2) out^2) at those outputs; 0 when the
-// outputs break the split feature's direction `mono` (left > right for +1, left < right for -1).  Out of line for d_leaf_gain's reason.
-__device__ __noinline__ double d_mono_split_gain(double lg, double lh, double rg, double rh, const SplitParams& p, double lo, double hi, int mono) {
-  const double lo_out = d_mono_output(lg, lh, p, lo, hi), ro_out = d_mono_output(rg, rh, p, lo, hi);
+// outputs break the split feature's direction `mono` (left > right for +1, left < right for -1).  Without monotone constraints the
+// bounds are (-inf, +inf) and mono is 0, which leaves the smoothed gain.  Out of line for d_leaf_gain's reason.
+__device__ __noinline__ double d_mono_split_gain(double lg, double lh, double rg, double rh, int lc, int rc, double parent_output, const SplitParams& p,
+                                                 double lo, double hi, int mono) {
+  const double lo_out = d_mono_output(lg, lh, lc, parent_output, p, lo, hi), ro_out = d_mono_output(rg, rh, rc, parent_output, p, lo, hi);
   if ((mono > 0 && lo_out > ro_out) || (mono < 0 && lo_out < ro_out)) return 0.0;
   const double slg = (p.l1 > 0) ? d_threshold_l1(lg, p.l1) : lg, srg = (p.l1 > 0) ? d_threshold_l1(rg, p.l1) : rg;
   return -(2.0 * slg * lo_out + (lh + p.l2) * lo_out * lo_out) + -(2.0 * srg * ro_out + (rh + p.l2) * ro_out * ro_out);
@@ -767,6 +796,9 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
     r.global_count = static_cast<int>(ctrl->root_q[2]);
     r.sum_g = static_cast<double>(ctrl->root_q[0]) * ctrl->inv_g;
     r.sum_h = static_cast<double>(ctrl->root_q[1]) * ctrl->inv_h;
+    // path smoothing: the root's parent_output is its own output, from the all-reduced sums without the scans' 2 kEpsilon; smoothing
+    // toward it gives it back
+    r.output = d_calc_output(r.sum_g, r.sum_h, p);
     ctrl->num_leaves = 1; ctrl->left_leaf = 0; ctrl->right_leaf = -1; ctrl->smaller = 0; ctrl->larger = -1;
     ctrl->go = 0; ctrl->finished = 0; ctrl->split_leaf = -1; ctrl->pending = 0; ctrl->round = 0; ctrl->trace_rows = 0;
     ctrl->col_state = col_state;
@@ -780,8 +812,10 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
 // monotone feature narrows them at mid = (left_out + right_out) / 2 — the left child's max and the right child's min for +1, the mirror
 // for -1.
 // Interaction constraints (interaction != 0): both children's set mask is the parent's & the split feature's sets_of word.
+// Path smoothing: each child keeps its output as the parent_output of its own scans.
 __device__ __noinline__ void d_constrain_children(LeafState& L, LeafState& R, int monotone_type, int is_cat, double left_out, double right_out,
                                                   int interaction, const unsigned long long& inter_sets) {
+  L.output = left_out; R.output = right_out;
   R.mono_min = L.mono_min; R.mono_max = L.mono_max;
   if (monotone_type != 0 && !is_cat) {
     const double mid = (left_out + right_out) / 2.0;
@@ -955,8 +989,9 @@ __device__ __forceinline__ void d_cat_walk(int used_bin, int max_num_cat, int nu
 // kExtra (extra_trees): xr is the feature's stream state before this scan's draw.  One-hot draws r over the num_bin - 1 category bins
 // and evaluates only bin r + 1; many-vs-many draws r over d_cat_rand_range and evaluates only the prefixes of r + 1 bins.  Returns the
 // number of draws taken (0 or 1), in every lane.
-// kMono (monotone constraints): every gain is d_mono_split_gain's at outputs clamped to the leaf's bounds; categorical features carry no
-// constraint of their own.
+// kMono (monotone constraints or path smoothing): every gain is d_mono_split_gain's at outputs smoothed toward the leaf's output and
+// clamped to the leaf's bounds, with the children's estimated counts (one-hot: num_data - cnt and cnt); categorical features carry no
+// constraint of their own.  min_gain_shift is d_smooth_leaf_gain's.
 template <bool kExtra, bool kMono>
 __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const long long (&qh)[8], int lane, const FeatMeta m, const LeafState& L,
                                                   double inv_g, double inv_h, const SplitParams& p, uint8_t* flag, SplitCand* outp, double* ws,
@@ -967,7 +1002,7 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
+  const double min_gain_shift = (kMono ? d_smooth_leaf_gain(sum_g, sum_h, num_data, L.output, p) : d_leaf_gain(sum_g, sum_h, p)) + p.min_gain_to_split;
   const bool onehot = m.num_bin <= p.max_cat_to_onehot;
   int drew = 0, rand_t = -1;      // rand_t: the one candidate index evaluated, -1: every candidate
   if (kExtra && onehot) { rand_t = d_extra_draw(&xr, m.num_bin - 1); drew = m.num_bin > 1 ? 1 : 0; }
@@ -987,7 +1022,7 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
         const int other = num_data - cnt;
         const double oh = sum_h - h - kEpsD;
         if (other >= p.min_data_in_leaf && oh >= p.min_sum_hessian && (!kExtra || b - 1 == rand_t)) {
-          const double gain = kMono ? d_mono_split_gain(sum_g - g, oh, g, h + kEpsD, p, L.mono_min, L.mono_max, 0)
+          const double gain = kMono ? d_mono_split_gain(sum_g - g, oh, g, h + kEpsD, other, cnt, L.output, p, L.mono_min, L.mono_max, 0)
                                     : d_leaf_gain(sum_g - g, oh, p) + d_leaf_gain(g, h + kEpsD, p);
           if (gain > min_gain_shift) {
             any_valid = true;
@@ -1063,7 +1098,8 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
       d_cat_walk<kExtra>(used_bin, max_num_cat, num_data, sum_h, cnt_factor, p, rand_t,
                          [&](double* g, double* h) { const int t = order[pos]; pos += dir; *g = sg[t]; *h = sh[t]; },
                          [&](int i, double slg, double slh, double srh, int left_count) {
-                           const double gain = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, srh, pc, L.mono_min, L.mono_max, 0)
+                           const double gain = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, srh, left_count, num_data - left_count, L.output, pc,
+                                                                         L.mono_min, L.mono_max, 0)
                                                      : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, srh, pc);
                            if (gain <= min_gain_shift) return;
                            any_valid = true;
@@ -1132,8 +1168,9 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
 // The two leaves of the round are handled side by side (threads 0..127: smaller, 128..255: larger) with warp-shuffle argmaxes — the
 // first version looped over the two leaves with an 8-step shared-memory tree each (18 block barriers) and ncu showed this serial tail
 // taking longer than the scan itself.  The order (gain desc, real feature index asc) is total, so any reduction shape picks the same winner.
-// kMono (monotone constraints): the outputs are clamped to the leaf's bounds ([UPSTREAM] CalculateSplittedLeafOutput<USE_MC>) and the
-// split feature's constraint (mono_type, per inner feature) is kept for the round controller's bound update.
+// kMono (monotone constraints or path smoothing): the outputs are smoothed toward the leaf's output with the candidate's estimated
+// counts, then clamped to the leaf's bounds ([UPSTREAM] CalculateSplittedLeafOutput<USE_MC, USE_SMOOTHING>), and the split feature's
+// constraint (mono_type, per inner feature) is kept for the round controller's bound update.
 // p.interaction (interaction constraints): a feature that may not split the leaf (sets_of[u] & the leaf's inter_mask == 0) is passed
 // over here and only here, after the scans, so the scans, their is_splittable flags and the extra_trees draws are what they are
 // without constraints ([UPSTREAM] SerialTreeLearner::ComputeBestSplitForFeature filters after FindBestThreshold).  The chosen
@@ -1187,8 +1224,8 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
       SplitParams pc = p;
       pc.l2 += c.l2_extra;
       if constexpr (kMono) {
-        b.left_out = d_mono_output(c.left_g, c.left_h, pc, L.mono_min, L.mono_max);
-        b.right_out = d_mono_output(L.sum_g - c.left_g, sum_h - c.left_h, pc, L.mono_min, L.mono_max);
+        b.left_out = d_mono_output(c.left_g, c.left_h, b.left_count, L.output, pc, L.mono_min, L.mono_max);
+        b.right_out = d_mono_output(L.sum_g - c.left_g, sum_h - c.left_h, b.right_count, L.output, pc, L.mono_min, L.mono_max);
         b.monotone_type = mono_type[c.feature];
       } else {
         b.left_out = d_calc_output(c.left_g, c.left_h, pc);
@@ -1667,8 +1704,9 @@ __device__ __forceinline__ void d_block_excl3(long long& a, long long& b, long l
 // lowest).  hist = the leaf's reduced histogram of the feature in its pool slot.  Returns through *outp (thread 0) and *flag.
 // kExtra (extra_trees): only the candidate with that threshold is evaluated, in either pass; the count and hessian tests before it
 // still skip and break as they do without it ([UPSTREAM] FindBestThresholdSequentially, USE_RAND: t - 1 + offset resp. t + offset).
-// kMono (monotone constraints): every gain, in both passes, is d_mono_split_gain's at outputs clamped to the leaf's bounds, 0 when they
-// break the feature's direction `mono`; min_gain_shift stays the leaf's unconstrained gain.
+// kMono (monotone constraints or path smoothing): every gain, in both passes, is d_mono_split_gain's at outputs smoothed toward the
+// leaf's output with the estimated counts and clamped to the leaf's bounds, 0 when they break the feature's direction `mono`;
+// min_gain_shift is d_smooth_leaf_gain's: the leaf's unconstrained gain, smoothed when path smoothing is on.
 template <bool kExtra, bool kMono>
 __device__ __noinline__ void d_scan_numeric(const long long* __restrict__ hist, const FeatMeta m, const LeafState& L, double inv_g, double inv_h,
                                             const SplitParams& p, uint8_t* flag, SplitCand* outp, int rand_thr, int mono) {
@@ -1680,7 +1718,7 @@ __device__ __noinline__ void d_scan_numeric(const long long* __restrict__ hist, 
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
+  const double min_gain_shift = (kMono ? d_smooth_leaf_gain(sum_g, sum_h, num_data, L.output, p) : d_leaf_gain(sum_g, sum_h, p)) + p.min_gain_to_split;
   const bool two_way = (m.num_bin > 2 && m.missing_type == 2);
   const int na = two_way ? 1 : 0;
   const int S = (m.num_bin + 255) / 256;
@@ -1715,7 +1753,7 @@ __device__ __noinline__ void d_scan_numeric(const long long* __restrict__ hist, 
       if (left_count < p.min_data_in_leaf || slh < p.min_sum_hessian) { stop = true; break; }
       if (kExtra && b - 1 != rand_thr) continue;
       const double slg = sum_g - srg;
-      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, p, L.mono_min, L.mono_max, mono)
+      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, left_count, right_count, L.output, p, L.mono_min, L.mono_max, mono)
                                 : d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       any_valid = true;
@@ -1778,7 +1816,7 @@ __device__ __noinline__ void d_scan_numeric(const long long* __restrict__ hist, 
       if (right_count < p.min_data_in_leaf || srh < p.min_sum_hessian) { f_stop = true; break; }
       if (kExtra && b != rand_thr) continue;
       const double srg = sum_g - slg;
-      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, p, L.mono_min, L.mono_max, mono)
+      const double gain = kMono ? d_mono_split_gain(slg, slh, srg, srh, left_count, right_count, L.output, p, L.mono_min, L.mono_max, mono)
                                 : d_leaf_gain(slg, slh, p) + d_leaf_gain(srg, srh, p);
       if (gain <= min_gain_shift) continue;
       f_valid = true;
@@ -1891,8 +1929,8 @@ __device__ __noinline__ void d_block_bitonic2(double* k, int* id, int stride, in
 // (smaller|larger, feature).  The histogram is reduced into the leaf's pool slot (parent - smaller for the larger child), the
 // max_cat_threshold smallest and largest ctr = g / (h + cat_smooth) among the bins that hold >= cat_smooth rows are selected in the
 // (ctr, bin) order of the reference's stable sort, and thread 0 accumulates from both ends exactly like the sequential code.
-// kMono (monotone constraints): constrained gains as in d_scan_numeric / d_scan_feature_cat, and a monotone numerical feature's
-// candidate gain times d_mono_penalty at the leaf's depth.
+// kMono (monotone constraints or path smoothing): output-based gains and min_gain_shift as in d_scan_numeric / d_scan_feature_cat, and
+// a monotone numerical feature's candidate gain times d_mono_penalty at the leaf's depth.
 template <bool kExtra, bool kMono>
 __global__ void __launch_bounds__(256)
 k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const FeatMeta* __restrict__ meta, const long long* __restrict__ H,
@@ -2080,14 +2118,15 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
                        });
   }
   __syncthreads();
-  const double min_gain_shift = d_leaf_gain(sum_g, sum_h, p) + p.min_gain_to_split;
+  const double min_gain_shift = (kMono ? d_smooth_leaf_gain(sum_g, sum_h, num_data, L.output, p) : d_leaf_gain(sum_g, sum_h, p)) + p.min_gain_to_split;
   if (threadIdx.x < 2 * kCatListMax) {
     const int d = threadIdx.x / kCatListMax, i = threadIdx.x % kCatListMax;
     if (s_pgain[d][i] == 0.0) {
       SplitParams pc = p;
       pc.l2 += p.cat_l2;
       const double slg = s_plg[d][i], slh = s_plh[d][i];
-      s_pgain[d][i] = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, sum_h - slh, pc, L.mono_min, L.mono_max, 0)
+      s_pgain[d][i] = kMono ? d_mono_split_gain(slg, slh, sum_g - slg, sum_h - slh, s_plc[d][i], num_data - s_plc[d][i], L.output, pc,
+                                                L.mono_min, L.mono_max, 0)
                             : d_leaf_gain(slg, slh, pc) + d_leaf_gain(sum_g - slg, sum_h - slh, pc);
     }
   }
@@ -2383,8 +2422,9 @@ __device__ __noinline__ void d_bynode_sample(TreeCtrl* ctrl, const LeafState* le
   __threadfence();      // every thread's mask bytes, before thread 0 takes the kernel's scan ticket
 }
 
-// kMono (monotone constraints): the constrained scans (d_scan_numeric, d_scan_feature_cat), a monotone feature's candidate gain
-// times d_mono_penalty at the leaf's depth, and outputs clamped to the leaf's bounds in the pick step.
+// kMono (monotone constraints or path smoothing): the output-based scans (d_scan_numeric, d_scan_feature_cat), a monotone feature's
+// candidate gain times d_mono_penalty at the leaf's depth, and outputs smoothed and clamped to the leaf's bounds in the pick step.
+// Without a constraint list the bounds stay (-inf, +inf) and every type is 0, so only the smoothing remains.
 template <int kMode, bool kExtra = false, bool kMono = false>
 __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,

@@ -10,8 +10,8 @@ constexpr int kPartTickets = 8;                   // k_partition: chunks a block
 // ColSampler's GetCnt: the size of a feature sample ([UPSTREAM] ColSampler::GetCnt)
 static int SampleCount(int total, double fraction) { return std::max(static_cast<int>(total * fraction + 0.5), std::min(2, total)); }
 
-// The split scans of one (extra_trees, monotone constraints) pair, indexed [extra_trees][monotone].  Each pair has its own instantiations,
-// so that the default one compiles to what it was without either.
+// The split scans of one (extra_trees, output-based gains) pair, indexed [extra_trees][monotone constraints or path smoothing].  Each pair
+// has its own instantiations, so that the default one compiles to what it was without either.
 struct ScanKernels {
   decltype(&k_scan<kScanPlain>) scan;
   decltype(&k_scan_wide<false, false>) scan_wide;
@@ -164,6 +164,10 @@ void TreeLearner::ResetConfig(const Config& cfg) {
   std::vector<signed char> types(train_.nf_pad, 0);
   if (monotone_)
     for (int u = 0; u < train_.nf; ++u) types[u] = static_cast<signed char>(cfg.monotone_constraints[train_.used[u]]);
+  // path smoothing runs the same output-based scans, with all-zero types when there is no list.  Never on for the voting learner
+  // (Booster rejects path_smooth for it).
+  sp_.path_smooth = cfg.path_smooth;
+  smooth_ = !voting_ && cfg.path_smooth > kPathSmoothEps;
   if (types != mono_host_) {
     mono_host_ = std::move(types);
     mono_.Upload(mono_host_.data(), mono_host_.size(), stream_);
@@ -485,7 +489,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
         comm_hist_bytes_ += static_cast<long long>(slot_elems_ * sizeof(long long));
       }
       mark();
-      const ScanKernels& k = kScanKernels[extra_trees_][monotone_];
+      const ScanKernels& k = kScanKernels[extra_trees_][monotone_ || smooth_];
       if (d.nw > 0) {
         k.scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
                                                                  cons);

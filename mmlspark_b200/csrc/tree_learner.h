@@ -54,6 +54,7 @@ class TreeLearner {
   bool extra_trees_ = false;     // cfg.extra_trees as of the last ResetConfig: launch the scans' extra_trees instantiations
   bool monotone_ = false;        // cfg.monotone_constraints non-empty as of the last ResetConfig: launch the scans' kMono instantiations
   double monotone_penalty_ = 0.0;
+  bool smooth_ = false;          // path_smooth > kPathSmoothEps as of the last ResetConfig: launch the kMono instantiations too
   std::vector<signed char> mono_host_;      // [nf_pad] each inner feature's monotone constraint, as uploaded to mono_
   DevBuf<signed char> mono_;
   std::vector<unsigned long long> sets_of_host_;      // [nf_pad] each inner feature's interaction-constraint sets, as uploaded to sets_of_

@@ -45,6 +45,7 @@ COMMON_DEFAULTS = dict(
     monotoneConstraints=(), monotoneConstraintsMethod="basic", monotonePenalty=0.0,      # monotone_constraints (per feature -1/0/1) etc.
     interactionConstraints=(),          # interaction_constraints: lists of feature indices; a branch splits on features of one list only
     featureFractionByNode=1.0,          # feature_fraction_bynode: the share of the tree's features each leaf's split is chosen from
+    pathSmooth=0.0,                     # path_smooth: smooths every split gain and leaf output toward the parent leaf's output
     delegate=None,
     # column params (core/contracts/Params.scala:93-208 + Spark ML)
     featuresCol="features", labelCol="label", predictionCol="prediction", weightCol=None, initScoreCol=None,
@@ -133,6 +134,8 @@ class TrainParams:
             s += "interaction_constraints=%s " % ",".join("[%s]" % ",".join(str(int(f)) for f in c) for c in p["interactionConstraints"])
         if p["featureFractionByNode"] != 1.0:      # only when set, so every other parameter string stays as the reference builds it
             s += "feature_fraction_bynode=%s " % scala_double(p["featureFractionByNode"])
+        if p["pathSmooth"] != 0.0:      # only when set, so every other parameter string stays as the reference builds it
+            s += "path_smooth=%s " % scala_double(p["pathSmooth"])
         return s
 
     def to_string(self):
