@@ -71,7 +71,16 @@ __global__ void k_renew_unweighted(const TreeCtrl* __restrict__ ctrl, const int*
   const double v1 = desc(pos - 1), v2 = desc(pos);
   out[l] = __dsub_rn(v1, __dmul_rn(__dsub_rn(v1, v2), bias));
 }
-// weighted cdf per leaf: one CTA per leaf, chunked block scan with a running carry
+// a + b; `inexact` is set when the sum rounds (TwoSum's error term is non-zero)
+__device__ __forceinline__ double d_add_flag(double a, double b, bool& inexact) {
+  const double s = __dadd_rn(a, b), bb = __dsub_rn(s, a);
+  inexact |= __dadd_rn(__dsub_rn(a, __dsub_rn(s, bb)), __dsub_rn(b, bb)) != 0.0;
+  return s;
+}
+// weighted cdf per leaf: one CTA per leaf, chunked block scan with a running carry.  Upstream adds the weights one by one in row
+// order.  While no add of the scan rounds (lane, warp-total and carry adds), every cdf value is the exact prefix sum, and so is every
+// sequential partial sum, so the two agree.  From the first chunk in which an add rounds, the leaf's cdf is summed in row order by one
+// thread, starting from the carry, which is still exact: wide weights get upstream's cdf too.
 __global__ void __launch_bounds__(1024)
 k_renew_cdf(const TreeCtrl* __restrict__ ctrl, const int* __restrict__ seg_begin, const unsigned* __restrict__ grouped_pos,
             const int* __restrict__ row_of_pos, const float* __restrict__ weight, double* __restrict__ cdf) {
@@ -79,28 +88,46 @@ k_renew_cdf(const TreeCtrl* __restrict__ ctrl, const int* __restrict__ seg_begin
   if (l >= ctrl->num_leaves) return;
   const int b = seg_begin[l], cnt = seg_begin[l + 1] - b;
   __shared__ double s_warp[32];
+  __shared__ double s_v[1024];
   __shared__ double s_carry;
   if (threadIdx.x == 0) s_carry = 0.0;
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  bool sequential = false;      // the same in every thread of the block
   for (int base = 0; base < cnt; base += 1024) {
     const int i = base + threadIdx.x;
     const double v = i < cnt ? static_cast<double>(weight[row_of_pos[grouped_pos[b + i]]]) : 0.0;
-    double incl = v;
-    for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      double w = s_warp[lane];
-      for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += t; }
-      s_warp[lane] = w;
+    if (!sequential) {
+      bool inexact = false;
+      double incl = v;
+      for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl = d_add_flag(incl, t, inexact); }
+      if (lane == 31) s_warp[warp] = incl;
+      __syncthreads();
+      if (warp == 0) {
+        double w = s_warp[lane];
+        for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w = d_add_flag(w, t, inexact); }
+        s_warp[lane] = w;
+      }
+      __syncthreads();
+      const double carry = s_carry, woff = warp ? s_warp[warp - 1] : 0.0;
+      const double c = d_add_flag(carry, d_add_flag(woff, incl, inexact), inexact);
+      sequential = __syncthreads_or(inexact);
+      if (!sequential) {
+        if (i < cnt) cdf[b + i] = c;
+        if (threadIdx.x == 1023) s_carry = c;
+      }
+      __syncthreads();
     }
-    __syncthreads();
-    const double carry = s_carry, woff = warp ? s_warp[warp - 1] : 0.0;
-    if (i < cnt) cdf[b + i] = carry + (woff + incl);
-    __syncthreads();
-    if (threadIdx.x == 1023) s_carry = carry + (woff + incl);
-    __syncthreads();
+    if (sequential) {
+      s_v[threadIdx.x] = v;
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        double c = s_carry;
+        for (int j = 0, m = min(1024, cnt - base); j < m; ++j) { c = __dadd_rn(c, s_v[j]); cdf[b + base + j] = c; }
+        s_carry = c;
+      }
+      __syncthreads();
+    }
   }
 }
 // WeightedPercentileFun(double, residual, weight, cnt, alpha) on the ascending order

@@ -102,10 +102,11 @@ def features(ds, F, cats):
             for f in range(F) if not infos[f]["is_trivial"]]
 
 
-def dataset(X, cats, max_bin):
-    """what the restatement needs of X's dataset: (features, bins, upper bounds, bin-to-category lists)"""
+def dataset(X, cats, max_bin, extra=""):
+    """what the restatement needs of X's dataset (built with ds_params and `extra`): (features, bins, upper bounds, bin-to-category
+    lists)"""
     from mmlspark_b200 import capi
-    ds = capi.Dataset.from_mat(X, ds_params(cats, max_bin)).set_field("label", np.zeros(len(X), np.float32))
+    ds = capi.Dataset.from_mat(X, ds_params(cats, max_bin) + " " + extra).set_field("label", np.zeros(len(X), np.float32))
     try:
         feats = features(ds, X.shape[1], cats)
         return (feats, ds.get_bins16(), {f.real_index: ds.upper_bounds(f.real_index) for f in feats},
@@ -114,10 +115,11 @@ def dataset(X, cats, max_bin):
         ds.free()
 
 
-def run(X, g, h, params, iters, ds_params, reset=None):
-    """the model text of `iters` trees on the same custom (g, h); reset = (after tree k, parameter string) calls ResetParameter"""
+def run(X, g, h, params, iters, ds_params, reset=None, label=None):
+    """the model text of `iters` trees on the same custom (g, h); reset = (after tree k, parameter string) calls ResetParameter; label:
+    the dataset's labels (zeros by default; multiclass needs every class present, or no class trains)"""
     from mmlspark_b200 import capi
-    ds = capi.Dataset.from_mat(X, ds_params).set_field("label", np.zeros(len(X), np.float32))
+    ds = capi.Dataset.from_mat(X, ds_params).set_field("label", np.zeros(len(X), np.float32) if label is None else np.asarray(label, np.float32))
     b = capi.Booster(ds, params)
     try:
         for k in range(iters):
@@ -322,18 +324,32 @@ def quantized(v):
     return np.rint(v.astype(np.float64) * 2.0 ** e) * 2.0 ** -e
 
 
-def bags(n, iters, fraction, seed):
-    """GBDT::Bagging with bagging_freq = 1 on one rank: per 1024-row block an LCG seeded seed + block, row j of a block takes the next
-    draw ((x >> 16) & 0x7fff) / 32768 < fraction; the states carry over to the next iteration's draw"""
+def lcg_next(x):
+    """LightGBM's Random: x <- 214013 x + 2531011 (mod 2^32); returns (x, float draw ((x >> 16) & 0x7fff) / 32768)"""
+    x = (x * np.uint64(214013) + np.uint64(2531011)) & np.uint64(0xFFFFFFFF)
+    return x, ((x >> np.uint64(16)) & np.uint64(0x7FFF)).astype(np.float64) / 32768.0
+
+
+def bags(n, iters, fraction, seed, freq=1, label=None, pos=1.0, neg=1.0):
+    """GBDT::Bagging on one rank: per 1024-row block an LCG seeded seed + block, row j of a block takes the next draw < its fraction:
+    `fraction`, or with `label` (balanced bagging) `pos` where label > 0 and `neg` elsewhere.  The first draw is at iteration 0, the next
+    ones at it % freq == 0; in between the bag and the states stay.  The states carry over to the next draw."""
     blocks = (n + 1023) // 1024
     x = np.arange(blocks, dtype=np.uint64) + np.uint64(seed)
+    frac = np.full(blocks * 1024, fraction, np.float64)
+    if label is not None:
+        frac[:n] = np.where(np.asarray(label) > 0, pos, neg)
     out = []
-    for _ in range(iters):
+    for it in range(iters):
+        if it > 0 and it % freq != 0:
+            out.append(out[-1])
+            continue
         take = np.zeros(blocks * 1024, bool)
         for j in range(1024):
             live = j < n - np.arange(blocks) * 1024
-            nx = (x * np.uint64(214013) + np.uint64(2531011)) & np.uint64(0xFFFFFFFF)
+            nx, draw = lcg_next(x)
             x = np.where(live, nx, x)
-            take[np.arange(blocks) * 1024 + j] = live & (((x >> np.uint64(16)) & np.uint64(0x7FFF)).astype(np.float64) / 32768.0 < fraction)
+            at = np.arange(blocks) * 1024 + j
+            take[at] = live & (draw < frac[at])
         out.append(take[:n])
     return out

@@ -12,7 +12,7 @@ Growth, with learning_rate 1 and no bias:
   sets the flag.  The leaf's best split is taken over the scanned features its interaction mask allows and its node sample holds.
 - The leaf with the best split (SplitInfo::operator>, then the first leaf) splits if its gain is positive.  Its children take the split's
   sums, outputs (clamped to the leaf's monotone bounds), the narrowed bounds, the narrowed mask and the parent's flags.  Their counts are
-  their rows, or under voting the split's hessian-rebuilt global counts."""
+  their rows, or under voting and data-parallel learning the split's hessian-rebuilt global counts."""
 import math
 
 import numpy as np
@@ -78,7 +78,7 @@ def _vote(bins, g, h, L, features, p, voting):
 
 
 def grow_tree(bins, g, h, features, p, num_leaves, *, used=None, streams=None, mono=None, penalty=0.0, constraints=None, sampler=None,
-              max_depth=-1, voting=None):
+              max_depth=-1, voting=None, estimated_counts=False):
     """One tree.  bins: [rows][real features] bin indices; g/h: fp64 values on an exact grid.  The options, each off by default:
     - used: the real indices the tree's feature_fraction sample holds (None: every feature);
     - streams: an extra_trees_ref.Streams, which turns extra trees on and carries the feature streams from tree to tree;
@@ -87,10 +87,12 @@ def grow_tree(bins, g, h, features, p, num_leaves, *, used=None, streams=None, m
     - constraints: the interaction constraint sets (None: one set of every feature, which allows every feature at every leaf);
     - sampler: a bynode_ref.ColSampler, which takes the tree's feature_fraction sample (instead of `used`) and every leaf's node sample;
     - max_depth: > 0 stops the rounds whose leaves are at that depth;
-    - voting: (rank_of_row, R, top_k), the rank holding each row; one rank is the serial learner.
+    - voting: (rank_of_row, R, top_k), the rank holding each row; one rank is the serial learner;
+    - estimated_counts: the children's counts are the split's hessian-rebuilt counts, as the data-parallel learner keeps them (voting
+      always does).
     Returns the tree arrays as the model text prints them (bins instead of threshold values, bin sets instead of categories) and:
     rounds: per round, (leaf, leaf state, scans) in scan order; picks: per pick, every leaf's best split; scanned_counts: per round, the
-    (leaf, row count) pairs in (left, right) order; bounds, masks, branches: every leaf's final monotone bounds, set mask and split
+    (leaf, row count) pairs in (left, right) order; leaf_rows: every leaf's rows (indices into g), ascending; bounds, masks, branches: every leaf's final monotone bounds, set mask and split
     features from the root; scan_masks and node_rounds: per round, each scanned leaf's mask and its (mask, node sample) in scan order;
     draws: the sampler's draws of the tree, its tree draw included; voted: per round, the (smaller, larger) voted feature lists (larger
     None at the root)."""
@@ -172,7 +174,7 @@ def grow_tree(bins, g, h, features, p, num_leaves, *, used=None, streams=None, m
         lb, rb = M.child_bounds(L["bounds"], 0 if mono is None or s.is_cat else mono[s.feature], s.is_cat, left_out, right_out)
         mask, branch = L["mask"] & sets[s.feature], L["branch"] + (s.feature,)
         lrows, rrows = L["rows"][left], L["rows"][~left]
-        lcount, rcount = (len(lrows), len(rrows)) if voting is None else (s.left_count, L["count"] - s.left_count)
+        lcount, rcount = (len(lrows), len(rrows)) if voting is None and not estimated_counts else (s.left_count, L["count"] - s.left_count)
         node, nl = len(leaves) - 1, len(leaves)
         par = parent_of[pick]
         if par >= 0:
@@ -200,6 +202,7 @@ def grow_tree(bins, g, h, features, p, num_leaves, *, used=None, streams=None, m
     T["leaf_value"] = [L["value"] if abs(L["value"]) > ref.K_ZERO else 0.0 for L in leaves]
     T["leaf_weight"] = [L["weight"] for L in leaves]
     T["leaf_count"] = [L["count"] for L in leaves]
+    T["leaf_rows"] = [L["rows"] for L in leaves]
     T["internal_value"] = [v if abs(v) > ref.K_ZERO else 0.0 for v in T["internal_value"]]
     T["bounds"] = [L["bounds"] for L in leaves]
     T["masks"] = [L["mask"] for L in leaves]
