@@ -284,16 +284,9 @@ int LGBM_BoosterPredictForCSRSingle(BoosterHandle handle, const void* indptr, in
   *out_len = b->model.PredictRow(row.data(), static_cast<int>(ncol), predict_type, start_iteration, num_iteration, out_result);
   API_END();
 }
-static int64_t PerRow(const HostModel& m, int predict_type, int start_iteration, int num_iteration) {
-  int t0, t1;
-  m.IterRange(start_iteration, num_iteration, &t0, &t1);
-  if (predict_type == C_API_PREDICT_LEAF_INDEX) return t1 - t0;
-  if (predict_type == C_API_PREDICT_CONTRIB) return static_cast<int64_t>(m.num_tree_per_iteration) * (m.max_feature_idx + 2);
-  return m.num_tree_per_iteration;
-}
 int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_type, int start_iteration, int num_iteration, int64_t* out_len) {
   API_BEGIN();
-  *out_len = PerRow(BS(handle)->model, predict_type, start_iteration, num_iteration) * num_row;
+  *out_len = BS(handle)->model.NumPredictPerRow(predict_type, start_iteration, num_iteration) * num_row;
   API_END();
 }
 int LGBM_BoosterPredictForMat(BoosterHandle handle, const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, int predict_type,
@@ -301,7 +294,7 @@ int LGBM_BoosterPredictForMat(BoosterHandle handle, const void* data, int data_t
   API_BEGIN();
   (void)parameter;
   const HostModel& m = BS(handle)->model;
-  const int64_t per = PerRow(m, predict_type, start_iteration, num_iteration);
+  const int64_t per = m.NumPredictPerRow(predict_type, start_iteration, num_iteration);
 #pragma omp parallel
   {
     std::vector<double> row(ncol);
@@ -611,9 +604,9 @@ int B200GBM_BoosterGetTiming(BoosterHandle handle, double* out6, int reset) {
 int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol, int predict_type,
                                        int start_iteration, int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms) {
   API_BEGIN();
-  Booster* b = BS(handle);
-  *out_len = b->PredictBatch(data, data_type, nrow, ncol, predict_type, start_iteration, num_iteration, out_result);
-  if (elapsed_ms) *elapsed_ms = b->last_predict_ms;
+  Predictor& p = *BS(handle)->predictor;
+  *out_len = p.PredictMat(data, data_type, nrow, ncol, predict_type, start_iteration, num_iteration, out_result);
+  if (elapsed_ms) *elapsed_ms = p.last_ms;
   API_END();
 }
 int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
@@ -621,9 +614,9 @@ int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr,
                                        int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms) {
   API_BEGIN();
   (void)num_col;      // like LGBM_BoosterPredictForCSRSingle: columns past the model's features are never read
-  Booster* b = BS(handle);
-  *out_len = b->PredictBatchCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, predict_type, start_iteration, num_iteration, out_result);
-  if (elapsed_ms) *elapsed_ms = b->last_predict_ms;
+  Predictor& p = *BS(handle)->predictor;
+  *out_len = p.PredictCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, predict_type, start_iteration, num_iteration, out_result);
+  if (elapsed_ms) *elapsed_ms = p.last_ms;
   API_END();
 }
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4) {

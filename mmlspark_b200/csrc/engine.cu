@@ -4,6 +4,7 @@
 #include "objective.h"
 #include "renew_kernel.cuh"
 #include "metrics.h"
+#include "predictor.h"
 
 #include <nvtx3/nvToolsExt.h>      // header-only NVTX v3: ranges are no-ops unless a profiler injects itself
 
@@ -1378,14 +1379,14 @@ static void CheckPathSmooth(const Config& cfg, bool voting_parallel) {
   if (cfg.path_smooth > kPathSmoothEps && voting_parallel) Fatal(kVotingPathSmooth);
 }
 
-Booster::Booster(const std::string& model_text) {
+Booster::Booster(const std::string& model_text) : predictor(new Predictor(model, stream_)) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
   K = model.num_tree_per_iteration;
   num_init_iteration = model.NumIterations();
 }
 
-Booster::Booster(const Dataset* tr, const char* params) : train(tr) {
+Booster::Booster(const Dataset* tr, const char* params) : train(tr), predictor(new Predictor(model, stream_)) {
   EnsureDevice();
   device_ = CurrentDevice();
   cfg.Parse(params);
@@ -1565,7 +1566,7 @@ void Booster::DroppingTrees() {
   if (!cfg.xgboost_dart_mode) shrinkage_ = cfg.learning_rate / (1.0f + static_cast<double>(drop_index_.size()));
   else if (drop_index_.empty()) shrinkage_ = cfg.learning_rate;
   else shrinkage_ = cfg.learning_rate / (cfg.learning_rate + static_cast<double>(drop_index_.size()));
-  if (!drop_index_.empty()) forest_.reset();
+  if (!drop_index_.empty()) predictor->Invalidate();
   dart_dropped_this_iter_ = true;
 }
 void Booster::DartNormalize() {
@@ -1586,7 +1587,7 @@ void Booster::DartNormalize() {
       else { sum_weight_ -= tree_weight_[i] * (1.0f / (k + cfg.learning_rate)); tree_weight_[i] *= (k / (k + cfg.learning_rate)); }
     }
   }
-  if (!drop_index_.empty()) forest_.reset();        // leaf values of earlier trees changed: the device forest for predict is stale
+  if (!drop_index_.empty()) predictor->Invalidate();        // leaf values of earlier trees changed: the device forest for predict is stale
 }
 
 // [LightGBM gbdt.cpp GBDT::Bagging / goss.hpp GOSS::Bagging] draws the in-bag flags on the device, compacts the in-bag rows
@@ -1884,14 +1885,8 @@ void Booster::GetPredict(int data_idx, int64_t* out_len, double* out) {
   EnsureDevice();
   if (is_dart_ && data_idx == 0 && !dart_dropped_this_iter_) DroppingTrees();      // DART::GetTrainingScore
   const int n = ScoredData(data_idx).first->num_data;
-  std::vector<double> raw(static_cast<size_t>(K) * n);
-  GetRawScores(data_idx, raw.data());
-  std::vector<double> r(K), o(K);
-  for (int i = 0; i < n; ++i) {
-    for (int k = 0; k < K; ++k) r[k] = raw[static_cast<size_t>(k) * n + i];
-    model.Convert(r.data(), o.data());
-    for (int k = 0; k < K; ++k) out[static_cast<size_t>(k) * n + i] = o[k];
-  }
+  GetRawScores(data_idx, out);
+  model.ConvertScores(out, n, 1, n, 0, false);
   *out_len = static_cast<int64_t>(K) * n;
 }
 void Booster::GetRawScores(int data_idx, double* out) {
@@ -1923,243 +1918,6 @@ void Booster::GetGradients(float* grad, float* hess) {
   B200_CUDA(cudaStreamSynchronize(stream_));
 }
 
-void Booster::UploadForest() {
-  if (forest_ && forest_->trees == model.trees.size()) return;
-  forest_.reset(new ForestBufs());
-  ForestBufs& f = *forest_;
-  const size_t T = model.trees.size();
-  std::vector<int> toff(T + 1, 0), loff(T + 1, 0), nl(T), sf, dt, lc, rc, cbeg, clen;
-  std::vector<unsigned> cwords;
-  std::vector<double> thr, lv, ncnt, lcnt, expv(T, 0.0);
-  for (size_t t = 0; t < T; ++t) {
-    const HostTree& tr = *model.trees[t];
-    nl[t] = tr.num_leaves;
-    expv[t] = tr.ExpectedValue();
-    if (tr.num_leaves > 1) f.max_depth = std::max(f.max_depth, tr.MaxDepth());
-    toff[t + 1] = toff[t] + std::max(tr.num_leaves - 1, 0);
-    loff[t + 1] = loff[t] + tr.num_leaves;
-    for (int i = 0; i < tr.num_leaves - 1; ++i) {
-      sf.push_back(tr.split_feature[i]); dt.push_back(tr.decision_type[i]); lc.push_back(tr.left_child[i]); rc.push_back(tr.right_child[i]);
-      thr.push_back(tr.threshold[i]); ncnt.push_back(tr.internal_count[i]);
-      if (tr.decision_type[i] & 1) {
-        const int ci = static_cast<int>(tr.threshold[i]);
-        cbeg.push_back(static_cast<int>(cwords.size())); clen.push_back(tr.cat_boundaries[ci + 1] - tr.cat_boundaries[ci]);
-        for (int w = tr.cat_boundaries[ci]; w < tr.cat_boundaries[ci + 1]; ++w) cwords.push_back(tr.cat_threshold[w]);
-      } else { cbeg.push_back(0); clen.push_back(0); }
-    }
-    for (int i = 0; i < tr.num_leaves; ++i) { lv.push_back(tr.leaf_value[i]); lcnt.push_back(tr.leaf_count[i]); }
-  }
-  if (!stream_) stream_ = AcquireStream();
-  auto up_i = [&](DevBuf<int>& d, std::vector<int>& h) { d.Alloc(std::max<size_t>(h.size(), 1)); if (!h.empty()) d.Upload(h.data(), h.size(), stream_); };
-  auto up_d = [&](DevBuf<double>& d, std::vector<double>& h) { d.Alloc(std::max<size_t>(h.size(), 1)); if (!h.empty()) d.Upload(h.data(), h.size(), stream_); };
-  up_i(f.tree_offset, toff); up_i(f.leaf_offset, loff); up_i(f.num_leaves, nl); up_i(f.split_feature, sf); up_i(f.decision_type, dt);
-  up_i(f.left_child, lc); up_i(f.right_child, rc); up_d(f.threshold, thr); up_d(f.leaf_value, lv); up_i(f.cat_begin, cbeg); up_i(f.cat_len, clen);
-  up_d(f.node_count, ncnt); up_d(f.leaf_count, lcnt); up_d(f.expected, expv);
-  f.cat_words.Alloc(std::max<size_t>(cwords.size(), 1));
-  if (!cwords.empty()) f.cat_words.Upload(cwords.data(), cwords.size(), stream_);
-  B200_CUDA(cudaStreamSynchronize(stream_));
-  f.trees = T;
-}
-
-const Booster::SlotBufs& Booster::UploadSlots(int t0, int t1) {
-  ForestBufs& fb = *forest_;
-  if (fb.slots && fb.slots->t0 == t0 && fb.slots->t1 == t1) return *fb.slots;
-  std::unique_ptr<SlotBufs> sl(new SlotBufs());
-  sl->t0 = t0; sl->t1 = t1;
-  const int nfeat = model.max_feature_idx + 1;
-  std::vector<int> slot_of(nfeat, -1), feature_of, split;
-  for (int t = t0; t < t1; ++t) {
-    const HostTree& tr = *model.trees[t];
-    for (int i = 0; i < tr.num_leaves - 1; ++i) slot_of[tr.split_feature[i]] = 0;
-  }
-  for (int j = 0; j < nfeat; ++j)
-    if (slot_of[j] == 0) { slot_of[j] = static_cast<int>(feature_of.size()); feature_of.push_back(j); }
-  for (size_t t = 0; t < model.trees.size(); ++t) {      // node order of UploadForest; trees outside [t0, t1) are not walked
-    const HostTree& tr = *model.trees[t];
-    const bool in = static_cast<int>(t) >= t0 && static_cast<int>(t) < t1;
-    for (int i = 0; i < tr.num_leaves - 1; ++i) split.push_back(in ? slot_of[tr.split_feature[i]] : 0);
-  }
-  sl->U = static_cast<int>(feature_of.size());
-  auto up = [&](DevBuf<int>& d, const std::vector<int>& h) { d.Alloc(std::max<size_t>(h.size(), 1)); if (!h.empty()) d.Upload(h.data(), h.size(), stream_); };
-  up(sl->slot_of_feature, slot_of); up(sl->feature_of_slot, feature_of); up(sl->split_slot, split);
-  B200_CUDA(cudaStreamSynchronize(stream_));
-  fb.slots = std::move(sl);
-  return *fb.slots;
-}
-
-// TreeSHAP scratch of k_predict_contrib: per thread (depth+2)(depth+3)/2 path elements + depth+3 stack frames
-struct Booster::ShapScratch {
-  static constexpr int kThreads = 128;
-  int grid = 0, path_stride = 0, frame_stride = 0;
-  DevBuf<ShapPathElem> paths;
-  DevBuf<ShapFrame> frames;
-  ShapScratch(int max_depth, int64_t rows, int sms) {
-    const int md = max_depth + 2;
-    path_stride = md * (md + 1) / 2 + md;
-    frame_stride = md + 2;
-    grid = static_cast<int>(std::min<int64_t>((rows + kThreads - 1) / kThreads, static_cast<int64_t>(sms) * 4));
-    paths.Alloc(static_cast<size_t>(grid) * kThreads * path_stride);
-    frames.Alloc(static_cast<size_t>(grid) * kThreads * frame_stride);
-  }
-};
-
-void Booster::LaunchPredict(const ForestDev& f, const void* X, int data_type, int64_t rows, int ncol, int predict_type, int t0, int t1, int F1,
-                            ShapScratch& shap, double* out) {
-  const int Kc = model.num_tree_per_iteration;
-  const int64_t per_row = predict_type == 2 ? (t1 - t0) : predict_type == 3 ? static_cast<int64_t>(Kc) * F1 : Kc;
-  if (rows * per_row == 0) return;
-  const int grid = static_cast<int>(std::min<int64_t>((rows * per_row + 255) / 256, static_cast<int64_t>(DeviceSMs()) * 16));
-  const float* xf = static_cast<const float*>(X);
-  const double* xd = static_cast<const double*>(X);
-  if (predict_type == 3) {
-    B200_CUDA(cudaMemsetAsync(out, 0, static_cast<size_t>(rows) * per_row * sizeof(double), stream_));
-    if (data_type == 0) k_predict_contrib<float><<<shap.grid, ShapScratch::kThreads, 0, stream_>>>(f, xf, rows, ncol, Kc, t0, t1, F1, shap.paths.p, shap.path_stride, shap.frames.p, shap.frame_stride, out);
-    else k_predict_contrib<double><<<shap.grid, ShapScratch::kThreads, 0, stream_>>>(f, xd, rows, ncol, Kc, t0, t1, F1, shap.paths.p, shap.path_stride, shap.frames.p, shap.frame_stride, out);
-  } else if (predict_type == 2) {
-    if (data_type == 0) k_predict_leaf<float><<<grid, 256, 0, stream_>>>(f, xf, rows, ncol, t0, t1, out);
-    else k_predict_leaf<double><<<grid, 256, 0, stream_>>>(f, xd, rows, ncol, t0, t1, out);
-  } else {
-    if (data_type == 0) k_predict_raw<float><<<grid, 256, 0, stream_>>>(f, xf, rows, ncol, Kc, t0, t1, out);
-    else k_predict_raw<double><<<grid, 256, 0, stream_>>>(f, xd, rows, ncol, Kc, t0, t1, out);
-  }
-  B200_CUDA(cudaGetLastError());
-}
-
-void Booster::FinishPredict(double* out, int64_t nrow, int predict_type, int t0, int t1) const {
-  const int Kc = model.num_tree_per_iteration;
-  const bool avg = model.average_output && t1 > t0 && predict_type < 2;       // rf: raw score = mean over the iterations
-  if (avg && predict_type == 1)
-    for (int64_t i = 0; i < nrow * Kc; ++i) out[i] /= ((t1 - t0) / Kc);
-  if (predict_type == 0) {          // objective transform on the host, identical to the single-row predictor
-    std::vector<double> r(Kc), o(Kc);
-    for (int64_t i = 0; i < nrow; ++i) {
-      double* p = out + i * Kc;
-      if (avg) for (int k = 0; k < Kc; ++k) p[k] /= ((t1 - t0) / Kc);
-      for (int k = 0; k < Kc; ++k) r[k] = p[k];
-      model.Convert(r.data(), o.data());
-      for (int k = 0; k < Kc; ++k) p[k] = o[k];
-    }
-  }
-}
-
-int64_t Booster::PredictBatch(const void* data, int data_type, int64_t nrow, int ncol, int predict_type, int start_iteration, int num_iteration,
-                              double* out) {
-  EnsureDevice();
-  if (data_type != 0 && data_type != 1) Fatal("PredictBatch: unknown data type");
-  if (predict_type < 0 || predict_type > 3) Fatal("PredictBatch: unknown predict type");
-  if (ncol < model.max_feature_idx + 1) Fatal("PredictBatch: the matrix has fewer columns than the model has features");
-  UploadForest();
-  const ForestDev f = forest_->View();
-  int t0, t1;
-  model.IterRange(start_iteration, num_iteration, &t0, &t1);
-  const int Kc = model.num_tree_per_iteration;
-  const int F1 = model.max_feature_idx + 2;            // contributions: one per feature + the expected value
-  const int64_t per_row = predict_type == 2 ? (t1 - t0) : predict_type == 3 ? static_cast<int64_t>(Kc) * F1 : Kc;
-  const size_t esz = data_type == 0 ? 4 : 8;
-  const bool on_device = IsDevicePointer(data);
-  int64_t chunk = on_device ? nrow : std::max<int64_t>(1, std::min<int64_t>(nrow, (512LL << 20) / (static_cast<int64_t>(ncol) * esz)));
-  chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, (1024LL << 20) / (std::max<int64_t>(per_row, 1) * 8)));      // bound the device output buffer too (contributions are wide)
-  ShapScratch shap(forest_->max_depth, predict_type == 3 ? std::min(chunk, nrow) : 0, DeviceSMs());
-  DevBuf<unsigned char> xin;
-  if (!on_device) xin.Alloc(static_cast<size_t>(chunk) * ncol * esz);
-  DevBuf<double> dout; dout.Alloc(static_cast<size_t>(std::min(chunk, nrow)) * per_row);
-  StreamTimer timer(stream_);
-  for (int64_t r0 = 0; r0 < nrow; r0 += chunk) {
-    const int64_t rows = std::min(chunk, nrow - r0);
-    const void* x = static_cast<const unsigned char*>(data) + static_cast<size_t>(r0) * ncol * esz;
-    if (!on_device) { B200_CUDA(cudaMemcpyAsync(xin.p, x, static_cast<size_t>(rows) * ncol * esz, cudaMemcpyHostToDevice, stream_)); x = xin.p; }
-    LaunchPredict(f, x, data_type, rows, ncol, predict_type, t0, t1, F1, shap, dout.p);
-    B200_CUDA(cudaMemcpyAsync(out + r0 * per_row, dout.p, static_cast<size_t>(rows) * per_row * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-    B200_CUDA(cudaStreamSynchronize(stream_));
-  }
-  last_predict_ms = timer.Ms();
-  FinishPredict(out, nrow, predict_type, t0, t1);
-  return nrow * per_row;
-}
-
-int64_t Booster::PredictBatchCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
-                                 int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out) {
-  if (indptr_type != 2 && indptr_type != 3) Fatal("PredictBatchCSR: indptr must be INT32 or INT64");
-  if (data_type != 1) Fatal("PredictBatchCSR: CSR values must be FLOAT64");
-  if (predict_type < 0 || predict_type > 3) Fatal("PredictBatchCSR: unknown predict type");
-  if (nindptr < 1) Fatal("PredictBatchCSR: nindptr must be at least 1");
-  auto ptr = [&](int64_t i) -> int64_t {
-    return indptr_type == 2 ? static_cast<const int32_t*>(indptr)[i] : static_cast<const int64_t*>(indptr)[i];
-  };
-  if (ptr(0) < 0) Fatal("PredictBatchCSR: indptr[0] is negative");
-  for (int64_t i = 1; i < nindptr; ++i)
-    if (ptr(i) < ptr(i - 1)) Fatal("PredictBatchCSR: indptr decreases at position " + std::to_string(i));
-  if (ptr(nindptr - 1) > nelem) Fatal("PredictBatchCSR: indptr[nindptr-1] is larger than nelem");
-  EnsureDevice();
-  UploadForest();
-  int t0, t1;
-  model.IterRange(start_iteration, num_iteration, &t0, &t1);
-  const SlotBufs& sl = UploadSlots(t0, t1);
-  ForestDev f = forest_->View();
-  f.split_feature = sl.split_slot.p;
-  const int U = sl.U;
-  const int Kc = model.num_tree_per_iteration;
-  const int F1 = model.max_feature_idx + 2;
-  const int64_t nrow = nindptr - 1;
-  const int64_t per_row = predict_type == 2 ? (t1 - t0) : predict_type == 3 ? static_cast<int64_t>(Kc) * F1 : Kc;
-  // chunks of rows bounded like PredictBatch's (slots as the input matrix, and the output), and by the nonzeros uploaded at once;
-  // a row with more nonzeros than that bound is a chunk of its own
-  const int64_t kChunkNnz = 32LL << 20;
-  int64_t max_rows = std::max<int64_t>(1, std::min<int64_t>(nrow, (512LL << 20) / (std::max(U, 1) * 8LL)));
-  max_rows = std::max<int64_t>(1, std::min<int64_t>(max_rows, (1024LL << 20) / (std::max<int64_t>(per_row, 1) * 8)));
-  std::vector<int64_t> bounds{0};
-  int64_t max_nnz = 0;
-  while (bounds.back() < nrow) {
-    const int64_t r0 = bounds.back();
-    int64_t lo = r0 + 1, hi = std::min(nrow, r0 + max_rows);
-    while (lo < hi) {
-      const int64_t mid = (lo + hi + 1) / 2;
-      if (ptr(mid) - ptr(r0) <= kChunkNnz) lo = mid; else hi = mid - 1;
-    }
-    max_nnz = std::max(max_nnz, ptr(lo) - ptr(r0));
-    bounds.push_back(lo);
-  }
-  const int64_t rows_max = std::min(max_rows, nrow);
-  ShapScratch shap(forest_->max_depth, predict_type == 3 ? rows_max : 0, DeviceSMs());
-  DevBuf<long long> d_ptr; d_ptr.Alloc(static_cast<size_t>(rows_max) + 1);
-  DevBuf<int> d_idx; d_idx.Alloc(static_cast<size_t>(max_nnz));
-  DevBuf<double> d_val; d_val.Alloc(static_cast<size_t>(max_nnz));
-  DevBuf<double> xs; xs.Alloc(static_cast<size_t>(rows_max) * U);
-  DevBuf<double> dslot;          // contributions per slot
-  if (predict_type == 3) dslot.Alloc(static_cast<size_t>(rows_max) * Kc * (U + 1));
-  DevBuf<double> dout; dout.Alloc(static_cast<size_t>(rows_max) * per_row);
-  std::vector<long long> hptr(static_cast<size_t>(rows_max) + 1);
-  const int sms = DeviceSMs();
-  StreamTimer timer(stream_);
-  for (size_t c = 0; c + 1 < bounds.size(); ++c) {
-    const int64_t r0 = bounds[c], rows = bounds[c + 1] - r0, a = ptr(r0), nnz = ptr(r0 + rows) - a;
-    for (int64_t i = 0; i <= rows; ++i) hptr[i] = ptr(r0 + i) - a;
-    d_ptr.Upload(hptr.data(), static_cast<size_t>(rows) + 1, stream_);
-    if (nnz > 0) {
-      d_idx.Upload(indices + a, static_cast<size_t>(nnz), stream_);
-      d_val.Upload(static_cast<const double*>(data) + a, static_cast<size_t>(nnz), stream_);
-    }
-    if (U > 0) {
-      const int grid = static_cast<int>(std::min<int64_t>((rows * 32 + 255) / 256, static_cast<int64_t>(sms) * 16));
-      k_csr_to_slots<<<grid, 256, 0, stream_>>>(d_ptr.p, d_idx.p, d_val.p, rows, sl.slot_of_feature.p, F1 - 1, U, xs.p);
-      B200_CUDA(cudaGetLastError());
-    }
-    if (predict_type == 3) {
-      LaunchPredict(f, xs.p, 1, rows, U, predict_type, t0, t1, U + 1, shap, dslot.p);
-      B200_CUDA(cudaMemsetAsync(dout.p, 0, static_cast<size_t>(rows) * per_row * sizeof(double), stream_));
-      const int grid = static_cast<int>(std::min<int64_t>((rows * Kc * (U + 1) + 255) / 256, static_cast<int64_t>(sms) * 16));
-      k_contrib_slots_to_features<<<grid, 256, 0, stream_>>>(dslot.p, rows * Kc, U, sl.feature_of_slot.p, F1, dout.p);
-      B200_CUDA(cudaGetLastError());
-    } else {
-      LaunchPredict(f, xs.p, 1, rows, U, predict_type, t0, t1, F1, shap, dout.p);
-    }
-    B200_CUDA(cudaMemcpyAsync(out + r0 * per_row, dout.p, static_cast<size_t>(rows) * per_row * sizeof(double), cudaMemcpyDeviceToHost, stream_));
-    B200_CUDA(cudaStreamSynchronize(stream_));
-  }
-  last_predict_ms = timer.Ms();
-  FinishPredict(out, nrow, predict_type, t0, t1);
-  return nrow * per_row;
-}
-
 }  // namespace b200gbm
 #include "metrics.cu"      // the booster's metrics, in this translation unit
+#include "predictor.cu"    // the booster's batched predictor, in this translation unit

@@ -189,6 +189,7 @@ struct ValidSet {
 class Objective;          // objective.h
 class TreeLearner;        // tree_learner.h
 class Metrics;            // metrics.h
+class Predictor;          // predictor.h
 
 class Booster {
  public:
@@ -209,14 +210,6 @@ class Booster {
   // the objective's gradients at the current training scores, class-major [K][n], computed into scratch buffers: the training state
   // (grad_ / hess_, which rf keeps from construction and GOSS rescales in place) is not touched
   void GetGradients(float* grad, float* hess);
-  // batched GPU prediction over a row-major matrix (host or device pointer); predict_type 0 normal, 1 raw, 2 leaf index.
-  // Returns the number of doubles written to `out` (host).  last_predict_ms = kernel time (CUDA events), incl. H2D for host input.
-  int64_t PredictBatch(const void* data, int data_type, int64_t nrow, int ncol, int predict_type, int start_iteration, int num_iteration, double* out);
-  // the same over a host CSR matrix (indptr_type 2 = int32, 3 = int64; data_type 1 = float64), uploaded in chunks of rows: every output
-  // equals PredictBatch's on the densified rows.  indptr must start at 0 or above, never decrease and end at most at nelem.
-  int64_t PredictBatchCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
-                          int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out);
-  double last_predict_ms = 0.0;
   void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = same_device_ ? 3 : 0; out4[3] = const_hessian_ ? 1 : 0; }
   std::string SaveModelToString(int start_iteration, int num_iteration, int importance_type) const;
   std::string DumpModelJson(int start_iteration, int num_iteration) const;
@@ -232,6 +225,7 @@ class Booster {
   Config cfg;
   HostModel model;
   const Dataset* train = nullptr;
+  std::unique_ptr<Predictor> predictor;      // batched prediction on the device; reads model and stream_, which it acquires when null
   int K = 1;
   int iter = 0;
   int num_init_iteration = 0;
@@ -276,22 +270,6 @@ class Booster {
   // device state
   DevBuf<double> score_;        // [K][n]
   DevBuf<float> grad_, hess_;   // [K][n]
-  // flattened forest for PredictBatch
-  // PredictBatchCSR's slots (kernels.cuh k_csr_to_slots) for the trees [t0, t1): the U distinct split features in ascending order
-  struct SlotBufs { int t0 = 0, t1 = 0, U = 0; DevBuf<int> slot_of_feature, feature_of_slot, split_slot; };
-  struct ForestBufs {
-    DevBuf<int> tree_offset, leaf_offset, num_leaves, split_feature, decision_type, left_child, right_child, cat_begin, cat_len; DevBuf<double> threshold, leaf_value, node_count, leaf_count, expected; DevBuf<unsigned> cat_words; size_t trees = 0; int max_depth = 0;
-    std::unique_ptr<SlotBufs> slots;      // built for the last iteration range PredictBatchCSR was asked for, dropped with the forest
-    ForestDev View() const { return ForestDev{tree_offset.p, leaf_offset.p, num_leaves.p, split_feature.p, threshold.p, decision_type.p, left_child.p, right_child.p, leaf_value.p, cat_begin.p, cat_len.p, cat_words.p, node_count.p, leaf_count.p, expected.p}; }
-  };
-  std::unique_ptr<ForestBufs> forest_;
-  void UploadForest();
-  const SlotBufs& UploadSlots(int t0, int t1);
-  // enqueues the predict kernel of predict_type on `rows` rows of X [rows][ncol] into out (contributions: [rows][K][F1], zero-filled here)
-  struct ShapScratch;
-  void LaunchPredict(const ForestDev& f, const void* X, int data_type, int64_t rows, int ncol, int predict_type, int t0, int t1, int F1,
-                     ShapScratch& shap, double* out);
-  void FinishPredict(double* out, int64_t nrow, int predict_type, int t0, int t1) const;      // rf averaging and the objective transform
   std::vector<ValidSet*> valids_;
   // data_idx 0: the training data and its scores, i > 0: validation set i - 1; fails for any other data_idx
   std::pair<const Dataset*, const DevBuf<double>*> ScoredData(int data_idx) const;

@@ -46,7 +46,7 @@ __device__ __forceinline__ double d_yent_loss(double p) {
   if (q > 1e-12) hp += q * log(q);
   return hp;
 }
-// single-output transforms of HostModel::Convert
+// single-output transforms of HostModel::ConvertScores
 __device__ __forceinline__ double d_output_transform(int kind, double sigmoid, double x) {
   switch (kind) {
     case 1: return 1.0 / (1.0 + exp(-sigmoid * x));

@@ -452,26 +452,39 @@ struct HostModel {
     *t = r;
     return true;
   }
-  void Convert(const double* raw, double* out) const {
-    OutputTransform t;
-    if (!ObjectiveTransform(objective_str, &t)) throw std::runtime_error("Unknown objective type name: " + objective_str);
+  // nrow rows of K raw scores, class k of row i at s[i * row_step + k * class_step], turned into outputs in place: the mean over
+  // `iterations` for an averaged (rf) model when iterations > 0, then the objective transform unless raw
+  void ConvertScores(double* s, int64_t nrow, int64_t row_step, int64_t class_step, int iterations, bool raw) const {
     const int K = num_tree_per_iteration;
-    switch (t.kind) {
-      case 1: out[0] = 1.0 / (1.0 + std::exp(-t.sigmoid * raw[0])); break;
-      case 2: {
-        double mx = raw[0];
-        for (int k = 1; k < num_class; ++k) mx = std::max(mx, raw[k]);
-        double s = 0;
-        for (int k = 0; k < num_class; ++k) { out[k] = std::exp(raw[k] - mx); s += out[k]; }
-        for (int k = 0; k < num_class; ++k) out[k] /= s;
-        break;
+    const bool avg = average_output && iterations > 0;
+    OutputTransform t;
+    if (!raw && !ObjectiveTransform(objective_str, &t)) throw std::runtime_error("Unknown objective type name: " + objective_str);
+    for (int64_t i = 0; i < nrow && (avg || !raw); ++i) {
+      double* p = s + i * row_step;
+      auto v = [&](int k) -> double& { return p[k * class_step]; };
+      if (avg) for (int k = 0; k < K; ++k) v(k) /= iterations;
+      if (raw) continue;
+      switch (t.kind) {
+        case 1: v(0) = 1.0 / (1.0 + std::exp(-t.sigmoid * v(0))); break;
+        case 2: {
+          double mx = v(0);
+          for (int k = 1; k < num_class; ++k) mx = std::max(mx, v(k));
+          double sum = 0;
+          for (int k = 0; k < num_class; ++k) { v(k) = std::exp(v(k) - mx); sum += v(k); }
+          for (int k = 0; k < num_class; ++k) v(k) /= sum;
+          break;
+        }
+        case 3: v(0) = std::exp(v(0)); break;
+        case 4: for (int k = 0; k < K; ++k) v(k) = 1.0 / (1.0 + std::exp(-t.sigmoid * v(k))); break;
+        case 5: v(0) = std::log1p(std::exp(v(0))); break;
+        case 6: v(0) = (v(0) >= 0 ? 1.0 : -1.0) * v(0) * v(0); break;
       }
-      case 3: out[0] = std::exp(raw[0]); break;
-      case 4: for (int k = 0; k < K; ++k) out[k] = 1.0 / (1.0 + std::exp(-t.sigmoid * raw[k])); break;
-      case 5: out[0] = std::log1p(std::exp(raw[0])); break;
-      case 6: out[0] = (raw[0] >= 0 ? 1.0 : -1.0) * raw[0] * raw[0]; break;
-      default: for (int k = 0; k < K; ++k) out[k] = raw[k];
     }
+  }
+  int64_t NumPredictPerRow(int predict_type, int start_iteration, int num_iteration) const {      // outputs per row of predict_type
+    int t0, t1;
+    IterRange(start_iteration, num_iteration, &t0, &t1);
+    return predict_type == 2 ? t1 - t0 : predict_type == 3 ? static_cast<int64_t>(num_tree_per_iteration) * (max_feature_idx + 2) : num_tree_per_iteration;
   }
   void IterRange(int start_iteration, int num_iteration, int* t0, int* t1) const {
     int total = NumIterations();
@@ -493,24 +506,16 @@ struct HostModel {
     }
     if (predict_type == 2) {
       for (int t = t0; t < t1; ++t) out[t - t0] = trees[t]->LeafIndex(row);
-      return t1 - t0;
-    }
-    if (predict_type == 3) {
+    } else if (predict_type == 3) {
       const int nf1 = max_feature_idx + 2;
       for (int k = 0; k < K * nf1; ++k) out[k] = 0;
       for (int t = t0; t < t1; ++t) trees[t]->AddContrib(row, max_feature_idx + 1, out + (t % K) * nf1);
-      return static_cast<int64_t>(K) * nf1;
+    } else {
+      for (int k = 0; k < K; ++k) out[k] = 0;
+      for (int t = t0; t < t1; ++t) out[t % K] += trees[t]->Predict(row);
+      ConvertScores(out, 1, K, 1, (t1 - t0) / K, predict_type == 1);
     }
-    double raw[64];
-    std::vector<double> rawv;
-    double* r = raw;
-    if (K > 64) { rawv.resize(K); r = rawv.data(); }
-    for (int k = 0; k < K; ++k) r[k] = 0;
-    for (int t = t0; t < t1; ++t) r[t % K] += trees[t]->Predict(row);
-    if (average_output && t1 > t0) for (int k = 0; k < K; ++k) r[k] /= ((t1 - t0) / K);
-    if (predict_type == 1) { for (int k = 0; k < K; ++k) out[k] = r[k]; }
-    else Convert(r, out);
-    return K;
+    return NumPredictPerRow(predict_type, start_iteration, num_iteration);
   }
 };
 
