@@ -204,6 +204,13 @@ int B200GBM_DatasetGetIngestMs(DatasetHandle handle, double* out_ms);
  * fp64 [num_feature][256][2]; grad/hess/idx are host arrays; idx == NULL means rows 0..cnt-1 */
 int B200GBM_DatasetHistogram(DatasetHandle handle, const float* grad, const float* hess, const int32_t* idx,
                              int32_t cnt, double* out);
+/* kernel-level entry of quantised training (use_quantized_grad): the training path's discretisation of grad/hess into
+ * num_grad_quant_bins levels (stochastic rounding keyed by seed = data_random_seed and tree_index) and its packed K4 histogram of the
+ * given rows.  out_q [num_data][2] the levels (q_g, q_h), out_scale2 {s_g, s_h}, out_hist [num_feature][256][2] the int64 sums of q.
+ * hess == NULL: constant hessians (q_h = 1 per row, s_h = 1); idx == NULL means rows 0..cnt-1 */
+int B200GBM_DatasetQuantizedHistogram(DatasetHandle handle, const float* grad, const float* hess, const int32_t* idx, int32_t cnt,
+                                      int num_grad_quant_bins, int stochastic_rounding, int seed, int tree_index, int32_t* out_q,
+                                      double* out_scale2, int64_t* out_hist);
 /* kernel-level entry: the objective's gradients and hessians (K1/K2) at the booster's current training scores, class-major [K][n]
  * host arrays; classes the objective does not train read back as 0.  Training state and the model are not changed. */
 int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess);

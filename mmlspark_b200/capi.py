@@ -326,6 +326,23 @@ class Dataset:
         check(load().B200GBM_DatasetHistogram(self.handle, _ptr(g), _ptr(h), ip, C.c_int32(cnt), _ptr(out)))
         return out
 
+    def quantized_histogram(self, grad, hess, num_grad_quant_bins, stochastic_rounding, seed, tree_index, idx=None):
+        """quantised training's discretisation and packed K4 histogram of the rows (all, or idx): returns (q [n][2] int32 levels (q_g, q_h),
+        (s_g, s_h), int64 sums of q [num_feature][256][2]); hess None: constant hessians (q_h = 1)"""
+        g = np.ascontiguousarray(grad, dtype=np.float32)
+        h = None if hess is None else np.ascontiguousarray(hess, dtype=np.float32)
+        n = self.num_data()
+        cnt, ip = n, None
+        if idx is not None:
+            idx = np.ascontiguousarray(idx, dtype=np.int32); cnt = len(idx); ip = _ptr(idx)
+        q = np.zeros((n, 2), dtype=np.int32)
+        scale = np.zeros(2, dtype=np.float64)
+        out = np.zeros((self.num_feature(), 256, 2), dtype=np.int64)
+        check(load().B200GBM_DatasetQuantizedHistogram(self.handle, _ptr(g), None if h is None else _ptr(h), ip, C.c_int32(cnt),
+                                                       C.c_int(num_grad_quant_bins), C.c_int(1 if stochastic_rounding else 0), C.c_int(seed),
+                                                       C.c_int(tree_index), _ptr(q), _ptr(scale), _ptr(out)))
+        return q, (float(scale[0]), float(scale[1])), out
+
     def free(self):
         if self.handle:
             check(load().LGBM_DatasetFree(self.handle))

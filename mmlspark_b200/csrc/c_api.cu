@@ -583,6 +583,14 @@ int B200GBM_DatasetHistogram(DatasetHandle handle, const float* grad, const floa
   DS(handle)->Histogram(grad, hess, idx, cnt, out);
   API_END();
 }
+int B200GBM_DatasetQuantizedHistogram(DatasetHandle handle, const float* grad, const float* hess, const int32_t* idx, int32_t cnt,
+                                      int num_grad_quant_bins, int stochastic_rounding, int seed, int tree_index, int32_t* out_q,
+                                      double* out_scale2, int64_t* out_hist) {
+  API_BEGIN();
+  DS(handle)->QuantizedHistogram(grad, hess, idx, cnt, Dataset::QuantSpec{num_grad_quant_bins, stochastic_rounding != 0, seed, tree_index}, out_q,
+                                 out_scale2, out_hist);
+  API_END();
+}
 int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess) {
   API_BEGIN();
   BS(handle)->GetGradients(grad, hess);

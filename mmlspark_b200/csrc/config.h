@@ -49,6 +49,12 @@ struct Config {
   // sets of real feature indices; a branch's split features stay inside one set (TreeLearner sets_of_, kernels.cuh d_pick_block)
   std::vector<std::vector<int>> interaction_constraints;
   std::string interaction_constraints_malformed;      // the value given when it does not parse (Booster fails at create)
+  // quantised training [UPSTREAM 4.x names and defaults, from knowledge]: each tree's g and h discretised to a few integer levels
+  // (kernels.cuh k_quantize_discrete) and histograms built with one packed atomic per cell (hist_kernel.cuh k4_hist_build_packed)
+  bool use_quantized_grad = false;
+  int num_grad_quant_bins = 4;              // B: q_g in [-floor(B/2), floor(B/2)], q_h in [-B, B]; 2..63 (Booster checks)
+  bool quant_train_renew_leaf = false;      // leaf values from the true in-bag sums of g and h after growth
+  bool stochastic_rounding = true;
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -223,6 +229,8 @@ struct Config {
     B("extra_trees", &extra_trees); I("extra_seed", &extra_seed);
     S("monotone_constraints_method", &monotone_constraints_method); D("monotone_penalty", &monotone_penalty);
     D("path_smooth", &path_smooth);
+    B("use_quantized_grad", &use_quantized_grad); I("num_grad_quant_bins", &num_grad_quant_bins);
+    B("quant_train_renew_leaf", &quant_train_renew_leaf); B("stochastic_rounding", &stochastic_rounding);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -310,6 +318,9 @@ struct Config {
     s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
     s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: " << Num(path_smooth) << "]\n";
     s << "[interaction_constraints: " << join_sets(interaction_constraints) << "]\n";
+    if (use_quantized_grad)      // only when on, so every other model text stays as it was
+      s << "[use_quantized_grad: 1]\n[num_grad_quant_bins: " << num_grad_quant_bins << "]\n[quant_train_renew_leaf: " << quant_train_renew_leaf
+        << "]\n[stochastic_rounding: " << stochastic_rounding << "]\n";
     s << "[verbosity: " << verbosity << "]\n[saved_feature_importance_type: 0]\n[linear_tree: 0]\n[max_bin: " << max_bin << "]\n";
     s << "[max_bin_by_feature: " << max_bin_by_feature << "]\n[min_data_in_bin: " << min_data_in_bin << "]\n";
     s << "[bin_construct_sample_cnt: " << bin_construct_sample_cnt << "]\n[data_random_seed: " << data_random_seed << "]\n";

@@ -914,10 +914,15 @@ RowBlockBound Dataset::BlockBound() const {
   return RowBlockBound{block_bound_.p, bound_blocks(num_data)};
 }
 
-void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const {
+// K4 on this dataset's bins for the given rows through the training path's K3 and launch_k4: quant.bins 0 quantises to the 36-bit
+// fixed-point grid, quant.bins = B discretises as use_quantized_grad does (hess null: constant hessians, the count plane).  Returns the
+// per-inner-feature int64 histograms [nfn][256][2] (bundle columns expanded, exact as in k_scan); ctrl holds the scales, q the words.
+std::vector<long long> Dataset::HistogramInt(const float* grad, const float* hess, const int32_t* idx, int cnt, const QuantSpec& quant,
+                                             DevBuf<TreeCtrl>& ctrl, DevBuf<int4>& q) const {
   EnsureDevice();
   B200_CUDA(set_k4_smem_limit());
   const int n = num_data;
+  const bool const_hessian = hess == nullptr;
   // K4 bounds an index-list item by the row blocks between its first and last row, so it needs a strictly ascending list; the
   // histogram does not depend on the order.  A list that repeats a row is bounded by row counts instead.
   std::vector<int32_t> rows;
@@ -929,26 +934,34 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
     if (std::adjacent_find(rows.begin(), rows.end()) != rows.end()) bound.prefix = nullptr;
   }
   DevBuf<float> g, h; g.Alloc(n); h.Alloc(n);
-  g.Upload(grad, n, stream); h.Upload(hess, n, stream);
-  DevBuf<int4> q; q.Alloc(n);
-  DevBuf<TreeCtrl> ctrl; ctrl.Alloc(1); ctrl.Zero(stream);
+  g.Upload(grad, n, stream);
+  if (const_hessian) h.Zero(stream); else h.Upload(hess, n, stream);
+  q.Alloc(n);
+  ctrl.Alloc(1); ctrl.Zero(stream);
   DevBuf<int> didx; didx.Alloc(std::max(cnt, 1));
   if (idx) didx.Upload(rows.data(), cnt, stream);
   const size_t elems = static_cast<size_t>(num_tiles) * 32 * 512;      // tile features only (wide features are covered by the model-level tests)
   DevBuf<long long> H; H.Alloc(elems); H.Zero(stream);
   const size_t felems = static_cast<size_t>(std::max(nfn, 1)) * 512;     // per feature
-  DevBuf<double> D; D.Alloc(felems);
   int sms = 0;
   B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  const int ch = const_hessian ? 1 : 0;
   k_absmax<<<sms * 4, 256, 0, stream>>>(g.p, h.p, n, ctrl.p);
-  k_set_scale<<<1, 1, 0, stream>>>(ctrl.p, 0, 1.0);
-  k_quantize<<<sms * 4, 256, 0, stream>>>(g.p, h.p, n, q.p, ctrl.p, 0, nullptr, 0);
+  k_set_scale<<<1, 1, 0, stream>>>(ctrl.p, ch, 1.0);
+  if (quant.bins > 0) {
+    k_set_quant_scale<<<1, 1, 0, stream>>>(ctrl.p, ch, quant.bins);
+    k_quantize_discrete<<<sms * 4, 256, 0, stream>>>(g.p, h.p, n, q.p, ctrl.p, ch, nullptr, 0, quant.bins, quant.stochastic ? 1 : 0, quant.seed,
+                                                     quant.tree);
+  } else {
+    k_quantize<<<sms * 4, 256, 0, stream>>>(g.p, h.p, n, q.p, ctrl.p, ch, nullptr, 0);
+  }
   HistWork w{0, cnt, idx ? 1 : 0, 0};
   B200_CUDA(cudaMemcpyAsync(&ctrl.p->hist_work, &w, sizeof(w), cudaMemcpyHostToDevice, stream));
   DevBuf<int4> qo; qo.Alloc(std::max(cnt, 1));
   k_gather_q<<<sms * 4, 256, 0, stream>>>(&ctrl.p->hist_work, didx.p, didx.p, q.p, qo.p);
-  launch_k4(/*const_hessian=*/false, bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
+  launch_k4(const_hessian, quant.bins, bins.p, rows_stride, num_tiles, q.p, qo.p, didx.p, didx.p, &ctrl.p->hist_work,
             reinterpret_cast<unsigned long long*>(H.p), bound, sms, stream);
+  B200_CUDA(cudaGetLastError());
   // per-feature histograms out of the column histograms, exact int64 as in k_scan: a bundle member's most frequent bin is the column total
   // minus the member's other bins
   std::vector<long long> hc(elems), hf(felems, 0);
@@ -968,6 +981,17 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
     }
     o[m.default_bin * 2] = tot[0]; o[m.default_bin * 2 + 1] = tot[1];
   }
+  return hf;
+}
+
+void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const {
+  DevBuf<TreeCtrl> ctrl;
+  DevBuf<int4> q;
+  const std::vector<long long> hf = HistogramInt(grad, hess, idx, cnt, QuantSpec{}, ctrl, q);
+  const size_t felems = hf.size();
+  int sms = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  DevBuf<double> D; D.Alloc(felems);
   DevBuf<long long> HF; HF.Alloc(felems); HF.Upload(hf.data(), felems, stream);
   k_hist_to_double<<<sms * 4, 256, 0, stream>>>(HF.p, D.p, felems, ctrl.p);
   B200_CUDA(cudaGetLastError());
@@ -976,6 +1000,26 @@ void Dataset::Histogram(const float* grad, const float* hess, const int32_t* idx
   B200_CUDA(cudaStreamSynchronize(stream));
   std::memset(out, 0, sizeof(double) * static_cast<size_t>(num_total_features) * 512);
   for (int u = 0; u < nfn; ++u) std::memcpy(out + static_cast<size_t>(used[u]) * 512, hd.data() + static_cast<size_t>(u) * 512, sizeof(double) * 512);
+}
+
+void Dataset::QuantizedHistogram(const float* grad, const float* hess, const int32_t* idx, int cnt, const QuantSpec& quant, int32_t* out_q,
+                                 double* out_scale2, int64_t* out_hist) const {
+  if (quant.bins < 2 || quant.bins > 63) Fatal("num_grad_quant_bins should be in [2, 63], got " + std::to_string(quant.bins));
+  DevBuf<TreeCtrl> ctrl;
+  DevBuf<int4> q;
+  const std::vector<long long> hf = HistogramInt(grad, hess, idx, cnt, quant, ctrl, q);
+  TreeCtrl c;
+  ctrl.Download(&c, 1, stream);
+  std::vector<int4> hq(num_data);
+  q.Download(hq.data(), hq.size(), stream);
+  B200_CUDA(cudaStreamSynchronize(stream));
+  for (int i = 0; i < num_data; ++i) {
+    out_q[2 * i] = (hq[i].x << kLoBits) + hq[i].y;
+    out_q[2 * i + 1] = hess ? (hq[i].z << kLoBits) + hq[i].w : 1;
+  }
+  out_scale2[0] = c.inv_g; out_scale2[1] = c.inv_h;
+  std::memset(out_hist, 0, sizeof(int64_t) * static_cast<size_t>(num_total_features) * 512);
+  for (int u = 0; u < nfn; ++u) std::memcpy(out_hist + static_cast<size_t>(used[u]) * 512, hf.data() + static_cast<size_t>(u) * 512, sizeof(int64_t) * 512);
 }
 
 // " (part i)" in the messages of a multi-part create
@@ -1379,6 +1423,19 @@ static void CheckPathSmooth(const Config& cfg, bool voting_parallel) {
   if (cfg.path_smooth > kPathSmoothEps && voting_parallel) Fatal(kVotingPathSmooth);
 }
 
+// quantised training: the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+static void CheckQuantized(const Config& cfg) {
+  if (!cfg.use_quantized_grad) return;
+  // K4's packed plane flushes a cell after at most floor(32767 / B) additions, and its row chunks are whole 512-row stages
+  if (cfg.num_grad_quant_bins < 2 || cfg.num_grad_quant_bins > 63)
+    Fatal("num_grad_quant_bins should be in [2, 63] with use_quantized_grad, got " + std::to_string(cfg.num_grad_quant_bins));
+  // the renewed leaf outputs would need the bounds and the parent outputs of the scans; not restated
+  if (cfg.quant_train_renew_leaf && !cfg.monotone_constraints.empty())
+    Fatal("quant_train_renew_leaf does not support monotone_constraints; use quant_train_renew_leaf=false or no monotone_constraints");
+  if (cfg.quant_train_renew_leaf && cfg.path_smooth > kPathSmoothEps)
+    Fatal("quant_train_renew_leaf does not support path_smooth > 0; use quant_train_renew_leaf=false or path_smooth=0");
+}
+
 Booster::Booster(const std::string& model_text) : predictor(new Predictor(model, stream_)) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1429,6 +1486,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr), predictor(n
   CheckInteraction(cfg, *train, voting_);
   CheckByNode(cfg, voting_);
   CheckPathSmooth(cfg, voting_);
+  CheckQuantized(cfg);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1668,7 +1726,10 @@ void Booster::TrainOneTree(int k, HostTree* out) {
   cudaStream_t s = stream_;
   const int egrid = num_sms_ * 8;
   const TreeLearner::Bag bag{in_bag_.p, bag_idx_.p, bag_count_};
-  learner_->Grow(grad_.p + static_cast<size_t>(k) * n, hess_.p + static_cast<size_t>(k) * n, const_hessian_, use_bag_ ? &bag : nullptr);
+  const float* g = grad_.p + static_cast<size_t>(k) * n;
+  const float* h = hess_.p + static_cast<size_t>(k) * n;
+  learner_->Grow(g, h, const_hessian_, use_bag_ ? &bag : nullptr, iter * K + k);
+  if (cfg.use_quantized_grad && cfg.quant_train_renew_leaf) learner_->RenewQuantized(g, h, const_hessian_);
   if (obj_->RenewsLeaves()) learner_->Renew(*obj_, is_rf_ ? nullptr : score_k, is_rf_ ? rf_init_scores_[k] : 0.0);
   // rf keeps scores as the running average of (tree + init score) over the iterations [LightGBM rf.hpp MultiplyScore / UpdateScore]
   const double bias = is_rf_ ? rf_init_scores_[k] : 0.0, pre = is_rf_ ? static_cast<double>(iter + num_init_iteration) : 1.0;
@@ -1773,6 +1834,7 @@ void Booster::ResetParameter(const char* params) {
       CheckInteraction(cfg, *train, voting_);
       CheckByNode(cfg, voting_);
       CheckPathSmooth(cfg, voting_);
+      CheckQuantized(cfg);
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;

@@ -107,6 +107,12 @@ class Dataset {
   void GetBinsOfRows(const int32_t* rows, int nrows, uint16_t* out) const;      // [nrows][num_total_features], gathered on the device
   // K4 on this dataset's bins for the given rows (kernel-level parity entry), fp64 [F][256][2] per feature (bundle columns expanded)
   void Histogram(const float* grad, const float* hess, const int32_t* idx, int cnt, double* out) const;
+  // quantised training's K3 discretisation (B = bins levels, draws keyed by seed and tree) and packed K4 on the given rows: per row
+  // (q_g, q_h) into out_q [num_data][2], the scales (s_g, s_h) into out_scale2, int64 sums of q [F][256][2] per feature into out_hist.
+  // hess null: constant hessians (q_h = 1, the count plane).
+  struct QuantSpec { int bins = 0; bool stochastic = false; int seed = 0; int tree = 0; };
+  void QuantizedHistogram(const float* grad, const float* hess, const int32_t* idx, int cnt, const QuantSpec& quant, int32_t* out_q,
+                          double* out_scale2, int64_t* out_hist) const;
   void SetField(const char* name, const void* data, int n, int type);
   void GetField(const char* name, int* out_len, const void** out_ptr, int* out_type) const;
   void SetFeatureNames(const char** names, int n);
@@ -114,6 +120,10 @@ class Dataset {
   // K4's per-block bin-count bound of the uint8 tiles (hist_kernel.cuh): computed from the bins on first use, reused by every
   // booster on this dataset and by Histogram, dropped when rows are binned again.  Safe to call from several host threads.
   RowBlockBound BlockBound() const;
+ private:
+  std::vector<long long> HistogramInt(const float* grad, const float* hess, const int32_t* idx, int cnt, const QuantSpec& quant,
+                                      DevBuf<TreeCtrl>& ctrl, DevBuf<int4>& q) const;
+ public:
 
   int device = 0;
   int num_data = 0, num_total_features = 0;

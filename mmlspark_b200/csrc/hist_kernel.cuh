@@ -36,6 +36,7 @@
 // The LSU data pipe is the binding unit (ncu: ~94 % busy): an ATOMS wavefront costs ~0.93 cycles, so the loop spends
 // 16 x 0.93 (atomics) + 1 (bin word) + 0.5 (q) cycles per 128 cells.  DESIGN.md §3 has the measurements and the rejected variants.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include <cub/block/block_scan.cuh>
@@ -233,13 +234,24 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 // generic-proxy shared-memory writes before this fence are visible to the async proxy (TMA) after the following barrier
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
-// NATOM selects how many planes are accumulated: 4 = (g_hi,g_lo,h_hi,h_lo) general case,
-// 3 = constant-hessian objectives (g_hi,g_lo,count) [UPSTREAM is_constant_hessian path].
+// Quantised training (use_quantized_grad): the (g,h) words hold small integers, |q_g| <= floor(B/2) and |q_h| <= B (B =
+// num_grad_quant_bins), or q_h = 1 on the count plane of constant hessians.  One packed plane then carries both: the lane builds
+// w = (q_g << 16) + q_h once per row and a cell takes ONE 32-bit atomic (wrapping), instead of 4 (or 3).  As long as neither sum leaves
+// [-32767, 32767], w's low 16 bits are the sign-extended h sum and (w - h) >> 16 the g sum.  A cell takes at most
+// packed_flush_cap(B, count_plane) additions before a field could leave that range; it replaces kFlushRows in the flush rule.
+inline int packed_flush_cap(int quant_bins, bool count_plane) {
+  return 32767 / std::max(quant_bins / 2, count_plane ? 1 : quant_bins);
+}
+
+// The body of every K4 instantiation.  NATOM selects the planes: 4 = (g_hi,g_lo,h_hi,h_lo) general case, 3 = constant-hessian objectives
+// (g_hi,g_lo,count) [UPSTREAM is_constant_hessian path], 1 = one packed plane of quantised training (above).  cap: the additions a
+// cell may take between flushes (kFlushRows, or packed_flush_cap for NATOM 1, at least kWsStageRows); count_plane (NATOM 1 only):
+// q_h is 1 per row instead of the words' h fields.
 template <int NATOM>
-__global__ void __launch_bounds__(kWsThreads, 1)
-k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
-                 const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1,
-                 const HistWork* __restrict__ work, unsigned long long* __restrict__ hist, RowBlockBound bound) {
+__device__ __forceinline__ void k4_hist_body(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
+                                             const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1,
+                                             const HistWork* __restrict__ work, unsigned long long* __restrict__ hist, RowBlockBound bound,
+                                             int cap, int count_plane) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned* plane = reinterpret_cast<unsigned*>(smem_raw);
   unsigned char* stage_bins = smem_raw + 4 * kPlaneWords * 4;
@@ -256,12 +268,12 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
 
   // Work items are (tile, row chunk) pairs in TILE-MAJOR order; every CTA takes one contiguous range of them, so
   // consecutive items of a CTA mostly belong to the same feature tile and the sub-histogram is flushed only when the
-  // tile changes or the bound of the items absorbed since the last flush could pass the 2^14 additions per cell (below).
+  // tile changes or the bound of the items absorbed since the last flush could pass the cap of additions per cell (below).
   long long cells_rows = static_cast<long long>(n) * num_tiles;
   int rpi = static_cast<int>((cells_rows + 4LL * gridDim.x - 1) / (4LL * gridDim.x));
   rpi = (rpi + kWsStageRows - 1) / kWsStageRows * kWsStageRows;
   rpi = max(rpi, kWsStageRows);
-  rpi = min(rpi, kFlushRows);
+  rpi = min(rpi, cap / kWsStageRows * kWsStageRows);
   const int chunks = (n + rpi - 1) / rpi;
   const long long items = static_cast<long long>(chunks) * num_tiles;
   const int i0 = static_cast<int>(items * blockIdx.x / gridDim.x);
@@ -383,6 +395,11 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
           const int r = g * 32 + lane;
           if (r < rows) {
             const int4 q = sq[r];
+            unsigned packed = 0u;
+            if (NATOM == 1) {
+              const int qg = (q.x << kLoBits) + q.y, qh = count_plane ? 1 : (q.z << kLoBits) + q.w;
+              packed = (static_cast<unsigned>(qg) << 16) + static_cast<unsigned>(qh);
+            }
             const unsigned* rw = sw + r * 8;
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -394,14 +411,19 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
                 const unsigned b = (word >> (8 * kk)) & 0xFFu;
                 const unsigned a = b * 32u + static_cast<unsigned>(w8 * 4 + kk);
 #if B200GBM_K4_EXPERIMENT == 0 || B200GBM_K4_EXPERIMENT == 4
-                atomicAdd(&plane[a], static_cast<unsigned>(q.x));
-                atomicAdd(&plane[kPlaneWords + a], static_cast<unsigned>(q.y));
-                atomicAdd(&plane[2 * kPlaneWords + a], static_cast<unsigned>(q.z));
-                if (NATOM == 4) atomicAdd(&plane[3 * kPlaneWords + a], static_cast<unsigned>(q.w));
+                if (NATOM == 1) {
+                  atomicAdd(&plane[a], packed);
+                } else {
+                  atomicAdd(&plane[a], static_cast<unsigned>(q.x));
+                  atomicAdd(&plane[kPlaneWords + a], static_cast<unsigned>(q.y));
+                  atomicAdd(&plane[2 * kPlaneWords + a], static_cast<unsigned>(q.z));
+                  if (NATOM == 4) atomicAdd(&plane[3 * kPlaneWords + a], static_cast<unsigned>(q.w));
+                }
 #else   // tools/ubench_hist.cu only: cost model of the loop with 0 / 1 / 2 atomics per cell
                 if (B200GBM_K4_EXPERIMENT >= 2) atomicAdd(&plane[a], static_cast<unsigned>(q.x));
                 if (B200GBM_K4_EXPERIMENT >= 3) atomicAdd(&plane[kPlaneWords + a], static_cast<unsigned>(q.y));
                 if (B200GBM_K4_EXPERIMENT == 1) exp_sink ^= a + static_cast<unsigned>(q.x ^ q.y ^ q.z ^ q.w);
+                (void)packed;
 #endif
               }
             }
@@ -413,8 +435,8 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[slot]);
       }
-      // rpi <= kFlushRows, so a single item never breaks the 2^14 bound
-      const bool flush = (item + 1 == i1) || ((item + 1) / chunks != tile) || (acc_bound + next_bound > kFlushRows);
+      // rpi <= cap, so a single item never breaks the bound
+      const bool flush = (item + 1 == i1) || ((item + 1) / chunks != tile) || (acc_bound + next_bound > cap);
       if (!flush) continue;
       acc_bound = 0;
       // All consumers finished: flush the sub-histogram into the int64 leaf histogram (consumer-only named barriers; the producers
@@ -434,6 +456,15 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           const int e = (b0 + sbin[i]) * kTileFeat + lane;          // plane index = bin*32 + feature
+          if (NATOM == 1) {
+            const unsigned pw = plane[e];
+            plane[e] = 0u;
+            nz |= pw != 0u;
+            const int ph = static_cast<int>(static_cast<short>(pw & 0xFFFFu));      // sext16 of the low field
+            g[i] = (static_cast<int>(pw) - ph) >> 16;
+            h[i] = ph;
+            continue;
+          }
           const unsigned ghi = plane[e], glo = plane[kPlaneWords + e], hhi = plane[2 * kPlaneWords + e];
           const unsigned hlo = (NATOM == 4) ? plane[3 * kPlaneWords + e] : 0u;
           plane[e] = 0u;
@@ -481,20 +512,43 @@ k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_t
   }
 }
 
-// K4's shared memory exceeds the 48 KB default: raise the limit of both instantiations on the current device.  Call it once per
+// The full-precision instantiations <4> and <3>: their cap is the compile-time kFlushRows.
+template <int NATOM>
+__global__ void __launch_bounds__(kWsThreads, 1)
+k4_hist_build_ws(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
+                 const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1,
+                 const HistWork* __restrict__ work, unsigned long long* __restrict__ hist, RowBlockBound bound) {
+  k4_hist_body<NATOM>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound, kFlushRows, 0);
+}
+
+// The packed instantiation of quantised training: cap = packed_flush_cap(B, count_plane), >= kWsStageRows for B <= 63.
+__global__ void __launch_bounds__(kWsThreads, 1)
+k4_hist_build_packed(const uint8_t* __restrict__ bins, size_t rows_stride, int num_tiles, const int4* __restrict__ qgh,
+                     const int4* __restrict__ qord, const int* __restrict__ idx0, const int* __restrict__ idx1,
+                     const HistWork* __restrict__ work, unsigned long long* __restrict__ hist, RowBlockBound bound, int cap, int count_plane) {
+  k4_hist_body<1>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound, cap, count_plane);
+}
+
+// K4's shared memory exceeds the 48 KB default: raise the limit of every instantiation on the current device.  Call it once per
 // device at set-up; it is host work that does not belong in the per-split launches.
 inline cudaError_t set_k4_smem_limit() {
-  const cudaError_t e = cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
+  cudaError_t e = cudaFuncSetAttribute(k4_hist_build_ws<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(k4_hist_build_ws<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
+  e = cudaFuncSetAttribute(k4_hist_build_ws<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(k4_hist_build_packed, cudaFuncAttributeMaxDynamicSharedMemorySize, kWsSmemBytes);
 }
 
 // One persistent K4 launch: `grid` is one CTA per SM; constant-hessian objectives accumulate 3 planes (g_hi, g_lo, count).
-// `bound` is the bins' per-block bound (launch_block_bound); index lists given with it must be strictly ascending.
-inline void launch_k4(bool const_hessian, const uint8_t* bins, size_t rows_stride, int num_tiles, const int4* qgh, const int4* qord,
-                      const int* idx0, const int* idx1, const HistWork* work, unsigned long long* hist, RowBlockBound bound, int grid,
-                      cudaStream_t stream) {
-  if (const_hessian)
+// quant_bins > 0 (quantised training, the words hold K3's discretised q): the packed plane with that B's cap, q_h = 1 per row when
+// const_hessian.  `bound` is the bins' per-block bound (launch_block_bound); index lists given with it must be strictly ascending.
+inline void launch_k4(bool const_hessian, int quant_bins, const uint8_t* bins, size_t rows_stride, int num_tiles, const int4* qgh,
+                      const int4* qord, const int* idx0, const int* idx1, const HistWork* work, unsigned long long* hist, RowBlockBound bound,
+                      int grid, cudaStream_t stream) {
+  if (quant_bins > 0)
+    k4_hist_build_packed<<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound,
+                                                                    packed_flush_cap(quant_bins, const_hessian), const_hessian ? 1 : 0);
+  else if (const_hessian)
     k4_hist_build_ws<3><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound);
   else
     k4_hist_build_ws<4><<<grid, kWsThreads, kWsSmemBytes, stream>>>(bins, rows_stride, num_tiles, qgh, qord, idx0, idx1, work, hist, bound);

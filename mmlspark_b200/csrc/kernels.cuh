@@ -751,6 +751,21 @@ __global__ void k_set_scale(TreeCtrl* ctrl, int const_hessian, double hess_const
   ctrl->inv_h = const_hessian ? hess_const : ldexp(1.0, -eh);
   ctrl->root_q[0] = 0; ctrl->root_q[1] = 0; ctrl->root_q[2] = 0; ctrl->root_q[3] = 0;
 }
+// a 256-thread block's share of the root sums: sum q_g, sum q_h over its in-bag rows, and (block 0) the rows of the root
+__device__ __forceinline__ void d_add_root_sums(long long sg, long long sh, TreeCtrl* ctrl, const uint8_t* in_bag, int bag_count, int n) {
+  for (int o = 16; o; o >>= 1) { sg += __shfl_xor_sync(0xffffffffu, sg, o); sh += __shfl_xor_sync(0xffffffffu, sh, o); }
+  __shared__ long long s_g[8], s_h[8];
+  int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { s_g[warp] = sg; s_h[warp] = sh; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long a = 0, b = 0;
+    for (int w = 0; w < 8; ++w) { a += s_g[w]; b += s_h[w]; }
+    atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[0]), static_cast<unsigned long long>(a));
+    atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[1]), static_cast<unsigned long long>(b));
+    if (blockIdx.x == 0) atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[2]), static_cast<unsigned long long>(in_bag ? bag_count : n));
+  }
+}
 __global__ void __launch_bounds__(256)
 k_quantize(const float* __restrict__ g, const float* __restrict__ h, int n, int4* __restrict__ qgh, TreeCtrl* ctrl, int const_hessian,
            const uint8_t* __restrict__ in_bag, int bag_count) {
@@ -766,17 +781,100 @@ k_quantize(const float* __restrict__ g, const float* __restrict__ h, int n, int4
     qgh[i] = q;
     if (!in_bag || in_bag[i]) { sg += qg; sh += qh; }       // root sums run over the in-bag rows only
   }
+  d_add_root_sums(sg, sh, ctrl, in_bag, bag_count, n);
+}
+
+// ---------------------------------------------------------------- quantised training (use_quantized_grad), K3's discretisation
+// [UPSTREAM 4.x GradientDiscretizer::DiscretizeGradients], restated from knowledge: per tree, g and h become a few integer levels,
+// q_g in [-floor(B/2), floor(B/2)] at scale s_g = max|g| / floor(B/2) and q_h in [-B, B] at s_h = max|h| / B (B = num_grad_quant_bins;
+// a zero maximum gives scale 1).  Constant hessians keep q_h = 1 (the count plane).  tests/quant_ref.py restates every fp64 operation.
+// The draws of stochastic rounding: u in [0, 1) from a counter-based hash of (data_random_seed, tree index, rank-local row, g or h), so
+// nothing carries from tree to tree and any tree's draws follow from its key whatever the launch shape.  (LightGBM's own stream is not
+// reproduced.)
+__device__ __forceinline__ unsigned long long d_mix64(unsigned long long z) {      // splitmix64's finaliser
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ double d_quant_uniform(int seed, int tree, int row, int which) {
+  unsigned long long z = d_mix64(static_cast<unsigned long long>(static_cast<unsigned>(seed)));
+  z = d_mix64(z ^ static_cast<unsigned long long>(static_cast<unsigned>(tree)));
+  z = d_mix64(z ^ (2ull * static_cast<unsigned>(row) + static_cast<unsigned>(which)));
+  return static_cast<double>(z >> 11) * 0x1.0p-53;
+}
+// One value's level: v = x / s; with stochastic rounding trunc(v + sign(v) u), else v rounded half away from zero; clamped to [-lim, lim]
+__device__ __forceinline__ int d_discretize(float x, double s, int lim, int stochastic, double u) {
+  const double v = static_cast<double>(x) / s;
+  double q;
+  if (stochastic) {
+    q = trunc(v + d_sign(v) * u);
+  } else {
+    q = trunc(v);
+    if (fabs(v - q) >= 0.5) q += d_sign(v);
+  }
+  return static_cast<int>(fmin(fmax(q, static_cast<double>(-lim)), static_cast<double>(lim)));
+}
+// after k_set_scale (whose exponents the leaf renewal keeps using): the scales of the discretised words
+__global__ void k_set_quant_scale(TreeCtrl* ctrl, int const_hessian, int quant_bins) {
+  const float mg = __uint_as_float(ctrl->absmax_bits[0]), mh = __uint_as_float(ctrl->absmax_bits[1]);
+  ctrl->inv_g = (mg > 0.f && isfinite(mg)) ? static_cast<double>(mg) / (quant_bins / 2) : 1.0;
+  if (!const_hessian) ctrl->inv_h = (mh > 0.f && isfinite(mh)) ? static_cast<double>(mh) / quant_bins : 1.0;
+}
+// q into K3's fixed-point words (the same {g_hi, g_lo, h_hi, h_lo} layout, so every later kernel reads them as it reads k_quantize's) and
+// the root sums over the in-bag rows.  tree: iteration * trees per iteration + class.
+__global__ void __launch_bounds__(256)
+k_quantize_discrete(const float* __restrict__ g, const float* __restrict__ h, int n, int4* __restrict__ qgh, TreeCtrl* ctrl, int const_hessian,
+                    const uint8_t* __restrict__ in_bag, int bag_count, int quant_bins, int stochastic, int seed, int tree) {
+  const double sg_scale = ctrl->inv_g, sh_scale = ctrl->inv_h;
+  long long sg = 0, sh = 0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int qg = d_discretize(g[i], sg_scale, quant_bins / 2, stochastic, stochastic ? d_quant_uniform(seed, tree, i, 0) : 0.0);
+    const int qh = const_hessian ? 1 : d_discretize(h[i], sh_scale, quant_bins, stochastic, stochastic ? d_quant_uniform(seed, tree, i, 1) : 0.0);
+    int4 q;
+    q.x = qg >> kLoBits; q.y = qg & ((1 << kLoBits) - 1);
+    if (const_hessian) { q.z = 1; q.w = 0; }
+    else { q.z = qh >> kLoBits; q.w = qh & ((1 << kLoBits) - 1); }
+    qgh[i] = q;
+    if (!in_bag || in_bag[i]) { sg += qg; sh += qh; }
+  }
+  d_add_root_sums(sg, sh, ctrl, in_bag, bag_count, n);
+}
+
+// quant_train_renew_leaf ([UPSTREAM 4.x GradientDiscretizer::RenewIntGradTreeOutput], from knowledge): each leaf's true in-bag sums of
+// g and h on K3's 36-bit fixed-point grid (k_set_scale's exponents), so they are exact and order-independent and ranks agree bit for bit.
+// grid x = num_leaves * blocks_per_leaf: block b sums part b % blocks_per_leaf of leaf b / blocks_per_leaf.  sums: [num_leaves][2], zeroed.
+__global__ void __launch_bounds__(256)
+k_quant_leaf_sums(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const int* __restrict__ idx0,
+                  const int* __restrict__ idx1, const float* __restrict__ g, const float* __restrict__ h, int const_hessian,
+                  int blocks_per_leaf, long long* __restrict__ sums) {
+  const int l = blockIdx.x / blocks_per_leaf, part = blockIdx.x - l * blocks_per_leaf;
+  if (l >= ctrl->num_leaves) return;
+  const LeafState& L = leaves[l];
+  const int* src = L.buf ? idx1 : idx0;
+  const int eg = ctrl->exp_g, eh = ctrl->exp_h;
+  long long sg = 0, sh = 0;
+  for (int i = part * blockDim.x + threadIdx.x; i < L.count; i += blocks_per_leaf * blockDim.x) {
+    const int r = L.identity ? (L.begin + i) : src[L.begin + i];
+    sg += __double2ll_rn(ldexp(static_cast<double>(g[r]), eg));
+    sh += const_hessian ? 1 : __double2ll_rn(ldexp(static_cast<double>(h[r]), eh));
+  }
   for (int o = 16; o; o >>= 1) { sg += __shfl_xor_sync(0xffffffffu, sg, o); sh += __shfl_xor_sync(0xffffffffu, sh, o); }
-  __shared__ long long s_g[8], s_h[8];
-  int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { s_g[warp] = sg; s_h[warp] = sh; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long a = 0, b = 0;
-    for (int w = 0; w < 8; ++w) { a += s_g[w]; b += s_h[w]; }
-    atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[0]), static_cast<unsigned long long>(a));
-    atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[1]), static_cast<unsigned long long>(b));
-    if (blockIdx.x == 0) atomicAdd(reinterpret_cast<unsigned long long*>(&ctrl->root_q[2]), static_cast<unsigned long long>(in_bag ? bag_count : n));
+  if ((threadIdx.x & 31) == 0 && (sg | sh)) {
+    atomicAdd(reinterpret_cast<unsigned long long*>(&sums[2 * l]), static_cast<unsigned long long>(sg));
+    atomicAdd(reinterpret_cast<unsigned long long*>(&sums[2 * l + 1]), static_cast<unsigned long long>(sh));
+  }
+}
+// leaf_value = d_calc_output at the (all-reduced) true sums; leaf_weight, internal values and counts keep the quantised sums.  A leaf
+// whose true h sum + lambda_l2 is 0 (custom hessians can cancel; the scans chose the split on the quantised sums) keeps its quantised
+// output instead of an inf or NaN.
+__global__ void k_quant_renew_apply(const TreeCtrl* __restrict__ ctrl, TreeDev tree, const long long* __restrict__ sums, int const_hessian,
+                                    SplitParams p) {
+  const int nl = ctrl->num_leaves;
+  const double ig = ldexp(1.0, -ctrl->exp_g), ih = const_hessian ? 1.0 : ldexp(1.0, -ctrl->exp_h);
+  for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < nl; l += gridDim.x * blockDim.x) {
+    const double sh = static_cast<double>(sums[2 * l + 1]) * ih;
+    if (sh + p.l2 != 0.0) tree.leaf_value[l] = d_calc_output(static_cast<double>(sums[2 * l]) * ig, sh, p);
   }
 }
 

@@ -84,6 +84,7 @@ TreeLearner::TreeLearner(const Dataset& train, const Config& cfg, const Objectiv
   }
 
   qgh_.Alloc(n); qord_.Alloc(n); idx0_.Alloc(n); idx1_.Alloc(n);
+  quant_sums_.Alloc(2 * static_cast<size_t>(L));      // whatever quant_train_renew_leaf says: a ResetParameter may set it
   slot_elems_ = train.hist_pairs * 2;
   H_.Alloc(slot_elems_); H_.Zero(stream_); pool_.Alloc(slot_elems_ * L);
   {
@@ -245,6 +246,21 @@ void TreeLearner::Renew(const Objective& obj, const double* score_k, double rf_p
   timing_.launches += wptr ? 7 : 6;
 }
 
+// quant_train_renew_leaf: the leaves' row lists are this rank's in-bag rows, so the sums are all-reduced as the histograms are
+void TreeLearner::RenewQuantized(const float* g, const float* h, bool const_hessian) {
+  const int L = cfg_.num_leaves;
+  cudaStream_t s = stream_;
+  B200_CUDA(cudaMemsetAsync(quant_sums_.p, 0, quant_sums_.n * sizeof(long long), s));
+  // about 8 blocks per SM in all, at least one per leaf; the grid's x dimension takes any num_leaves
+  const int per_leaf = std::max(1, num_sms_ * 8 / L);
+  k_quant_leaf_sums<<<static_cast<unsigned>(static_cast<long long>(per_leaf) * L), 256, 0, s>>>(ctrl_.p, leaves_.p, idx0_.p, idx1_.p, g, h,
+                                                                                                const_hessian ? 1 : 0, per_leaf, quant_sums_.p);
+  if (parallel_) Net().AllReduce(quant_sums_.p, quant_sums_.n, ncclInt64, ncclSum, s);
+  k_quant_renew_apply<<<(L + 127) / 128, 128, 0, s>>>(ctrl_.p, tree_dev_, quant_sums_.p, const_hessian ? 1 : 0, sp_);
+  B200_CUDA(cudaGetLastError());
+  timing_.launches += 2;
+}
+
 // k_partition is launched cooperatively: its software grid barriers need every block resident
 // Column-major copies of the training tiles for k_partition, so that its phase 1 reads one byte per row instead of a 32-byte sector —
 // same results either way.  Set up once, before the first tree, after every other buffer of the booster exists, and only within a
@@ -390,7 +406,7 @@ void TreeLearner::LaunchPartition(int grid, int last) {
 
 // One tree: the whole leaf-wise growth is enqueued without a host sync; leaf choice, smaller/larger
 // selection, partition sizes all live in TreeCtrl / LeafState on the device.
-void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const Bag* bag) {
+void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const Bag* bag, int tree_index) {
   EnsureColumnCopy();
   const Dataset& d = train_;
   const int n = d.num_data;
@@ -404,7 +420,16 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
   k_absmax<<<egrid, 256, 0, s>>>(g, h, n, ctrl);
   if (parallel_) Net().AllReduce(&ctrl->absmax_bits[0], 2, ncclUint32, ncclMax, s);
   k_set_scale<<<1, 1, 0, s>>>(ctrl, const_hessian ? 1 : 0, 1.0);
-  k_quantize<<<egrid, 256, 0, s>>>(g, h, n, qgh_.p, ctrl, const_hessian ? 1 : 0, bag ? bag->in_bag : nullptr, rows_);
+  // quantised training: B = num_grad_quant_bins levels instead of the 36-bit grid, and K4's packed plane below
+  const int quant_bins = cfg_.use_quantized_grad ? cfg_.num_grad_quant_bins : 0;
+  if (quant_bins > 0) {
+    k_set_quant_scale<<<1, 1, 0, s>>>(ctrl, const_hessian ? 1 : 0, quant_bins);
+    k_quantize_discrete<<<egrid, 256, 0, s>>>(g, h, n, qgh_.p, ctrl, const_hessian ? 1 : 0, bag ? bag->in_bag : nullptr, rows_, quant_bins,
+                                              cfg_.stochastic_rounding ? 1 : 0, cfg_.data_random_seed, tree_index);
+    timing_.launches += 1;
+  } else {
+    k_quantize<<<egrid, 256, 0, s>>>(g, h, n, qgh_.p, ctrl, const_hessian ? 1 : 0, bag ? bag->in_bag : nullptr, rows_);
+  }
   if (parallel_) Net().AllReduce(&ctrl->root_q[0], 3, ncclInt64, ncclSum, s);
   ResetFeaturesByTree();
   if (bag)      // the root leaf is the ascending in-bag row list (SetBaggingData); partitions then ping-pong idx0/idx1 as usual
@@ -434,7 +459,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
     mark();
     // the scratch histogram H is zero here: zeroed at set-up and by every partition kernel after the scan consumed it
     nvtxRangePushA("b200gbm:K4 histogram");
-    launch_k4(const_hessian, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
+    launch_k4(const_hessian, quant_bins, d.bins.p, d.rows_stride, d.num_tiles, qgh_.p, qord_.p, idx0_.p, idx1_.p, &ctrl->hist_work,
               reinterpret_cast<unsigned long long*>(H_.p), bound, num_sms_, s);
     if (d.nw > 0) {      // the features with more than 256 bins: own sub-histogram layout (k4_hist_wide)
       int max_nb = 0, units = 0;

@@ -18,8 +18,11 @@ class TreeLearner {
 
   // the rows a bagged tree is grown on: the in-bag flags and the ascending in-bag row list
   struct Bag { const uint8_t* in_bag; const int* rows; int count; };
-  // enqueues the whole leaf-wise growth of one tree on (g, h) without a host sync; bag null: every row
-  void Grow(const float* g, const float* h, bool const_hessian, const Bag* bag);
+  // enqueues the whole leaf-wise growth of one tree on (g, h) without a host sync; bag null: every row.  tree_index (iteration * trees
+  // per iteration + class) keys the draws of quantised training's stochastic rounding.
+  void Grow(const float* g, const float* h, bool const_hessian, const Bag* bag, int tree_index);
+  // quant_train_renew_leaf: the grown tree's leaf values from the leaves' true in-bag sums of the (g, h) it was grown on
+  void RenewQuantized(const float* g, const float* h, bool const_hessian);
   // percentile objectives: patch the grown tree's leaf values (score_k null: residuals against rf_pred)
   void Renew(const Objective& obj, const double* score_k, double rf_pred);
   // score_k[row] += shrinkage * leaf value of the row's leaf, walking the leaves' row lists (every row is in a leaf)
@@ -68,6 +71,7 @@ class TreeLearner {
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built
   DevBuf<int> idx0_, idx1_;
+  DevBuf<long long> quant_sums_;   // quant_train_renew_leaf: [num_leaves][2] the leaves' true sums on K3's fixed-point grid
   DevBuf<long long> H_;          // scratch histogram of the current smaller leaf
   DevBuf<long long> pool_;       // [num_leaves] leaf histograms
   size_t slot_elems_ = 0;

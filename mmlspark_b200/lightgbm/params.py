@@ -46,6 +46,8 @@ COMMON_DEFAULTS = dict(
     interactionConstraints=(),          # interaction_constraints: lists of feature indices; a branch splits on features of one list only
     featureFractionByNode=1.0,          # feature_fraction_bynode: the share of the tree's features each leaf's split is chosen from
     pathSmooth=0.0,                     # path_smooth: smooths every split gain and leaf output toward the parent leaf's output
+    # LightGBM 4's quantised training: use_quantized_grad, num_grad_quant_bins, quant_train_renew_leaf, stochastic_rounding
+    useQuantizedGrad=False, numGradQuantBins=4, quantTrainRenewLeaf=False, stochasticRounding=True,
     delegate=None,
     # column params (core/contracts/Params.scala:93-208 + Spark ML)
     featuresCol="features", labelCol="label", predictionCol="prediction", weightCol=None, initScoreCol=None,
@@ -136,6 +138,9 @@ class TrainParams:
             s += "feature_fraction_bynode=%s " % scala_double(p["featureFractionByNode"])
         if p["pathSmooth"] != 0.0:      # only when set, so every other parameter string stays as the reference builds it
             s += "path_smooth=%s " % scala_double(p["pathSmooth"])
+        if p["useQuantizedGrad"]:      # only when set, so every other parameter string stays as the reference builds it
+            s += "use_quantized_grad=true num_grad_quant_bins=%d quant_train_renew_leaf=%s stochastic_rounding=%s " % (
+                p["numGradQuantBins"], scala_bool(p["quantTrainRenewLeaf"]), scala_bool(p["stochasticRounding"]))
         return s
 
     def to_string(self):

@@ -1,7 +1,8 @@
 // Microbenchmarks that decide the K4 histogram design (build() compiles it to build/ubench_hist).
 //  Part A: shared-memory scatter-add throughput per SM for the candidate accumulator schemes
 //          (native ATOMS.ADD.32 owner-bank / random-bank, CAS float, non-atomic owner RMW ...).
-//  Part B: the engine's K4 kernel (k4_hist_build_ws<4> and <3>, launched through launch_k4 with the per-block bin-count
+//  Part B: the engine's K4 kernel (k4_hist_build_ws<4> and <3>, and quantised training's packed k4_hist_build_packed, with and
+//          without the count plane, all launched through launch_k4 with the per-block bin-count
 //          bound of launch_block_bound) on synthetic tile-major bins, uniform and skewed: checked exactly against an int64
 //          host computation, then timed with CUDA events and reported as cells/s and algorithmic GB/s.
 // Usage: ubench_hist [ROWS] [SKIP_PART_A]   (ROWS defaults to 10M; SKIP_PART_A = 1 skips Part A)
@@ -136,6 +137,15 @@ __global__ void gen_q(int4* q, size_t n, unsigned seed) {
     q[i] = make_int4(g_hi, g_lo, h_hi, h_lo);
   }
 }
+// quantised (g,h) words of the packed instantiation, in K3's layout: q_g = +-floor(B/2) and q_h = +-B (1 in 8 negative), the field
+// limits, so that a cell that takes more than packed_flush_cap additions between flushes leaves its 16-bit field and mismatches
+__global__ void gen_q_packed(int4* q, size_t n, int B, unsigned seed) {
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  for (; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const int qg = (hash32((unsigned)i ^ seed) & 7u) ? B / 2 : -(B / 2), qh = (hash32((unsigned)i * 3u + seed) & 7u) ? B : -B;
+    q[i] = make_int4(qg >> kLoBits, qg & ((1 << kLoBits) - 1), qh >> kLoBits, qh & ((1 << kLoBits) - 1));
+  }
+}
 __global__ void gen_idx(int* idx, int n, int stride) {   // every `stride`-th row, ascending
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   for (; i < n; i += gridDim.x * blockDim.x) idx[i] = i * stride;
@@ -185,7 +195,8 @@ int main(int argc, char** argv) {
   size_t slot_elems = (size_t)F * 256 * 2;
   CK(cudaMalloc(&d_bins, (size_t)num_tiles * rows_stride * 32));
   CK(cudaMalloc(&d_q, N * sizeof(int4)));
-  CK(cudaMalloc(&d_qord, N * sizeof(int4)));
+  int4* d_qp; CK(cudaMalloc(&d_qp, N * sizeof(int4)));      // the packed instantiation's words (gen_q_packed)
+  CK(cudaMalloc(&d_qord, 2 * N * sizeof(int4)));      // the second half: the packed words in leaf order (k4_check)
   CK(cudaMalloc(&d_idx, N * sizeof(int)));
   CK(cudaMalloc(&d_hist, slot_elems * 8));
   CK(cudaMalloc(&d_work, sizeof(HistWork) * 2));
@@ -200,6 +211,17 @@ int main(int argc, char** argv) {
     CK(cudaDeviceSynchronize());
   };
   gen_q<<<nsm * 8, 256>>>(d_q, N, 777u);
+  // kinds of K4 launch: NATOM 4 and 3 on d_q; packed (quantised training) on d_qp at kPackedB, with the words' q_h ("packed") or
+  // q_h = 1 ("packed_count")
+  const int kPackedB = 63;      // the largest B: the smallest cap (520 additions), so the flush rule is tested hardest
+  gen_q_packed<<<nsm * 8, 256>>>(d_qp, N, kPackedB, 999u);
+  enum Kind { kN4, kN3, kPacked, kPackedCount };
+  const char* kind_name[] = {"natom4", "natom3", "packed", "packed_count"};
+  auto launch = [&](Kind k, int quant_bins, int4* qord, RowBlockBound rb) {
+    const bool packed = k == kPacked || k == kPackedCount;
+    launch_k4(k == kN3 || k == kPackedCount, packed ? quant_bins : 0, d_bins, rows_stride, num_tiles, packed ? d_qp : d_q, qord, d_idx, d_idx,
+              d_work, d_hist, rb, nsm, 0);
+  };
   set_bins(0, 0);
   CK(set_k4_smem_limit());
 
@@ -212,9 +234,11 @@ int main(int argc, char** argv) {
   {
     const int n_chk = (int)std::min<size_t>(N, 1000000);
     std::vector<uint8_t> hb((size_t)num_tiles * n_chk * 32);      // [tile][row][32] of the checked rows
-    std::vector<int4> hq(n_chk);
+    std::vector<int4> hq(n_chk), hqp(n_chk);
     CK(cudaMemcpy(hq.data(), d_q, (size_t)n_chk * 16, cudaMemcpyDeviceToHost));
-    std::vector<long long> got(slot_elems), want4(slot_elems), want3(slot_elems);
+    CK(cudaMemcpy(hqp.data(), d_qp, (size_t)n_chk * 16, cudaMemcpyDeviceToHost));
+    std::vector<long long> got(slot_elems), want[4];
+    for (auto& v : want) v.resize(slot_elems);
     printf(" \"k4_check\": {\"rows\": %d, \"mismatches\": {", n_chk);
     struct State { const char* name; int skew_r0, skew_r1, stride; };
     const State states[] = {{"uniform", 0, 0, 3}, {"skew", 0, n_chk, 2}, {"skew_second_half", n_chk / 2, n_chk, 37}};
@@ -227,33 +251,33 @@ int main(int argc, char** argv) {
         const int step = pass ? st.stride : 1;
         const HistWork hw = {0, n_chk / step, pass, 0};
         CK(cudaMemcpy(d_work, &hw, sizeof(hw), cudaMemcpyHostToDevice));
+        int4* d_qpord = d_qord + n_chk;      // the packed words in leaf order, beside d_q's
         if (pass) {
           gen_idx<<<nsm, 256>>>(d_idx, hw.count, step);
           k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);
+          k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_qp, d_qpord);
         }
-        std::fill(want4.begin(), want4.end(), 0LL);
-        std::fill(want3.begin(), want3.end(), 0LL);
+        for (auto& v : want) std::fill(v.begin(), v.end(), 0LL);
         for (int i = 0; i < hw.count * step; i += step) {
           const long long g = ((long long)hq[i].x << kLoBits) + hq[i].y;
-          const long long h4 = ((long long)hq[i].z << kLoBits) + hq[i].w, h3 = hq[i].z;
+          const long long gp = ((long long)hqp[i].x << kLoBits) + hqp[i].y, hp = ((long long)hqp[i].z << kLoBits) + hqp[i].w;
+          const long long gh[4][2] = {{g, ((long long)hq[i].z << kLoBits) + hq[i].w}, {g, hq[i].z}, {gp, hp}, {gp, 1}};
           for (int t = 0; t < num_tiles; ++t) {
             const uint8_t* row = &hb[((size_t)t * n_chk + i) * 32];
             for (int l = 0; l < 32; ++l) {
               size_t o = ((size_t)(t * 32 + l) * 256 + row[l]) * 2;
-              want4[o] += g; want4[o + 1] += h4;
-              want3[o] += g; want3[o + 1] += h3;
+              for (int k = 0; k < 4; ++k) { want[k][o] += gh[k][0]; want[k][o + 1] += gh[k][1]; }
             }
           }
         }
-        for (int natom : {4, 3}) {
+        for (Kind k : {kN4, kN3, kPacked, kPackedCount}) {
           CK(cudaMemset(d_hist, 0, slot_elems * 8));
-          launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, kb, nsm, 0);
+          launch(k, kPackedB, (k == kPacked || k == kPackedCount) ? d_qpord : d_qord, kb);
           CK(cudaGetLastError());
           CK(cudaDeviceSynchronize());
           CK(cudaMemcpy(got.data(), d_hist, slot_elems * 8, cudaMemcpyDeviceToHost));
-          const std::vector<long long>& want = natom == 4 ? want4 : want3;
-          size_t bad = 0; for (size_t i = 0; i < want.size(); ++i) bad += (got[i] != want[i]);
-          printf("%s\"%s_natom%d_%s\": %zu", first ? "" : ", ", st.name, natom, pass ? "gathered" : "contiguous", bad);
+          size_t bad = 0; for (size_t i = 0; i < slot_elems; ++i) bad += (got[i] != want[k][i]);
+          printf("%s\"%s_%s_%s\": %zu", first ? "" : ", ", st.name, kind_name[k], pass ? "gathered" : "contiguous", bad);
           first = false;
           k4_bad += bad;
         }
@@ -266,7 +290,7 @@ int main(int argc, char** argv) {
   // timing: full pass (contiguous) and gathered passes, NATOM 4 and 3.  The two skew = 1 rows run on bins whose column 5 of tile 1
   // has nearly every row in one bin, where the block bound lets that tile flush only every ~2^14 rows: once with the block bound
   // and once (bound = 0) with the row-count bound, i.e. a flush every 2^14 rows, what the kernel does for an index list that repeats rows.
-  auto time_it = [&](int natom, int n, int use_idx, RowBlockBound rb, int reps) -> float {
+  auto time_it = [&](Kind kind, int quant_bins, int n, int use_idx, RowBlockBound rb, int reps) -> float {
     HistWork hw = {0, n, use_idx, 0};
     CK(cudaMemcpy(d_work, &hw, sizeof(hw), cudaMemcpyHostToDevice));
     cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
@@ -274,8 +298,9 @@ int main(int argc, char** argv) {
     for (int r = 0; r < reps + 2; ++r) {
       CK(cudaMemsetAsync(d_hist, 0, slot_elems * 8));
       CK(cudaEventRecord(e0));
-      if (use_idx) k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, d_q, d_qord);     // part of a leaf pass: timed
-      launch_k4(natom == 3, d_bins, rows_stride, num_tiles, d_q, d_qord, d_idx, d_idx, d_work, d_hist, rb, nsm, 0);
+      const bool packed = kind == kPacked || kind == kPackedCount;
+      if (use_idx) k_gather_q<<<nsm * 8, 256>>>(d_work, d_idx, d_idx, packed ? d_qp : d_q, d_qord);     // part of a leaf pass: timed
+      launch(kind, quant_bins, d_qord, rb);
       CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
       float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
       if (r >= 2) { best = std::min(best, ms); tot += ms; }
@@ -292,18 +317,21 @@ int main(int argc, char** argv) {
     printf(" \"block_bound\": {\"ms\": %.3f, \"bin_bytes\": %zu},\n", ms, (size_t)num_tiles * N * 32);
   }
   printf(" \"k4_timing\": [\n");
-  struct Cfg { int natom; double frac; int use_idx; int skew; int bound; };
-  Cfg cfgs[] = {{4, 1.0, 0, 0, 1}, {3, 1.0, 0, 0, 1}, {4, 0.5, 1, 0, 1}, {4, 0.1, 1, 0, 1}, {4, 0.01, 1, 0, 1}, {4, 0.001, 1, 0, 1},
-                {4, 1.0, 0, 1, 1}, {4, 1.0, 0, 1, 0}};
+  // packed rows (quantised training) at B = 4 and 16 beside <4> and <3>: their cap is 8191 and 2047 additions (a flush at least every
+  // 7680 and 1536 rows of a bin-dense column).  The packed words are gen_q_packed's at B = 63; the timing does not depend on their values.
+  struct Cfg { Kind kind; int quant_bins; double frac; int use_idx; int skew; int bound; };
+  Cfg cfgs[] = {{kN4, 0, 1.0, 0, 0, 1}, {kN3, 0, 1.0, 0, 0, 1}, {kPacked, 4, 1.0, 0, 0, 1}, {kPacked, 16, 1.0, 0, 0, 1}, {kPackedCount, 4, 1.0, 0, 0, 1},
+                {kN4, 0, 0.5, 1, 0, 1}, {kN4, 0, 0.1, 1, 0, 1}, {kPacked, 4, 0.1, 1, 0, 1}, {kN4, 0, 0.01, 1, 0, 1}, {kN4, 0, 0.001, 1, 0, 1},
+                {kN4, 0, 1.0, 0, 1, 1}, {kN4, 0, 1.0, 0, 1, 0}, {kPacked, 4, 1.0, 0, 1, 1}};
   for (size_t c = 0; c < sizeof(cfgs) / sizeof(cfgs[0]); ++c) {
     int n = (int)(N * cfgs[c].frac);
     if (cfgs[c].use_idx) { gen_idx<<<nsm, 256>>>(d_idx, n, (int)(1.0 / cfgs[c].frac)); CK(cudaDeviceSynchronize()); }
     if (cfgs[c].skew && !cfgs[c - 1].skew) set_bins(0, (int)N);
-    float ms = time_it(cfgs[c].natom, n, cfgs[c].use_idx, cfgs[c].bound ? kb : RowBlockBound{nullptr, 0}, 5);
+    float ms = time_it(cfgs[c].kind, cfgs[c].quant_bins, n, cfgs[c].use_idx, cfgs[c].bound ? kb : RowBlockBound{nullptr, 0}, 5);
     double cells = (double)n * F;
     double bytes = (double)n * (F + 16.0 * num_tiles + (cfgs[c].use_idx ? 4.0 * num_tiles : 0.0)) + (double)F * 256 * 16;
-    printf("  {\"natom\": %d, \"rows\": %d, \"gather\": %d, \"skew\": %d, \"bound\": %d, \"ms\": %.4f, \"gcells_per_s\": %.2f, \"algo_GBps\": %.1f}%s\n",
-           cfgs[c].natom, n, cfgs[c].use_idx, cfgs[c].skew, cfgs[c].bound, ms, cells / ms * 1e-6, bytes / ms * 1e-6,
+    printf("  {\"kind\": \"%s\", \"quant_bins\": %d, \"rows\": %d, \"gather\": %d, \"skew\": %d, \"bound\": %d, \"ms\": %.4f, \"gcells_per_s\": %.2f, \"algo_GBps\": %.1f}%s\n",
+           kind_name[cfgs[c].kind], cfgs[c].quant_bins, n, cfgs[c].use_idx, cfgs[c].skew, cfgs[c].bound, ms, cells / ms * 1e-6, bytes / ms * 1e-6,
            c + 1 < sizeof(cfgs) / sizeof(cfgs[0]) ? "," : "");
   }
   printf(" ]\n}\n");
