@@ -112,6 +112,11 @@ int LGBM_BoosterUpdateOneIterCustom(BoosterHandle handle, const float* grad, con
 /* LGB/booster/LightGBMBooster.scala:315-318 ("learning_rate=<x>") */
 int LGBM_BoosterResetParameter(BoosterHandle handle, const char* parameters);
 
+/* LightGBM's LGBM_BoosterRefit (Booster.refit / task=refit): leaf_preds is row-major nrow x ncol, the leaf of training row i in model
+ * j (nrow = the training rows, ncol = the models).  Every tree keeps its structure; each leaf value becomes
+ * refit_decay_rate * leaf + (1 - refit_decay_rate) * the leaf output of its rows' gradients at the current training scores. */
+int LGBM_BoosterRefit(BoosterHandle handle, const int32_t* leaf_preds, int32_t nrow, int32_t ncol);
+
 /* ---- evaluation / introspection ---------------------------------------------------------- */
 int LGBM_BoosterGetEvalCounts(BoosterHandle handle, int* out_len);
 /* LGB/booster/LightGBMBooster.scala:279-294 (through the SWIG string-array helper) */
@@ -214,6 +219,9 @@ int B200GBM_DatasetQuantizedHistogram(DatasetHandle handle, const float* grad, c
 /* kernel-level entry: the objective's gradients and hessians (K1/K2) at the booster's current training scores, class-major [K][n]
  * host arrays; classes the objective does not train read back as 0.  Training state and the model are not changed. */
 int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess);
+/* the last LGBM_BoosterRefit: out = {staging ms, per-tree work ms (host clock, each ending in a device sync), batches of models,
+ * row blocks staged} */
+int B200GBM_BoosterGetRefitTiming(BoosterHandle handle, double* out4);
 /* timing of the engine stream, CUDA events: out = {hist_ms, total_ms, hist_rows, hist_launches, launches, iterations} */
 int B200GBM_BoosterSetProfile(BoosterHandle handle, int profile_hist);
 int B200GBM_BoosterGetTiming(BoosterHandle handle, double* out6, int reset);

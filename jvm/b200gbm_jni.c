@@ -1,7 +1,7 @@
 /*
  * JNI shim: com.microsoft.ml.lightgbm.lightgbmlibJNI  ->  libb200gbm.so.  This image has no JDK, so the file is type- and link-checked
  * against jvm/stub/jni.h + libb200gbm.so by tests/test_capi_cpu.py::test_jni_shim_compiles_and_links; it has never run inside a JVM.
- * It covers every lightgbmlib.* method and ChunkedArray proxy the reference's Scala code calls (90 natives).
+ * It covers every lightgbmlib.* method and ChunkedArray proxy the reference's Scala code calls (90 natives), and LGBM_BoosterRefit.
  *
  * The reference loads `_lightgbm` and `_lightgbm_swig` from the lightgbmlib jar
  * (lightgbm/src/main/scala/com/microsoft/ml/spark/lightgbm/LightGBMUtils.scala:38-41) and calls the SWIG-generated
@@ -71,6 +71,11 @@ JNI_FN(LGBM_1BoosterLoadModelFromString)(JNIEnv* env, jclass cls, jstring model,
 JNI_FN(LGBM_1BoosterMerge)(JNIEnv* env, jclass cls, jlong h, jlong other) { (void)env; (void)cls; return LGBM_BoosterMerge(P(h), P(other)); }
 JNI_FN(LGBM_1BoosterAddValidData)(JNIEnv* env, jclass cls, jlong h, jlong v) { (void)env; (void)cls; return LGBM_BoosterAddValidData(P(h), P(v)); }
 JNI_FN(LGBM_1BoosterFree)(JNIEnv* env, jclass cls, jlong h) { (void)env; (void)cls; return LGBM_BoosterFree(P(h)); }
+/* leaf_preds: an int32 array pointer (new_intArray) of nrow x ncol leaf indices */
+JNI_FN(LGBM_1BoosterRefit)(JNIEnv* env, jclass cls, jlong h, jlong leaf_preds, jint nrow, jint ncol) {
+  (void)env; (void)cls;
+  return LGBM_BoosterRefit(P(h), (const int32_t*)P(leaf_preds), nrow, ncol);
+}
 /* the hot call: one boosting iteration on the GPU */
 JNI_FN(LGBM_1BoosterUpdateOneIter)(JNIEnv* env, jclass cls, jlong h, jlong is_finished) {
   (void)env; (void)cls;

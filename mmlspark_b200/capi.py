@@ -372,6 +372,21 @@ class Booster:
         check(load().LGBM_BoosterUpdateOneIterCustom(self.handle, _ptr(g), _ptr(h), C.byref(fin)))
         return fin.value == 1
 
+    def refit(self, leaf_preds):
+        """LGBM_BoosterRefit: keep every tree's structure and re-estimate its leaf values from the training rows.  leaf_preds: int32
+        (num_data, num_models), the leaf of training row i in model j (PREDICT_LEAF_INDEX of the training rows); read in place when it is
+        already a C-contiguous int32 array.  The decay is the booster's refit_decay_rate parameter (default 0.9)."""
+        a = np.ascontiguousarray(leaf_preds, dtype=np.int32)
+        if a.ndim != 2:
+            raise LightGBMError("refit: leaf_preds must be a 2-D (num_data, num_models) array")
+        check(load().LGBM_BoosterRefit(self.handle, _ptr(a), C.c_int32(a.shape[0]), C.c_int32(a.shape[1])))
+
+    def refit_timing(self):
+        """the last refit (B200GBM_BoosterGetRefitTiming): staging and per-tree host milliseconds, batches of models, row blocks"""
+        out = np.zeros(4, dtype=np.float64)
+        check(load().B200GBM_BoosterGetRefitTiming(self.handle, _ptr(out)))
+        return dict(stage_ms=float(out[0]), tree_ms=float(out[1]), batches=int(out[2]), blocks=int(out[3]))
+
     def reset_parameter(self, params):
         check(load().LGBM_BoosterResetParameter(self.handle, params.encode()))
 
@@ -552,6 +567,30 @@ class Booster:
         if self.handle:
             check(load().LGBM_BoosterFree(self.handle))
             self.handle = None
+
+
+def refit(model_str, X, label, params="", decay_rate=0.9, weight=None, group=None, init_score=None):
+    """LightGBM's Booster.refit flow: the leaf indices of X's rows under the model, a booster on a dataset of X (with the label and the
+    optional weight, group and init_score) and `params` plus refit_decay_rate=decay_rate, the model merged into it (its scores stay at
+    the init score, as a merge does not replay them), then LGBM_BoosterRefit.  Returns that booster, which holds the refit model."""
+    old = Booster(model_str=model_str)
+    try:
+        leaf = old.predict_device(X, PREDICT_LEAF_INDEX).astype(np.int32)
+        ds = Dataset.from_mat(X, params)
+        ds.set_field("label", label)
+        for name, v in (("weight", weight), ("group", group), ("init_score", init_score)):
+            if v is not None:
+                ds.set_field(name, v)
+        b = Booster(ds, "%s refit_decay_rate=%r" % (params, float(decay_rate)))
+        try:
+            b.merge(old)
+            b.refit(leaf)
+        except Exception:
+            b.free(); ds.free()
+            raise
+        return b
+    finally:
+        old.free()
 
 
 class ChunkedArray:

@@ -149,6 +149,11 @@ int LGBM_BoosterFree(BoosterHandle handle) {
   delete static_cast<Booster*>(handle);
   API_END();
 }
+int LGBM_BoosterRefit(BoosterHandle handle, const int32_t* leaf_preds, int32_t nrow, int32_t ncol) {
+  API_BEGIN();
+  BS(handle)->Refit(leaf_preds, nrow, ncol);
+  API_END();
+}
 int LGBM_BoosterUpdateOneIter(BoosterHandle handle, int* is_finished) {
   API_BEGIN();
   *is_finished = BS(handle)->UpdateOneIter() ? 1 : 0;
@@ -594,6 +599,12 @@ int B200GBM_DatasetQuantizedHistogram(DatasetHandle handle, const float* grad, c
 int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess) {
   API_BEGIN();
   BS(handle)->GetGradients(grad, hess);
+  API_END();
+}
+int B200GBM_BoosterGetRefitTiming(BoosterHandle handle, double* out4) {
+  API_BEGIN();
+  const Booster::RefitTiming& t = BS(handle)->refit_timing;
+  out4[0] = t.stage_ms; out4[1] = t.tree_ms; out4[2] = t.batches; out4[3] = t.blocks;
   API_END();
 }
 int B200GBM_BoosterSetProfile(BoosterHandle handle, int profile_hist) {

@@ -55,6 +55,8 @@ struct Config {
   int num_grad_quant_bins = 4;              // B: q_g in [-floor(B/2), floor(B/2)], q_h in [-B, B]; 2..63 (Booster checks)
   bool quant_train_renew_leaf = false;      // leaf values from the true in-bag sums of g and h after growth
   bool stochastic_rounding = true;
+  // LGBM_BoosterRefit: leaf = decay * leaf + (1 - decay) * refit output (refit.cu); [0, 1] is checked by the refit, not here
+  double refit_decay_rate = 0.9;
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -231,6 +233,7 @@ struct Config {
     D("path_smooth", &path_smooth);
     B("use_quantized_grad", &use_quantized_grad); I("num_grad_quant_bins", &num_grad_quant_bins);
     B("quant_train_renew_leaf", &quant_train_renew_leaf); B("stochastic_rounding", &stochastic_rounding);
+    D("refit_decay_rate", &refit_decay_rate);
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -315,7 +318,7 @@ struct Config {
     s << "[cat_smooth: " << Num(cat_smooth) << "]\n[max_cat_to_onehot: " << max_cat_to_onehot << "]\n";
     s << "[top_k: " << top_k << "]\n[monotone_constraints: " << join_i(monotone_constraints) << "]\n";
     s << "[monotone_constraints_method: " << monotone_constraints_method << "]\n[monotone_penalty: " << Num(monotone_penalty) << "]\n";
-    s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: 0.9]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
+    s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: " << Num(refit_decay_rate) << "]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
     s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: " << Num(path_smooth) << "]\n";
     s << "[interaction_constraints: " << join_sets(interaction_constraints) << "]\n";
     if (use_quantized_grad)      // only when on, so every other model text stays as it was

@@ -1767,6 +1767,7 @@ bool Booster::TrainTrees(const float* custom_g, const float* custom_h) {
     grad_.Upload(custom_g, static_cast<size_t>(K) * n, s);
     hess_.Upload(custom_h, static_cast<size_t>(K) * n, s);
     const_hessian_ = false;
+    custom_grad_ = true;
   }
   Bagging(iter);
   bool should_continue = is_rf_;        // a random forest never stops early
@@ -1983,3 +1984,4 @@ void Booster::GetGradients(float* grad, float* hess) {
 }  // namespace b200gbm
 #include "metrics.cu"      // the booster's metrics, in this translation unit
 #include "predictor.cu"    // the booster's batched predictor, in this translation unit
+#include "refit.cu"       // the booster's refit, in this translation unit

@@ -220,6 +220,11 @@ class Booster {
   // the objective's gradients at the current training scores, class-major [K][n], computed into scratch buffers: the training state
   // (grad_ / hess_, which rf keeps from construction and GOSS rescales in place) is not touched
   void GetGradients(float* grad, float* hess);
+  // LGBM_BoosterRefit (refit.cu): leaf_preds [nrow][ncol] row-major host memory, the leaf of training row i in model j.  Every check
+  // (and with data-parallel ranks every rank's outcome) comes before anything changes, so a failed refit leaves the model as it was.
+  void Refit(const int32_t* leaf_preds, int nrow, int ncol);
+  struct RefitTiming { double stage_ms = 0, tree_ms = 0; int batches = 0, blocks = 0; };
+  RefitTiming refit_timing;      // of the last refit: host time of the staging and of the per-tree work, batches of models, row blocks
   void GetInfo(int* out4) const { out4[0] = parallel_ ? Net().world : 1; out4[1] = parallel_ ? Net().rank : 0; out4[2] = same_device_ ? 3 : 0; out4[3] = const_hessian_ ? 1 : 0; }
   std::string SaveModelToString(int start_iteration, int num_iteration, int importance_type) const;
   std::string DumpModelJson(int start_iteration, int num_iteration) const;
@@ -256,6 +261,7 @@ class Booster {
   bool same_device_ = false;            // parallel_ over the same-device communicator: all ranks are threads of this process on this device
   bool const_hessian_ = false;
   bool has_init_score_ = false;
+  bool custom_grad_ = false;            // trained on custom gradients at least once: refit has no objective to take gradients from
   double shrinkage_ = 0.1;
   // row subsampling: bagging / GOSS / random forest (SURVEY §8f-3)
   bool is_rf_ = false, is_goss_ = false, bagging_ = false, balanced_bagging_ = false, use_bag_ = false, need_re_bagging_ = false;

@@ -729,6 +729,8 @@ __global__ void k_grad_xentlambda(const double* __restrict__ score, const float*
 }
 
 // ---------------------------------------------------------------- quantisation + root sums (K3)
+// one value's word on K3's fixed-point grid: q = rint(x * 2^e), e from k_set_scale (the quantisation, the renewed and the refit leaf sums)
+__device__ __forceinline__ long long d_fixed(float x, int e) { return __double2ll_rn(ldexp(static_cast<double>(x), e)); }
 __global__ void k_absmax(const float* __restrict__ g, const float* __restrict__ h, int n, TreeCtrl* ctrl) {
   float mg = 0.f, mh = 0.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -772,12 +774,12 @@ k_quantize(const float* __restrict__ g, const float* __restrict__ h, int n, int4
   const int eg = ctrl->exp_g, eh = ctrl->exp_h;
   long long sg = 0, sh = 0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    long long qg = __double2ll_rn(ldexp(static_cast<double>(g[i]), eg));
+    long long qg = d_fixed(g[i], eg);
     int4 q;
     q.x = static_cast<int>(qg >> kLoBits); q.y = static_cast<int>(qg & ((1LL << kLoBits) - 1));
     long long qh;
     if (const_hessian) { qh = 1; q.z = 1; q.w = 0; }
-    else { qh = __double2ll_rn(ldexp(static_cast<double>(h[i]), eh)); q.z = static_cast<int>(qh >> kLoBits); q.w = static_cast<int>(qh & ((1LL << kLoBits) - 1)); }
+    else { qh = d_fixed(h[i], eh); q.z = static_cast<int>(qh >> kLoBits); q.w = static_cast<int>(qh & ((1LL << kLoBits) - 1)); }
     qgh[i] = q;
     if (!in_bag || in_bag[i]) { sg += qg; sh += qh; }       // root sums run over the in-bag rows only
   }
@@ -856,8 +858,8 @@ k_quant_leaf_sums(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict
   long long sg = 0, sh = 0;
   for (int i = part * blockDim.x + threadIdx.x; i < L.count; i += blocks_per_leaf * blockDim.x) {
     const int r = L.identity ? (L.begin + i) : src[L.begin + i];
-    sg += __double2ll_rn(ldexp(static_cast<double>(g[r]), eg));
-    sh += const_hessian ? 1 : __double2ll_rn(ldexp(static_cast<double>(h[r]), eh));
+    sg += d_fixed(g[r], eg);
+    sh += const_hessian ? 1 : d_fixed(h[r], eh);
   }
   for (int o = 16; o; o >>= 1) { sg += __shfl_xor_sync(0xffffffffu, sg, o); sh += __shfl_xor_sync(0xffffffffu, sh, o); }
   if ((threadIdx.x & 31) == 0 && (sg | sh)) {
