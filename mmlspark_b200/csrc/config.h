@@ -57,6 +57,9 @@ struct Config {
   bool stochastic_rounding = true;
   // LGBM_BoosterRefit: leaf = decay * leaf + (1 - decay) * refit output (refit.cu); [0, 1] is checked by the refit, not here
   double refit_decay_rate = 0.9;
+  // forced splits: a JSON file of splits every tree starts with (forced_splits.h); empty for none.  Booster reads it at create and when a
+  // ResetParameter gives the key
+  std::string forcedsplits_filename;
   int early_stopping_round = 0;
   double max_delta_step = 0.0, lambda_l1 = 0.0, lambda_l2 = 0.0, min_gain_to_split = 0.0;
   double cat_l2 = 10.0, cat_smooth = 10.0;
@@ -126,6 +129,8 @@ struct Config {
         {"num_classes", "num_class"}, {"unbalance", "is_unbalance"}, {"unbalanced_sets", "is_unbalance"},
         {"max_position", "lambdarank_truncation_level"}, {"metrics", "metric"}, {"metric_types", "metric"},
         {"ndcg_eval_at", "eval_at"}, {"ndcg_at", "eval_at"}, {"map_eval_at", "eval_at"}, {"map_at", "eval_at"},
+        {"fs", "forcedsplits_filename"}, {"forced_splits_filename", "forcedsplits_filename"},
+        {"forced_splits_file", "forcedsplits_filename"}, {"forced_splits", "forcedsplits_filename"},
         {"num_machine", "num_machines"}, {"local_port", "local_listen_port"}, {"port", "local_listen_port"}};
     return a;
   }
@@ -234,6 +239,10 @@ struct Config {
     B("use_quantized_grad", &use_quantized_grad); I("num_grad_quant_bins", &num_grad_quant_bins);
     B("quant_train_renew_leaf", &quant_train_renew_leaf); B("stochastic_rounding", &stochastic_rounding);
     D("refit_decay_rate", &refit_decay_rate);
+    {   // an empty value clears it
+      auto it = raw.find("forcedsplits_filename");
+      forcedsplits_filename = it != raw.end() ? it->second : "";
+    }
     D("max_delta_step", &max_delta_step); D("lambda_l1", &lambda_l1); D("lambda_l2", &lambda_l2);
     D("min_gain_to_split", &min_gain_to_split); D("cat_l2", &cat_l2); D("cat_smooth", &cat_smooth);
     I("max_cat_threshold", &max_cat_threshold); I("max_cat_to_onehot", &max_cat_to_onehot); I("min_data_per_group", &min_data_per_group);
@@ -318,7 +327,7 @@ struct Config {
     s << "[cat_smooth: " << Num(cat_smooth) << "]\n[max_cat_to_onehot: " << max_cat_to_onehot << "]\n";
     s << "[top_k: " << top_k << "]\n[monotone_constraints: " << join_i(monotone_constraints) << "]\n";
     s << "[monotone_constraints_method: " << monotone_constraints_method << "]\n[monotone_penalty: " << Num(monotone_penalty) << "]\n";
-    s << "[feature_contri: ]\n[forcedsplits_filename: ]\n[refit_decay_rate: " << Num(refit_decay_rate) << "]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
+    s << "[feature_contri: ]\n[forcedsplits_filename: " << forcedsplits_filename << "]\n[refit_decay_rate: " << Num(refit_decay_rate) << "]\n[cegb_tradeoff: 1]\n[cegb_penalty_split: 0]\n";
     s << "[cegb_penalty_feature_lazy: ]\n[cegb_penalty_feature_coupled: ]\n[path_smooth: " << Num(path_smooth) << "]\n";
     s << "[interaction_constraints: " << join_sets(interaction_constraints) << "]\n";
     if (use_quantized_grad)      // only when on, so every other model text stays as it was

@@ -1352,6 +1352,7 @@ void Dataset::SetFeatureNames(const char** names, int n) {
 // =============================================================================== booster
 }  // namespace b200gbm
 #include "tree_learner.cu"      // the booster's tree learner, in this translation unit
+#include "forced_splits.h"
 namespace b200gbm {
 
 // the voting learner's local and global scans would each need their own draw order of the extra_trees streams; not restated
@@ -1436,6 +1437,39 @@ static void CheckQuantized(const Config& cfg) {
     Fatal("quant_train_renew_leaf does not support path_smooth > 0; use quant_train_renew_leaf=false or path_smooth=0");
 }
 
+// the voting learner's local scans and vote would need every rank to evaluate the plan on the global histograms; not restated
+static const char* const kVotingForced = "tree_learner=voting does not support forcedsplits_filename with more than one machine; "
+                                         "use tree_learner=data_parallel or no forcedsplits_filename";
+// upstream tightens the children's bounds after a forced split with the same update as after any split; not restated and tested here
+static const char* const kForcedMonotone = "forcedsplits_filename does not support monotone_constraints; "
+                                           "use no monotone_constraints or no forcedsplits_filename";
+
+// forced splits: the same checks at LGBM_BoosterCreate and ResetParameter.  Reads and flattens the plan (forced_splits.h).  With several
+// ranks every rank then takes part in one all-reduce of (failed, digest, -digest), whatever happened before it, so that all of them fail
+// together when any rank could not load its plan or the plans differ, and none is left waiting in a collective.
+static std::vector<ForcedNode> CheckForcedSplits(const Config& cfg, const Dataset& train, bool voting_parallel, bool parallel) {
+  std::vector<ForcedNode> plan;
+  std::string err;
+  try {
+    plan = LoadForcedPlan(cfg.forcedsplits_filename, train);
+  } catch (const std::exception& e) {
+    err = "forcedsplits_filename=" + cfg.forcedsplits_filename + ": " + e.what();
+  }
+  if (err.empty() && !plan.empty() && voting_parallel) err = kVotingForced;
+  if (err.empty() && !plan.empty() && !cfg.monotone_constraints.empty()) err = kForcedMonotone;
+  if (parallel) {
+    const double d = ForcedPlanDigest(plan);
+    double v[3] = {err.empty() ? 0.0 : 1.0, d, -d};
+    cudaStream_t ts = AcquireStream();
+    try { AllReduceHost(v, 3, ncclMax, ts); } catch (...) { ReleaseStream(ts); throw; }
+    ReleaseStream(ts);
+    if (err.empty() && v[0] > 0.0) err = "forcedsplits_filename: another rank could not load its forced split plan";
+    if (err.empty() && v[1] != -v[2]) err = "forcedsplits_filename: the ranks were given different forced split plans";
+  }
+  if (!err.empty()) Fatal(err);
+  return plan;
+}
+
 Booster::Booster(const std::string& model_text) : predictor(new Predictor(model, stream_)) {
   std::unique_ptr<HostModel> m = HostModel::FromString(model_text);
   model = std::move(*m);
@@ -1487,6 +1521,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr), predictor(n
   CheckByNode(cfg, voting_);
   CheckPathSmooth(cfg, voting_);
   CheckQuantized(cfg);
+  const std::vector<ForcedNode> forced_plan = CheckForcedSplits(cfg, *train, voting_, parallel_);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
     if (parallel_) {
@@ -1506,6 +1541,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr), predictor(n
   for (int f = 0; f < train->num_total_features; ++f) model.feature_infos.push_back(train->mappers[f].InfoString());
   model.monotone_constraints = cfg.monotone_constraints;
   InitTraining();
+  learner_->SetForcedPlan(forced_plan);
   model.objective_str = obj_->ToString();
 }
 
@@ -1827,6 +1863,8 @@ void Booster::ResetParameter(const char* params) {
   int keep_machines = cfg.num_machines;
   cfg.Refresh();
   cfg.num_machines = keep_machines;
+  std::vector<ForcedNode> forced_plan;
+  bool reload_plan = false;
   if (train) {      // metrics named by the reset meet the checks of LGBM_BoosterCreate / AddValidData; a rejected reset changes nothing
     try {
       // the voting checks follow the learner built at create: a reset's tree_learner does not change it
@@ -1836,6 +1874,9 @@ void Booster::ResetParameter(const char* params) {
       CheckByNode(cfg, voting_);
       CheckPathSmooth(cfg, voting_);
       CheckQuantized(cfg);
+      // a reset that gives the key (set, changed or cleared) reloads the plan on every rank
+      if (nc.raw.count("forcedsplits_filename")) { forced_plan = CheckForcedSplits(cfg, *train, voting_, parallel_); reload_plan = true; }
+      else if (learner_ && learner_->HasForcedPlan() && !cfg.monotone_constraints.empty()) Fatal(kForcedMonotone);
       metrics_->Reset(cfg, valids_);      // last: it takes the new metrics only when they pass every check
     } catch (...) {
       cfg = before;
@@ -1846,6 +1887,7 @@ void Booster::ResetParameter(const char* params) {
   if (is_dart_) { drop_rand_ = LcgRandom(cfg.drop_seed); sum_weight_ = 0.0; }      // [LightGBM dart.hpp DART::ResetConfig]
   if (train) model.monotone_constraints = cfg.monotone_constraints;
   if (learner_) learner_->ResetConfig(cfg);
+  if (learner_ && reload_plan) learner_->SetForcedPlan(forced_plan);
 }
 
 void Booster::AddValidData(const Dataset* valid) {

@@ -145,6 +145,14 @@ struct ConstraintArgs { const signed char* type; double penalty; const unsigned 
 // without per-node sampling (nothing is read then).  k = GetCnt(|tree sample|, feature_fraction_bynode); order: the used features in
 // real-index order (Dataset::sample_order); tree_used: the tree's feature_fraction sample; work: [2][4][nf_pad] ints of scratch.
 struct NodeSampleArgs { uint8_t* mask; int* work; const int* order; const uint8_t* tree_used; int k; };
+// Forced splits ([UPSTREAM] SerialTreeLearner::ForceSplits; forced_splits.h builds the plan): the plan's nodes in breadth-first order.
+// Node j is the j-th split of the tree while the forced phase lasts, so it splits leaf `leaf` (the root's is 0, a left child keeps its
+// parent's leaf, a right child of node j gets leaf j + 1).  bin: the threshold's bin (numerical) or the category's bin (categorical, 0
+// when the category has no bin of its own); left / right: the child plan nodes, -1 for none.  A node is evaluated by the scan block of
+// (its leaf, its feature) in the round that scans its leaf (d_forced_eval) into evals[node]; the evals are zeroed before each tree, so
+// a gain that is not > 0 is a node that was never evaluated or is invalid.  nodes null: no plan, and nothing else is read.
+struct ForcedNode { int feature, bin, is_cat, leaf, left, right; };
+struct ForcedArgs { const ForcedNode* nodes; SplitCand* evals; int n; };
 
 struct TreeCtrl {
   int num_leaves, left_leaf, right_leaf, smaller, larger, go, finished, split_leaf;
@@ -168,6 +176,9 @@ struct TreeCtrl {
   // per-node feature sampling: the ColSampler stream's state.  k_tree_init takes it from the host after the tree's feature_fraction
   // draw, the pick step advances it to col_next (written by d_bynode_sample) each round, and ReadTree hands it back to the host.
   unsigned col_state, col_next;
+  // forced splits: the plan node the next forced split applies, -1 once the forced phase is over (k_tree_init starts it at 0; read only
+  // with a plan)
+  int forced_next;
 };
 
 struct TreeDev {               // SoA tree under construction (sizes: num_leaves / num_leaves-1)
@@ -901,7 +912,7 @@ k_tree_init(TreeCtrl* ctrl, LeafState* leaves, TreeDev tree, uint8_t* flags, Spl
     r.output = d_calc_output(r.sum_g, r.sum_h, p);
     ctrl->num_leaves = 1; ctrl->left_leaf = 0; ctrl->right_leaf = -1; ctrl->smaller = 0; ctrl->larger = -1;
     ctrl->go = 0; ctrl->finished = 0; ctrl->split_leaf = -1; ctrl->pending = 0; ctrl->round = 0; ctrl->trace_rows = 0;
-    ctrl->col_state = col_state;
+    ctrl->col_state = col_state; ctrl->forced_next = 0;
     *tree.num_leaves = 1;
   }
 }
@@ -1219,7 +1230,9 @@ __device__ __noinline__ int d_scan_feature_cat(const long long (&qg)[8], const l
   return drew;
 }
 
-__device__ __forceinline__ void d_choose_leaf(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitParams& p, int lane) {
+// forced_leaf >= 0: the forced phase splits that leaf (its best is the plan node's split) instead of the arg-max
+__device__ __forceinline__ void d_choose_leaf(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitParams& p, int lane,
+                                              int forced_leaf) {
   double bg = kNegInf; int bf = 0x7fffffff, bl = 0x7fffffff;
   const int nl = ctrl->num_leaves;
   for (int l = lane; l < nl; l += 32) {
@@ -1234,7 +1247,7 @@ __device__ __forceinline__ void d_choose_leaf(TreeCtrl* ctrl, LeafState* leaves,
     if (og > bg || (og == bg && (of < bf || (of == bf && ol < bl)))) { bg = og; bf = of; bl = ol; }
   }
   if (lane != 0) return;
-  const int best_leaf = bl == 0x7fffffff ? 0 : bl;
+  const int best_leaf = forced_leaf >= 0 ? forced_leaf : (bl == 0x7fffffff ? 0 : bl);
   const LeafBest& b = leaves[best_leaf].best;
   if (!(b.gain > 0.0) || ctrl->num_leaves >= p.num_leaves) {
     ctrl->finished = 1; ctrl->split_leaf = -1; ctrl->part_count = 0;
@@ -1264,6 +1277,59 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
   for (int i = 0; i < static_cast<int>(sizeof(SplitCand) / 8); ++i) dst[i] = __ldcg(src + i);
   return out;
 }
+// a leaf's best split from its candidate c ([UPSTREAM] SplitInfo as FindBestThreshold leaves it): sums without the scans' epsilon, the
+// children's outputs (kMono: smoothed toward the leaf's output and clamped to its bounds) and what the round controller's constraint
+// update needs
+template <bool kMono>
+__device__ __forceinline__ void d_leaf_best(const SplitCand& c, const LeafState& L, const SplitParams& p, const signed char* __restrict__ mono_type,
+                                            const unsigned long long* __restrict__ sets_of, LeafBest* out) {
+  LeafBest& b = *out;
+  b.monotone_type = 0; b.inter_sets = 0ull;
+  b.cat_list_len = c.cat_list_len;
+  for (int k = 0; k < c.cat_list_len && k < kCatListMax; ++k) b.cat_list[k] = c.cat_list[k];
+  const double sum_h = L.sum_h + 2 * kEpsD;
+  b.gain = c.gain; b.feature = c.feature; b.threshold = c.threshold; b.default_left = c.default_left;
+  b.left_count = c.left_count; b.right_count = L.global_count - c.left_count;
+  b.left_g = c.left_g; b.left_h = c.left_h - kEpsD;
+  b.right_g = L.sum_g - c.left_g; b.right_h = sum_h - c.left_h - kEpsD;
+  SplitParams pc = p;
+  pc.l2 += c.l2_extra;
+  if constexpr (kMono) {
+    b.left_out = d_mono_output(c.left_g, c.left_h, b.left_count, L.output, pc, L.mono_min, L.mono_max);
+    b.right_out = d_mono_output(L.sum_g - c.left_g, sum_h - c.left_h, b.right_count, L.output, pc, L.mono_min, L.mono_max);
+    b.monotone_type = mono_type[c.feature];
+  } else {
+    b.left_out = d_calc_output(c.left_g, c.left_h, pc);
+    b.right_out = d_calc_output(L.sum_g - c.left_g, sum_h - c.left_h, pc);
+  }
+  if (p.interaction) b.inter_sets = sets_of[c.feature];
+  b.is_cat = c.is_cat;
+  for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = c.cat_bits[wd];
+}
+
+// Forced splits, the pick step's thread 0 once every leaf's best is in place ([UPSTREAM] the queue loop of SerialTreeLearner::ForceSplits):
+// while the phase lasts, plan node j = forced_next splits its leaf when its stored evaluation is valid; that leaf's best becomes the
+// node's split and the leaf is returned.  Otherwise (the node is invalid or was never evaluated, the plan has run out, or the tree is
+// full) the phase ends and this round picks as it would without a plan (-1).  The leaf being split loses its own best split, which
+// the round controller resets anyway.
+template <bool kMono>
+__device__ __noinline__ int d_forced_pick(TreeCtrl* ctrl, LeafState* leaves, const ForcedArgs& forced, const SplitParams& p,
+                                          const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of) {
+  const int j = ctrl->forced_next;
+  if (j < 0 || ctrl->finished) return -1;
+  if (j < forced.n && ctrl->num_leaves < p.num_leaves) {
+    const SplitCand c = d_load_cand(&forced.evals[j]);
+    if (c.gain > 0.0) {
+      const int leaf = forced.nodes[j].leaf;
+      d_leaf_best<kMono>(c, leaves[leaf], p, mono_type, sets_of, &leaves[leaf].best);
+      ctrl->forced_next = j + 1;
+      return leaf;
+    }
+  }
+  ctrl->forced_next = -1;
+  return -1;
+}
+
 // best candidate per leaf (argmax over features, ties -> smaller real feature index), then the leaf to split; one 256-thread block.
 // The two leaves of the round are handled side by side (threads 0..127: smaller, 128..255: larger) with warp-shuffle argmaxes — the
 // first version looped over the two leaves with an 8-step shared-memory tree each (18 block barriers) and ncu showed this serial tail
@@ -1277,10 +1343,13 @@ __device__ __forceinline__ SplitCand d_load_cand(const SplitCand* c) {
 // feature's sets_of word is kept for the round controller's mask update.
 // node_mask non-null (per-node feature sampling): likewise a feature the leaf did not sample (written by d_bynode_sample in this kernel)
 // is passed over, and the ColSampler stream moves past the round's draws.
+// forced.nodes non-null (forced splits): while the forced phase lasts, the next plan node's stored evaluation replaces the arg-max when it
+// is valid (d_forced_pick).
 template <bool kMono>
 __device__ __noinline__ void
 d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta, const SplitCand* cands, const SplitParams& p,
-             const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of, const uint8_t* node_mask) {
+             const signed char* __restrict__ mono_type, const unsigned long long* __restrict__ sets_of, const uint8_t* node_mask,
+             const ForcedArgs& forced) {
   __shared__ double s_gain[8];
   __shared__ int s_feat[8], s_idx[8];
   const int which = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -1312,34 +1381,19 @@ d_pick_block(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ met
     b.left_g = b.left_h = b.right_g = b.right_h = b.left_out = b.right_out = 0; b.is_cat = 0; b.cat_list_len = 0; b.monotone_type = 0;
     b.inter_sets = 0ull;
     for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = 0u;
-    if (bi >= 0 && bg > kNegInf) {
-      const SplitCand c = d_load_cand(&cands[which * p.nf_pad + bi]);
-      b.cat_list_len = c.cat_list_len;
-      for (int k = 0; k < c.cat_list_len && k < kCatListMax; ++k) b.cat_list[k] = c.cat_list[k];
-      const double sum_h = L.sum_h + 2 * kEpsD;
-      b.gain = c.gain; b.feature = c.feature; b.threshold = c.threshold; b.default_left = c.default_left;
-      b.left_count = c.left_count; b.right_count = L.global_count - c.left_count;
-      b.left_g = c.left_g; b.left_h = c.left_h - kEpsD;
-      b.right_g = L.sum_g - c.left_g; b.right_h = sum_h - c.left_h - kEpsD;
-      SplitParams pc = p;
-      pc.l2 += c.l2_extra;
-      if constexpr (kMono) {
-        b.left_out = d_mono_output(c.left_g, c.left_h, b.left_count, L.output, pc, L.mono_min, L.mono_max);
-        b.right_out = d_mono_output(L.sum_g - c.left_g, sum_h - c.left_h, b.right_count, L.output, pc, L.mono_min, L.mono_max);
-        b.monotone_type = mono_type[c.feature];
-      } else {
-        b.left_out = d_calc_output(c.left_g, c.left_h, pc);
-        b.right_out = d_calc_output(L.sum_g - c.left_g, sum_h - c.left_h, pc);
-      }
-      if (p.interaction) b.inter_sets = sets_of[c.feature];
-      b.is_cat = c.is_cat;
-      for (int wd = 0; wd < 8; ++wd) b.cat_bits[wd] = c.cat_bits[wd];
-    }
+    if (bi >= 0 && bg > kNegInf) d_leaf_best<kMono>(d_load_cand(&cands[which * p.nf_pad + bi]), L, p, mono_type, sets_of, &b);
     L.best = b;
   }
   if (node_mask && threadIdx.x == 0 && ctrl->go) ctrl->col_state = __ldcg(&ctrl->col_next);
   __syncthreads();
-  if (threadIdx.x < 32 && !ctrl->finished) d_choose_leaf(ctrl, leaves, meta, p, threadIdx.x);
+  int forced_leaf = -1;
+  if (forced.nodes) {      // the same in every thread: a kernel argument
+    __shared__ int s_forced_leaf;
+    if (threadIdx.x == 0) s_forced_leaf = d_forced_pick<kMono>(ctrl, leaves, forced, p, mono_type, sets_of);
+    __syncthreads();
+    forced_leaf = s_forced_leaf;
+  }
+  if (threadIdx.x < 32 && !ctrl->finished) d_choose_leaf(ctrl, leaves, meta, p, threadIdx.x, forced_leaf);
 }
 
 // ---------------------------------------------------------------- same-device all-reduce (rank-threads of one process on one device)
@@ -1964,6 +2018,86 @@ __device__ __forceinline__ SplitCand d_empty_cand(int u) {
   for (int wd = 0; wd < 8; ++wd) out.cat_bits[wd] = 0u;
   return out;
 }
+// ---- forced splits ([UPSTREAM] FeatureHistogram::GatherInfoForThreshold{Numerical,Categorical}): plan node nd on the leaf's reduced
+// histogram column `hist` of its feature m, by every thread of the scan block of (leaf, feature); thread 0 stores the result in *outp.
+// - numerical: the right side sums the bins above nd.bin, the NaN bin left out; the left side is the leaf total minus it, so NaN goes
+//   left (default_left = 1).  Counts are rounded per bin from the hessians, as in the scans.
+// - categorical: the left side is the single bin nd.bin, which must be one of the feature's category bins (not 0).
+// The gain and min_gain_shift are the scans' (kMono: smoothed toward the leaf's output); the node is valid only when the gain exceeds
+// min_gain_shift, and min_data_in_leaf and min_sum_hessian_in_leaf do not apply.  An invalid node stores gain -inf.  Out of line, with
+// barriers before and after: the scan of the same block may overwrite `hist` when it is the block's scratch (a bundle member).
+template <bool kMono>
+__device__ __noinline__ void d_forced_eval(const long long* __restrict__ hist, const FeatMeta m, const ForcedNode nd, int u, int wide,
+                                           const LeafState& L, double inv_g, double inv_h, const SplitParams& p, SplitCand* outp) {
+  __shared__ long long s_fr[3][8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
+  const int num_data = L.global_count;
+  const double cnt_factor = num_data / sum_h;
+  long long r[3] = {0, 0, 0};
+  if (!nd.is_cat) {
+    const int hi = m.num_bin - 1 - (m.missing_type == 2 ? 1 : 0);
+    for (int b = nd.bin + 1 + static_cast<int>(threadIdx.x); b <= hi; b += blockDim.x) {
+      const long long qh = hist[b * 2 + 1];
+      r[0] += hist[b * 2]; r[1] += qh; r[2] += static_cast<int>(static_cast<double>(qh) * inv_h * cnt_factor + 0.5);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    for (int o = 16; o; o >>= 1) r[i] += __shfl_xor_sync(0xffffffffu, r[i], o);
+  __syncthreads();
+  if (lane == 0) for (int i = 0; i < 3; ++i) s_fr[i][warp] = r[i];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 3; ++i) { r[i] = 0; for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) r[i] += s_fr[i][w]; }
+    bool ok = true;
+    double lg, lh, rg, rh;
+    int lc, rc;
+    if (!nd.is_cat) {
+      rg = static_cast<double>(r[0]) * inv_g; rh = kEpsD + static_cast<double>(r[1]) * inv_h; rc = static_cast<int>(r[2]);
+      lc = num_data - rc; lg = sum_g - rg; lh = sum_h - rh;
+    } else {
+      ok = nd.bin > 0 && nd.bin < m.num_bin;
+      const double g = ok ? static_cast<double>(hist[nd.bin * 2]) * inv_g : 0.0, h = ok ? static_cast<double>(hist[nd.bin * 2 + 1]) * inv_h : 0.0;
+      lc = static_cast<int>(h * cnt_factor + 0.5); rc = num_data - lc;
+      lg = g; lh = h + kEpsD; rg = sum_g - g; rh = sum_h - lh;
+    }
+    const double min_gain_shift = (kMono ? d_smooth_leaf_gain(sum_g, sum_h, num_data, L.output, p) : d_leaf_gain(sum_g, sum_h, p)) + p.min_gain_to_split;
+    const double gain = kMono ? d_mono_split_gain(lg, lh, rg, rh, lc, rc, L.output, p, L.mono_min, L.mono_max, 0)
+                              : d_leaf_gain(lg, lh, p) + d_leaf_gain(rg, rh, p);
+    SplitCand out = d_empty_cand(u);
+    if (ok && gain > min_gain_shift) {
+      out.gain = gain - min_gain_shift; out.left_g = lg; out.left_h = lh; out.left_count = lc;
+      out.threshold = nd.is_cat ? 0 : nd.bin; out.default_left = nd.is_cat ? 0 : 1; out.is_cat = nd.is_cat;
+      if (nd.is_cat && wide) { out.cat_list_len = 1; out.cat_list[0] = static_cast<unsigned short>(nd.bin); }
+      else if (nd.is_cat) out.cat_bits[nd.bin >> 5] = 1u << (nd.bin & 31);
+    }
+    *outp = out;
+    __threadfence();      // before the block takes the kernel's scan ticket: the pick step reads it
+  }
+  __syncthreads();
+}
+// the plan node the scan block of `leaf` evaluates in this round, or -1: while the phase lasts, the round after node j - 1 was applied
+// scans that node's two new leaves, and each of its child nodes is evaluated on its own leaf (the root's node 0 on leaf 0 in round 0)
+__device__ __forceinline__ int d_forced_node(const TreeCtrl* ctrl, const ForcedArgs& f, int leaf) {
+  const int j = ctrl->forced_next;
+  if (j < 0) return -1;
+  if (j == 0) return leaf == 0 ? 0 : -1;
+  const ForcedNode& par = f.nodes[j - 1];
+  if (par.left >= 0 && f.nodes[par.left].leaf == leaf) return par.left;
+  if (par.right >= 0 && f.nodes[par.right].leaf == leaf) return par.right;
+  return -1;
+}
+// the forced-split step of a scan block of (leaf, feature u) whose column `hist` holds the leaf's histogram: evaluates the plan node of
+// this leaf and round if it splits on u.  Called by every thread; the condition is the same in all of them.
+template <bool kMono>
+__device__ __forceinline__ void d_forced_step(const TreeCtrl* ctrl, const ForcedArgs& f, int leaf, int u, const long long* hist, const FeatMeta& m,
+                                              const LeafState& L, const SplitParams& p) {
+  const int k = d_forced_node(ctrl, f, leaf);
+  if (k >= 0 && f.nodes[k].feature == u)
+    d_forced_eval<kMono>(hist, m, f.nodes[k], u, u >= p.nfn, L, ctrl->inv_g, ctrl->inv_h, p, &f.evals[k]);
+}
+
 // one thread: the candidate of (leaf `which`, feature u) and, for extra_trees, the scan's number of draws (see d_lcg_next), then a fence
 // that makes both visible to the block that runs the pick step
 template <bool kExtra>
@@ -2035,7 +2169,7 @@ template <bool kExtra, bool kMono>
 __global__ void __launch_bounds__(256)
 k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ leaves, const FeatMeta* __restrict__ meta, const long long* __restrict__ H,
             long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags, SplitCand* __restrict__ cands, SplitParams p,
-            unsigned* __restrict__ xrand, ConstraintArgs cons) {
+            unsigned* __restrict__ xrand, ConstraintArgs cons, ForcedArgs forced) {
   extern __shared__ __align__(16) unsigned char sw_smem[];
   double* s_key = reinterpret_cast<double*>(sw_smem);                          // [num_bin] ctr keys of the used bins, +inf otherwise
   __shared__ int s_used;
@@ -2044,15 +2178,22 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   if (!ctrl->go || leaf < 0) return;
   SplitCand out = d_empty_cand(u);
   uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
+  const FeatMeta m = meta[u];
+  const LeafState& L = leaves[leaf];
+  long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(m.hist_off) * 2;
+  const long long* src = H + static_cast<size_t>(m.hist_off) * 2;
+  // forced splits: while the phase lasts every column of the scanned leaves is reduced, flagged or not, so that a plan node can be
+  // evaluated on any used feature (its leaf's ancestors were all scanned in the phase)
+  const bool forcing = forced.nodes && ctrl->forced_next >= 0;
   if (!*flag) {
+    if (forcing) {
+      d_reduce_column(src, dst, m.num_bin, which);
+      d_forced_step<kMono>(ctrl, forced, leaf, u, dst, m, L, p);
+    }
     if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, 0);
     return;
   }
-  const FeatMeta m = meta[u];
-  const LeafState& L = leaves[leaf];
   const double inv_g = ctrl->inv_g, inv_h = ctrl->inv_h;
-  long long* dst = pool + static_cast<size_t>(L.hist_slot) * slot_elems + static_cast<size_t>(m.hist_off) * 2;
-  const long long* src = H + static_cast<size_t>(m.hist_off) * 2;
   const double sum_g = L.sum_g, sum_h = L.sum_h + 2 * kEpsD;
   const int num_data = L.global_count;
   const double cnt_factor = num_data / sum_h;
@@ -2061,6 +2202,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   if (kExtra && which && d_smaller_drew(src, m, ctrl, leaves, p, min(p.max_cat_threshold, kCatListMax))) xr = d_lcg_next(xr);
   if (!m.is_categorical) {        // wide numerical feature (max_bin > 255): reduce into the pool slot, then the block-wide two-pass scan
     d_reduce_column(src, dst, m.num_bin, which);
+    if (forcing) d_forced_step<kMono>(ctrl, forced, leaf, u, dst, m, L, p);
     const int drew = d_scan_numeric_feature<kExtra, kMono>(dst, m, u, L, inv_g, inv_h, p, flag, &out, xr, cons);
     if (threadIdx.x == 0) d_publish_cand<kExtra>(cands, xrand, p, which, u, out, drew);
     return;
@@ -2096,6 +2238,7 @@ k_scan_wide(const TreeCtrl* __restrict__ ctrl, const LeafState* __restrict__ lea
   }
   if (my_used) atomicAdd(&s_used, my_used);
   __syncthreads();
+  if (forcing) d_forced_step<kMono>(ctrl, forced, leaf, u, dst, m, L, p);
   const int used_bin = s_used;
   const int max_num_cat = min(min(p.max_cat_threshold, kCatListMax), (used_bin + 1) / 2);
   int rand_i = 0, drew = 0;      // extra_trees: the one prefix length - 1 evaluated
@@ -2530,7 +2673,7 @@ __global__ void __launch_bounds__(256, 4)
 k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
        const long long* __restrict__ H, long long* __restrict__ pool, size_t slot_elems, uint8_t* __restrict__ flags,
        SplitCand* cands, SplitParams p, const int* __restrict__ bundle_base, VoteBufs vote, unsigned* __restrict__ xrand, ConstraintArgs cons,
-       NodeSampleArgs node) {
+       NodeSampleArgs node, ForcedArgs forced) {
   // dynamic scratch (kScanSmem, only when the dataset has categorical tile features or a bundle): the categorical search's work space,
   // or a bundle member's histogram (d_unbundle_hist)
   extern __shared__ double scan_ws[];
@@ -2566,7 +2709,9 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
       }
     } else {
       uint8_t* flag = &flags[static_cast<size_t>(leaf) * p.nf_pad + u];
-      if (kMode == kScanLocal || *flag) {
+      // forced splits: while the phase lasts every column of the scanned leaves is reduced, as in k_scan_wide
+      const bool forcing = kMode == kScanPlain && forced.nodes && ctrl->forced_next >= 0;
+      if (kMode == kScanLocal || *flag || forcing) {
         const FeatMeta fm = meta[u];
         long long* dst = pool + static_cast<size_t>(leaves[leaf].hist_slot) * slot_elems + static_cast<size_t>(fm.hist_off) * 2;
         const long long* src = H + static_cast<size_t>(fm.hist_off) * 2;
@@ -2592,6 +2737,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
           Lloc.global_count = Lw.count;
         }
         const LeafState& L = kMode == kScanLocal ? Lloc : leaves[leaf];
+        if (forcing) d_forced_step<kMono>(ctrl, forced, leaf, u, dst, fm, L, p);
         if (*flag) {
           // extra_trees: the stream state before this scan's draw (see d_smaller_drew)
           unsigned xr = kExtra ? xrand[u] : 0u;
@@ -2624,7 +2770,7 @@ k_scan(TreeCtrl* ctrl, LeafState* leaves, const FeatMeta* __restrict__ meta,
     if constexpr (kMode == kScanLocal) d_topk_block(ctrl, leaves, meta, cands, p, vote.recs, vote.top_k);
     else {
       if constexpr (kExtra) d_extra_commit(ctrl, xrand, p);
-      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, cons.type, cons.sets_of, node.mask);
+      d_pick_block<kMono>(ctrl, leaves, meta, cands, p, cons.type, cons.sets_of, node.mask, forced);
     }
     if (threadIdx.x == 0) ctrl->scan_ticket = 0u;
   }

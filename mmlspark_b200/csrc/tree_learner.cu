@@ -192,6 +192,15 @@ void TreeLearner::ResetConfig(const Config& cfg) {
   bynode_k_ = bynode_ ? SampleCount(pool, cfg.feature_fraction_bynode) : 0;
 }
 
+void TreeLearner::SetForcedPlan(const std::vector<ForcedNode>& plan) {
+  const bool same = plan.size() == forced_host_.size() &&
+                    (plan.empty() || std::memcmp(plan.data(), forced_host_.data(), plan.size() * sizeof(ForcedNode)) == 0);
+  if (same) return;
+  forced_host_ = plan;
+  forced_.Alloc(plan.size()); forced_evals_.Alloc(plan.size());      // frees the old buffers: cudaFree waits for the trees enqueued
+  if (!plan.empty()) forced_.Upload(forced_host_.data(), plan.size(), stream_);
+}
+
 // extra_trees streams (kernels.cuh d_lcg_next): used feature i in real-index order starts at extra_seed + i.  One small kernel on the
 // stream, ordered after the trees already enqueued; nothing is copied from the host.  With extra_trees off the states are never read.
 void TreeLearner::SeedExtraStreams(const Config& cfg) {
@@ -438,6 +447,9 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
   k_tree_init<<<1, 256, 0, s>>>(ctrl, leaves_.p, tree_dev_, flags_.p, sp_, rows_, feature_used_.p, bag ? 1 : 0, col_rand_.state());
   nvtxRangePop();
   timing_.launches += 4;
+  // forced splits: the plan's evaluations start as "not evaluated" (gain 0) in every tree
+  const ForcedArgs forced = forced_host_.empty() ? ForcedArgs{} : ForcedArgs{forced_.p, forced_evals_.p, static_cast<int>(forced_host_.size())};
+  if (forced.nodes) forced_evals_.Zero(s);
   const int pgrid = std::max(1, std::min(n / kPartChunk + 1, part_max_blocks_));
   // one block per (leaf, tile feature); the pick step in the last block also sees the wide features' candidates.  Per-node feature
   // sampling adds one column: each leaf's d_bynode_sample block
@@ -491,7 +503,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       nvtxRangePushA("b200gbm:voting local scan + vote + C2 reduce + global scan + pick");
       const VoteBufs vote{recs_.p, voted_.p, packed_.p, top_k_};
       k_scan<kScanLocal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_local, d.BundleBase(), vote, xrand_.p,
-                                                        cons, NodeSampleArgs{});
+                                                        cons, NodeSampleArgs{}, ForcedArgs{});
       mark();
       Net().AllGather(recs_.p, all_recs_.p, recs_.n * sizeof(VoteRec), s);
       mark();
@@ -502,7 +514,7 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       Net().AllReduce(packed_.p, packed_.n, ncclInt64, ncclSum, s);
       mark();
       k_scan<kScanGlobal><<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), vote, xrand_.p,
-                                                         cons, NodeSampleArgs{});
+                                                         cons, NodeSampleArgs{}, ForcedArgs{});
       nvtxRangePop();
       comm_hist_bytes_ += static_cast<long long>(packed_.n * sizeof(long long));
       comm_rec_bytes_ += static_cast<long long>(all_recs_.n * sizeof(VoteRec));
@@ -517,13 +529,13 @@ void TreeLearner::Grow(const float* g, const float* h, bool const_hessian, const
       const ScanKernels& k = kScanKernels[extra_trees_][monotone_ || smooth_];
       if (d.nw > 0) {
         k.scan_wide<<<dim3(d.nw, 2), 256, kWideMaxBins * 8, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, xrand_.p,
-                                                                 cons);
+                                                                 cons, forced);
         timing_.launches += 1;
       }
       // scan + (last block) pick
       const NodeSampleArgs node = bynode_ ? NodeSampleArgs{node_mask_.p, node_work_.p, real_order_.p, feature_used_.p, bynode_k_} : NodeSampleArgs{};
       k.scan<<<sgrid, 256, scan_smem, s>>>(ctrl, leaves_.p, d.meta.p, H_.p, pool_.p, slot_elems_, flags_.p, cands_.p, sp_, d.BundleBase(), VoteBufs{}, xrand_.p,
-                                           cons, node);
+                                           cons, node, forced);
       nvtxRangePop();
     }
     mark();

@@ -15,6 +15,9 @@ class TreeLearner {
               cudaStream_t stream, Booster::Timing& timing);
   ~TreeLearner();
   void ResetConfig(const Config& cfg);      // the split parameters a ResetParameter may change
+  // forced splits: the plan every later tree starts with (forced_splits.h), empty for none; uploaded when it changes
+  void SetForcedPlan(const std::vector<ForcedNode>& plan);
+  bool HasForcedPlan() const { return !forced_host_.empty(); }
 
   // the rows a bagged tree is grown on: the in-bag flags and the ascending in-bag row list
   struct Bag { const uint8_t* in_bag; const int* rows; int count; };
@@ -67,6 +70,9 @@ class TreeLearner {
   DevBuf<uint8_t> node_mask_;      // per-node feature sampling: [2][nf_pad] the round's leaf samples (kernels.cuh d_bynode_sample)
   DevBuf<int> node_work_;          // [2][4][nf_pad] the sampler's scratch
   DevBuf<int> real_order_;         // [nf_pad] Dataset::sample_order: the used features in real-index order
+  std::vector<ForcedNode> forced_host_;      // forced splits: the plan as uploaded to forced_, empty for none
+  DevBuf<ForcedNode> forced_;
+  DevBuf<SplitCand> forced_evals_;           // [plan nodes] each node's evaluation (kernels.cuh d_forced_eval), zeroed before each tree
   int rows_ = 0;                 // rows of the tree being grown (the bag's count when bagged)
   // device state of the tree being grown
   DevBuf<int4> qgh_, qord_;      // per-row fixed-point (g,h) words; the same in leaf order for the leaf being built

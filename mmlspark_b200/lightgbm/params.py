@@ -46,6 +46,7 @@ COMMON_DEFAULTS = dict(
     interactionConstraints=(),          # interaction_constraints: lists of feature indices; a branch splits on features of one list only
     featureFractionByNode=1.0,          # feature_fraction_bynode: the share of the tree's features each leaf's split is chosen from
     pathSmooth=0.0,                     # path_smooth: smooths every split gain and leaf output toward the parent leaf's output
+    forcedSplitsFilename="",            # forcedsplits_filename: a JSON file of splits every tree starts with (no spaces in the path)
     # LightGBM 4's quantised training: use_quantized_grad, num_grad_quant_bins, quant_train_renew_leaf, stochastic_rounding
     useQuantizedGrad=False, numGradQuantBins=4, quantTrainRenewLeaf=False, stochasticRounding=True,
     delegate=None,
@@ -138,6 +139,8 @@ class TrainParams:
             s += "feature_fraction_bynode=%s " % scala_double(p["featureFractionByNode"])
         if p["pathSmooth"] != 0.0:      # only when set, so every other parameter string stays as the reference builds it
             s += "path_smooth=%s " % scala_double(p["pathSmooth"])
+        if p["forcedSplitsFilename"]:      # only when set, so every other parameter string stays as the reference builds it
+            s += "forcedsplits_filename=%s " % p["forcedSplitsFilename"]
         if p["useQuantizedGrad"]:      # only when set, so every other parameter string stays as the reference builds it
             s += "use_quantized_grad=true num_grad_quant_bins=%d quant_train_renew_leaf=%s stochastic_rounding=%s " % (
                 p["numGradQuantBins"], scala_bool(p["quantTrainRenewLeaf"]), scala_bool(p["stochasticRounding"]))
