@@ -219,6 +219,11 @@ int B200GBM_DatasetQuantizedHistogram(DatasetHandle handle, const float* grad, c
 /* kernel-level entry: the objective's gradients and hessians (K1/K2) at the booster's current training scores, class-major [K][n]
  * host arrays; classes the objective does not train read back as 0.  Training state and the model are not changed. */
 int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess);
+/* the ranking objectives' position factors (a training set with the "position" field, lambdarank or rank_xendcg): out_len = the number
+ * of distinct position values over every rank's training rows; when buffer_len >= out_len, out_ids [out_len] gets those values in
+ * ascending order and out_factors [out_len] the factor of each.  A booster with no position field (or another objective, or loaded from
+ * a model string) gives out_len = 0.  The factors are training state: model text and predictions do not contain them. */
+int B200GBM_BoosterGetPositionBias(BoosterHandle handle, int64_t buffer_len, int* out_len, int32_t* out_ids, double* out_factors);
 /* the last LGBM_BoosterRefit: out = {staging ms, per-tree work ms (host clock, each ending in a device sync), batches of models,
  * row blocks staged} */
 int B200GBM_BoosterGetRefitTiming(BoosterHandle handle, double* out4);

@@ -247,6 +247,12 @@ class Dataset:
             a = np.ascontiguousarray(arr, dtype=np.float64); t = DTYPE_FLOAT64
         elif name == "group":
             a = np.ascontiguousarray(arr, dtype=np.int32); t = DTYPE_INT32
+        elif name == "position":      # integer arrays go as int32; float arrays keep their type, which the library rejects
+            a = np.ascontiguousarray(arr)
+            if a.dtype.kind in "iub":
+                a = a.astype(np.int32); t = DTYPE_INT32
+            else:
+                t = _np_dtype_code(a)
         else:
             raise LightGBMError("Unknown field name: " + name)
         check(load().LGBM_DatasetSetField(self.handle, name.encode(), _ptr(a), C.c_int(len(a)), C.c_int(t)))
@@ -380,6 +386,17 @@ class Booster:
         if a.ndim != 2:
             raise LightGBMError("refit: leaf_preds must be a 2-D (num_data, num_models) array")
         check(load().LGBM_BoosterRefit(self.handle, _ptr(a), C.c_int32(a.shape[0]), C.c_int32(a.shape[1])))
+
+    def position_bias(self):
+        """(ids, factors): the distinct position values of the training data in ascending order, int32, and the ranking objective's
+        factor of each, float64 (B200GBM_BoosterGetPositionBias); both empty without a position field"""
+        n = C.c_int(0)
+        check(load().B200GBM_BoosterGetPositionBias(self.handle, C.c_int64(0), C.byref(n), None, None))
+        ids = np.zeros(n.value, dtype=np.int32)
+        factors = np.zeros(n.value, dtype=np.float64)
+        if n.value:
+            check(load().B200GBM_BoosterGetPositionBias(self.handle, C.c_int64(n.value), C.byref(n), _ptr(ids), _ptr(factors)))
+        return ids, factors
 
     def refit_timing(self):
         """the last refit (B200GBM_BoosterGetRefitTiming): staging and per-tree host milliseconds, batches of models, row blocks"""

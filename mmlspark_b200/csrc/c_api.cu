@@ -601,6 +601,18 @@ int B200GBM_BoosterGetGradients(BoosterHandle handle, float* grad, float* hess) 
   BS(handle)->GetGradients(grad, hess);
   API_END();
 }
+int B200GBM_BoosterGetPositionBias(BoosterHandle handle, int64_t buffer_len, int* out_len, int32_t* out_ids, double* out_factors) {
+  API_BEGIN();
+  std::vector<int32_t> ids;
+  std::vector<double> factors;
+  BS(handle)->GetPositionBias(&ids, &factors);
+  *out_len = static_cast<int>(ids.size());
+  if (static_cast<int64_t>(ids.size()) <= buffer_len && out_ids && out_factors) {
+    std::copy(ids.begin(), ids.end(), out_ids);
+    std::copy(factors.begin(), factors.end(), out_factors);
+  }
+  API_END();
+}
 int B200GBM_BoosterGetRefitTiming(BoosterHandle handle, double* out4) {
   API_BEGIN();
   const Booster::RefitTiming& t = BS(handle)->refit_timing;

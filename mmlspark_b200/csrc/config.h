@@ -89,6 +89,9 @@ struct Config {
   int lambdarank_truncation_level = 30;
   bool lambdarank_norm = true;
   std::vector<double> label_gain;
+  // [UPSTREAM 4.1, from knowledge] L2 regularisation of the ranking objectives' position factors (a training set with a position field);
+  // >= 0, Booster checks at create and reset
+  double lambdarank_position_bias_regularization = 0.0;
   std::vector<int> eval_at;
   std::vector<double> auc_mu_weights;       // auc_mu's K x K class-pair weights, row-major; empty = 1 off the diagonal, 0 on it
   // --- network
@@ -258,6 +261,7 @@ struct Config {
     D("tweedie_variance_power", &tweedie_variance_power); D("fair_c", &fair_c); D("poisson_max_delta_step", &poisson_max_delta_step); I("objective_seed", &objective_seed);
     I("lambdarank_truncation_level", &lambdarank_truncation_level);
     B("lambdarank_norm", &lambdarank_norm); I("num_machines", &num_machines);
+    D("lambdarank_position_bias_regularization", &lambdarank_position_bias_regularization);
     {
       auto it = raw.find("label_gain");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &label_gain, [](const std::string& x) { return std::atof(x.c_str()); });
@@ -343,7 +347,10 @@ struct Config {
     s << "[scale_pos_weight: " << Num(scale_pos_weight) << "]\n[sigmoid: " << Num(sigmoid) << "]\n[boost_from_average: " << boost_from_average << "]\n";
     s << "[reg_sqrt: 0]\n[alpha: " << Num(alpha) << "]\n[fair_c: " << Num(fair_c) << "]\n[poisson_max_delta_step: " << Num(poisson_max_delta_step) << "]\n";
     s << "[tweedie_variance_power: " << Num(tweedie_variance_power) << "]\n[lambdarank_truncation_level: " << lambdarank_truncation_level << "]\n";
-    s << "[lambdarank_norm: " << lambdarank_norm << "]\n[label_gain: " << join_d(label_gain) << "]\n[eval_at: " << join_i(eval_at) << "]\n";
+    s << "[lambdarank_norm: " << lambdarank_norm << "]\n[label_gain: " << join_d(label_gain) << "]\n";
+    if (lambdarank_position_bias_regularization != 0.0)      // only when set, so every other model text stays as it was
+      s << "[lambdarank_position_bias_regularization: " << Num(lambdarank_position_bias_regularization) << "]\n";
+    s << "[eval_at: " << join_i(eval_at) << "]\n";
     s << "[multi_error_top_k: 1]\n[auc_mu_weights: " << join_d(auc_mu_weights) << "]\n[num_machines: " << num_machines << "]\n[local_listen_port: 12400]\n";
     s << "[time_out: 120]\n[machine_list_filename: ]\n[machines: ]\n[gpu_platform_id: -1]\n[gpu_device_id: -1]\n[gpu_use_dp: 0]\n[num_gpu: 1]";
     return s.str();

@@ -1317,6 +1317,13 @@ void Dataset::SetField(const char* name, const void* data, int n, int type) {
     for (int i = 0; i < n; ++i) query_boundaries.push_back(query_boundaries.back() + g[i]);
     if (query_boundaries.back() != num_data) Fatal("Sum of query counts is not same with #data");
     d_qb.Alloc(query_boundaries.size()); d_qb.Upload(query_boundaries.data(), query_boundaries.size(), stream);
+  } else if (s == "position") {
+    if (n == 0 || data == nullptr) { position.clear(); d_position.Free(); return; }
+    if (type != 2) Fatal("Input type error for position (expect int32)");
+    if (n != num_data) Fatal("Length of position (" + std::to_string(n) + ") is not same with #data (" + std::to_string(num_data) + ")");
+    const int32_t* p = static_cast<const int32_t*>(data);
+    position.assign(p, p + n);
+    d_position.Alloc(n); d_position.Upload(position.data(), n, stream);
   } else {
     Fatal("Unknown field name: " + s);
   }
@@ -1329,6 +1336,7 @@ void Dataset::GetField(const char* name, int* out_len, const void** out_ptr, int
   else if (s == "weight" || s == "weights") { *out_len = static_cast<int>(weight.size()); *out_ptr = weight.empty() ? nullptr : weight.data(); *out_type = 0; }
   else if (s == "init_score") { *out_len = static_cast<int>(init_score.size()); *out_ptr = init_score.empty() ? nullptr : init_score.data(); *out_type = 1; }
   else if (s == "group" || s == "query") { *out_len = static_cast<int>(query_boundaries.size()); *out_ptr = query_boundaries.empty() ? nullptr : query_boundaries.data(); *out_type = 2; }
+  else if (s == "position") { *out_len = static_cast<int>(position.size()); *out_ptr = position.empty() ? nullptr : position.data(); *out_type = 2; }
   else Fatal("Unknown field name: " + s);
 }
 
@@ -1425,6 +1433,12 @@ static void CheckPathSmooth(const Config& cfg, bool voting_parallel) {
 }
 
 // quantised training: the same checks at LGBM_BoosterCreate and ResetParameter, identical on every rank
+// [UPSTREAM 4.1, from knowledge] the position factors' L2 regularisation
+static void CheckPositionBias(const Config& cfg) {
+  if (!(cfg.lambdarank_position_bias_regularization >= 0.0))
+    Fatal("lambdarank_position_bias_regularization should be >= 0, got " + Config::Num(cfg.lambdarank_position_bias_regularization));
+}
+
 static void CheckQuantized(const Config& cfg) {
   if (!cfg.use_quantized_grad) return;
   // K4's packed plane flushes a cell after at most floor(32767 / B) additions, and its row chunks are whole 512-row stages
@@ -1521,6 +1535,7 @@ Booster::Booster(const Dataset* tr, const char* params) : train(tr), predictor(n
   CheckByNode(cfg, voting_);
   CheckPathSmooth(cfg, voting_);
   CheckQuantized(cfg);
+  CheckPositionBias(cfg);
   const std::vector<ForcedNode> forced_plan = CheckForcedSplits(cfg, *train, voting_, parallel_);
   if (balanced_bagging_) {      // [LightGBM GBDT::ResetBaggingConfig] needs (globally) at least one positive row
     double npos = static_cast<double>(std::count_if(train->label.begin(), train->label.end(), [](float v) { return v > 0; }));
@@ -1874,6 +1889,7 @@ void Booster::ResetParameter(const char* params) {
       CheckByNode(cfg, voting_);
       CheckPathSmooth(cfg, voting_);
       CheckQuantized(cfg);
+      CheckPositionBias(cfg);
       // a reset that gives the key (set, changed or cleared) reloads the plan on every rank
       if (nc.raw.count("forcedsplits_filename")) { forced_plan = CheckForcedSplits(cfg, *train, voting_, parallel_); reload_plan = true; }
       else if (learner_ && learner_->HasForcedPlan() && !cfg.monotone_constraints.empty()) Fatal(kForcedMonotone);
@@ -2021,6 +2037,13 @@ void Booster::GetGradients(float* grad, float* hess) {
   B200_CUDA(cudaGetLastError());
   g.Download(grad, m, stream_); h.Download(hess, m, stream_);
   B200_CUDA(cudaStreamSynchronize(stream_));
+}
+
+void Booster::GetPositionBias(std::vector<int32_t>* values, std::vector<double>* factors) const {
+  values->clear(); factors->clear();
+  if (!obj_) return;
+  EnsureDevice();
+  obj_->PositionBias(values, factors);
 }
 
 }  // namespace b200gbm

@@ -158,8 +158,9 @@ class Dataset {
   std::vector<float> label, weight;
   std::vector<double> init_score;
   std::vector<int32_t> query_boundaries, group_sizes;
+  std::vector<int32_t> position;             // display position of each row (any int32 values), empty for none: the ranking objectives' factors
   DevBuf<float> d_label, d_weight;
-  DevBuf<int> d_qb;
+  DevBuf<int> d_qb, d_position;
   std::vector<std::string> feature_names;
   cudaStream_t stream = nullptr;
   double ingest_ms = 0.0;                    // H2D + binning time of a matrix / CSR create, or the sum over PushRows calls (CUDA events)
@@ -220,6 +221,9 @@ class Booster {
   // the objective's gradients at the current training scores, class-major [K][n], computed into scratch buffers: the training state
   // (grad_ / hess_, which rf keeps from construction and GOSS rescales in place) is not touched
   void GetGradients(float* grad, float* hess);
+  // the ranking objectives' position factors: the distinct position values of the training data (over every rank, sorted) and the
+  // factor of each; empty without a position field, for other objectives and for a prediction-only booster
+  void GetPositionBias(std::vector<int32_t>* values, std::vector<double>* factors) const;
   // LGBM_BoosterRefit (refit.cu): leaf_preds [nrow][ncol] row-major host memory, the leaf of training row i in model j.  Every check
   // (and with data-parallel ranks every rank's outcome) comes before anything changes, so a failed refit leaves the model as it was.
   void Refit(const int32_t* leaf_preds, int nrow, int ncol);

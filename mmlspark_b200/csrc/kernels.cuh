@@ -516,6 +516,15 @@ __global__ void k_grad_softmax(const double* __restrict__ score, const float* __
   }
 }
 
+// The score a ranking objective sees for row i.  [UPSTREAM 4.1, from knowledge] unbiased lambdarank: with a position field, both ranking
+// objectives take their gradients at s_i + b[id_i], the row's position factor added; pos_id null is the plain score.
+__device__ __forceinline__ double d_rank_score(const double* __restrict__ score, const int* __restrict__ pos_id, const double* __restrict__ pos_bias,
+                                               int i) {
+  double s = score[i];
+  if (pos_id) s += pos_bias[pos_id[i]];
+  return s;
+}
+
 // [UPSTREAM LambdarankNDCG::GetGradientsForOneQuery] — one block per query (K2).
 // Sorting: stable rank by score descending (rank counting out of shared memory; queries are ~100 docs).
 // Pairs (i, j), i < min(truncation, cnt-1), j > i, are evaluated ONCE, tile by tile over j, by all threads (balanced) into a
@@ -533,7 +542,8 @@ __host__ __device__ inline int lr_tile(int truncation) {          // j-tile widt
   return max(t & ~31, 32);
 }
 __global__ void __launch_bounds__(kLrThreads)
-k_grad_lambdarank(const double* __restrict__ score, const float* __restrict__ label, const float* __restrict__ weight,
+k_grad_lambdarank(const double* __restrict__ score, const int* __restrict__ pos_id, const double* __restrict__ pos_bias,
+                  const float* __restrict__ label, const float* __restrict__ weight,
                   const int* __restrict__ qb, int nq, const double* __restrict__ inv_max_dcg, const double* __restrict__ label_gain,
                   const double* __restrict__ discount, const float* __restrict__ sig_table, int sig_bins, double min_in, double max_in,
                   double idx_factor, double sigmoid, int truncation, int norm, float* __restrict__ g, float* __restrict__ h, int max_q) {
@@ -550,7 +560,9 @@ k_grad_lambdarank(const double* __restrict__ score, const float* __restrict__ la
   for (int q = blockIdx.x; q < nq; q += gridDim.x) {
     const int start = qb[q], cnt = qb[q + 1] - start;
     __syncthreads();
-    for (int i = threadIdx.x; i < cnt; i += blockDim.x) r_score[i] = score[start + i];
+    // two loops rather than d_rank_score's test per row: one loop holds 8 more registers through the whole kernel
+    if (pos_id) for (int i = threadIdx.x; i < cnt; i += blockDim.x) r_score[i] = score[start + i] + pos_bias[pos_id[start + i]];
+    else for (int i = threadIdx.x; i < cnt; i += blockDim.x) r_score[i] = score[start + i];
     __syncthreads();
     for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
       const double si = r_score[i];
@@ -646,7 +658,8 @@ k_grad_lambdarank(const double* __restrict__ score, const float* __restrict__ la
 __device__ __forceinline__ float d_lcg_float(unsigned x) { return static_cast<float>((x >> 16) & 0x7FFFu) / 32768.0f; }
 constexpr int kXeThreads = 128;
 __global__ void __launch_bounds__(kXeThreads)
-k_grad_xendcg(const double* __restrict__ score, const float* __restrict__ label, const float* __restrict__ weight, const int* __restrict__ qb,
+k_grad_xendcg(const double* __restrict__ score, const int* __restrict__ pos_id, const double* __restrict__ pos_bias, const float* __restrict__ label,
+              const float* __restrict__ weight, const int* __restrict__ qb,
               int nq, unsigned* __restrict__ lcg_state, const unsigned* __restrict__ jump_mul, const unsigned* __restrict__ jump_add, int advance,
               double* __restrict__ scratch, size_t n, float* __restrict__ g, float* __restrict__ h) {
   __shared__ double s_sum;
@@ -663,7 +676,7 @@ k_grad_xendcg(const double* __restrict__ score, const float* __restrict__ label,
     double* pa = params + start;
     // softmax: max (order-free), exp, denominator in document order
     double wmax = -INFINITY;
-    for (int i = threadIdx.x; i < cnt; i += blockDim.x) wmax = fmax(wmax, score[start + i]);
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) wmax = fmax(wmax, d_rank_score(score, pos_id, pos_bias, start + i));
     for (int o = 16; o; o >>= 1) wmax = fmax(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
     __shared__ double s_max[kXeThreads / 32];
     if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = wmax;
@@ -671,7 +684,7 @@ k_grad_xendcg(const double* __restrict__ score, const float* __restrict__ label,
     wmax = s_max[0];
     for (int w = 1; w < kXeThreads / 32; ++w) wmax = fmax(wmax, s_max[w]);
     for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
-      r[i] = exp(score[start + i] - wmax);
+      r[i] = exp(d_rank_score(score, pos_id, pos_bias, start + i) - wmax);
       const unsigned x = jump_mul[i] * x0 + jump_add[i];
       pa[i] = ldexp(1.0, static_cast<int>(label[start + i])) - static_cast<double>(d_lcg_float(x));
     }
@@ -763,6 +776,34 @@ __global__ void k_set_scale(TreeCtrl* ctrl, int const_hessian, double hess_const
   ctrl->inv_g = ldexp(1.0, -eg);
   ctrl->inv_h = const_hessian ? hess_const : ldexp(1.0, -eh);
   ctrl->root_q[0] = 0; ctrl->root_q[1] = 0; ctrl->root_q[2] = 0; ctrl->root_q[3] = 0;
+}
+
+// Position row ids (Objective): ids[i] = the index of pos[i] in the sorted distinct values `values` [P], which hold every value of pos
+__global__ void __launch_bounds__(256)
+k_position_ids(const int* __restrict__ pos, int n, const int* __restrict__ values, int P, int* __restrict__ ids) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int v = pos[i];
+    int lo = 0, hi = P - 1;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (values[mid] < v) lo = mid + 1; else hi = mid; }
+    ids[i] = lo;
+  }
+}
+// [UPSTREAM 4.1 RankingObjective::UpdatePositionBiasFactors, from knowledge] one thread per position id p, at k_refit_leaf_sums' (all-reduced)
+// sums of the weighted g and h over the rows of p (sums [3][P]: Q_g, Q_h, rows):
+//   d1 = -sum_g - b_p * reg * cnt,  d2 = -sum_h - reg * cnt,  b_p += learning_rate * d1 / (|d2| + 0.001)
+// sum_g = Q_g 2^-e_g and sum_h = Q_h 2^-e_h on K3's grid.  Every fp64 operation is rounded on its own, in this order, so a restatement
+// can follow it bit for bit.
+__global__ void k_position_bias_update(const long long* __restrict__ sums, int P, const TreeCtrl* __restrict__ ctrl, double learning_rate,
+                                       double reg, double* __restrict__ bias) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const double sg = __dmul_rn(static_cast<double>(sums[p]), ldexp(1.0, -ctrl->exp_g));
+  const double sh = __dmul_rn(static_cast<double>(sums[P + p]), ldexp(1.0, -ctrl->exp_h));
+  const double cnt = static_cast<double>(sums[2 * P + p]);
+  const double b = bias[p];
+  const double d1 = __dsub_rn(-sg, __dmul_rn(__dmul_rn(b, reg), cnt));
+  const double d2 = __dsub_rn(-sh, __dmul_rn(reg, cnt));
+  bias[p] = __dadd_rn(b, __ddiv_rn(__dmul_rn(learning_rate, d1), __dadd_rn(fabs(d2), 0.001)));
 }
 // a 256-thread block's share of the root sums: sum q_g, sum q_h over its in-bag rows, and (block 0) the rows of the root
 __device__ __forceinline__ void d_add_root_sums(long long sg, long long sh, TreeCtrl* ctrl, const uint8_t* in_bag, int bag_count, int n) {

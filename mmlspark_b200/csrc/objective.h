@@ -5,6 +5,7 @@
 #include <functional>
 #include <numeric>
 #include "engine.h"
+#include "refit_kernels.cuh"      // k_refit_leaf_sums: the per-position sums of the position factors' update
 
 namespace b200gbm {
 
@@ -201,6 +202,7 @@ class Objective {
       if (smem > 200 * 1024) Fatal("a query group is too large for the lambdarank kernel");
       B200_CUDA(cudaFuncSetAttribute(k_grad_lambdarank, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(std::max<size_t>(smem, 1024))));
     }
+    if (kind_ == Kind::kLambdarank || kind_ == Kind::kRankXendcg) InitPositions();
   }
 
   // init score of class k, the same on every rank
@@ -250,18 +252,29 @@ class Objective {
       case Kind::kCrossEntropyLambda: k_grad_xentlambda<<<grid, 256, 0, stream_>>>(score, y, w, g, h, n); break;
       case Kind::kRankXendcg: {
         const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
-        k_grad_xendcg<<<std::max(1, std::min(nq, num_sms * 16)), kXeThreads, 0, stream_>>>(score, y, w, train_.d_qb.p, nq, xe_state_.p, xe_jump_.p,
-                                                                                         xe_jump_.p + xe_max_q_, advance ? 1 : 0, xe_scratch_.p, n, g, h);
+        k_grad_xendcg<<<std::max(1, std::min(nq, num_sms * 16)), kXeThreads, 0, stream_>>>(score, PositionIds(), pos_bias_.p, y, w, train_.d_qb.p, nq,
+                                                                                         xe_state_.p, xe_jump_.p, xe_jump_.p + xe_max_q_,
+                                                                                         advance ? 1 : 0, xe_scratch_.p, n, g, h);
         break;
       }
       case Kind::kLambdarank: {
         const int nq = static_cast<int>(train_.query_boundaries.size()) - 1;
         const size_t smem = std::max<size_t>(LambdarankSmem(lr_max_q_, cfg_.lambdarank_truncation_level), 1024);
         k_grad_lambdarank<<<std::min(nq, num_sms * 16), kLrThreads, smem, stream_>>>(
-            score, y, w, train_.d_qb.p, nq, lr_inv_max_dcg_.p, lr_label_gain_.p, lr_discount_.p, lr_sig_table_.p, 1024 * 1024, lr_min_in_,
+            score, PositionIds(), pos_bias_.p, y, w, train_.d_qb.p, nq, lr_inv_max_dcg_.p, lr_label_gain_.p, lr_discount_.p, lr_sig_table_.p, 1024 * 1024, lr_min_in_,
             lr_max_in_, lr_idx_factor_, cfg_.sigmoid, cfg_.lambdarank_truncation_level, cfg_.lambdarank_norm ? 1 : 0, g, h, lr_max_q_); break;
       }
     }
+    if (advance && !pos_values_.empty()) UpdatePositionBias(g, h, num_sms);
+  }
+
+  // the distinct position values (sorted, over every rank) and their factors; empty without a position field or for another objective
+  void PositionBias(std::vector<int32_t>* values, std::vector<double>* factors) const {
+    *values = pos_values_;
+    factors->assign(pos_values_.size(), 0.0);
+    if (pos_values_.empty()) return;
+    pos_bias_.Download(factors->data(), factors->size(), stream_);
+    B200_CUDA(cudaStreamSynchronize(stream_));
   }
 
   std::string ToString() const {      // objective= value of the model header
@@ -276,6 +289,77 @@ class Objective {
   void ClassWeights(double pos, double neg, double* cw) const {
     if (cfg_.is_unbalance && pos > 0 && neg > 0) { if (pos > neg) cw[0] = pos / neg; else cw[1] = neg / pos; }
     cw[1] *= cfg_.scale_pos_weight;
+  }
+
+  const int* PositionIds() const { return pos_values_.empty() ? nullptr : pos_id_.p; }
+
+  // [UPSTREAM 4.1 Metadata::SetPosition, from knowledge] one factor per distinct position value, starting at 0.  The ids are global: the
+  // sorted union of every rank's values, gathered padded to the largest count, so that every rank updates the same factors.  Every rank
+  // of a ranking booster takes part in the first collective, so ranks that disagree on having the field all fail here.
+  void InitPositions() {
+    const int n = train_.num_data;
+    std::vector<int32_t> local(train_.position);
+    std::sort(local.begin(), local.end());
+    local.erase(std::unique(local.begin(), local.end()), local.end());
+    const bool has = !train_.position.empty();
+    const bool net = Net().active && Net().world > 1;
+    if (net) {
+      double v[3] = {has ? 1.0 : 0.0, has ? -1.0 : 0.0, static_cast<double>(local.size())};      // max: any rank has it, not every rank has it
+      AllReduceHost(v, 3, ncclMax, stream_);
+      if (v[0] != -v[1]) Fatal("the position field is set on some ranks' training data and not on others; set it on every rank or on none");
+      if (!has) return;
+      const size_t stride = 1 + static_cast<size_t>(v[2]);      // [count, values padded with 0]
+      std::vector<int32_t> send(stride, 0), recv(stride * Net().world);
+      send[0] = static_cast<int32_t>(local.size());
+      std::copy(local.begin(), local.end(), send.begin() + 1);
+      DevBuf<int32_t> d_send, d_recv;
+      d_send.Alloc(stride); d_recv.Alloc(recv.size());
+      d_send.Upload(send.data(), stride, stream_);
+      Net().AllGather(d_send.p, d_recv.p, stride * sizeof(int32_t), stream_);
+      d_recv.Download(recv.data(), recv.size(), stream_);
+      B200_CUDA(cudaStreamSynchronize(stream_));
+      local.clear();
+      for (int r = 0; r < Net().world; ++r) local.insert(local.end(), recv.begin() + r * stride + 1, recv.begin() + r * stride + 1 + recv[r * stride]);
+      std::sort(local.begin(), local.end());
+      local.erase(std::unique(local.begin(), local.end()), local.end());
+    }
+    if (!has) return;
+    pos_values_ = local;
+    const int P = static_cast<int>(pos_values_.size());
+    DevBuf<int32_t> d_values;
+    d_values.Alloc(P); d_values.Upload(pos_values_.data(), P, stream_);
+    pos_id_.Alloc(n);
+    if (n > 0) k_position_ids<<<std::max(1, std::min((n + 255) / 256, DeviceSMs() * 8)), 256, 0, stream_>>>(train_.d_position.p, n, d_values.p, P, pos_id_.p);
+    B200_CUDA(cudaGetLastError());
+    pos_bias_.Alloc(P); pos_bias_.Zero(stream_);
+    pos_sums_.Alloc(3 * static_cast<size_t>(P));
+    pos_ctrl_.Alloc(1); pos_ctrl_.Zero(stream_);
+    if (P <= kRefitSharedLeaves)
+      B200_CUDA(cudaFuncSetAttribute(k_refit_leaf_sums<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     static_cast<int>(3 * kRefitSharedLeaves * sizeof(long long))));
+    B200_CUDA(cudaStreamSynchronize(stream_));
+  }
+
+  // After a training pass's gradients, on the stream and without a host wait: the fixed-point exponents of max|g| and max|h| over every
+  // rank's rows, the per-position sums of g, h and rows (k_refit_leaf_sums with rows mapped to position ids, exact and order-free, then
+  // all-reduced), and one Newton step per factor.  learning_rate and the regularisation are read from the current config.
+  void UpdatePositionBias(const float* g, const float* h, int num_sms) const {
+    const int n = train_.num_data, P = static_cast<int>(pos_values_.size());
+    const bool net = Net().active && Net().world > 1;
+    B200_CUDA(cudaMemsetAsync(&pos_ctrl_.p->absmax_bits[0], 0, 8, stream_));
+    k_absmax<<<num_sms * 8, 256, 0, stream_>>>(g, h, n, pos_ctrl_.p);
+    if (net) Net().AllReduce(&pos_ctrl_.p->absmax_bits[0], 2, ncclUint32, ncclMax, stream_);
+    k_set_scale<<<1, 1, 0, stream_>>>(pos_ctrl_.p, 0, 1.0);
+    B200_CUDA(cudaMemsetAsync(pos_sums_.p, 0, pos_sums_.n * sizeof(long long), stream_));
+    if (P <= kRefitSharedLeaves)
+      k_refit_leaf_sums<true><<<num_sms * 4, 256, 3 * static_cast<size_t>(P) * sizeof(long long), stream_>>>(pos_id_.p, g, h, n, P, 0, pos_ctrl_.p,
+                                                                                                              pos_sums_.p);
+    else
+      k_refit_leaf_sums<false><<<num_sms * 8, 256, 0, stream_>>>(pos_id_.p, g, h, n, P, 0, pos_ctrl_.p, pos_sums_.p);
+    if (net) Net().AllReduce(pos_sums_.p, pos_sums_.n, ncclInt64, ncclSum, stream_);
+    k_position_bias_update<<<(P + 127) / 128, 128, 0, stream_>>>(pos_sums_.p, P, pos_ctrl_.p, cfg_.learning_rate,
+                                                                 cfg_.lambdarank_position_bias_regularization, pos_bias_.p);
+    B200_CUDA(cudaGetLastError());
   }
 
   const Config& cfg_;
@@ -293,6 +377,9 @@ class Objective {
   DevBuf<float> lr_sig_table_;
   double lr_min_in_ = -50, lr_max_in_ = 50, lr_idx_factor_ = 0; int lr_max_q_ = 0;
   DevBuf<unsigned> xe_state_, xe_jump_; DevBuf<double> xe_scratch_; int xe_max_q_ = 1;      // rank_xendcg: LCG per query, jump table, [2][n] rho / params
+  // ranking with a position field: the sorted distinct values (global), every row's id into them, the factors, the update's sums and scales
+  std::vector<int32_t> pos_values_;
+  DevBuf<int> pos_id_; DevBuf<double> pos_bias_; DevBuf<long long> pos_sums_; DevBuf<TreeCtrl> pos_ctrl_;
 };
 
 }  // namespace b200gbm

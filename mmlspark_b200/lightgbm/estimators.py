@@ -438,6 +438,9 @@ class LightGBMBase(Params):
         gcol = self.get("groupCol") if "groupCol" in self._defaults else None
         if gcol:      # partitions never split a query, so the parts' runs are the runs of their concatenation
             ds.set_field("group", np.asarray([c for p in parts for c in tu.count_cardinality(p[gcol].tolist())], dtype=np.int32))
+        pcol = self.get("positionCol") if "positionCol" in self._defaults else None
+        if pcol:      # display positions of the ranker's rows: the ranking objectives learn one score factor per position
+            ds.set_field("position", column(pcol, np.int32))
         names = list(self.get("slotNames"))
         if names:
             ds.set_feature_names(names)
@@ -491,7 +494,10 @@ class LightGBMBase(Params):
 
 _CLS_DEFAULTS = dict(COMMON_DEFAULTS, objective="binary", isUnbalance=False, probabilityCol="probability", rawPredictionCol="rawPrediction", thresholds=None)
 _REG_DEFAULTS = dict(COMMON_DEFAULTS, objective="regression", alpha=0.9, tweedieVariancePower=1.5)
-_RNK_DEFAULTS = dict(COMMON_DEFAULTS, objective="lambdarank", maxPosition=20, labelGain=(), evalAt=(1, 2, 3, 4, 5), groupCol=None)
+# positionCol / lambdarankPositionBiasRegularization: LightGBM 4.1's unbiased lambdarank (the dataset's position field and
+# lambdarank_position_bias_regularization); the reference has no such parameters
+_RNK_DEFAULTS = dict(COMMON_DEFAULTS, objective="lambdarank", maxPosition=20, labelGain=(), evalAt=(1, 2, 3, 4, 5), groupCol=None,
+                     positionCol=None, lambdarankPositionBiasRegularization=0.0)
 
 
 class LightGBMClassifier(LightGBMBase):

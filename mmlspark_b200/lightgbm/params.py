@@ -156,7 +156,10 @@ class TrainParams:
                 scala_double(p["alpha"]), scala_double(p["tweedieVariancePower"]), scala_bool(p["boostFromAverage"]), self._base())
         lg = "label_gain=%s" % ",".join(scala_double(x) for x in p["labelGain"]) if p["labelGain"] else ""   # :131-137
         ea = "eval_at=%s" % ",".join(str(i) for i in p["evalAt"]) if p["evalAt"] else ""
-        return "max_position=%d %s %s %s" % (p["maxPosition"], lg, ea, self._base())
+        s = "max_position=%d %s %s %s" % (p["maxPosition"], lg, ea, self._base())
+        if p.get("lambdarankPositionBiasRegularization", 0.0) != 0.0:      # only when set, so every other parameter string stays as it was
+            s += "lambdarank_position_bias_regularization=%s " % scala_double(p["lambdarankPositionBiasRegularization"])
+        return s
 
     __str__ = to_string
 
