@@ -80,10 +80,9 @@ struct HostTree {
   inline int Decide(double fval, int node) const {
     int mt = (decision_type[node] >> 2) & 3;
     if (decision_type[node] & 1) {       // [UPSTREAM] Tree::CategoricalDecision
-      if (std::isnan(fval)) {
-        if (mt == MISSING_NAN) return right_child[node];
-        fval = 0.0;
-      }
+      // NaN goes right whatever the missing type: upstream converts it to int first, which on x86 gives INT_MIN (< 0 => right), so
+      // its "NaN -> category 0" branch never runs.  Binning agrees: NaN falls in bin 0, which no left set holds.
+      if (std::isnan(fval)) return right_child[node];
       const int iv = static_cast<int>(fval);
       if (iv < 0) return right_child[node];
       const int ci = static_cast<int>(threshold[node]);

@@ -32,10 +32,10 @@ __device__ __forceinline__ int d_node_child(const ForestDev& f, int g, const T* 
   const int dt = f.decision_type[g];
   const int mt = (dt >> 2) & 3;
   bool left;
-  if (dt & 1) {                 // categorical decision
+  if (dt & 1) {                 // categorical decision: NaN goes right whatever the missing type (HostTree::Decide)
     left = false;
-    if (!(isnan(fval) && mt == 2)) {
-      const int iv = isnan(fval) ? 0 : static_cast<int>(fval);
+    if (!isnan(fval)) {
+      const int iv = static_cast<int>(fval);
       const int w = iv >> 5;
       if (iv >= 0 && w < f.cat_len[g]) left = (f.cat_words[f.cat_begin[g] + w] >> (iv & 31)) & 1u;
     }

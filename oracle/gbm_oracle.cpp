@@ -1398,10 +1398,10 @@ struct Tree {
     while (node >= 0) {
       double fval = row[split_feature[node]];
       int mt = (decision_type[node] >> 2) & 3;
-      if (decision_type[node] & 1) {     // CategoricalDecision
+      if (decision_type[node] & 1) {     // CategoricalDecision: NaN goes right whatever the missing type (int(NaN) = INT_MIN on x86)
         bool left = false;
-        if (!(std::isnan(fval) && mt == kMissNaN)) {
-          int iv = std::isnan(fval) ? 0 : static_cast<int>(fval);
+        if (!std::isnan(fval)) {
+          int iv = static_cast<int>(fval);
           if (iv >= 0) {
             int ci = static_cast<int>(threshold[node]);
             left = FindInBitset(cat_threshold.data() + cat_boundaries[ci], cat_boundaries[ci + 1] - cat_boundaries[ci], iv);

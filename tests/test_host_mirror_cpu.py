@@ -254,61 +254,6 @@ def test_model_shap_accessors_dense_and_sparse_agree():
     np.testing.assert_allclose(dense.sum(), m.predict(x), rtol=0, atol=1e-12)          # contributions + expected value = prediction
 
 
-def _brute_force_shap(tree, x):
-    """Shapley values of one tree by the DEFINITION: v(S) = E[f(x) | x_S] with the features outside S integrated out along the tree by
-    the training cover of the children (the path-dependent expectation TreeSHAP computes), phi_i = sum over subsets of the weighted
-    marginal contributions.  Exponential in the number of features a tree uses — a known-answer generator, not an algorithm."""
-    import itertools
-    import math
-    if int(tree["num_leaves"]) <= 1:
-        return {}, float(tree["leaf_value"][0])
-    sf = [int(v) for v in tree["split_feature"]]
-    thr = [float(v) for v in tree["threshold"]]
-    dt = [int(v) for v in tree["decision_type"]]
-    lc, rc = [int(v) for v in tree["left_child"]], [int(v) for v in tree["right_child"]]
-    lv = [float(v) for v in tree["leaf_value"]]
-    lcnt, icnt = [float(v) for v in tree["leaf_count"]], [float(v) for v in tree["internal_count"]]
-    cb = [int(v) for v in tree.get("cat_boundaries", [])]
-    ct = [int(v) for v in tree.get("cat_threshold", [])]
-
-    def cover(n):
-        return icnt[n] if n >= 0 else lcnt[~n]
-
-    def goes_left(n):
-        v = x[sf[n]]
-        if dt[n] & 1:                                   # categorical: the threshold indexes a bitset of categories that go left
-            if np.isnan(v) or v < 0:
-                return False
-            c, k = int(v), int(thr[n])
-            words = ct[cb[k]:cb[k + 1]]
-            return (c >> 5) < len(words) and bool((words[c >> 5] >> (c & 31)) & 1)
-        mt = (dt[n] >> 2) & 3
-        if np.isnan(v) and mt != 2:
-            v = 0.0
-        if (mt == 2 and np.isnan(v)) or (mt == 1 and abs(v) <= 1e-35):
-            return bool(dt[n] & 2)
-        return v <= thr[n]
-
-    def ev(n, S):
-        if n < 0:
-            return lv[~n]
-        if sf[n] in S:
-            return ev(lc[n] if goes_left(n) else rc[n], S)
-        return (cover(lc[n]) * ev(lc[n], S) + cover(rc[n]) * ev(rc[n], S)) / cover(n)
-
-    feats = sorted(set(sf))
-    M = len(feats)
-    phi = {f: 0.0 for f in feats}
-    for i in feats:
-        others = [f for f in feats if f != i]
-        for k in range(len(others) + 1):
-            wgt = math.factorial(k) * math.factorial(M - k - 1) / math.factorial(M)
-            for S in itertools.combinations(others, k):
-                S = set(S)
-                phi[i] += wgt * (ev(0, S | {i}) - ev(0, S))
-    return phi, ev(0, set())
-
-
 @pytest.mark.parametrize("name", ["regression", "binary", "regression_categorical|categorical_feature=4", "regression_quantile"])
 def test_feature_shap_equals_brute_force_shapley_values(name):
     """Independent known-answer test of the TreeSHAP predictor (C_API_PREDICT_CONTRIB, LightGBMBooster.featuresShap :412-423): the
@@ -318,6 +263,7 @@ def test_feature_shap_equals_brute_force_shapley_values(name):
     import os
     from mmlspark_b200.lightgbm import LightGBMRegressionModel
     from mmlspark_b200.modeltext import parse_model
+    from tree_walk_ref import brute_force_shap
     here = os.path.dirname(os.path.abspath(__file__))
     text = json.load(open(os.path.join(here, "golden", "oracle_golden.json")))["models"][name]["model"]
     trees = parse_model(text)["trees"]
@@ -334,7 +280,7 @@ def test_feature_shap_equals_brute_force_shapley_values(name):
     for x in rows:
         want = np.zeros(F + 1)
         for t in trees:
-            phi, e = _brute_force_shap(t, x)
+            phi, e = brute_force_shap(t, x)
             used = max(used, len(phi))
             for f, v in phi.items():
                 want[f] += v
