@@ -145,6 +145,8 @@ int LGBM_BoosterDumpModel(BoosterHandle handle, int start_iteration, int num_ite
                           int64_t buffer_len, int64_t* out_len, char* out_str);
 
 /* ---- prediction (per-row UDF semantics of the reference; host side) ------------------------ */
+/* `parameter` (NULL or "" = no keys): only the prediction early-stopping keys pred_early_stop, pred_early_stop_freq and
+ * pred_early_stop_margin are read (see B200GBM_BoosterPredictForMatDeviceWithParameter); every other key is ignored. */
 /* LGB/booster/LightGBMBooster.scala:528-545 */
 int LGBM_BoosterPredictForMatSingle(BoosterHandle handle, const void* data, int data_type, int ncol, int is_row_major,
                                     int predict_type, int start_iteration, int num_iteration, const char* parameter,
@@ -237,6 +239,15 @@ int B200GBM_BoosterGetScores(BoosterHandle handle, int data_idx, double* out);  
  * NULL) = CUDA-event time.  Replaces the per-row UDF calls of LightGBMBooster.scala:390-423,528-545 for whole partitions. */
 int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol, int predict_type,
                                        int start_iteration, int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms);
+/* B200GBM_BoosterPredictForMatDevice with the predict call's parameter string, in the position LightGBM's predict functions take it
+ * (NULL or "" = no keys, the same outputs bit for bit).  The keys read are pred_early_stop, pred_early_stop_freq (default 10) and
+ * pred_early_stop_margin (default 10.0), as LGBM_BoosterPredictForMat* read them: for a binary, multiclass, multiclassova, lambdarank or
+ * rank_xendcg model and a NORMAL or RAW_SCORE prediction, a row walks no more trees once, after a multiple of freq iterations, its
+ * margin (2|s| for one score, the largest minus the second largest score otherwise) exceeds the margin.  Outputs equal the single-row
+ * entries' with the same string bit for bit.  freq <= 0 or a margin < 0 (or NaN) fails the call when early stopping applies. */
+int B200GBM_BoosterPredictForMatDeviceWithParameter(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol,
+                                                    int predict_type, int start_iteration, int num_iteration, const char* parameter,
+                                                    int64_t* out_len, double* out_result, double* elapsed_ms);
 /* batched GPU prediction of a host CSR matrix (indptr INT32 or INT64, data FLOAT64), arguments of LGBM_BoosterPredictForCSRSingle plus
  * elapsed_ms.  Every output equals B200GBM_BoosterPredictForMatDevice on the densified rows bit for bit (a missing entry is 0, of
  * repeated indices the last wins, indices outside the model's features are ignored), and so LGBM_BoosterPredictForCSRSingle on the row:
@@ -246,6 +257,11 @@ int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, i
 int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
                                        int data_type, int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration,
                                        int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms);
+/* B200GBM_BoosterPredictForCSRDevice with the predict call's parameter string, read as by B200GBM_BoosterPredictForMatDeviceWithParameter */
+int B200GBM_BoosterPredictForCSRDeviceWithParameter(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices,
+                                                    const void* data, int data_type, int64_t nindptr, int64_t nelem, int64_t num_col,
+                                                    int predict_type, int start_iteration, int num_iteration, const char* parameter,
+                                                    int64_t* out_len, double* out_result, double* elapsed_ms);
 /* out = {num_machines, rank, histogram reduce mode (0 = ncclAllReduce, 3 = same-device all-reduce: every rank a thread of this process
  * on this device), constant_hessian} */
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4);

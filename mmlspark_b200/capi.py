@@ -114,6 +114,15 @@ class PinnedBuffer:
             self.ptr = C.c_void_p()
 
 
+def _param(parameter):
+    """a predict call's parameter string as a C string; None is a NULL pointer"""
+    return None if parameter is None else parameter.encode()
+
+
+def _single_row_param(parameter):
+    return b"max_bin=255" if parameter == "" else _param(parameter)
+
+
 def _vp(p):
     return p if isinstance(p, C.c_void_p) else C.c_void_p(int(p))
 
@@ -465,16 +474,19 @@ class Booster:
     def dump_model(self, start_iteration=0, num_iteration=-1):
         return self._string_call("LGBM_BoosterDumpModel", start_iteration, num_iteration, 10000)
 
-    def predict_for_mat_single(self, row, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1):
+    def predict_for_mat_single(self, row, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1, parameter=""):
+        """LGBM_BoosterPredictForMatSingle.  parameter: the predict call's key=value string (of which the pred_early_stop keys are
+        read); "" sends "max_bin=255" as the reference's UDFs do, None a NULL pointer."""
         row = np.ascontiguousarray(row, dtype=np.float64)
         n = C.c_int64(0)
         check(load().LGBM_BoosterCalcNumPredict(self.handle, C.c_int(1), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=np.float64)
         check(load().LGBM_BoosterPredictForMatSingle(self.handle, _ptr(row), C.c_int(DTYPE_FLOAT64), C.c_int(len(row)), C.c_int(1), C.c_int(predict_type),
-                                                     C.c_int(start_iteration), C.c_int(num_iteration), b"max_bin=255", C.byref(n), _ptr(out)))
+                                                     C.c_int(start_iteration), C.c_int(num_iteration), _single_row_param(parameter), C.byref(n), _ptr(out)))
         return out[:n.value].copy()
 
-    def predict_for_csr_single(self, indices, values, num_col, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1):
+    def predict_for_csr_single(self, indices, values, num_col, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1, parameter=""):
+        """LGBM_BoosterPredictForCSRSingle of one row; parameter as predict_for_mat_single's"""
         indices = np.ascontiguousarray(indices, dtype=np.int32); values = np.ascontiguousarray(values, dtype=np.float64)
         indptr = np.array([0, len(values)], dtype=np.int32)
         n = C.c_int64(0)
@@ -482,22 +494,24 @@ class Booster:
         out = np.zeros(max(n.value, 1), dtype=np.float64)
         check(load().LGBM_BoosterPredictForCSRSingle(self.handle, _ptr(indptr), C.c_int(DTYPE_INT32), _ptr(indices), _ptr(values), C.c_int(DTYPE_FLOAT64),
                                                      C.c_int64(2), C.c_int64(len(values)), C.c_int64(num_col), C.c_int(predict_type), C.c_int(start_iteration),
-                                                     C.c_int(num_iteration), b"max_bin=255", C.byref(n), _ptr(out)))
+                                                     C.c_int(num_iteration), _single_row_param(parameter), C.byref(n), _ptr(out)))
         return out[:n.value].copy()
 
-    def predict_for_mat(self, X, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1):
+    def predict_for_mat(self, X, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1, parameter=""):
+        """LGBM_BoosterPredictForMat (host); parameter: the predict call's key=value string, None for a NULL pointer"""
         X = np.ascontiguousarray(X, dtype=np.float64)
         nrow, ncol = X.shape
         n = C.c_int64(0)
         check(load().LGBM_BoosterCalcNumPredict(self.handle, C.c_int(nrow), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=np.float64)
         check(load().LGBM_BoosterPredictForMat(self.handle, _ptr(X), C.c_int(DTYPE_FLOAT64), C.c_int32(nrow), C.c_int32(ncol), C.c_int(1), C.c_int(predict_type),
-                                               C.c_int(start_iteration), C.c_int(num_iteration), b"", C.byref(n), _ptr(out)))
+                                               C.c_int(start_iteration), C.c_int(num_iteration), _param(parameter), C.byref(n), _ptr(out)))
         return out[:n.value].reshape(nrow, -1)
 
     # --- engine extensions
-    def predict_device(self, X, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1, return_ms=False):
-        """Batched GPU prediction (B200GBM_BoosterPredictForMatDevice); X: float32/float64 [nrow, ncol] host array."""
+    def predict_device(self, X, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1, return_ms=False, parameter=""):
+        """Batched GPU prediction (B200GBM_BoosterPredictForMatDeviceWithParameter); X: float32/float64 [nrow, ncol] host array.
+        parameter: the predict call's key=value string (pred_early_stop, pred_early_stop_freq, pred_early_stop_margin), None for NULL."""
         X = np.ascontiguousarray(X)
         if X.dtype not in (np.float32, np.float64):
             X = X.astype(np.float64)
@@ -506,15 +520,17 @@ class Booster:
         check(load().LGBM_BoosterCalcNumPredict(self.handle, C.c_int(nrow), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=np.float64)
         ms = C.c_double(0)
-        check(load().B200GBM_BoosterPredictForMatDevice(self.handle, _ptr(X), C.c_int(_np_dtype_code(X)), C.c_int64(nrow), C.c_int32(ncol), C.c_int(predict_type),
-                                                        C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n), _ptr(out), C.byref(ms)))
+        check(load().B200GBM_BoosterPredictForMatDeviceWithParameter(
+            self.handle, _ptr(X), C.c_int(_np_dtype_code(X)), C.c_int64(nrow), C.c_int32(ncol), C.c_int(predict_type), C.c_int(start_iteration),
+            C.c_int(num_iteration), _param(parameter), C.byref(n), _ptr(out), C.byref(ms)))
         res = out[:n.value].reshape(nrow, -1)
         return (res, ms.value) if return_ms else res
 
     def predict_csr_device(self, indptr, indices=None, data=None, num_col=None, predict_type=PREDICT_NORMAL, start_iteration=0, num_iteration=-1,
-                           return_ms=False):
-        """Batched GPU prediction of CSR rows (B200GBM_BoosterPredictForCSRDevice): host indptr (int32/int64), indices, float64 data,
-        or a scipy.sparse matrix as the first argument.  Same values as predict_for_csr_single row by row."""
+                           return_ms=False, parameter=""):
+        """Batched GPU prediction of CSR rows (B200GBM_BoosterPredictForCSRDeviceWithParameter): host indptr (int32/int64), indices, float64
+        data, or a scipy.sparse matrix as the first argument.  Same values as predict_for_csr_single row by row; parameter as
+        predict_device's."""
         if not isinstance(indptr, np.ndarray) and hasattr(indptr, "tocsr"):      # scipy.sparse
             m = indptr.tocsr()
             indptr, indices, data, num_col = m.indptr, m.indices, m.data, m.shape[1]
@@ -528,10 +544,10 @@ class Booster:
         check(load().LGBM_BoosterCalcNumPredict(self.handle, C.c_int(max(nrow, 0)), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=np.float64)
         ms = C.c_double(0)
-        check(load().B200GBM_BoosterPredictForCSRDevice(self.handle, _ptr(indptr), C.c_int(DTYPE_INT32 if indptr.dtype == np.int32 else DTYPE_INT64),
-                                                        _ptr(indices), _ptr(data), C.c_int(DTYPE_FLOAT64), C.c_int64(len(indptr)), C.c_int64(len(data)),
-                                                        C.c_int64(num_col), C.c_int(predict_type), C.c_int(start_iteration), C.c_int(num_iteration),
-                                                        C.byref(n), _ptr(out), C.byref(ms)))
+        check(load().B200GBM_BoosterPredictForCSRDeviceWithParameter(
+            self.handle, _ptr(indptr), C.c_int(DTYPE_INT32 if indptr.dtype == np.int32 else DTYPE_INT64), _ptr(indices), _ptr(data),
+            C.c_int(DTYPE_FLOAT64), C.c_int64(len(indptr)), C.c_int64(len(data)), C.c_int64(num_col), C.c_int(predict_type),
+            C.c_int(start_iteration), C.c_int(num_iteration), _param(parameter), C.byref(n), _ptr(out), C.byref(ms)))
         res = out[:n.value].reshape(nrow, n.value // max(nrow, 1))
         return (res, ms.value) if return_ms else res
 

@@ -262,21 +262,30 @@ static void RowToDouble(const void* data, int data_type, int ncol, std::vector<d
   else if (data_type == C_API_DTYPE_FLOAT32) for (int i = 0; i < ncol; ++i) (*row)[i] = static_cast<const float*>(data)[i];
   else Fatal("Unknown data type in predict");
 }
+// the early-stop setting of a predict call's parameter string (NULL or empty: no keys); the only predict keys read
+static EarlyStop PredictParams(const char* parameter, const HostModel& m, int predict_type) {
+  Config c;
+  c.Parse(parameter);
+  return PredictEarlyStop(c, m, predict_type);
+}
 int LGBM_BoosterPredictForMatSingle(BoosterHandle handle, const void* data, int data_type, int ncol, int is_row_major, int predict_type,
                                     int start_iteration, int num_iteration, const char* parameter, int64_t* out_len, double* out_result) {
   API_BEGIN();
-  (void)is_row_major; (void)parameter;
+  (void)is_row_major;
+  const HostModel& m = BS(handle)->model;
+  const EarlyStop es = PredictParams(parameter, m, predict_type);
   std::vector<double> row;
   RowToDouble(data, data_type, ncol, &row);
-  *out_len = BS(handle)->model.PredictRow(row.data(), ncol, predict_type, start_iteration, num_iteration, out_result);
+  *out_len = m.PredictRow(row.data(), ncol, predict_type, start_iteration, num_iteration, out_result, es);
   API_END();
 }
 int LGBM_BoosterPredictForCSRSingle(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type,
                                     int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration, int num_iteration,
                                     const char* parameter, int64_t* out_len, double* out_result) {
   API_BEGIN();
-  (void)parameter; (void)nindptr;
+  (void)nindptr;
   Booster* b = BS(handle);
+  const EarlyStop es = PredictParams(parameter, b->model, predict_type);
   int64_t ncol = std::max<int64_t>(num_col, b->model.max_feature_idx + 1);
   std::vector<double> row(ncol, 0.0);
   int64_t a = indptr_type == C_API_DTYPE_INT32 ? static_cast<const int32_t*>(indptr)[0] : static_cast<const int64_t*>(indptr)[0];
@@ -286,7 +295,7 @@ int LGBM_BoosterPredictForCSRSingle(BoosterHandle handle, const void* indptr, in
     double v = data_type == C_API_DTYPE_FLOAT32 ? static_cast<const float*>(data)[k] : static_cast<const double*>(data)[k];
     if (indices[k] >= 0 && indices[k] < ncol) row[indices[k]] = v;
   }
-  *out_len = b->model.PredictRow(row.data(), static_cast<int>(ncol), predict_type, start_iteration, num_iteration, out_result);
+  *out_len = b->model.PredictRow(row.data(), static_cast<int>(ncol), predict_type, start_iteration, num_iteration, out_result, es);
   API_END();
 }
 int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_type, int start_iteration, int num_iteration, int64_t* out_len) {
@@ -297,8 +306,8 @@ int LGBM_BoosterCalcNumPredict(BoosterHandle handle, int num_row, int predict_ty
 int LGBM_BoosterPredictForMat(BoosterHandle handle, const void* data, int data_type, int32_t nrow, int32_t ncol, int is_row_major, int predict_type,
                               int start_iteration, int num_iteration, const char* parameter, int64_t* out_len, double* out_result) {
   API_BEGIN();
-  (void)parameter;
   const HostModel& m = BS(handle)->model;
+  const EarlyStop es = PredictParams(parameter, m, predict_type);
   const int64_t per = m.NumPredictPerRow(predict_type, start_iteration, num_iteration);
 #pragma omp parallel
   {
@@ -309,7 +318,7 @@ int LGBM_BoosterPredictForMat(BoosterHandle handle, const void* data, int data_t
         size_t at = is_row_major ? static_cast<size_t>(i) * ncol + f : static_cast<size_t>(f) * nrow + i;
         row[f] = data_type == C_API_DTYPE_FLOAT32 ? static_cast<const float*>(data)[at] : static_cast<const double*>(data)[at];
       }
-      m.PredictRow(row.data(), ncol, predict_type, start_iteration, num_iteration, out_result + per * i);
+      m.PredictRow(row.data(), ncol, predict_type, start_iteration, num_iteration, out_result + per * i, es);
     }
   }
   *out_len = per * nrow;
@@ -632,23 +641,41 @@ int B200GBM_BoosterGetTiming(BoosterHandle handle, double* out6, int reset) {
   if (reset) b->timing = Booster::Timing();
   API_END();
 }
+int B200GBM_BoosterPredictForMatDeviceWithParameter(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol,
+                                                    int predict_type, int start_iteration, int num_iteration, const char* parameter,
+                                                    int64_t* out_len, double* out_result, double* elapsed_ms) {
+  API_BEGIN();
+  Booster* b = BS(handle);
+  const EarlyStop es = PredictParams(parameter, b->model, predict_type);
+  Predictor& p = *b->predictor;
+  *out_len = p.PredictMat(data, data_type, nrow, ncol, predict_type, start_iteration, num_iteration, es, out_result);
+  if (elapsed_ms) *elapsed_ms = p.last_ms;
+  API_END();
+}
 int B200GBM_BoosterPredictForMatDevice(BoosterHandle handle, const void* data, int data_type, int64_t nrow, int32_t ncol, int predict_type,
                                        int start_iteration, int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms) {
+  return B200GBM_BoosterPredictForMatDeviceWithParameter(handle, data, data_type, nrow, ncol, predict_type, start_iteration, num_iteration,
+                                                         nullptr, out_len, out_result, elapsed_ms);
+}
+int B200GBM_BoosterPredictForCSRDeviceWithParameter(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices,
+                                                    const void* data, int data_type, int64_t nindptr, int64_t nelem, int64_t num_col,
+                                                    int predict_type, int start_iteration, int num_iteration, const char* parameter,
+                                                    int64_t* out_len, double* out_result, double* elapsed_ms) {
   API_BEGIN();
-  Predictor& p = *BS(handle)->predictor;
-  *out_len = p.PredictMat(data, data_type, nrow, ncol, predict_type, start_iteration, num_iteration, out_result);
+  (void)num_col;      // like LGBM_BoosterPredictForCSRSingle: columns past the model's features are never read
+  Booster* b = BS(handle);
+  const EarlyStop es = PredictParams(parameter, b->model, predict_type);
+  Predictor& p = *b->predictor;
+  *out_len = p.PredictCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, predict_type, start_iteration, num_iteration, es,
+                          out_result);
   if (elapsed_ms) *elapsed_ms = p.last_ms;
   API_END();
 }
 int B200GBM_BoosterPredictForCSRDevice(BoosterHandle handle, const void* indptr, int indptr_type, const int32_t* indices, const void* data,
                                        int data_type, int64_t nindptr, int64_t nelem, int64_t num_col, int predict_type, int start_iteration,
                                        int num_iteration, int64_t* out_len, double* out_result, double* elapsed_ms) {
-  API_BEGIN();
-  (void)num_col;      // like LGBM_BoosterPredictForCSRSingle: columns past the model's features are never read
-  Predictor& p = *BS(handle)->predictor;
-  *out_len = p.PredictCSR(indptr, indptr_type, indices, data, data_type, nindptr, nelem, predict_type, start_iteration, num_iteration, out_result);
-  if (elapsed_ms) *elapsed_ms = p.last_ms;
-  API_END();
+  return B200GBM_BoosterPredictForCSRDeviceWithParameter(handle, indptr, indptr_type, indices, data, data_type, nindptr, nelem, num_col,
+                                                         predict_type, start_iteration, num_iteration, nullptr, out_len, out_result, elapsed_ms);
 }
 int B200GBM_BoosterGetInfo(BoosterHandle handle, int* out4) {
   API_BEGIN();

@@ -94,6 +94,11 @@ struct Config {
   double lambdarank_position_bias_regularization = 0.0;
   std::vector<int> eval_at;
   std::vector<double> auc_mu_weights;       // auc_mu's K x K class-pair weights, row-major; empty = 1 off the diagonal, 0 on it
+  // --- predict: read from a predict call's parameter string only, never printed (the saved params block has no predict section).
+  // HostModel::PredictEarlyStop decides whether they apply and checks them.
+  bool pred_early_stop = false;
+  int pred_early_stop_freq = 10;
+  double pred_early_stop_margin = 10.0;
   // --- network
   int num_machines = 1;
   std::map<std::string, std::string> raw;
@@ -262,6 +267,7 @@ struct Config {
     I("lambdarank_truncation_level", &lambdarank_truncation_level);
     B("lambdarank_norm", &lambdarank_norm); I("num_machines", &num_machines);
     D("lambdarank_position_bias_regularization", &lambdarank_position_bias_regularization);
+    B("pred_early_stop", &pred_early_stop); I("pred_early_stop_freq", &pred_early_stop_freq); D("pred_early_stop_margin", &pred_early_stop_margin);
     {
       auto it = raw.find("label_gain");
       if (it != raw.end() && !it->second.empty()) SplitList(it->second, &label_gain, [](const std::string& x) { return std::atof(x.c_str()); });

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "bin_mapper.h"
+#include "config.h"
 
 namespace b200gbm {
 
@@ -279,6 +280,25 @@ struct HostTree {
   }
 };
 
+// prediction early stopping ([UPSTREAM] prediction_early_stop.cpp, from knowledge): after every `freq` iterations a row whose margin
+// exceeds `margin` walks no more trees.  freq 0 is off.  PredictEarlyStop below makes the setting; the host predictor
+// (HostModel::PredictRow) and the device one (k_predict_raw_es) run it.
+struct EarlyStop {
+  int freq = 0;
+  double margin = 0.0;
+  bool on() const { return freq > 0; }
+  // K == 1: 2|s|; K >= 2: the largest score minus the second largest (tied maxima give 0), as upstream's partial_sort
+  static double Margin(const double* s, int K) {
+    if (K == 1) return 2.0 * std::fabs(s[0]);
+    double a = -INFINITY, b = -INFINITY;
+    for (int k = 0; k < K; ++k) {
+      if (s[k] > a) { b = a; a = s[k]; }
+      else if (s[k] > b) b = s[k];
+    }
+    return a - b;
+  }
+};
+
 struct HostModel {
   int num_class = 1;
   int num_tree_per_iteration = 1;
@@ -451,6 +471,17 @@ struct HostModel {
     *t = r;
     return true;
   }
+  // objectives whose raw scores may stop summing once a row's margin is decided: [UPSTREAM] NeedAccuratePrediction() is false for
+  // BinaryLogloss, MulticlassSoftmax, MulticlassOVA and the ranking objectives (from knowledge).  Every other objective, a custom one and
+  // a model without one needs every tree.
+  static bool AllowsPredictEarlyStop(const std::string& o) {
+    static const char* const kNames[] = {"binary", "multiclass", "multiclassova", "lambdarank", "rank_xendcg"};
+    std::istringstream is(o);
+    std::string name;
+    is >> name;
+    for (const char* n : kNames) if (name == n) return true;
+    return false;
+  }
   // nrow rows of K raw scores, class k of row i at s[i * row_step + k * class_step], turned into outputs in place: the mean over
   // `iterations` for an averaged (rf) model when iterations > 0, then the objective transform unless raw
   void ConvertScores(double* s, int64_t nrow, int64_t row_step, int64_t class_step, int iterations, bool raw) const {
@@ -492,8 +523,10 @@ struct HostModel {
     *t0 = start_iteration * num_tree_per_iteration;
     *t1 = end * num_tree_per_iteration;
   }
-  // predict_type: 0 normal, 1 raw, 2 leaf index, 3 contrib.  Returns number of outputs written.
-  int64_t PredictRow(const double* row, int ncol, int predict_type, int start_iteration, int num_iteration, double* out) const {
+  // predict_type: 0 normal, 1 raw, 2 leaf index, 3 contrib.  Returns number of outputs written.  `es` (PredictEarlyStop) ends the raw
+  // sums of normal and raw predictions once the row's margin is decided.
+  int64_t PredictRow(const double* row, int ncol, int predict_type, int start_iteration, int num_iteration, double* out,
+                     const EarlyStop& es = EarlyStop()) const {
     int t0, t1;
     IterRange(start_iteration, num_iteration, &t0, &t1);
     const int K = num_tree_per_iteration;
@@ -511,11 +544,31 @@ struct HostModel {
       for (int t = t0; t < t1; ++t) trees[t]->AddContrib(row, max_feature_idx + 1, out + (t % K) * nf1);
     } else {
       for (int k = 0; k < K; ++k) out[k] = 0;
-      for (int t = t0; t < t1; ++t) out[t % K] += trees[t]->Predict(row);
+      int c = 0;      // [UPSTREAM] GBDT::PredictRaw: the margin is checked after every es.freq iterations; freq 0 never matches
+      for (int t = t0; t < t1; t += K) {
+        for (int k = 0; k < K; ++k) out[k] += trees[t + k]->Predict(row);
+        if (++c == es.freq) {
+          if (es.Margin(out, K) > es.margin) break;
+          c = 0;
+        }
+      }
       ConvertScores(out, 1, K, 1, (t1 - t0) / K, predict_type == 1);
     }
     return NumPredictPerRow(predict_type, start_iteration, num_iteration);
   }
 };
+
+// The early-stop setting of one predict call: on when the call's parameters give pred_early_stop=true, the predict type is normal (0) or
+// raw (1) and the model's objective allows it (HostModel::AllowsPredictEarlyStop); otherwise off, whatever the other two keys say.
+// When on, [UPSTREAM] Predictor's checks run and fail the call.
+inline EarlyStop PredictEarlyStop(const Config& cfg, const HostModel& m, int predict_type) {
+  EarlyStop es;
+  if (!cfg.pred_early_stop || (predict_type != 0 && predict_type != 1) || !HostModel::AllowsPredictEarlyStop(m.objective_str)) return es;
+  if (!(cfg.pred_early_stop_freq > 0)) throw std::runtime_error("Check failed: (early_stop_freq) > (0)");
+  if (!(cfg.pred_early_stop_margin >= 0)) throw std::runtime_error("Check failed: (early_stop_margin) >= (0)");
+  es.freq = cfg.pred_early_stop_freq;
+  es.margin = cfg.pred_early_stop_margin;
+  return es;
+}
 
 }  // namespace b200gbm

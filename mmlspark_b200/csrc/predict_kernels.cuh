@@ -67,6 +67,62 @@ k_predict_raw(ForestDev f, const T* __restrict__ X, long long nrow, int ncol, in
     out[e] = acc;
   }
 }
+// Raw scores with prediction early stopping (EarlyStop, model.h): the iterations [i0, i1) of K trees each, and after every `freq` of
+// them a row whose margin exceeds `margin` walks no more trees.  The K class walks of a row meet at each check, so a group of G lanes
+// (a power of two, G <= 32) owns one row: with K <= G lane k walks class k and keeps its sum in a register; with K > G (K > 32, G = 32)
+// lane l walks the classes l, l + G, ... and keeps their sums in the row's output slots, which only it touches.  Per class the additions
+// are HostModel::PredictRow's, in its order, from 0.0, so every score is the host's bit for bit.  The margin is taken from the sums
+// exactly as EarlyStop::Margin: 2|s| for K == 1, else the largest minus the second largest, the group's top two combined over xor
+// shuffles so every lane of the group gets the same pair and takes the same branch.  The launch gives each group one row, so a
+// stopped row's lanes fall idle until the rows of the rest of their warp finish.
+__device__ __forceinline__ void d_top2_merge(double& a, double& b, double a2, double b2) {      // (a, b), (a2, b2): top two, a >= b
+  const double lo = a < a2 ? a : a2;
+  b = b > b2 ? b : b2;
+  b = b > lo ? b : lo;
+  a = a > a2 ? a : a2;
+}
+template <typename T, int G>
+__global__ void __launch_bounds__(256)
+k_predict_raw_es(ForestDev f, const T* __restrict__ X, long long nrow, int ncol, int K, int i0, int i1, int freq, double margin,
+                 double* __restrict__ out) {
+  const int lane = threadIdx.x & (G - 1);
+  const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1));
+  const long long groups = (static_cast<long long>(gridDim.x) * blockDim.x) / G;
+  for (long long r = (blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x) / G; r < nrow; r += groups) {
+    const T* row = X + r * ncol;
+    double* o = out + r * K;
+    double s = 0.0;                                    // K <= G: class `lane`'s sum
+    if (K > G) for (int k = lane; k < K; k += G) o[k] = 0.0;
+    int c = 0;
+    for (int it = i0; it < i1; ++it) {
+      const int tb = it * K;
+      if (K <= G) {
+        if (lane < K) s += f.leaf_value[f.leaf_offset[tb + lane] + d_tree_leaf(f, tb + lane, row)];
+      } else {
+        for (int k = lane; k < K; k += G) o[k] += f.leaf_value[f.leaf_offset[tb + k] + d_tree_leaf(f, tb + k, row)];
+      }
+      if (++c != freq) continue;
+      c = 0;
+      if (K == 1) {
+        if (2.0 * fabs(s) > margin) break;
+        continue;
+      }
+      double a = -INFINITY, b = -INFINITY;
+      if (K <= G) {
+        if (lane < K) a = s;
+      } else {
+        for (int k = lane; k < K; k += G) d_top2_merge(a, b, o[k], -INFINITY);
+      }
+#pragma unroll
+      for (int m = 1; m < G; m <<= 1) {
+        const double a2 = __shfl_xor_sync(gmask, a, m, G), b2 = __shfl_xor_sync(gmask, b, m, G);
+        d_top2_merge(a, b, a2, b2);
+      }
+      if (a - b > margin) break;
+    }
+    if (K <= G && lane < K) o[lane] = s;
+  }
+}
 template <typename T>
 __global__ void __launch_bounds__(256)
 k_predict_leaf(ForestDev f, const T* __restrict__ X, long long nrow, int ncol, int t0, int t1, double* __restrict__ out) {

@@ -87,12 +87,31 @@ struct ShapScratch {
   }
 };
 
+// k_predict_raw_es with a group of G lanes per row: one lane for K == 1, the next power of two up to 32 for K <= 32, a warp beyond.
+// One group per row of the chunk (no grid-stride reuse): every group of a warp starts at the first iteration and walks the same tree
+// index as the others until it stops, so the still-active rows of a warp stay converged.  A group that took a second row after its
+// first stopped would walk other trees than its warp neighbours, and the warp would run both walks one after the other.
+template <typename T>
+void Predictor::LaunchRawEarlyStop(const ForestDev& f, const T* X, int64_t rows, int ncol, int K, int i0, int i1, const EarlyStop& es, double* y) {
+  const int G = K == 1 ? 1 : K <= 2 ? 2 : K <= 4 ? 4 : K <= 8 ? 8 : K <= 16 ? 16 : 32;
+  const int grid = static_cast<int>((rows * G + 255) / 256);
+  switch (G) {
+    case 1: k_predict_raw_es<T, 1><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+    case 2: k_predict_raw_es<T, 2><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+    case 4: k_predict_raw_es<T, 4><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+    case 8: k_predict_raw_es<T, 8><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+    case 16: k_predict_raw_es<T, 16><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+    default: k_predict_raw_es<T, 32><<<grid, 256, 0, stream_>>>(f, X, rows, ncol, K, i0, i1, es.freq, es.margin, y); break;
+  }
+}
+
 // The chunk loop of dense and CSR input: chunk [r0, end(r0)) has at most `chunk` rows.  stage(r0, rows, launch, dout) puts the chunk's
 // rows on the device and calls launch(f, X, data_type, rows, ncol, F1, y), which enqueues the predict kernel of predict_type on X
 // [rows][ncol] into y (contributions: [rows][K][F1], zero-filled here).  Each chunk's dout is copied out and waited for.  last_ms spans
 // the loop; the rf averaging and the objective transform run on the host after it.
 template <typename End, typename Stage>
-int64_t Predictor::Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict_type, int t0, int t1, double* out, End end, Stage stage) {
+int64_t Predictor::Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict_type, int t0, int t1, const EarlyStop& es, double* out, End end,
+                       Stage stage) {
   const int Kc = model_.num_tree_per_iteration;
   const int64_t rows_max = std::min(chunk, nrow);
   ShapScratch shap(forest_->max_depth, predict_type == 3 ? rows_max : 0, DeviceSMs());
@@ -109,6 +128,9 @@ int64_t Predictor::Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict
     } else if (predict_type == 2) {
       if (data_type == 0) k_predict_leaf<float><<<grid, 256, 0, stream_>>>(f, xf, rows, ncol, t0, t1, y);
       else k_predict_leaf<double><<<grid, 256, 0, stream_>>>(f, xd, rows, ncol, t0, t1, y);
+    } else if (es.on()) {
+      if (data_type == 0) LaunchRawEarlyStop(f, xf, rows, ncol, Kc, t0 / Kc, t1 / Kc, es, y);
+      else LaunchRawEarlyStop(f, xd, rows, ncol, Kc, t0 / Kc, t1 / Kc, es, y);
     } else {
       if (data_type == 0) k_predict_raw<float><<<grid, 256, 0, stream_>>>(f, xf, rows, ncol, Kc, t0, t1, y);
       else k_predict_raw<double><<<grid, 256, 0, stream_>>>(f, xd, rows, ncol, Kc, t0, t1, y);
@@ -129,7 +151,7 @@ int64_t Predictor::Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict
 }
 
 int64_t Predictor::PredictMat(const void* data, int data_type, int64_t nrow, int ncol, int predict_type, int start_iteration, int num_iteration,
-                              double* out) {
+                              const EarlyStop& es, double* out) {
   EnsureDevice();
   if (data_type != 0 && data_type != 1) Fatal("PredictBatch: unknown data type");
   if (predict_type < 0 || predict_type > 3) Fatal("PredictBatch: unknown predict type");
@@ -143,7 +165,7 @@ int64_t Predictor::PredictMat(const void* data, int data_type, int64_t nrow, int
   const int64_t chunk = ChunkRows(nrow, on_device ? 0 : static_cast<int64_t>(ncol) * esz, per_row);
   DevBuf<unsigned char> xin;
   if (!on_device) xin.Alloc(static_cast<size_t>(chunk) * ncol * esz);
-  return Run(nrow, chunk, per_row, predict_type, t0, t1, out, [&](int64_t r0) { return std::min(nrow, r0 + chunk); },
+  return Run(nrow, chunk, per_row, predict_type, t0, t1, es, out, [&](int64_t r0) { return std::min(nrow, r0 + chunk); },
              [&](int64_t r0, int64_t rows, auto& launch, double* dout) {
     const void* x = static_cast<const unsigned char*>(data) + static_cast<size_t>(r0) * ncol * esz;
     if (!on_device) { B200_CUDA(cudaMemcpyAsync(xin.p, x, static_cast<size_t>(rows) * ncol * esz, cudaMemcpyHostToDevice, stream_)); x = xin.p; }
@@ -152,7 +174,7 @@ int64_t Predictor::PredictMat(const void* data, int data_type, int64_t nrow, int
 }
 
 int64_t Predictor::PredictCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
-                              int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out) {
+                              int64_t nelem, int predict_type, int start_iteration, int num_iteration, const EarlyStop& es, double* out) {
   if (indptr_type != 2 && indptr_type != 3) Fatal("PredictBatchCSR: indptr must be INT32 or INT64");
   if (data_type != 1) Fatal("PredictBatchCSR: CSR values must be FLOAT64");
   if (predict_type < 0 || predict_type > 3) Fatal("PredictBatchCSR: unknown predict type");
@@ -196,7 +218,7 @@ int64_t Predictor::PredictCSR(const void* indptr, int indptr_type, const int32_t
   DevBuf<double> xs; xs.Alloc(static_cast<size_t>(rows_max) * U);
   DevBuf<double> dslot; dslot.Alloc(predict_type == 3 ? static_cast<size_t>(rows_max) * Kc * (U + 1) : 0);      // contributions per slot
   std::vector<long long> hptr(static_cast<size_t>(rows_max) + 1);
-  return Run(nrow, chunk, per_row, predict_type, t0, t1, out, end, [&](int64_t r0, int64_t rows, auto& launch, double* dout) {
+  return Run(nrow, chunk, per_row, predict_type, t0, t1, es, out, end, [&](int64_t r0, int64_t rows, auto& launch, double* dout) {
     const int64_t a = ptr(r0), nnz = ptr(r0 + rows) - a;
     for (int64_t i = 0; i <= rows; ++i) hptr[i] = ptr(r0 + i) - a;
     d_ptr.Upload(hptr.data(), static_cast<size_t>(rows) + 1, stream_);

@@ -12,13 +12,14 @@ class Predictor {
   Predictor(const HostModel& model, cudaStream_t& stream) : model_(model), stream_(stream) {}
   void Invalidate() { forest_.reset(); }      // leaf values on the device are stale (DART); a new tree count is noticed without this
   // a row-major matrix (host or device pointer); predict_type 0 normal, 1 raw, 2 leaf index, 3 contributions.
+  // `es` (PredictEarlyStop) on: normal and raw scores stop early per row (k_predict_raw_es), bit for bit HostModel::PredictRow's.
   // Returns the number of doubles written to `out` (host).  last_ms = kernel time (CUDA events), incl. H2D for host input.
   int64_t PredictMat(const void* data, int data_type, int64_t nrow, int ncol, int predict_type, int start_iteration, int num_iteration,
-                     double* out);
+                     const EarlyStop& es, double* out);
   // the same over a host CSR matrix (indptr_type 2 = int32, 3 = int64; data_type 1 = float64), uploaded in chunks of rows: every output
   // equals PredictMat's on the densified rows.  indptr must start at 0 or above, never decrease and end at most at nelem.
   int64_t PredictCSR(const void* indptr, int indptr_type, const int32_t* indices, const void* data, int data_type, int64_t nindptr,
-                     int64_t nelem, int predict_type, int start_iteration, int num_iteration, double* out);
+                     int64_t nelem, int predict_type, int start_iteration, int num_iteration, const EarlyStop& es, double* out);
   double last_ms = 0.0;
 
  private:
@@ -31,8 +32,11 @@ class Predictor {
   };
   void UploadForest();
   const SlotBufs& UploadSlots(int t0, int t1);
+  template <typename T>
+  void LaunchRawEarlyStop(const ForestDev& f, const T* X, int64_t rows, int ncol, int K, int i0, int i1, const EarlyStop& es, double* y);
   template <typename End, typename Stage>
-  int64_t Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict_type, int t0, int t1, double* out, End end, Stage stage);
+  int64_t Run(int64_t nrow, int64_t chunk, int64_t per_row, int predict_type, int t0, int t1, const EarlyStop& es, double* out, End end,
+              Stage stage);
 
   const HostModel& model_;
   cudaStream_t& stream_;
